@@ -3,6 +3,7 @@
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config c1|c2|c2h|c3|c4|c5] [--impl ours|reference]
                     [--engine auto|simt_fp32|tc_3x|tc_3x_w1 (reduced precision, labelled so)] [--graph 0|1] [--device cpu|cuda (reference arm)]
+                    [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one synthetic ray batch of a BASELINE config, through the public API
 (`Graph.render_image_at_specific_rays` + the loss module's `compute_loss` + `backward()`), gradients zeroed each step:
@@ -21,6 +22,10 @@ Timing: W warm-up steps, then K steps between a barrier + synchronize on both si
 CUDA events on the launching stream, with an L2 flush (256 MiB memset) between steps outside the event pairs and (default)
 a synchronize after each step; ms_per_step = mean of the K intervals, MAX over ranks.  `--sync-each-step 0` enqueues the K
 steps back to back instead.  Clocks / throttle reasons are sampled with nvidia-smi during the timed region.  Prints ONE JSON line (rank 0).
+
+`--dump-outputs DIR` (rank 0): after the timed steps, writes what the last step returned to its caller -- DIR/loss.npy
+(float64 [1]) and DIR/grad.npy (float32, the flat gradient buffer [d theta_coarse | d theta_fine | d pose]).  Inputs
+depend only on the arguments (seeded scene, weights and ray draws), so two builds can be compared output for output.
 
 `--impl reference` times the UNMODIFIED reference (oracle/_ref, made by oracle/build_ref.py) on the host cores
 (`--device cuda`: on the GPU, the torch/cuBLAS path SURVEY 8d calls "the kernel to beat"); without oracle/_ref it
@@ -71,8 +76,8 @@ CONFIGS = {
                desc="Replica-shaped 9 views 340x600, 9x455=4095 rays sharded over the GPUs, hierarchical 128 + 256 samples, pose gradients in the reduced buffer, photometric loss, fwd+bwd"),
 }
 METRIC = "rays/sec (fwd+bwd, 128 samples/ray)"
-DTYPE = ("fp32 in / out; GEMMs on tcgen05 kind::f16 with a 3-pass error-compensated split (fp16 halves forward, bf16 "
-         "halves backward), fp32 TMEM accumulation; fp32 CUDA cores for encoding / activations / compositing")
+DTYPE = ("fp32 in / out; GEMMs on Hopper wgmma with a 3-pass error-compensated split (fp16 halves forward, bf16 "
+         "halves backward), fp32 accumulation; fp32 CUDA cores for encoding / activations / compositing")
 ENGINE_DTYPE = {"auto": DTYPE, "tc_3x": DTYPE,
                 "tc_3x_w1": "REDUCED PRECISION (non-default engine, not a parity number): as tc_3x, but the weight gradients in "
                             "ONE bf16 pass over the hi halves of the saved images",
@@ -85,7 +90,8 @@ def load_peaks():
         d = json.load(open(path))
         return dict(bf16_tflops=d["bf16_tflops"], bf16_tflops_sustained=d.get("bf16_tflops_sustained"),
                     hbm_gbs=d["hbm_gbs"], source="measured (MEASURED_PEAKS.json)")
-    return dict(bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, hbm_gbs=6650.0, source="fallback (B200_PROFILING.md)")
+    return dict(bf16_tflops=989.0, bf16_tflops_sustained=None, hbm_gbs=3350.0,
+                source="NVIDIA H100 SXM data sheet (dense bf16, 700 W card; not measured)")
 
 
 # ------------------------------------------------------------------------------------------------ clocks
@@ -336,9 +342,7 @@ def run_ours(args):
     def timed(n_warm, n_steps, e2e, use_graph=False):
         # every step is bracketed by its own pair of CUDA events on the launching stream with the L2 flush outside the
         # pair; barrier + synchronize on both sides of the whole loop.  By default the host also synchronises after each
-        # step (--sync-each-step 0: the steps are enqueued back to back; measured 1.364 vs 1.350 ms on the same
-        # power-capped box, the launch latency of a graph replay on an idle device is below the noise).  The
-        # end-to-end arm always waits for every step's loss on the host (a caller that reads its result).
+        # step (--sync-each-step 0: the steps are enqueued back to back).  The end-to-end arm always waits for every step's loss on the host (a caller that reads its result).
         if world > 1:
             dist.barrier()
         torch.cuda.synchronize()
@@ -388,6 +392,11 @@ def run_ours(args):
         total_ms, times = timed(0, args.steps, False, use_graph=True)
         launches = launches_per_graph * args.steps
     e2e_ms, _ = timed(args.warmup, args.steps, True, use_graph=graphed is not None)
+    if args.dump_outputs and rank == 0:     # what the last timed step returned: its loss and the gradient buffer
+        torch.cuda.synchronize()
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "loss.npy"), np.array([float(loss_host)], dtype=np.float64))
+        np.save(os.path.join(args.dump_outputs, "grad.npy"), flat.detach().float().cpu().numpy())
     # cost of the collective alone (rank 0's view): the all-reduce of the flat buffer, timed back to back
     ar_us = None
     if world > 1:
@@ -425,8 +434,8 @@ def run_ours(args):
     # step time is the (conservative) upper bound of the group's duration.
     group_ms = min(mlp_ms_per_step, ms_per_step) if mlp_ms_per_step else ms_per_step
     achieved = flop_step_gpu / (group_ms * 1e-3) / 1e12
-    roofline = dict(bound="tensor", kernel="MLP fwd+bwd kernels of one step (sparf_mlp_forward_tape + sparf_mlp_backward_tape: "
-                                           "tc_mlp_fwd / dgrad / wgrad + small kernels)",
+    roofline = dict(bound="tensor", kernel="MLP fwd+bwd kernels of one step (sparf_mlp_forward + sparf_mlp_backward: "
+                                           "wgmma GEMMs + small kernels)",
                     achieved=achieved, peak=peaks["bf16_tflops"], unit="TFLOP/s", frac=achieved / peaks["bf16_tflops"],
                     peak_source=peaks["source"] + ", burst bf16",
                     frac_of_sustained=(achieved / peaks["bf16_tflops_sustained"]) if peaks["bf16_tflops_sustained"] else None,
@@ -434,8 +443,7 @@ def run_ours(args):
                     flop_per_launch_group=flop_step_gpu, ms_per_launch_group=group_ms,
                     ms_per_launch_group_eager_events=mlp_ms_per_step,
                     mlp_sample_evals_per_step=evals_per_step,
-                    traffic=TRAFFIC.get((args.engine if args.engine != "auto" else "tc_3x", args.config)),
-                    traffic_source=TRAFFIC_SOURCE.get(args.engine if args.engine != "auto" else "tc_3x"), engine=args.engine)
+                    engine=args.engine)
     cpu = tgb = None
     if world == 1 and not args.no_baselines:   # reported on rank 0 at N = 1 only
         graphed = None
@@ -484,13 +492,6 @@ def shutdown_distributed(dist, grace_s=15.0):
         dist.destroy_process_group()
     finally:
         done.set()
-
-
-# dram__bytes_read.sum + dram__bytes_write.sum of the MLP kernel group of one step, from `ncu --set full` captures
-# (taped forward 1.228 GB, dgrad 1.138 GB, wgrad 2.391 GB at the c2 shape)
-TRAFFIC = {("tc_3x", "c2"): 4.770e9, ("tc_3x_w1", "c2"): 2.582e9}
-TRAFFIC_SOURCE = {"tc_3x": "profiles/r02_ncu_chain.md (ncu --set full of tc_mlp_fwd / dgrad / wgrad, per step)",
-                  "tc_3x_w1": "profiles/r02_ncu_chain_w1.md (ncu --set full of tc_mlp_fwd / dgrad / wgrad, per step)"}
 
 
 # ------------------------------------------------------------------------------------------------ reference arms
@@ -618,7 +619,7 @@ def torch_gpu_baseline(cfg_name, dev, steps=10, warmup=3):
             out[tag + "_ms_per_step"] = ms
     finally:
         torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
-    out["note"] = "same config, same step definition, eager PyTorch on the same B200, %d steps after %d warm-up" % (steps, warmup)
+    out["note"] = "same config, same step definition, eager PyTorch on the same GPU, %d steps after %d warm-up" % (steps, warmup)
     return out
 
 
@@ -668,11 +669,13 @@ def main():
     ap.add_argument("--engine", default="auto")
     ap.add_argument("--sync-each-step", type=int, default=1,
                     help="1 (default): synchronise after every timed step, each step starts on an idle device; 0: the K "
-                         "steps are enqueued back to back (measured ~1 %% slower on a power-capped B200: lower clocks)")
+                         "steps are enqueued back to back")
     ap.add_argument("--device", default="cpu", choices=["cpu", "cuda"], help="reference arm only")
     ap.add_argument("--graph", type=int, default=1, help="1: replay the step as one CUDA graph (default), 0: eager")
     ap.add_argument("--allreduce-in-graph", type=int, default=1)
     ap.add_argument("--no-baselines", action="store_true", help="skip the cpu_baseline / torch_gpu_baseline legs")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's loss and gradients as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * sparf_b200 -- C ABI of the B200-native SPARF ray-marching hot path.
+ * sparf_b200 -- C ABI of the SPARF ray-marching hot path on the H100 (sm_90a).
  *
  * The reference (google-research/sparf) has NO FFI: its boundary for this path is the Python class
  * contract `Graph` / `NeRF` (source/models/renderer.py:28, source/models/frequency_nerf.py:72).  This
@@ -19,17 +19,8 @@
  *     render passes of one step can share one flat gradient buffer (the caller zeroes it once).
  *
  * Process-level state (all of it): the thread-local error string; a launch counter (sparf_launch_count); per device,
- * lazily: the SM count, the kernels' shared-memory attributes, and up to three internal side streams + a few events on which
- * sparf_mlp_backward* runs its small CUDA-core reductions beside the weight-gradient kernel (fork after the dgrad
- * chain, join before the call returns control of `stream`: callers see ordinary stream order, and the pattern is
- * capturable into a CUDA graph).  A workspace must not be shared by calls running concurrently on different streams.
- * Environment knobs, read once, for A/B timing only (defaults are the measured-fastest settings):
- *   SPARF_TC_OVERLAP=0   no side stream (everything on `stream`)
- *   SPARF_TC_OVERLAP_BWD=0   only the backward's leftovers back on `stream` (the forward's packing stays on the side stream)
- *   SPARF_TC_TMEMA=0     chain kernels with shared-memory A operands (round-1 generation; also serves the single-pass
- *                        engine and the recompute backward)
- *   SPARF_TC_BWD_SPLIT=n, SPARF_TC_BWD_ND=k   backward pipelined in n sub-chunks, dgrad on k SMs beside wgrad (off)
- *   SPARF_TC_WCOPIES=n   replicas of the packed forward weight stream (L2 hot-spot experiment)
+ * lazily: the SM count.  Every call enqueues on `stream` only, so a call sequence is capturable into a CUDA graph.
+ * A workspace must not be shared by calls running concurrently on different streams.
  */
 #ifndef SPARF_B200_H_
 #define SPARF_B200_H_
@@ -57,14 +48,12 @@ enum {
 enum {
   SPARF_ENGINE_AUTO = 0,
   SPARF_ENGINE_SIMT_FP32 = 1, /* CUDA-core FFMA, fp32 throughout (bit-level twin of the reference) */
-  SPARF_ENGINE_TC_3X = 2, /* tcgen05: x*W = x_hi*W_hi + x_lo*W_hi + x_hi*W_lo on 16-bit halves (fp16 in the
-                             forward, bf16 for gradients), fp32 TMEM accumulation: the parity engine */
-  SPARF_ENGINE_TC_1X = 3, /* tcgen05, single 16-bit pass ("fast", NOT within the 1e-4 parity bound) */
-  SPARF_ENGINE_TC_3X_W1 = 4 /* TC_3X forward and input / pose gradients (parity), but the wide layers' WEIGHT gradients
-                               dW = G^T X in ONE bf16 pass over the hi halves of the saved images (and their bias gradients
-                               as column sums of G_hi): the weight-gradient kernel reads half the bytes.  Non-default,
-                               reduced precision (8-bit factors; the rounding errors average over the batch):
-                               profiles/r02_engine_errors.md tabulates its error against fp64 */
+  SPARF_ENGINE_TC_3X = 2, /* Hopper wgmma: x*W = x_lo*W_hi + x_hi*W_lo + x_hi*W_hi on 16-bit halves (fp16 in the
+                             forward, bf16 for gradients), fp32 accumulation: the parity engine */
+  SPARF_ENGINE_TC_1X = 3, /* wgmma, single 16-bit pass ("fast", NOT within the 1e-4 parity bound) */
+  SPARF_ENGINE_TC_3X_W1 = 4 /* TC_3X forward and input / pose gradients (parity), but the weight gradients dW = G^T X in
+                               ONE bf16 pass over the hi halves.  Non-default, reduced precision (8-bit factors; the
+                               rounding errors average over the batch) */
 };
 
 typedef void* sparf_stream_t; /* cudaStream_t */
@@ -108,7 +97,7 @@ int sparf_version(void);
 const char* sparf_last_error(void);
 /* number of CUDA kernels this library has launched so far in this process (bench.py: gpu_launches) */
 uint64_t sparf_launch_count(void);
-/* 1 if the library was built with the tcgen05 engine and the current device is sm_100 */
+/* 1 if `engine` can run on the current device (the tensor-core engines need an sm_90 device) */
 int sparf_engine_available(int engine);
 
 /* ---------------------------------------------------------------- rays
@@ -163,12 +152,11 @@ int sparf_mlp_backward(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S
                        const float* d_rgb, const SparfMLPGrad* grad, float* d_origins, float* d_dirs,
                        void* workspace, size_t workspace_bytes, sparf_stream_t stream);
 
-/* Tape variants (tcgen05 engine): the TRAINING forward additionally dumps, into a caller-held `tape`, the per-layer
- * operand images the backward needs, so that sparf_mlp_backward_tape skips the recompute.  The tape must stay
- * untouched between the two calls.  sparf_mlp_tape_bytes returns 0 when no tape is available for this call
- * (SIMT engine, unsupported shape, or a tape above 64 GB): use the recompute pair then.  Batches larger than one
- * backward chunk (1024 row tiles) keep ONE tape and walk it chunk by chunk in the backward.
- * Outputs and numerics of the forward are identical to sparf_mlp_forward. */
+/* Tape variants: the TRAINING forward additionally keeps, in a caller-held `tape`, what the backward needs (encodings,
+ * trunk and colour-head activations, the softplus argument), so that sparf_mlp_backward_tape skips the recompute.  The
+ * tape must stay untouched between the two calls, and both take the same `engine`; sparf_mlp_backward_tape reads the
+ * forward's `rgb` output.  sparf_mlp_tape_bytes returns 0 when no tape is offered (a tape above 16 GB): use the
+ * recompute pair then.  Outputs and numerics are identical to sparf_mlp_forward / sparf_mlp_backward. */
 size_t sparf_mlp_tape_bytes(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S);
 int sparf_mlp_forward_tape(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S, const float* origins,
                            const float* dirs, const float* t, const float* noise, float* sigma, float* rgb,
@@ -230,20 +218,12 @@ int sparf_adam_step(int64_t n, float* param, float* grad, float* exp_avg, float*
                     double eps, double max_norm, sparf_stream_t stream);
 
 /* ---------------------------------------------------------------- diagnostics
- * Minimal tcgen05 GEMM exercising every Blackwell primitive of the tensor-core engine (operand layout,
- * descriptors, bulk copy, TMEM): D[128,128] = bf16(A[128,K]) * bf16(B[128,K])^T, K in {64,...,256}.
- * `packed` is >= 128*K*2 bytes of scratch.  Used by tests/test_tc_engine.py. */
+ * The forward GEMM kernel of the tensor-core engines in one bf16 pass (operand layout, wgmma descriptors, accumulator
+ * fragment mapping): D[128,128] = bf16(A[128,K]) * bf16(B[128,K])^T, K in {64,...,256}.  `packed` is unused (kept for
+ * ABI stability).  Used by tests/test_tc_engine.py. */
 int sparf_tc_selftest(const float* A, const float* B, int32_t K, void* packed, float* D, sparf_stream_t stream);
-/* Same GEMM with the A operand written to and read from tensor memory (tcgen05.st, tcgen05.mma with A in TMEM). */
-int sparf_tc_selftest_ts(const float* A, const float* B, int32_t K, void* packed, float* D, sparf_stream_t stream);
-/* Same for the weight-gradient shape: D[128,128] = G[rows,128]^T X[rows,128] through MN-major descriptors. */
+/* Same for the weight-gradient kernel: D[128,128] = G[rows,128]^T X[rows,128], rows in {64, 128}. */
 int sparf_tc_selftest_tn(const float* G, const float* X, int32_t rows, float* D, sparf_stream_t stream);
-/* probe: same with G in bf16 and X in fp16 (mixed operand formats in one kind::f16 instruction) */
-int sparf_tc_selftest_tn_mixed(const float* G, const float* X, int32_t rows, float* D, sparf_stream_t stream);
-
-/* Micro-benchmark of cp.async.bulk L2->shared throughput per SM vs copies in flight (tools/probe_bulkcopy.py). */
-int sparf_tc_bulkcopy_probe(const void* src, uint32_t src_bytes, int32_t stages, uint32_t chunk, int32_t iters,
-                            int32_t grid, long long* cycles, sparf_stream_t stream);
 
 #ifdef __cplusplus
 }

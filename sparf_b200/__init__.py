@@ -1,7 +1,7 @@
-"""sparf_b200: B200-native volumetric renderer for SPARF's ray-marching hot path.
+"""sparf_b200: volumetric renderer for SPARF's ray-marching hot path on the H100 (sm_90a).
 
 Host side (this package) mirrors the reference's Python API (`Graph`, `NeRF`, loss modules); all
-arithmetic runs in hand-written sm_100a CUDA behind the C ABI in include/sparf_b200.h.
+arithmetic runs in hand-written sm_90a CUDA behind the C ABI in include/sparf_b200.h.
 """
 from . import ops  # noqa: F401
 from .ops import set_engine, get_engine  # noqa: F401

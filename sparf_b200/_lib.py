@@ -59,10 +59,7 @@ _SIGNATURES = {
     "sparf_distortion_fwd_bwd": (c_int32, [c_int32, c_int32, _P, _P, c_float, _P, _P, _P, _P]),
     "sparf_adam_step": (c_int32, [c_int64, _P, _P, _P, _P, _P, _P] + [ctypes.c_double] * 7 + [_P]),
     "sparf_tc_selftest": (c_int32, [_P, _P, c_int32, _P, _P, _P]),
-    "sparf_tc_selftest_ts": (c_int32, [_P, _P, c_int32, _P, _P, _P]),
     "sparf_tc_selftest_tn": (c_int32, [_P, _P, c_int32, _P, _P]),
-    "sparf_tc_selftest_tn_mixed": (c_int32, [_P, _P, c_int32, _P, _P]),
-    "sparf_tc_bulkcopy_probe": (c_int32, [_P, ctypes.c_uint32, c_int32, ctypes.c_uint32, c_int32, c_int32, _P, _P]),
 }
 
 _lib = None
@@ -79,7 +76,7 @@ def lib():
     if _lib is not None:
         return _lib
     path = _build.LIB_PATH
-    override = os.environ.get("SPARF_B200_LIB")     # debug builds (python -m sparf_b200.build --trace), tools only
+    override = os.environ.get("SPARF_B200_LIB")     # experiment builds (python -m sparf_b200.build --variant), tools only
     if override:
         if not os.path.exists(override):
             raise RuntimeError("SPARF_B200_LIB=%s does not exist" % override)

@@ -1,7 +1,7 @@
-"""Build the C-ABI shared library (sparf_b200/lib/libsparf_b200.so) with nvcc for sm_100a.
+"""Build the C-ABI shared library (sparf_b200/lib/libsparf_b200.so) with nvcc for the H100 (sm_90a).
 
-nvcc cross-compiles without a GPU; the .so is git-ignored but travels to the GPU box with the
-working tree.  `python -m sparf_b200.build [--force]`.
+nvcc cross-compiles without a GPU; the .so is git-ignored and built in the source tree.
+`python -m sparf_b200.build [--force]`.
 """
 from __future__ import annotations
 
@@ -18,7 +18,7 @@ LIB_PATH = os.path.join(LIB_DIR, "libsparf_b200.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
     "--expt-relaxed-constexpr",
@@ -41,8 +41,8 @@ HASH_PATH = LIB_PATH + ".srchash"
 
 
 def _source_hash() -> str:
-    """Content hash of everything the library is built from (+ the flags).  File times are useless here: the tree is
-    copied to the GPU box, where every file gets a fresh mtime and N ranks would all decide to rebuild at once."""
+    """Content hash of everything the library is built from (+ the flags).  File times are not used: a copied tree gets
+    fresh mtimes, and N ranks of one job would all decide to rebuild at once."""
     import hashlib
     h = hashlib.sha256(" ".join(NVCC_FLAGS).encode())
     for d in sorted(sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(INCLUDE, "*.h"))):
@@ -62,16 +62,12 @@ def _stale() -> bool:
         return True
 
 
-TRACE_LIB_PATH = os.path.join(LIB_DIR, "libsparf_b200_trace.so")   # debug build (tools/trace_chain.py), never loaded by default
-
-
-def build(force: bool = False, verbose: bool = False, trace: bool = False, variant: str = "", defines_extra=()) -> str:
-    """Compile every .cu under csrc/ into one shared library.  Returns its path.  trace=True builds the wait-time
-    tracing variant (-DSPARF_TC_TRACE) next to it; `SPARF_B200_LIB=<path>` makes sparf_b200._lib load that instead."""
-    out_path = TRACE_LIB_PATH if trace else LIB_PATH
+def build(force: bool = False, verbose: bool = False, variant: str = "", defines_extra=()) -> str:
+    """Compile every .cu under csrc/ into one shared library.  Returns its path."""
+    out_path = LIB_PATH
     if variant:     # experiment builds: lib/libsparf_b200_<variant>.so with extra -D flags (tools only, via SPARF_B200_LIB)
         out_path = os.path.join(LIB_DIR, "libsparf_b200_%s.so" % variant)
-    if not trace and not variant and not force and not _stale():
+    if not variant and not force and not _stale():
         return LIB_PATH
     os.makedirs(LIB_DIR, exist_ok=True)
     # one builder at a time (several ranks of one job may get here together); whoever waited re-checks first
@@ -79,20 +75,17 @@ def build(force: bool = False, verbose: bool = False, trace: bool = False, varia
     lock = open(os.path.join(LIB_DIR, ".build.lock"), "w")
     fcntl.flock(lock, fcntl.LOCK_EX)
     try:
-        if not trace and not variant and not force and not _stale():
+        if not variant and not force and not _stale():
             return LIB_PATH
-        return _build_locked(out_path, verbose, trace, defines_extra, main_lib=not trace and not variant)
+        return _build_locked(out_path, verbose, defines_extra, main_lib=not variant)
     finally:
         fcntl.flock(lock, fcntl.LOCK_UN)
         lock.close()
 
 
-def _build_locked(out_path, verbose, trace, defines_extra, main_lib):
+def _build_locked(out_path, verbose, defines_extra, main_lib):
     srcs = sources()
-    defines = ["-DSPARF_WITH_TC"] if os.path.exists(os.path.join(CSRC, "mlp_tc.cu")) else []
-    defines += os.environ.get("SPARF_NVCC_DEFINES", "").split()   # extra debug defines
-    if trace:
-        defines.append("-DSPARF_TC_TRACE")
+    defines = os.environ.get("SPARF_NVCC_DEFINES", "").split()   # extra debug defines
     defines += list(defines_extra)
     tmp = "%s.tmp.%d" % (out_path, os.getpid())
     cmd = [_nvcc()] + NVCC_FLAGS + defines + ["-I", INCLUDE, "-o", tmp] + srcs
@@ -115,5 +108,4 @@ def _build_locked(out_path, verbose, trace, defines_extra, main_lib):
 if __name__ == "__main__":
     _variant = sys.argv[sys.argv.index("--variant") + 1] if "--variant" in sys.argv else ""
     _defs = sys.argv[sys.argv.index("--defines") + 1].split() if "--defines" in sys.argv else []
-    print(build(force="--force" in sys.argv, verbose="-v" in sys.argv, trace="--trace" in sys.argv, variant=_variant,
-                defines_extra=_defs))
+    print(build(force="--force" in sys.argv, verbose="-v" in sys.argv, variant=_variant, defines_extra=_defs))

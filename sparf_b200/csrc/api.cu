@@ -3,9 +3,6 @@
 
 #include "common.cuh"
 #include "mlp_simt.cuh"
-#ifdef SPARF_WITH_TC
-#include "mlp_tc.cuh"
-#endif
 
 namespace sparf {
 
@@ -26,30 +23,27 @@ int num_sms() {
   int& n = cache[dev & 63];           // per device ordinal (several devices in one process)
   if (n == 0) {
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
 
-static bool device_is_sm100() {
-  int dev = 0, major = 0;
+// the wgmma kernels exist for sm_90a only
+static bool device_is_sm90() {
+  int dev = 0, major = 0, minor = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return false;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  return major == 10;
+  cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+  return major == 9 && minor == 0;
 }
 
-// AUTO -> the tensor-core engine when this MLP shape is covered by it, else SIMT
 static bool is_tc(int engine) { return engine == SPARF_ENGINE_TC_3X || engine == SPARF_ENGINE_TC_1X || engine == SPARF_ENGINE_TC_3X_W1; }
-static bool is_tc3(int engine) { return engine == SPARF_ENGINE_TC_3X || engine == SPARF_ENGINE_TC_3X_W1; }   // engines that keep a tape
 
-static int resolve_engine(const SparfMLP* mlp, int engine) {
-#ifdef SPARF_WITH_TC
-  if (engine == SPARF_ENGINE_AUTO) return tc_supports(mlp) && device_is_sm100() ? SPARF_ENGINE_TC_3X : SPARF_ENGINE_SIMT_FP32;
-  if (is_tc(engine) && !tc_supports(mlp)) return -1;
-#else
-  if (engine == SPARF_ENGINE_AUTO) return SPARF_ENGINE_SIMT_FP32;
-#endif
-  return engine;
+// AUTO -> the 3-pass tensor-core engine; both AUTO choices are parity engines
+static int resolve_engine(const SparfMLP*, int engine) {
+  if (engine == SPARF_ENGINE_AUTO) return device_is_sm90() ? SPARF_ENGINE_TC_3X : SPARF_ENGINE_SIMT_FP32;
+  if (engine == SPARF_ENGINE_SIMT_FP32) return engine;
+  return is_tc(engine) && device_is_sm90() ? engine : -1;
 }
 
 }  // namespace sparf
@@ -62,19 +56,15 @@ extern "C" uint64_t sparf_launch_count(void) { return g_launch_count; }
 
 extern "C" int sparf_engine_available(int engine) {
   if (engine == SPARF_ENGINE_SIMT_FP32) return 1;
-#ifdef SPARF_WITH_TC
-  if (is_tc(engine)) return device_is_sm100() ? 1 : 0;
-#endif
+  if (is_tc(engine)) return device_is_sm90() ? 1 : 0;
   return 0;
 }
 
 extern "C" size_t sparf_mlp_workspace_bytes(const SparfMLP* mlp, int32_t R, int32_t S, int32_t backward, int32_t engine) {
   if (!mlp || R <= 0 || S <= 0) return 0;
-  engine = resolve_engine(mlp, engine);
-#ifdef SPARF_WITH_TC
-  if (is_tc(engine)) return tc_workspace_bytes(mlp, R, S, backward, engine);
-#endif
-  return simt_workspace_bytes(mlp, R, S, backward);
+  const int e = resolve_engine(mlp, engine);
+  if (e < 0 || backward < 0 || backward > 2) return 0;
+  return simt_workspace_bytes(mlp, R, S, backward, e);
 }
 
 extern "C" int sparf_mlp_forward(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S, const float* origins,
@@ -83,15 +73,12 @@ extern "C" int sparf_mlp_forward(const SparfMLP* mlp, int32_t engine, int32_t R,
   SPARF_REQUIRE(mlp && R >= 0 && S > 0, "mlp_forward: bad arguments");
   SPARF_REQUIRE(origins && dirs && t && sigma && rgb, "mlp_forward: NULL tensor");
   if (R == 0) return SPARF_OK;
-  engine = resolve_engine(mlp, engine);
-  if (engine == SPARF_ENGINE_SIMT_FP32)
-    return simt_mlp_forward(mlp, R, S, origins, dirs, t, noise, sigma, rgb, workspace, workspace_bytes, (cudaStream_t)stream);
-#ifdef SPARF_WITH_TC
-  if (is_tc(engine))
-    return tc_mlp_forward(mlp, engine, R, S, origins, dirs, t, noise, sigma, rgb, workspace, workspace_bytes, (cudaStream_t)stream);
-#endif
-  set_error("mlp_forward: engine %d not available in this build", engine);
-  return SPARF_ERR_UNSUPPORTED;
+  const int e = resolve_engine(mlp, engine);
+  if (e < 0) {
+    set_error("mlp_forward: engine %d not available in this build", engine);
+    return SPARF_ERR_UNSUPPORTED;
+  }
+  return simt_mlp_forward(mlp, e, R, S, origins, dirs, t, noise, sigma, rgb, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int sparf_mlp_backward(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S, const float* origins,
@@ -101,26 +88,20 @@ extern "C" int sparf_mlp_backward(const SparfMLP* mlp, int32_t engine, int32_t R
   SPARF_REQUIRE(mlp && R >= 0 && S > 0, "mlp_backward: bad arguments");
   SPARF_REQUIRE(origins && dirs && t && d_sigma && d_rgb && grad, "mlp_backward: NULL tensor");
   if (R == 0) return SPARF_OK;
-  engine = resolve_engine(mlp, engine);
-  if (engine == SPARF_ENGINE_SIMT_FP32)
-    return simt_mlp_backward(mlp, R, S, origins, dirs, t, noise, d_sigma, d_rgb, grad, d_origins, d_dirs, workspace, workspace_bytes, (cudaStream_t)stream);
-#ifdef SPARF_WITH_TC
-  if (is_tc(engine))
-    return tc_mlp_backward(mlp, engine, R, S, origins, dirs, t, noise, d_sigma, d_rgb, grad, d_origins, d_dirs, workspace, workspace_bytes, (cudaStream_t)stream);
-#endif
-  set_error("mlp_backward: engine %d not available in this build", engine);
-  return SPARF_ERR_UNSUPPORTED;
+  const int e = resolve_engine(mlp, engine);
+  if (e < 0) {
+    set_error("mlp_backward: engine %d not available in this build", engine);
+    return SPARF_ERR_UNSUPPORTED;
+  }
+  return simt_mlp_backward(mlp, e, R, S, origins, dirs, t, noise, d_sigma, d_rgb, grad, d_origins, d_dirs, workspace,
+                           workspace_bytes, (cudaStream_t)stream);
 }
 
-// ---------------------------------------------------------------- tape variants (training forward keeps the
-// operand images so that the backward does not recompute the forward)
+// ---------------------------------------------------------------- tape variants: the training forward keeps what the
+// backward needs, so that the backward does not recompute the forward
 extern "C" size_t sparf_mlp_tape_bytes(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S) {
-  if (!mlp || R <= 0 || S <= 0) return 0;
-  engine = resolve_engine(mlp, engine);
-#ifdef SPARF_WITH_TC
-  if (is_tc3(engine)) return tc_tape_bytes(mlp, R, S);
-#endif
-  return 0;
+  if (!mlp || R <= 0 || S <= 0 || resolve_engine(mlp, engine) < 0) return 0;
+  return simt_tape_bytes(mlp, R, S);
 }
 
 extern "C" int sparf_mlp_forward_tape(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S, const float* origins,
@@ -128,13 +109,13 @@ extern "C" int sparf_mlp_forward_tape(const SparfMLP* mlp, int32_t engine, int32
                                       void* tape, size_t tape_bytes, void* workspace, size_t workspace_bytes,
                                       sparf_stream_t stream) {
   SPARF_REQUIRE(mlp && R > 0 && S > 0 && origins && dirs && t && sigma && rgb && tape, "mlp_forward_tape: bad arguments");
-#ifdef SPARF_WITH_TC
-  if (is_tc3(resolve_engine(mlp, engine)))
-    return tc_mlp_forward_tape(mlp, resolve_engine(mlp, engine), R, S, origins, dirs, t, noise, sigma, rgb, tape, tape_bytes, workspace,
-                               workspace_bytes, (cudaStream_t)stream);
-#endif
-  set_error("mlp_forward_tape: only the tcgen05 engine keeps a tape (sparf_mlp_tape_bytes returned 0)");
-  return SPARF_ERR_UNSUPPORTED;
+  const int e = resolve_engine(mlp, engine);
+  if (e < 0) {
+    set_error("mlp_forward_tape: engine %d not available", engine);
+    return SPARF_ERR_UNSUPPORTED;
+  }
+  return simt_mlp_forward_tape(mlp, e, R, S, origins, dirs, t, noise, sigma, rgb, tape, tape_bytes, workspace, workspace_bytes,
+                               (cudaStream_t)stream);
 }
 
 extern "C" int sparf_mlp_backward_tape(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S, const float* origins,
@@ -144,11 +125,11 @@ extern "C" int sparf_mlp_backward_tape(const SparfMLP* mlp, int32_t engine, int3
                                        size_t workspace_bytes, sparf_stream_t stream) {
   SPARF_REQUIRE(mlp && R > 0 && S > 0 && origins && dirs && t && sigma && rgb && d_sigma && d_rgb && grad && tape,
                 "mlp_backward_tape: bad arguments");
-#ifdef SPARF_WITH_TC
-  if (is_tc3(resolve_engine(mlp, engine)))
-    return tc_mlp_backward_tape(mlp, resolve_engine(mlp, engine), R, S, origins, dirs, t, sigma, rgb, d_sigma, d_rgb, grad, d_origins,
-                                d_dirs, tape, tape_bytes, workspace, workspace_bytes, (cudaStream_t)stream);
-#endif
-  set_error("mlp_backward_tape: only the tcgen05 engine keeps a tape");
-  return SPARF_ERR_UNSUPPORTED;
+  const int e = resolve_engine(mlp, engine);
+  if (e < 0) {
+    set_error("mlp_backward_tape: engine %d not available", engine);
+    return SPARF_ERR_UNSUPPORTED;
+  }
+  return simt_mlp_backward_tape(mlp, e, R, S, origins, dirs, t, rgb, d_sigma, d_rgb, grad, d_origins, d_dirs, tape, tape_bytes,
+                                workspace, workspace_bytes, (cudaStream_t)stream);
 }

@@ -1,4 +1,4 @@
-// Shared helpers for the sparf_b200 CUDA sources (sm_100a only).
+// Shared helpers for the sparf_b200 CUDA sources (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdarg>

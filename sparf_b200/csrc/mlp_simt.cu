@@ -1,14 +1,16 @@
-// SIMT fp32 engine for the NeRF MLP (SPARF_ENGINE_SIMT_FP32): CUDA-core FFMA GEMMs, layer by layer,
-// activations in a caller-provided HBM workspace, processed in row chunks so memory stays bounded.
-// It is the bit-level twin of the reference's fp32 path (same per-element arithmetic, fp32 accumulate)
-// and serves (a) as the always-available exact engine, (b) as the on-device cross-check for the
-// tcgen05 engine (mlp_tc.cu).  Works for any width that is a multiple of 8 and any L_xyz/L_view <= 16.
+// Layer-by-layer engines for the NeRF MLP, activations in a caller-provided HBM workspace, processed in row chunks so
+// memory stays bounded.  Works for any width that is a multiple of 8 and any L_xyz/L_view <= 16.
+//   SPARF_ENGINE_SIMT_FP32: CUDA-core FFMA GEMMs, the bit-level twin of the reference's fp32 path (same per-element
+//     arithmetic, fp32 accumulate): the exact engine and the on-device cross-check of the tensor-core engines.
+//   SPARF_ENGINE_TC_3X / TC_1X / TC_3X_W1: the same orchestration with every wide GEMM on Hopper tensor cores
+//     (gemm_wgmma.cu); encoders, narrow layers and reductions are the shared CUDA-core kernels below.
 //
 // Reference: NeRF.compute_raw_density / NeRF.forward (source/models/frequency_nerf.py:149-227),
 // FrequencyEmbedder (:47-69), positional_encoding (:229-258).
 #include <algorithm>
 
 #include "common.cuh"
+#include "gemm_wgmma.cuh"
 #include "mlp_simt.cuh"
 
 namespace sparf {
@@ -240,10 +242,56 @@ __global__ void __launch_bounds__(256) gemm_tn_kernel(int M, int N, int K, int K
   }
 }
 
+// GEMM dispatch: CUDA-core kernels above (passes == 0) or the wgmma kernels of gemm_wgmma.cu
+static int gemm_nt(TcPrec p, int M, int N, const float* X1, int ld1, int K1, int K1v, const float* X2, int ld2, int K2, int K2v,
+                   int div2, const float* W, int ldw, int wcol2, const float* bias, float* Y, int ldy, cudaStream_t st) {
+  if (p.passes) return tc_gemm_nt(p, 1, M, N, X1, ld1, K1, K1v, X2, ld2, K2, K2v, div2, W, ldw, wcol2, bias, Y, ldy, st);
+  gemm_nt_kernel<1><<<dim3(ceil_div(N, BN), ceil_div(M, BM)), 256, 0, st>>>(M, N, X1, ld1, K1, K1v, X2, ld2, K2, K2v, div2, W,
+                                                                           ldw, wcol2, bias, Y, ldy);
+  SPARF_CHECK_LAUNCH("gemm_nt_kernel");
+  return SPARF_OK;
+}
+
+static int gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, const float* G, int ldg, const float* W, int ldw, int wcol,
+                   const float* mask_src, int ldmask, const float* r1_vec, const float* r1_row, float* D, int ldd, int accumulate,
+                   cudaStream_t st) {
+  if (p.passes)
+    return tc_gemm_nn(p, M, N, Kout, Kv, G, ldg, W, ldw, wcol, mask_src, ldmask, r1_vec, r1_row, D, ldd, accumulate, st);
+  gemm_nn_kernel<<<dim3(ceil_div(Kout, BN), ceil_div(M, BM)), 256, 0, st>>>(M, N, Kout, Kv, G, ldg, W, ldw, wcol, mask_src,
+                                                                           ldmask, r1_vec, r1_row, D, ldd, accumulate);
+  SPARF_CHECK_LAUNCH("gemm_nn_kernel");
+  return SPARF_OK;
+}
+
+static int gemm_tn(TcPrec p, int M, int N, int K, int Kv, int rows_per_slab, const float* G, int ldg, const float* X, int ldx,
+                   int div, float* dW, int ldw, int wcol, cudaStream_t st) {
+  if (p.passes) return tc_gemm_tn(p, M, N, K, Kv, rows_per_slab, G, ldg, X, ldx, div, dW, ldw, wcol, st);
+  gemm_tn_kernel<<<dim3(ceil_div(K, BN), ceil_div(N, BM), ceil_div(M, rows_per_slab)), 256, 0, st>>>(
+      M, N, K, Kv, rows_per_slab, G, ldg, X, ldx, div, dW, ldw, wcol);
+  SPARF_CHECK_LAUNCH("gemm_tn_kernel");
+  return SPARF_OK;
+}
+
+#define SPARF_TRY(expr)      \
+  do {                       \
+    int _rc = (expr);        \
+    if (_rc) return _rc;     \
+  } while (0)
+
+EnginePrec engine_prec(int engine) {
+  const TcPrec fp32{false, 0}, f16x3{true, 3}, f16x1{true, 1}, bf16x3{false, 3}, bf16x1{false, 1};
+  switch (engine) {
+    case SPARF_ENGINE_TC_3X: return EnginePrec{f16x3, bf16x3, bf16x3};
+    case SPARF_ENGINE_TC_1X: return EnginePrec{f16x1, bf16x1, bf16x1};
+    case SPARF_ENGINE_TC_3X_W1: return EnginePrec{f16x3, bf16x3, bf16x1};
+    default: return EnginePrec{fp32, fp32, fp32};
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // narrow layers (1 or 3 outputs): one warp per row
 // ------------------------------------------------------------------------------------------------
-// MODE 0: density row:  raw = X.W[0] + b ; raw_out[m] = raw ; sigma[m] = softplus(raw + noise)
+// MODE 0: density row:  raw = X.W[0] + b ; z = raw + noise ; raw_out[m] = z ; sigma[m] = softplus(z)
 // MODE 1: colour head:  rgb[m][j] = sigmoid(X.W[j] + b[j]), j < 3
 template <int MODE>
 __global__ void rowdot_kernel(long long M, int K, const float* __restrict__ X, int ldx, const float* __restrict__ W,
@@ -269,8 +317,8 @@ __global__ void rowdot_kernel(long long M, int K, const float* __restrict__ X, i
   if (lane == 0) {
     if (MODE == 0) {
       float raw = acc[0] + bias[0];
-      if (raw_out) raw_out[m] = raw;
       float z = noise ? add_rn(raw, noise[m]) : raw;
+      if (raw_out) raw_out[m] = z;     // the softplus argument, what the backward needs
       if (out) out[m] = softplus_f(z);
     } else {
 #pragma unroll
@@ -487,20 +535,64 @@ struct Carver {
   }
 };
 
-size_t simt_workspace_bytes(const SparfMLP* mlp, int R, int S, int backward) {
-  SimtDims d = simt_dims(mlp);
-  size_t nr = (size_t)std::min(R, chunk_rays(S, backward));
-  size_t Mc = nr * S;
-  auto a = [](size_t n) { return align_up(n * sizeof(float), 256); };
-  size_t total = a(32) + a(Mc * d.E3p) + a(nr * d.Evp) + a(Mc * d.HW) + a(Mc) + a(Mc * 3);
-  if (!backward) {
-    total += 2 * a(Mc * d.W);
-  } else {
-    total += (size_t)d.nt * a(Mc * d.W);            // h0..h_{nt-1}
-    total += 2 * a(Mc * d.W);                         // G ping-pong
-    total += a(Mc * d.E3p) + a(Mc * d.HW) + a(Mc * 4) + a(Mc) + a(Mc * d.Evp) + a(nr * d.Evp);
+// Workspace of one call, per chunk of nrc rays.  mode 0: forward, 1: backward (recomputes the forward), 2: backward from a
+// tape, 3: taped forward (the activations go to the tape).  Tensor-core engines add two operand-image buffers.
+struct Ws {
+  float *wts, *enc, *denc, *hid, *raw, *rgbv, *G0, *G1, *Genc, *Ghid, *gpre, *graw, *Gdtmp, *Gdenc;
+  float* H[SPARF_MAX_TRUNK];
+  uint16_t *pack_a, *pack_b;
+  size_t pack_elems;
+};
+
+static size_t carve(const SimtDims& d, bool tc, int nrc, int S, int mode, char* base, Ws* out) {
+  const size_t Mc = (size_t)nrc * S;
+  Carver cv{base, 0, 0};
+  Ws w{};
+  w.wts = cv.take(32);
+  if (mode == 0 || mode == 1) {
+    w.enc = cv.take(Mc * d.E3p);
+    w.denc = cv.take((size_t)nrc * d.Evp);
+    w.hid = cv.take(Mc * d.HW);
+    w.raw = cv.take(Mc);
+    w.rgbv = cv.take(Mc * 3);
+    const int nH = mode == 0 ? 2 : d.nt;            // the forward ping-pongs, the backward keeps every layer
+    for (int l = 0; l < nH; ++l) w.H[l] = cv.take(Mc * d.W);
+    for (int l = nH; l < d.nt; ++l) w.H[l] = w.H[l & 1];
   }
-  return total + 256;
+  if (mode == 1 || mode == 2) {
+    w.G0 = cv.take(Mc * d.W);
+    w.G1 = cv.take(Mc * d.W);
+    w.Genc = cv.take(Mc * d.E3p);
+    w.Ghid = cv.take(Mc * d.HW);
+    w.gpre = cv.take(Mc * 4);
+    w.graw = cv.take(Mc);
+    w.Gdtmp = cv.take(Mc * d.Evp);
+    w.Gdenc = cv.take((size_t)nrc * d.Evp);
+  }
+  if (tc) {     // largest operand images: [max(Mc, width) x (W + encoding)] forward, [width x Mc] weight gradient
+    const int wmax = std::max(std::max(d.W, d.HW), std::max(d.E3p, d.Evp));
+    w.pack_elems = std::max(tc_pack_elems((int)Mc, ceil_div(wmax, 32) + ceil_div(std::max(d.E3p, d.Evp), 32), wmax),
+                            tc_pack_elems(wmax, ceil_div((long long)Mc, 32), 0));
+    w.pack_a = reinterpret_cast<uint16_t*>(cv.take((w.pack_elems + 1) / 2));
+    w.pack_b = reinterpret_cast<uint16_t*>(cv.take((w.pack_elems + 1) / 2));
+  }
+  if (out) *out = w;
+  return cv.used + 256;
+}
+
+static bool uses_tc(int engine) { return engine_prec(engine).fwd.passes != 0; }
+
+size_t simt_workspace_bytes(const SparfMLP* mlp, int R, int S, int mode, int engine) {
+  return carve(simt_dims(mlp), uses_tc(engine), std::min(R, chunk_rays(S, mode == 1 || mode == 2)), S, mode, nullptr, nullptr);
+}
+
+static EnginePrec with_images(EnginePrec ep, const Ws& w) {
+  for (TcPrec* p : {&ep.fwd, &ep.dgrad, &ep.wgrad}) {
+    p->pack_a = w.pack_a;
+    p->pack_b = w.pack_b;
+    p->pack_elems = w.pack_elems;
+  }
+  return ep;
 }
 
 static inline int trunk_in_main(const SimtDims& d, int l) { return l == 0 ? d.E3p : d.W; }
@@ -513,7 +605,7 @@ static inline int trunk_ldw(const SimtDims& d, int l) {
 
 // forward through the MLP for one chunk.  H: array of nt activation buffers (may alias in pairs when
 // !keep), raw may be NULL.
-static int simt_chunk_forward(const SparfMLP* mlp, const SimtDims& d, int nr, int S, const float* origins,
+static int simt_chunk_forward(const SparfMLP* mlp, const EnginePrec& ep, const SimtDims& d, int nr, int S, const float* origins,
                               const float* dirs, const float* t, const float* noise, float* wts, float* enc,
                               float* denc, float** H, float* raw, float* hid, float* sigma, float* rgb,
                               cudaStream_t st) {
@@ -531,12 +623,9 @@ static int simt_chunk_forward(const SparfMLP* mlp, const SimtDims& d, int nr, in
     const int ldw = trunk_ldw(d, l);
     const float* Wl = mlp->trunk_w[l] + (last ? ldw : 0);  // last layer: row 0 is the density row
     const float* bl = mlp->trunk_b[l] + (last ? 1 : 0);
-    dim3 grid(ceil_div(d.W, BN), ceil_div(Mc, BM));
     const bool sk = l == d.skip;
-    gemm_nt_kernel<1><<<grid, 256, 0, st>>>((int)Mc, d.W, in, trunk_in_main(d, l), trunk_in_main(d, l),
-                                            trunk_in_main_valid(d, l), sk ? enc : nullptr, d.E3p, d.E3p, d.E3, 1, Wl, ldw,
-                                            d.W, bl, H[l], d.W);
-    LAUNCH_OK("gemm_nt_kernel");
+    SPARF_TRY(gemm_nt(ep.fwd, (int)Mc, d.W, in, trunk_in_main(d, l), trunk_in_main(d, l), trunk_in_main_valid(d, l),
+                      sk ? enc : nullptr, d.E3p, d.E3p, d.E3, 1, Wl, ldw, d.W, bl, H[l], d.W, st));
     if (last) {
       rowdot_kernel<0><<<ceil_div(Mc, 8), 256, 0, st>>>(Mc, d.W, in, d.W, mlp->trunk_w[l], ldw, mlp->trunk_b[l], noise, raw, sigma);
       LAUNCH_OK("rowdot_kernel<0>");
@@ -544,80 +633,145 @@ static int simt_chunk_forward(const SparfMLP* mlp, const SimtDims& d, int nr, in
     in = H[l];
   }
   {
-    dim3 grid(ceil_div(d.HW, BN), ceil_div(Mc, BM));
-    gemm_nt_kernel<1><<<grid, 256, 0, st>>>((int)Mc, d.HW, H[d.nt - 1], d.W, d.W, d.W, denc, d.Evp, d.Evp, d.Ev, S,
-                                            mlp->head_w[0], d.W + d.Ev, d.W, mlp->head_b[0], hid, d.HW);
-    LAUNCH_OK("gemm_nt_kernel(head)");
+    SPARF_TRY(gemm_nt(ep.fwd, (int)Mc, d.HW, H[d.nt - 1], d.W, d.W, d.W, denc, d.Evp, d.Evp, d.Ev, S, mlp->head_w[0],
+                      d.W + d.Ev, d.W, mlp->head_b[0], hid, d.HW, st));
     rowdot_kernel<1><<<ceil_div(Mc, 8), 256, 0, st>>>(Mc, d.HW, hid, d.HW, mlp->head_w[1], d.HW, mlp->head_b[1], nullptr, nullptr, rgb);
     LAUNCH_OK("rowdot_kernel<1>");
   }
   return SPARF_OK;
 }
 
-int simt_mlp_forward(const SparfMLP* mlp, int R, int S, const float* origins, const float* dirs, const float* t,
+int simt_mlp_forward(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs, const float* t,
                      const float* noise, float* sigma, float* rgb, void* workspace, size_t workspace_bytes,
                      cudaStream_t st) {
   int rc = simt_validate(mlp);
   if (rc) return rc;
-  if (workspace_bytes < simt_workspace_bytes(mlp, R, S, 0)) {
-    set_error("mlp_forward: workspace %zu < %zu bytes", workspace_bytes, simt_workspace_bytes(mlp, R, S, 0));
+  if (workspace_bytes < simt_workspace_bytes(mlp, R, S, 0, engine)) {
+    set_error("mlp_forward: workspace %zu < %zu bytes", workspace_bytes, simt_workspace_bytes(mlp, R, S, 0, engine));
     return SPARF_ERR_WORKSPACE;
   }
   SimtDims d = simt_dims(mlp);
   const int nrc = std::min(R, chunk_rays(S, 0));
-  const size_t Mc = (size_t)nrc * S;
-  Carver cv{reinterpret_cast<char*>(workspace), 0, workspace_bytes};
-  float* wts = cv.take(32);
-  float* enc = cv.take(Mc * d.E3p);
-  float* denc = cv.take((size_t)nrc * d.Evp);
-  float* hid = cv.take(Mc * d.HW);
-  cv.take(Mc);
-  cv.take(Mc * 3);
-  float* ha = cv.take(Mc * d.W);
-  float* hb = cv.take(Mc * d.W);
-  float* H[SPARF_MAX_TRUNK];
-  for (int l = 0; l < d.nt; ++l) H[l] = (l & 1) ? hb : ha;
+  Ws w;
+  carve(d, uses_tc(engine), nrc, S, 0, reinterpret_cast<char*>(workspace), &w);
+  const EnginePrec ep = with_images(engine_prec(engine), w);
   for (int r0 = 0; r0 < R; r0 += nrc) {
     int nr = std::min(nrc, R - r0);
     size_t m0 = (size_t)r0 * S;
-    rc = simt_chunk_forward(mlp, d, nr, S, origins + (size_t)r0 * 3, dirs + (size_t)r0 * 3, t + m0,
-                            noise ? noise + m0 : nullptr, wts, enc, denc, H, nullptr, hid, sigma + m0, rgb + m0 * 3, st);
+    rc = simt_chunk_forward(mlp, ep, d, nr, S, origins + (size_t)r0 * 3, dirs + (size_t)r0 * 3, t + m0,
+                            noise ? noise + m0 : nullptr, w.wts, w.enc, w.denc, w.H, nullptr, w.hid, sigma + m0, rgb + m0 * 3, st);
     if (rc) return rc;
   }
   return SPARF_OK;
 }
 
-int simt_mlp_backward(const SparfMLP* mlp, int R, int S, const float* origins, const float* dirs, const float* t,
+// Tape: what the backward reads of the forward, for the whole batch (one forward pass over all rays, no recompute):
+// the encodings, the nt trunk activations, the colour-head activations and the softplus argument of the density.
+struct Tape {
+  float *enc, *denc, *hid, *raw;
+  float* H[SPARF_MAX_TRUNK];
+};
+
+static size_t tape_layout(const SimtDims& d, int R, int S, char* base, Tape* tp) {
+  const size_t M = (size_t)R * S;
+  Carver cv{base, 0, 0};
+  Tape t;
+  t.enc = cv.take(M * d.E3p);
+  t.denc = cv.take((size_t)R * d.Evp);
+  t.hid = cv.take(M * d.HW);
+  t.raw = cv.take(M);
+  for (int l = 0; l < d.nt; ++l) t.H[l] = cv.take(M * d.W);
+  if (tp) *tp = t;
+  return cv.used + 256;
+}
+
+constexpr size_t kMaxTapeBytes = (size_t)16 << 30;   // larger batches take the recompute backward
+
+size_t simt_tape_bytes(const SparfMLP* mlp, int R, int S) {
+  if (simt_validate(mlp)) return 0;
+  size_t n = tape_layout(simt_dims(mlp), R, S, nullptr, nullptr);
+  return n <= kMaxTapeBytes ? n : 0;
+}
+
+int simt_mlp_forward_tape(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs,
+                          const float* t, const float* noise, float* sigma, float* rgb, void* tape, size_t tape_bytes,
+                          void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  int rc = simt_validate(mlp);
+  if (rc) return rc;
+  SimtDims d = simt_dims(mlp);
+  SPARF_REQUIRE(tape_bytes >= tape_layout(d, R, S, nullptr, nullptr), "mlp_forward_tape: tape %zu bytes too small", tape_bytes);
+  if (workspace_bytes < simt_workspace_bytes(mlp, R, S, 3, engine)) {
+    set_error("mlp_forward_tape: workspace %zu < %zu bytes", workspace_bytes, simt_workspace_bytes(mlp, R, S, 3, engine));
+    return SPARF_ERR_WORKSPACE;
+  }
+  Tape tp;
+  tape_layout(d, R, S, reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(tape), 256)), &tp);
+  const int nrc = std::min(R, chunk_rays(S, 0));
+  Ws w;
+  carve(d, uses_tc(engine), nrc, S, 3, reinterpret_cast<char*>(workspace), &w);
+  const EnginePrec ep = with_images(engine_prec(engine), w);
+  for (int r0 = 0; r0 < R; r0 += nrc) {       // chunk by chunk, straight into the tape
+    const int nr = std::min(nrc, R - r0);
+    const size_t m0 = (size_t)r0 * S;
+    float* H[SPARF_MAX_TRUNK];
+    for (int l = 0; l < d.nt; ++l) H[l] = tp.H[l] + m0 * d.W;
+    rc = simt_chunk_forward(mlp, ep, d, nr, S, origins + (size_t)r0 * 3, dirs + (size_t)r0 * 3, t + m0,
+                            noise ? noise + m0 : nullptr, w.wts, tp.enc + m0 * d.E3p, tp.denc + (size_t)r0 * d.Evp, H,
+                            tp.raw + m0, tp.hid + m0 * d.HW, sigma + m0, rgb + m0 * 3, st);
+    if (rc) return rc;
+  }
+  return SPARF_OK;
+}
+
+static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs,
+                             const float* t, const float* noise, const float* rgb_fwd, void* tape, const float* d_sigma,
+                             const float* d_rgb, const SparfMLPGrad* grad, float* d_origins, float* d_dirs, void* workspace,
+                             size_t workspace_bytes, cudaStream_t st);
+
+int simt_mlp_backward(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs, const float* t,
                       const float* noise, const float* d_sigma, const float* d_rgb, const SparfMLPGrad* grad,
                       float* d_origins, float* d_dirs, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  return mlp_backward_impl(mlp, engine, R, S, origins, dirs, t, noise, nullptr, nullptr, d_sigma, d_rgb, grad, d_origins, d_dirs,
+                           workspace, workspace_bytes, st);
+}
+
+int simt_mlp_backward_tape(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs,
+                           const float* t, const float* rgb, const float* d_sigma, const float* d_rgb, const SparfMLPGrad* grad,
+                           float* d_origins, float* d_dirs, void* tape, size_t tape_bytes, void* workspace,
+                           size_t workspace_bytes, cudaStream_t st) {
+  int rc = simt_validate(mlp);
+  if (rc) return rc;
+  SPARF_REQUIRE(tape_bytes >= tape_layout(simt_dims(mlp), R, S, nullptr, nullptr), "mlp_backward_tape: tape too small");
+  return mlp_backward_impl(mlp, engine, R, S, origins, dirs, t, nullptr, rgb, tape, d_sigma, d_rgb, grad, d_origins, d_dirs,
+                           workspace, workspace_bytes, st);
+}
+
+// tape == NULL: recompute the forward per chunk (noise as in the forward call); else read it from the tape (rgb_fwd =
+// the forward's colour output)
+static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs,
+                             const float* t, const float* noise, const float* rgb_fwd, void* tape, const float* d_sigma,
+                             const float* d_rgb, const SparfMLPGrad* grad, float* d_origins, float* d_dirs, void* workspace,
+                             size_t workspace_bytes, cudaStream_t st) {
   int rc = simt_validate(mlp);
   if (rc) return rc;
   SPARF_REQUIRE(grad != nullptr, "mlp_backward: grad is NULL");
-  if (workspace_bytes < simt_workspace_bytes(mlp, R, S, 1)) {
-    set_error("mlp_backward: workspace %zu < %zu bytes", workspace_bytes, simt_workspace_bytes(mlp, R, S, 1));
+  const int mode = tape ? 2 : 1;
+  if (workspace_bytes < simt_workspace_bytes(mlp, R, S, mode, engine)) {
+    set_error("mlp_backward: workspace %zu < %zu bytes", workspace_bytes, simt_workspace_bytes(mlp, R, S, mode, engine));
     return SPARF_ERR_WORKSPACE;
   }
   SimtDims d = simt_dims(mlp);
   const bool need_rays = d_origins != nullptr || d_dirs != nullptr;
   const int nrc = std::min(R, chunk_rays(S, 1));
-  const size_t Mcap = (size_t)nrc * S;
-  Carver cv{reinterpret_cast<char*>(workspace), 0, workspace_bytes};
-  float* wts = cv.take(32);
-  float* enc = cv.take(Mcap * d.E3p);
-  float* denc = cv.take((size_t)nrc * d.Evp);
-  float* hid = cv.take(Mcap * d.HW);
-  float* raw = cv.take(Mcap);
-  float* rgbv = cv.take(Mcap * 3);
-  float* H[SPARF_MAX_TRUNK];
-  for (int l = 0; l < d.nt; ++l) H[l] = cv.take(Mcap * d.W);
-  float* G0 = cv.take(Mcap * d.W);
-  float* G1 = cv.take(Mcap * d.W);
-  float* Genc = cv.take(Mcap * d.E3p);
-  float* Ghid = cv.take(Mcap * d.HW);
-  float* gpre = cv.take(Mcap * 4);
-  float* graw = cv.take(Mcap);
-  float* Gdtmp = cv.take(Mcap * d.Evp);
-  float* Gdenc = cv.take((size_t)nrc * d.Evp);
+  Ws w;
+  carve(d, uses_tc(engine), nrc, S, mode, reinterpret_cast<char*>(workspace), &w);
+  const EnginePrec ep = with_images(engine_prec(engine), w);
+  float *wts = w.wts, *enc_w = w.enc, *denc_w = w.denc, *hid_w = w.hid, *raw_w = w.raw, *rgbv_w = w.rgbv;
+  float** H_w = w.H;
+  Tape tp{};
+  if (tape) tape_layout(d, R, S, reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(tape), 256)), &tp);
+  float *G0 = w.G0, *G1 = w.G1, *Genc = w.Genc, *Ghid = w.Ghid, *gpre = w.gpre, *graw = w.graw, *Gdtmp = w.Gdtmp,
+        *Gdenc = w.Gdenc;
 
   for (int r0 = 0; r0 < R; r0 += nrc) {
     const int nr = std::min(nrc, R - r0);
@@ -627,12 +781,24 @@ int simt_mlp_backward(const SparfMLP* mlp, int R, int S, const float* origins, c
     const float* d_c = dirs + (size_t)r0 * 3;
     const float* t_c = t + m0;
     const float* nz = noise ? noise + m0 : nullptr;
-    rc = simt_chunk_forward(mlp, d, nr, S, o_c, d_c, t_c, nz, wts, enc, denc, H, raw, hid, nullptr, rgbv, st);
-    if (rc) return rc;
-    const int slab = 2048;  // rows per wgrad slab
+    float *enc = enc_w, *denc = denc_w, *hid = hid_w, *raw = raw_w, *rgbv = rgbv_w;
+    float* H[SPARF_MAX_TRUNK];
+    if (tape) {
+      enc = tp.enc + m0 * d.E3p;
+      denc = tp.denc + (size_t)r0 * d.Evp;
+      hid = tp.hid + m0 * d.HW;
+      raw = tp.raw + m0;
+      rgbv = const_cast<float*>(rgb_fwd) + m0 * 3;
+      for (int l = 0; l < d.nt; ++l) H[l] = tp.H[l] + m0 * d.W;
+    } else {
+      for (int l = 0; l < d.nt; ++l) H[l] = H_w[l];
+      rc = simt_chunk_forward(mlp, ep, d, nr, S, o_c, d_c, t_c, nz, wts, enc, denc, H, raw, hid, nullptr, rgbv, st);
+      if (rc) return rc;
+    }
+    const int slab = ep.wgrad.passes ? 512 : 2048;  // rows per wgrad slab (tensor cores: >= 2 waves of CTAs per layer)
     const int nslab = ceil_div(Mc, slab);
 
-    head_grad_kernel<<<ceil_div(Mc, 256), 256, 0, st>>>(Mc, d_rgb + m0 * 3, rgbv, d_sigma + m0, raw, nz, gpre, graw);
+    head_grad_kernel<<<ceil_div(Mc, 256), 256, 0, st>>>(Mc, d_rgb + m0 * 3, rgbv, d_sigma + m0, raw, nullptr, gpre, graw);
     LAUNCH_OK("head_grad_kernel");
     // colour head, layer 1 (HW -> 3)
     narrow_wgrad_kernel<3><<<ceil_div(Mc, 512), 128, 0, st>>>(Mc, d.HW, 512, gpre, 4, hid, d.HW, grad->head_w[1], d.HW, grad->head_b[1]);
@@ -642,17 +808,13 @@ int simt_mlp_backward(const SparfMLP* mlp, int R, int S, const float* origins, c
     // colour head, layer 0 ([feat | denc] -> HW)
     const int ldw8 = d.W + d.Ev;
     float* feat = H[d.nt - 1];
-    gemm_tn_kernel<<<dim3(ceil_div(d.W, BN), ceil_div(d.HW, BM), nslab), 256, 0, st>>>((int)Mc, d.HW, d.W, d.W, slab, Ghid, d.HW, feat, d.W, 1, grad->head_w[0], ldw8, 0);
-    LAUNCH_OK("gemm_tn_kernel(head feat)");
-    gemm_tn_kernel<<<dim3(ceil_div(d.Evp, BN), ceil_div(d.HW, BM), nslab), 256, 0, st>>>((int)Mc, d.HW, d.Evp, d.Ev, slab, Ghid, d.HW, denc, d.Evp, S, grad->head_w[0], ldw8, d.W);
-    LAUNCH_OK("gemm_tn_kernel(head dir)");
+    SPARF_TRY(gemm_tn(ep.wgrad, (int)Mc, d.HW, d.W, d.W, slab, Ghid, d.HW, feat, d.W, 1, grad->head_w[0], ldw8, 0, st));
+    SPARF_TRY(gemm_tn(ep.wgrad, (int)Mc, d.HW, d.Evp, d.Ev, slab, Ghid, d.HW, denc, d.Evp, S, grad->head_w[0], ldw8, d.W, st));
     colsum_kernel<<<dim3(ceil_div(d.HW, 32), ceil_div(Mc, 1024)), 256, 0, st>>>(Mc, d.HW, 1024, Ghid, d.HW, grad->head_b[0]);
     LAUNCH_OK("colsum_kernel(head)");
-    gemm_nn_kernel<<<dim3(ceil_div(d.W, BN), ceil_div(Mc, BM)), 256, 0, st>>>((int)Mc, d.HW, d.W, d.W, Ghid, d.HW, mlp->head_w[0], ldw8, 0, feat, d.W, nullptr, nullptr, G0, d.W, 0);
-    LAUNCH_OK("gemm_nn_kernel(head)");
+    SPARF_TRY(gemm_nn(ep.dgrad, (int)Mc, d.HW, d.W, d.W, Ghid, d.HW, mlp->head_w[0], ldw8, 0, feat, d.W, nullptr, nullptr, G0, d.W, 0, st));
     if (d_dirs) {
-      gemm_nn_kernel<<<dim3(ceil_div(d.Evp, BN), ceil_div(Mc, BM)), 256, 0, st>>>((int)Mc, d.HW, d.Evp, d.Ev, Ghid, d.HW, mlp->head_w[0], ldw8, d.W, nullptr, 0, nullptr, nullptr, Gdtmp, d.Evp, 0);
-      LAUNCH_OK("gemm_nn_kernel(head dir)");
+      SPARF_TRY(gemm_nn(ep.dgrad, (int)Mc, d.HW, d.Evp, d.Ev, Ghid, d.HW, mlp->head_w[0], ldw8, d.W, nullptr, 0, nullptr, nullptr, Gdtmp, d.Evp, 0, st));
       ray_reduce_kernel<<<ceil_div((long long)nr * d.Evp, 256), 256, 0, st>>>(nr, S, d.Evp, Gdtmp, Gdenc);
       LAUNCH_OK("ray_reduce_kernel");
       direnc_bwd_kernel<<<ceil_div(nr, 128), 128, 0, st>>>(nr, mlp->L_view, d.Evp, denc, Gdenc, d_c, d_dirs + (size_t)r0 * 3);
@@ -670,12 +832,8 @@ int simt_mlp_backward(const SparfMLP* mlp, int R, int S, const float* origins, c
       const int rowoff = last ? 1 : 0;
       float* dWl = grad->trunk_w[l] + (size_t)rowoff * ldw;
       const float* Wl = mlp->trunk_w[l] + (size_t)rowoff * ldw;
-      gemm_tn_kernel<<<dim3(ceil_div(Kin, BN), ceil_div(d.W, BM), nslab), 256, 0, st>>>((int)Mc, d.W, Kin, Kinv, slab, G, d.W, in, Kin, 1, dWl, ldw, 0);
-      LAUNCH_OK("gemm_tn_kernel(trunk)");
-      if (l == d.skip) {
-        gemm_tn_kernel<<<dim3(ceil_div(d.E3p, BN), ceil_div(d.W, BM), nslab), 256, 0, st>>>((int)Mc, d.W, d.E3p, d.E3, slab, G, d.W, enc, d.E3p, 1, dWl, ldw, d.W);
-        LAUNCH_OK("gemm_tn_kernel(skip)");
-      }
+      SPARF_TRY(gemm_tn(ep.wgrad, (int)Mc, d.W, Kin, Kinv, slab, G, d.W, in, Kin, 1, dWl, ldw, 0, st));
+      if (l == d.skip) SPARF_TRY(gemm_tn(ep.wgrad, (int)Mc, d.W, d.E3p, d.E3, slab, G, d.W, enc, d.E3p, 1, dWl, ldw, d.W, st));
       colsum_kernel<<<dim3(ceil_div(d.W, 32), ceil_div(Mc, 1024)), 256, 0, st>>>(Mc, d.W, 1024, G, d.W, grad->trunk_b[l] + rowoff);
       LAUNCH_OK("colsum_kernel(trunk)");
       if (last) {
@@ -683,12 +841,12 @@ int simt_mlp_backward(const SparfMLP* mlp, int R, int S, const float* origins, c
         LAUNCH_OK("narrow_wgrad_kernel<1>");
       }
       if (l > 0) {
-        gemm_nn_kernel<<<dim3(ceil_div(d.W, BN), ceil_div(Mc, BM)), 256, 0, st>>>((int)Mc, d.W, d.W, d.W, G, d.W, Wl, ldw, 0, in, d.W, last ? graw : nullptr, last ? mlp->trunk_w[l] : nullptr, Gn, d.W, 0);
-        LAUNCH_OK("gemm_nn_kernel(trunk)");
+        SPARF_TRY(gemm_nn(ep.dgrad, (int)Mc, d.W, d.W, d.W, G, d.W, Wl, ldw, 0, in, d.W, last ? graw : nullptr,
+                          last ? mlp->trunk_w[l] : nullptr, Gn, d.W, 0, st));
       }
       if (need_rays && (l == d.skip || l == 0)) {
-        gemm_nn_kernel<<<dim3(ceil_div(d.E3p, BN), ceil_div(Mc, BM)), 256, 0, st>>>((int)Mc, d.W, d.E3p, d.E3, G, d.W, Wl, ldw, l == 0 ? 0 : d.W, nullptr, 0, nullptr, nullptr, Genc, d.E3p, genc_written ? 1 : 0);
-        LAUNCH_OK("gemm_nn_kernel(enc)");
+        SPARF_TRY(gemm_nn(ep.dgrad, (int)Mc, d.W, d.E3p, d.E3, G, d.W, Wl, ldw, l == 0 ? 0 : d.W, nullptr, 0, nullptr, nullptr, Genc,
+                          d.E3p, genc_written ? 1 : 0, st));
         genc_written = true;
       }
       float* tmp = G; G = Gn; Gn = tmp;

@@ -1,6 +1,7 @@
-// Internal interface of the SIMT fp32 MLP engine (mlp_simt.cu).
+// Internal interface of the layer-by-layer MLP engines (mlp_simt.cu).
 #pragma once
 #include "common.cuh"
+#include "gemm_wgmma.cuh"
 
 namespace sparf {
 
@@ -8,20 +9,29 @@ struct SimtDims {
   int E3, E3p, Ev, Evp, W, HW, nt, skip;
 };
 
+// GEMM precision per role: forward, input gradient (dgrad), weight gradient (wgrad)
+struct EnginePrec {
+  TcPrec fwd, dgrad, wgrad;
+};
+EnginePrec engine_prec(int engine);
+
 SimtDims simt_dims(const SparfMLP* mlp);
 int simt_validate(const SparfMLP* mlp);
-size_t simt_workspace_bytes(const SparfMLP* mlp, int R, int S, int backward);
-int simt_mlp_forward(const SparfMLP* mlp, int R, int S, const float* origins, const float* dirs, const float* t,
+// mode 0: forward, 1: backward (recompute), 2: backward from a tape, 3: taped forward
+size_t simt_workspace_bytes(const SparfMLP* mlp, int R, int S, int mode, int engine);
+int simt_mlp_forward(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs, const float* t,
                      const float* noise, float* sigma, float* rgb, void* workspace, size_t workspace_bytes,
                      cudaStream_t st);
-int simt_mlp_backward(const SparfMLP* mlp, int R, int S, const float* origins, const float* dirs, const float* t,
+size_t simt_tape_bytes(const SparfMLP* mlp, int R, int S);
+int simt_mlp_forward_tape(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs,
+                          const float* t, const float* noise, float* sigma, float* rgb, void* tape, size_t tape_bytes,
+                          void* workspace, size_t workspace_bytes, cudaStream_t st);
+int simt_mlp_backward_tape(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs,
+                           const float* t, const float* rgb, const float* d_sigma, const float* d_rgb, const SparfMLPGrad* grad,
+                           float* d_origins, float* d_dirs, void* tape, size_t tape_bytes, void* workspace,
+                           size_t workspace_bytes, cudaStream_t st);
+int simt_mlp_backward(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs, const float* t,
                       const float* noise, const float* d_sigma, const float* d_rgb, const SparfMLPGrad* grad,
                       float* d_origins, float* d_dirs, void* workspace, size_t workspace_bytes, cudaStream_t st);
-
-// shared small kernels reused by the tensor-core engine
-__global__ void c2f_weights_kernel(C2F c, int L_xyz, int L_view, float* __restrict__ wts);
-// view-direction encoding backward (d denc -> d dirs through unit = d/|d|), denc/Gdenc rows of Evp floats
-__global__ void direnc_bwd_kernel(int nrays, int L, int Evp, const float* __restrict__ denc, const float* __restrict__ Gdenc,
-                                  const float* __restrict__ dirs, float* __restrict__ d_d);
 
 }  // namespace sparf

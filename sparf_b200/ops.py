@@ -15,7 +15,7 @@ from . import _lib
 from ._lib import SparfMLP, SparfMLPGrad, check
 
 _ENGINE = [_lib.ENGINE_AUTO]
-# keep the training forward's operand images for the backward (tcgen05 engine); False = always recompute
+# keep the training forward's activations for the backward when offered (sparf_mlp_tape_bytes > 0); False = always recompute
 USE_TAPE = [True]
 # Opt-in: let the MLP backward accumulate straight into existing `param.grad` storage (the C ABI accumulates, +=)
 # instead of returning fresh gradient tensors for autograd to add.  Saves ~20 tiny kernels and a 2 MB memset per
@@ -196,7 +196,7 @@ class MLPFunction(torch.autograd.Function):
         nbytes = L.sparf_mlp_workspace_bytes(ctypes.byref(m), R, S, 0, engine)
         ws = _workspace(nbytes, t.device)
         # Training forward: when a gradient will be asked for and the engine offers it, keep a "tape" (the
-        # per-layer operand images) so that the backward skips the forward recompute.
+        # fp32 encodings and activations) so that the backward skips the forward recompute.
         # (grad_mode: autograd is recording at the call site -- under torch.no_grad() nothing is kept)
         EVALS["fwd"] += R * S
         wants_grad = grad_mode and (any(ctx.needs_input_grad[i] for i in (3, 4)) or any(ctx.needs_input_grad[8:]))

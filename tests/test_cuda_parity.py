@@ -19,7 +19,7 @@ from helpers import check_grads, load_golden, rel_err, replay_graph
 
 pytestmark = pytest.mark.gpu
 
-ENGINES = ["simt_fp32", "tc_3x"]   # fp32 CUDA-core engine and the tcgen05 split-precision engine
+ENGINES = ["simt_fp32", "tc_3x"]   # fp32 CUDA-core engine and the wgmma split-precision engine
 # stage tests need the reference's intermediate tensors (origins / viewdirs / t), which render_by_slices drops
 STAGE_CASES = [n for n in common.CASES if not common.CASES[n].get("full_image")]
 
@@ -89,7 +89,7 @@ def test_mlp_and_composite_stage(name, engine):
         else:
             pred = nerf.forward_samples(opt, center, ray, t, mode=c["mode"])
         pred = nerf.composite(opt, ray, pred, t)
-        # fp32 engine: the reference's op order, 2e-5; tcgen05 3-pass fp16 split: fp32-level products in a different
+        # fp32 engine: the reference's op order, 2e-5; tensor-core 3-pass fp16 split: fp32-level products in a different
         # summation order, measured <= 3e-5 against the fp32 engine (tests/test_tc_engine.py)
         tol = 2e-5 if engine == "simt_fp32" else 3e-5
         if common.CASES[name].get("depth_param", "metric") == "inverse":
@@ -156,7 +156,7 @@ def test_graph_end_to_end_vs_reference(name, engine):
     # gradients: fp32 accumulation over ~1e4 rows in a different order + the input-side noise above
     # The reference's own fp32 gradient sits ~3e-2 from the exact (fp64) gradient on these random nets
     # (tests/test_tc_engine.py::test_tc_backward_matches_simt measures both engines against fp64): the SIMT
-    # engine shares the reference's op order and lands closer to IT; the tcgen05 engine is equally close to
+    # engine shares the reference's op order and lands closer to IT; the tensor-core engine is equally close to
     # the truth but not to the reference's particular rounding.
     # (c8: with the Charbonnier / distortion terms the reference's fp32 gradient is itself 1.2e-1 from the fp64 one)
     # (c13: near plane 0.1, nine views: the fine network's gradients sit behind resampled positions close to the cameras
@@ -211,7 +211,7 @@ def test_c4_inverse_depth_error_vs_fp64(engine):
 def test_coarse_cases_error_vs_fp64(name, engine):
     """The same yardstick for the metric-depth goldens without a resampling step (c1; c3 with pose gradients, BARF mask
     and sigma noise): outputs within 2x and gradient tensors within 3x (relative L2) of the reference's own fp32 distance
-    from the exact result, floors 1e-4 / 1e-3 -- the tight gate of the tcgen05 engine's gradients, which the comparison
+    from the exact result, floors 1e-4 / 1e-3 -- the tight gate of the tensor-core engine's gradients, which the comparison
     with the golden alone (6e-2, the reference's own noise) cannot give.  (Hierarchical cases are excluded: a last-bit
     change of a coarse weight moves a resampled position discontinuously, in exact arithmetic as well; the headline-shape
     test tests/test_headline_parity.py covers the full-size batch the same way.)  The fp32 CUDA-core engine accumulates the

@@ -141,7 +141,7 @@ def test_full_sparf_step_vs_reference(name, engine):
     # test_tc_engine.py); inverse depth (samples out to t = 256, arguments ~1e5 rad in the top encoding bands, plus the
     # hard visibility / validity thresholds of the SPARF losses): the reference's fp32 gradients are themselves 7e-2 from
     # exact on the photometric-only case c4 (test_inverse_depth_conditioning_c4) and single entries behave like phase
-    # noise (max-norm measured 0.2 .. 0.41, relative L2 0.2 (fp32 engine) .. 0.36 (tcgen05 engine) per tensor): the gate is the relative L2 distance per tensor
+    # noise (max-norm measured 0.2 .. 0.41, relative L2 0.2 (fp32 engine) .. 0.36 (tensor-core engine) per tensor): the gate is the relative L2 distance per tensor
     inv = c.get("depth_param") == "inverse"
     _run_and_check(name, engine, gold, c, opt, data, ray_idx, net, loss_module, pose_net.pose_embedding,
                    gtol=0.5 if inv else 6e-2, gnorm="l2" if inv else "max")

@@ -1,8 +1,8 @@
-"""Pose-parameter modules vs the reference's own modules, imported from /root/reference when it is mounted (the build
-container); on the GPU box the reference is absent and the comparison is skipped (the golden-backed tests remain)."""
+"""Pose-parameter modules vs the reference's own modules.  The reference module's outputs on the same inputs are
+stored in tests/golden/ref_pose_quaternion.npz (tests/golden/make_module_golden.py)."""
 import os
-import sys
 
+import numpy as np
 import pytest
 import torch
 
@@ -10,7 +10,7 @@ import common
 from sparf_b200.poses_models import QuaternionsPoseParameters
 from sparf_b200.utils.edict import edict
 
-HAVE_REF = os.path.isdir("/root/reference/source")
+REF_CASES = [(False, False, True, True), (True, True, True, True), (True, False, False, True), (False, True, True, False)]
 
 
 def _opt(c2w, rel, rot=True, trans=True):
@@ -37,24 +37,22 @@ def test_quaternion_pose_model_round_trip_and_gradients(c2w, rel):
     assert m.rot_embedding.grad.abs().sum() > 0 and m.trans_embedding.grad.abs().sum() > 0
 
 
-@pytest.mark.skipif(not HAVE_REF, reason="reference checkout not mounted")
-@pytest.mark.parametrize("c2w,rel,rot,trans", [(False, False, True, True), (True, True, True, True), (True, False, False, True),
-                                               (False, True, True, False)])
+def _move(m, rot, trans):
+    """move a pose model off its initial value (same way for ours and the reference's)"""
+    with torch.no_grad():
+        if rot:
+            m.rot_embedding += 0.05 * torch.arange(m.rot_embedding.numel()).view_as(m.rot_embedding).float().cos()
+        if trans:
+            m.trans_embedding += 0.1
+
+
+@pytest.mark.parametrize("c2w,rel,rot,trans", REF_CASES)
 def test_quaternion_pose_model_matches_reference_module(c2w, rel, rot, trans):
-    here = os.path.dirname(os.path.abspath(__file__))
-    for p in (os.path.join(here, "golden", "_shims"), "/root/reference"):
-        if p not in sys.path:
-            sys.path.insert(0, p)
-    from source.models.poses_models.quaternion import QuaternionsPoseParameters as Ref
-    w2c = _poses(5)
-    opt = _opt(c2w, rel, rot, trans)
-    ours, ref = QuaternionsPoseParameters(opt, 4, w2c, torch.device("cpu")), Ref(opt, 4, w2c, torch.device("cpu"))
-    assert torch.allclose(torch.as_tensor(ours.rot_embedding), torch.as_tensor(ref.rot_embedding), atol=1e-6)
-    with torch.no_grad():       # move both off the initial value the same way
-        for m in (ours, ref):
-            if rot:
-                m.rot_embedding += 0.05 * torch.arange(m.rot_embedding.numel()).view_as(m.rot_embedding).float().cos()
-            if trans:
-                m.trans_embedding += 0.1
-    assert torch.allclose(ours.get_w2c_poses(), ref.get_w2c_poses(), atol=1e-6)
-    assert torch.allclose(ours.get_c2w_poses(), ref.get_c2w_poses(), atol=1e-6)
+    gold = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_pose_quaternion.npz"))
+    i = REF_CASES.index((c2w, rel, rot, trans))
+    w2c = torch.from_numpy(gold["pose%d_input_w2c" % i])     # the poses the reference module was built from
+    ours = QuaternionsPoseParameters(_opt(c2w, rel, rot, trans), 4, w2c, torch.device("cpu"))
+    assert torch.allclose(torch.as_tensor(ours.rot_embedding), torch.from_numpy(gold["pose%d_rot_init" % i]), atol=1e-6)
+    _move(ours, rot, trans)
+    assert torch.allclose(ours.get_w2c_poses(), torch.from_numpy(gold["pose%d_w2c" % i]), atol=1e-6)
+    assert torch.allclose(ours.get_c2w_poses(), torch.from_numpy(gold["pose%d_c2w" % i]), atol=1e-6)

@@ -1,5 +1,5 @@
-"""tcgen05 engine: hardware self-test of the Blackwell primitives, then the fused MLP kernels against
-the SIMT fp32 engine (same C ABI, same inputs, on the device) and the reference goldens."""
+"""Tensor-core engines: exact-integer self-tests of the wgmma GEMM kernels, then the engines against the SIMT fp32
+engine (same C ABI, same inputs, on the device) and the fp64 oracle."""
 import ctypes
 
 import numpy as np
@@ -15,8 +15,8 @@ def _p(t):
 
 @pytest.mark.parametrize("K", [64, 128, 256])
 def test_tcgen05_selftest_gemm_exact(K):
-    """Small-integer operands are exact in bf16 and their dot products exact in fp32: bit-exact result
-    proves operand layout, descriptors, K stepping, bulk copy and TMEM addressing."""
+    """Small-integer operands are exact in bf16 and their dot products exact in fp32: a bit-exact result
+    proves the shared-memory operand layout, the wgmma descriptors, K stepping and the accumulator fragment mapping."""
     from sparf_b200 import _lib
     L = _lib.lib()
     g = torch.Generator(device="cpu").manual_seed(K)
@@ -26,24 +26,6 @@ def test_tcgen05_selftest_gemm_exact(K):
     D = torch.full((128, 128), -777.0, device="cuda")
     _lib.check(L.sparf_tc_selftest(_p(A), _p(B), K, _p(packed), _p(D), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)),
                "tc_selftest")
-    torch.cuda.synchronize()
-    ref = A @ B.t()
-    assert torch.equal(D, ref), (D - ref).abs().max().item()
-
-
-@pytest.mark.parametrize("K", [64, 128, 256])
-def test_tcgen05_selftest_a_operand_in_tmem(K):
-    """Same exact-integer GEMM with the A operand written to tensor memory by tcgen05.st and consumed from there
-    (lane = row, column c = K elements 2c, 2c+1; +8 columns per K16 step)."""
-    from sparf_b200 import _lib
-    L = _lib.lib()
-    g = torch.Generator(device="cpu").manual_seed(100 + K)
-    A = torch.randint(-4, 5, (128, K), generator=g).float().cuda()
-    B = torch.randint(-4, 5, (128, K), generator=g).float().cuda()
-    packed = torch.zeros(128 * K * 2, dtype=torch.uint8, device="cuda")
-    D = torch.full((128, 128), -777.0, device="cuda")
-    _lib.check(L.sparf_tc_selftest_ts(_p(A), _p(B), K, _p(packed), _p(D), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)),
-               "tc_selftest_ts")
     torch.cuda.synchronize()
     ref = A @ B.t()
     assert torch.equal(D, ref), (D - ref).abs().max().item()
@@ -69,10 +51,10 @@ def _rand_problem(R, S, seed=0, c2f=None, peaky=True):
 
 @pytest.mark.parametrize("R,S,c2f", [(8, 128, None), (1023, 128, None), (333, 96, (0.4, 0.7)), (37, 384, None), (5, 1, None)])
 def test_tc_forward_matches_simt(R, S, c2f):
-    """Fused tcgen05 forward (3-pass bf16 split) vs the fp32 SIMT engine on identical device inputs."""
+    """Tensor-core forward (3-pass fp16 split) vs the fp32 SIMT engine on identical device inputs."""
     from sparf_b200 import _lib, ops
     if not _lib.lib().sparf_engine_available(_lib.ENGINE_TC_3X):
-        pytest.skip("tcgen05 engine not available")
+        pytest.skip("tensor-core engine not available")
     spec, params, o, d, t, prog = _rand_problem(R, S, seed=R, c2f=c2f)
     noise = torch.randn(R, S, device="cuda") * 0.5
     with torch.no_grad():
@@ -96,7 +78,7 @@ def test_tc_single_pass_is_a_fast_mode_outside_the_bound():
     """TC_1X (one bf16 pass) runs and is close, but is NOT the parity engine (error ~1e-3)."""
     from sparf_b200 import _lib, ops
     if not _lib.lib().sparf_engine_available(_lib.ENGINE_TC_1X):
-        pytest.skip("tcgen05 engine not available")
+        pytest.skip("tensor-core engine not available")
     spec, params, o, d, t, prog = _rand_problem(256, 128, seed=3)
     with torch.no_grad():
         s_ref, c_ref = ops.mlp_forward(spec, o, d, t, params, progress=prog, engine=_lib.ENGINE_SIMT_FP32)
@@ -108,7 +90,7 @@ def test_tc_single_pass_is_a_fast_mode_outside_the_bound():
 
 @pytest.mark.parametrize("rows", [64, 128])
 def test_tcgen05_selftest_tn_mn_major(rows):
-    """D = G^T X through MN-major descriptors on the forward's operand image (weight-gradient GEMM shape)."""
+    """D = G^T X through the weight-gradient kernel (contraction over rows, operands read transposed)."""
     from sparf_b200 import _lib
     L = _lib.lib()
     g = torch.Generator(device="cpu").manual_seed(rows)
@@ -122,16 +104,15 @@ def test_tcgen05_selftest_tn_mn_major(rows):
     assert torch.equal(D, ref), (D - ref).abs().max().item()
 
 
-# the last three batches exceed one backward chunk (1024 row tiles): the taped forward keeps ONE tape and the backward
-# walks it chunk by chunk (tile-aligned chunk starts, accumulating gradients); the recompute path chunks as well
+# the last three batches exceed one backward chunk (32768 rows): gradients accumulate over the chunks
 @pytest.mark.parametrize("R,S,c2f", [(8, 128, None), (1023, 128, None), (100, 96, (0.4, 0.7)), (37, 384, None),
                                      (1100, 128, None), (600, 256, (0.4, 0.7)), (1400, 96, None)])
 def test_tc_backward_matches_simt(R, S, c2f):
-    """tcgen05 backward (bf16 3-pass recompute + dgrad chain + MN-major wgrad) vs the fp32 SIMT engine:
-    every parameter gradient, same upstream gradients, same device inputs."""
+    """Tensor-core backward (recomputed fp16 3-pass forward, bf16 3-pass input and weight gradients) vs the fp32 SIMT
+    engine: every parameter gradient, same upstream gradients, same device inputs."""
     from sparf_b200 import _lib, ops
     if not _lib.lib().sparf_engine_available(_lib.ENGINE_TC_3X):
-        pytest.skip("tcgen05 engine not available")
+        pytest.skip("tensor-core engine not available")
     spec, params, o, d, t, prog = _rand_problem(R, S, seed=R + 1, c2f=c2f)
     noise = torch.randn(R, S, device="cuda") * 0.3
     g = torch.Generator(device="cuda").manual_seed(7)
@@ -139,7 +120,7 @@ def test_tc_backward_matches_simt(R, S, c2f):
     gc = torch.randn(R, S, 3, device="cuda", generator=g) * 1e-3
     grads = {}
     for eng, tape in ((_lib.ENGINE_SIMT_FP32, True), (_lib.ENGINE_TC_3X, True), (_lib.ENGINE_TC_3X, False)):
-        ops.USE_TAPE[0] = tape     # tcgen05: taped training forward (no recompute) and the recompute path
+        ops.USE_TAPE[0] = tape     # with and without a tape request (engines without a tape recompute either way)
         ps = [p.clone().requires_grad_(True) for p in params]
         s, c = ops.mlp_forward(spec, o, d, t, ps, noise=noise, progress=prog, engine=eng)
         ((s * gs).sum() + (c * gc).sum()).backward()
@@ -170,16 +151,16 @@ def test_tc_backward_matches_simt(R, S, c2f):
         assert e_tc < max(2e-3, 4 * e_simt), (keys[i], e_tc, e_simt)
         e_rc = ((grads["tc_recompute"][i].double() - tr).abs().max() / den).item()
         assert e_rc < max(2e-3, 4 * e_simt), (keys[i], "recompute path", e_rc, e_simt)
-    print("R=%d S=%d: worst grad rel err vs fp64: tcgen05 %.2e, simt fp32 %.2e" % (R, S, worst_tc, worst_simt))
+    print("R=%d S=%d: worst grad rel err vs fp64: tensor cores %.2e, simt fp32 %.2e" % (R, S, worst_tc, worst_simt))
 
 
 @pytest.mark.parametrize("R,S,c2f", [(64, 128, None), (341, 128, (0.4, 0.7)), (50, 96, (0.1, 0.9)), (1100, 128, (0.4, 0.7))])
 def test_tc_ray_gradients_match_simt(R, S, c2f):
-    """dL/d origins, dL/d dirs (camera-pose optimisation) from the tcgen05 path (G4.W4e + G0.W0 on tensor
-    cores + encoding backward in the epilogue + view-direction chain) vs the fp32 SIMT engine."""
+    """dL/d origins, dL/d dirs (camera-pose optimisation) from the tensor-core path (G4.W4e + G0.W0 on tensor cores,
+    encoding backward, view-direction chain) vs the fp32 SIMT engine."""
     from sparf_b200 import _lib, ops
     if not _lib.lib().sparf_engine_available(_lib.ENGINE_TC_3X):
-        pytest.skip("tcgen05 engine not available")
+        pytest.skip("tensor-core engine not available")
     spec, params, o, d, t, prog = _rand_problem(R, S, seed=R + 5, c2f=c2f, peaky=False)
     g = torch.Generator(device="cuda").manual_seed(3)
     gs = torch.randn(R, S, device="cuda", generator=g) * 1e-2
@@ -200,11 +181,10 @@ def test_tc_ray_gradients_match_simt(R, S, c2f):
 @pytest.mark.parametrize("R,S,c2f", [(1023, 128, None), (300, 96, (0.4, 0.7)), (1100, 128, None)])
 def test_tc_3x_w1_reduced_weight_gradient_engine(R, S, c2f):
     """SPARF_ENGINE_TC_3X_W1 (non-default): same forward and same ray gradients as TC_3X, the wide layers' weight / bias
-    gradients from ONE bf16 pass over the hi halves of the saved images -- close to TC_3X, but outside the parity bound
-    (its error against fp64 is tabulated in profiles/r02_engine_errors.md)."""
+    gradients from ONE bf16 pass over the hi halves -- close to TC_3X, but outside the parity bound."""
     from sparf_b200 import _lib, ops
     if not _lib.lib().sparf_engine_available(_lib.ENGINE_TC_3X_W1):
-        pytest.skip("tcgen05 engine not available")
+        pytest.skip("tensor-core engine not available")
     spec, params, o, d, t, prog = _rand_problem(R, S, seed=R + 9, c2f=c2f)
     g = torch.Generator(device="cuda").manual_seed(11)
     gs = torch.randn(R, S, device="cuda", generator=g) * 1e-3

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Secondary measurements for profiles/r01_notes.md (not the bench line): full-image inference through
+"""Secondary measurements (not the bench line): full-image inference through
 Graph.render_by_slices (SURVEY 8f.3) and the hierarchical (coarse + fine network) training step, DTU-shaped."""
 import os
 import sys

@@ -3,7 +3,7 @@
 photometric loss, gradients of the 20 MLP tensors and of the 9-D pose embedding), next to the error of the reference's
 own fp32 arithmetic (the oracle run in fp32 on the same GPU, TF32 off), and the time of one forward + backward.
 
-    python tools/engine_error_table.py [--out profiles/r02_engine_errors.md]
+    python tools/engine_error_table.py [--out FILE.md]
 
 Columns: max-normalised error  max|x - exact| / max|exact|  and relative L2 error  ||x - exact|| / ||exact||, the worst
 tensor of each group.  (Test infrastructure: imports oracle/ through tests/test_headline_parity.py.)
@@ -95,7 +95,7 @@ def main(argv=None):
         rows.append(("sparf_b200 `%s`" % eng,) + run_ours(eng, opt, sd, data_dev, init_w2c, ray_idx, dev))
 
     lines = ["# Engine error against the fp64 oracle, headline shape (1023 rays x 128 samples, loss + all gradients)", "",
-             "`python tools/engine_error_table.py` on one B200.  Each cell: max-normalised error / relative L2 error of the worst",
+             "`python tools/engine_error_table.py` on one H100.  Each cell: max-normalised error / relative L2 error of the worst",
              "tensor of the group; ms = best of 5 eager forward + backward passes through the public API (no CUDA graph).", "",
              "| arithmetic | rgb | depth | loss (rel) | " + " | ".join(g for g, _ in GROUPS) + " | ms |",
              "|---|---|---|---|" + "---|" * len(GROUPS) + "---:|"]

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""A few taped MLP training steps at the bench shape (1023 rays x 128 samples): the target of the ncu captures.
+"""A few taped MLP training steps at the bench shape (1023 rays x 128 samples), e.g. to run under torch.profiler.
 [SPARF_OS_ENGINE=tc_3x|tc_3x_w1] python tools/one_step.py [steps]"""
 import os
 import sys

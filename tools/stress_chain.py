@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Repeat the taped MLP training step with a cold L2 (weights arrive late, the warp roles drift apart) and check that
-every repetition reproduces the first one: forward outputs bit-exactly, gradients to rounding of the atomics."""
+"""Repeat the MLP training step with a cold L2 and check that every repetition reproduces the first one: forward outputs
+bit-exactly, gradients to rounding of the atomics.  STRESS_ENGINE=tc_3x (default) | tc_1x | tc_3x_w1 | simt_fp32."""
 import os
 import sys
 
@@ -16,7 +16,6 @@ from sparf_b200 import _lib, ops
 def main():
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 200
     R, S = (int(sys.argv[2]), int(sys.argv[3])) if len(sys.argv) > 3 else (1023, 128)
-    ops.USE_TAPE[0] = os.environ.get("STRESS_TAPE", "1") != "0"    # 0: the recompute (no tape) backward
     opt = common.make_opt(S=S)
     sd = common.det_weights(opt, 0)
     keys = sum([["mlp_feat.%d.weight" % i, "mlp_feat.%d.bias" % i] for i in range(8)], []) + \
@@ -26,6 +25,7 @@ def main():
     d = torch.nn.functional.normalize(torch.randn(R, 3, device="cuda"), dim=-1).requires_grad_(True)
     t = torch.sort(torch.rand(R, S, device="cuda") * 4 + 1.2, dim=1).values
     spec = ops.MLPSpec()
+    engine = _lib.ENGINES[os.environ.get("STRESS_ENGINE", "tc_3x")]
     gs, gc = torch.randn(R, S, device="cuda"), torch.randn(R, S, 3, device="cuda")
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     ref = None
@@ -34,7 +34,7 @@ def main():
         flush.fill_(it & 255)
         for p in params + [o, d]:
             p.grad = None
-        s, c = ops.mlp_forward(spec, o, d, t, params, engine=_lib.ENGINE_TC_3X)
+        s, c = ops.mlp_forward(spec, o, d, t, params, engine=engine)
         torch.autograd.backward([s, c], [gs, gc])
         torch.cuda.synchronize()
         cur = [s.detach().clone(), c.detach().clone()] + [p.grad.clone() for p in params + [o, d]]

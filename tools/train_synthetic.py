@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""End-to-end training loop on the B200-native path, reference-shaped: `RaySamplingStrategy` -> `Graph.render...` ->
+"""End-to-end training loop on the CUDA path, reference-shaped: `RaySamplingStrategy` -> `Graph.render...` ->
 `define_loss(...).compute_loss` -> `backward()` -> fused clip + Adam + ExponentialLR, the WHOLE iteration captured once
 as a CUDA graph and replayed (source/training/nerf_trainer.py:207-275 `train_iteration` + iter_based_trainer.py:128-147).
 
