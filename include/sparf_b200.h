@@ -224,6 +224,12 @@ int sparf_adam_step(int64_t n, float* param, float* grad, float* exp_avg, float*
 int sparf_tc_selftest(const float* A, const float* B, int32_t K, void* packed, float* D, sparf_stream_t stream);
 /* Same for the weight-gradient kernel: D[128,128] = G[rows,128]^T X[rows,128], rows in {64, 128}. */
 int sparf_tc_selftest_tn(const float* G, const float* X, int32_t rows, float* D, sparf_stream_t stream);
+/* The operand images a GEMM epilogue writes, chained through three 3-pass bf16 GEMMs, M in [1, 1024]:
+ * D = X W1 (X [M,128], W1 [128,96]) is written only as a row image, a transposed image and db[96] = column sums of D;
+ * Y[M,128] = [D | E] W2^T (E [M,40], W2 [128,136]) reads the row image as the first segment of a two-segment operand;
+ * Z[96,128] = D^T X reads the transposed image.  Exact on small integers. */
+int sparf_tc_selftest_images(const float* X, const float* W1, const float* E, const float* W2, int32_t M, float* Y, float* Z,
+                             float* db, sparf_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -60,6 +60,7 @@ _SIGNATURES = {
     "sparf_adam_step": (c_int32, [c_int64, _P, _P, _P, _P, _P, _P] + [ctypes.c_double] * 7 + [_P]),
     "sparf_tc_selftest": (c_int32, [_P, _P, c_int32, _P, _P, _P]),
     "sparf_tc_selftest_tn": (c_int32, [_P, _P, c_int32, _P, _P]),
+    "sparf_tc_selftest_images": (c_int32, [_P, _P, _P, _P, c_int32, _P, _P, _P, _P]),
 }
 
 _lib = None

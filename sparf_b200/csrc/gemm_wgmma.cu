@@ -1,15 +1,17 @@
 // wgmma GEMMs of the tensor-core MLP engines (SPARF_ENGINE_TC_3X / TC_1X / TC_3X_W1), sm_90a.
 //
-// Two kernels per GEMM:
-//   pack: the fp32 operands (with the GEMM's own indexing: concatenated sources, transposes, per-ray rows, bounds) are
-//     split once into 16-bit (hi, lo) halves and written as an image of [128 rows x 32 K] tiles, each tile already in the
-//     canonical no-swizzle K-major shared-memory layout (8 x 8 core matrices of 128 contiguous bytes, core matrices
-//     adjacent in K 128 B apart = leading byte offset, 8-row groups 512 B apart = stride byte offset), hi and lo halves of
-//     a tile adjacent (16 KB);
+// The GEMMs read both operands as images: 16-bit (hi, lo) halves in [128 rows x 32 K] tiles, each tile already in the
+// canonical no-swizzle K-major shared-memory layout (8 x 8 core matrices of 128 contiguous bytes, core matrices adjacent
+// in K 128 B apart = leading byte offset, 8-row groups 512 B apart = stride byte offset), hi and lo halves of a tile
+// adjacent (16 KB).
+//   pack: splits an fp32 operand (with the GEMM's own indexing: transposes, per-ray rows, bounds) into an image; the
+//     weights, the encodings and the colour-head gradient take this path;
 //   gemm: one CTA = two warpgroups = one 128 x 128 output tile; one thread streams the tiles of both operands with
 //     cp.async.bulk into a STAGES-deep ring of shared-memory stages, each completing on its own mbarrier (complete_tx);
 //     both warpgroups wait on the stage's barrier and issue wgmma.m64n128k16 (register accumulators); one MMA group stays
-//     in flight while the stage consumed before it is refilled, so STAGES - 1 tile copies overlap the MMAs.
+//     in flight while the stage consumed before it is refilled, so STAGES - 1 tile copies overlap the MMAs.  The
+//     epilogue can write the output's own images (row and transposed) for the next GEMMs, so trunk activations and
+//     gradients are never packed from fp32.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -105,14 +107,12 @@ __device__ __forceinline__ void tile_pos(int i, int& r, int& k) {
 }
 
 // ---- operand views: f(k-step, row, k within the step) -> fp32 element (0 outside the operand)
-struct NtA {    // X1[m][k] for k-steps < s1, then X2[m / div2][k]
-  const float *X1, *X2;
-  int ld1, K1, ld2, K2, div2, M, s1;
+struct Rows {   // X[m / div][k]
+  const float* X;
+  int ldx, K, div, M;
   __device__ float operator()(int kt, int m, int kk) const {
-    const bool two = kt >= s1;
-    const int k = (two ? kt - s1 : kt) * TK + kk;
-    if (m >= M || k >= (two ? K2 : K1)) return 0.f;
-    return two ? X2[(size_t)(m / div2) * ld2 + k] : X1[(size_t)m * ld1 + k];
+    const int k = kt * TK + kk;
+    return (m < M && k < K) ? X[(size_t)(m / div) * ldx + k] : 0.f;
   }
 };
 struct NtB {    // W[n][k] (first source), W[n][wcol2 + k] (second source)
@@ -125,14 +125,6 @@ struct NtB {    // W[n][k] (first source), W[n][wcol2 + k] (second source)
     return W[(size_t)n * ldw + (two ? wcol2 : 0) + k];
   }
 };
-struct NnA {    // G[m][n], contraction over n
-  const float* G;
-  int ldg, M, N;
-  __device__ float operator()(int kt, int m, int nn) const {
-    const int n = kt * TK + nn;
-    return (m < M && n < N) ? G[(size_t)m * ldg + n] : 0.f;
-  }
-};
 struct NnB {    // W[n][wcol + k] as rows k, contraction over n
   const float* W;
   int ldw, wcol, Kv, N;
@@ -141,12 +133,12 @@ struct NnB {    // W[n][wcol + k] as rows k, contraction over n
     return (n < N && k < Kv) ? W[(size_t)n * ldw + wcol + k] : 0.f;
   }
 };
-struct TnA {    // G[m][n] as rows n, contraction over m
-  const float* G;
-  int ldg, M, N;
+struct Cols {   // X[m][n] as rows n, contraction over m
+  const float* X;
+  int ldx, M, N;
   __device__ float operator()(int kt, int n, int mm) const {
     const int m = kt * TK + mm;
-    return (m < M && n < N) ? G[(size_t)m * ldg + n] : 0.f;
+    return (m < M && n < N) ? X[(size_t)m * ldx + n] : 0.f;
   }
 };
 struct TnB {    // X[m / div][k] as rows k, contraction over m
@@ -207,12 +199,21 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 }
 __device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;\n" ::: "memory"); }
 
+// A GEMM operand as images: k-steps [0, ks0) of each row tile from image p0 (ks0 k-steps per row tile), the rest from
+// p1 (ks1 k-steps per row tile), e.g. [H3 | enc] at the skip layer
+struct Opnd {
+  const uint16_t *p0, *p1;
+  int ks0, ks1;
+  __device__ const uint16_t* tile(int rt, int kt) const {
+    return kt < ks0 ? p0 + ((size_t)rt * ks0 + kt) * 2 * TILE_ELEMS : p1 + ((size_t)rt * ks1 + kt - ks0) * 2 * TILE_ELEMS;
+  }
+};
+
 // acc[64] of this thread = its fragment of the warpgroup's [64 x 128] block: acc[4 j + 2 h + c] is
-// row 16 warp + lane/4 + 8 h, column 8 j + 2 (lane % 4) + c.  Operands: A image row tile blockIdx.y, B image row tile
-// blockIdx.x, k-steps [kt0, kt0 + nk) of images with a_ks / b_ks k-steps per row tile.
+// row 16 warp + lane/4 + 8 h, column 8 j + 2 (lane % 4) + c.  Operands: A row tile blockIdx.y, B row tile blockIdx.x,
+// k-steps [kt0, kt0 + nk).
 template <bool F16, int PASSES>
-__device__ __forceinline__ void wg_pipeline(float (&acc)[64], const uint16_t* __restrict__ pa, int a_ks,
-                                            const uint16_t* __restrict__ pb, int b_ks, int kt0, int nk) {
+__device__ __forceinline__ void wg_pipeline(float (&acc)[64], const Opnd& a, const Opnd& b, int kt0, int nk) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   const int tid = threadIdx.x, wg = tid >> 7;
@@ -228,14 +229,12 @@ __device__ __forceinline__ void wg_pipeline(float (&acc)[64], const uint16_t* __
   __syncthreads();
   if (nk <= 0) return;
   const uint32_t bytes = PASSES == 3 ? 2 * TILE_BYTES : TILE_BYTES;
-  const uint16_t* a0 = pa + ((size_t)blockIdx.y * a_ks + kt0) * 2 * TILE_ELEMS;
-  const uint16_t* b0 = pb + ((size_t)blockIdx.x * b_ks + kt0) * 2 * TILE_ELEMS;
   auto issue = [&](int j) {       // k-step j of this CTA -> stage j % STAGES
     uint8_t* st = smem + (j % STAGES) * STAGE_BYTES;
     uint64_t* bar = &full[j % STAGES];
     mbar_expect_tx(bar, 2 * bytes);
-    bulk_g2s(st, a0 + (size_t)j * 2 * TILE_ELEMS, bytes, bar);
-    bulk_g2s(st + 2 * TILE_BYTES, b0 + (size_t)j * 2 * TILE_ELEMS, bytes, bar);
+    bulk_g2s(st, a.tile(blockIdx.y, kt0 + j), bytes, bar);
+    bulk_g2s(st + 2 * TILE_BYTES, b.tile(blockIdx.x, kt0 + j), bytes, bar);
   };
   if (tid == 0)
     for (int j = 0; j < STAGES - 1 && j < nk; ++j) issue(j);
@@ -272,6 +271,23 @@ __device__ __forceinline__ int frag_row(int i) {
 }
 __device__ __forceinline__ int frag_col(int i) { return (i >> 2) * 8 + (threadIdx.x & 3) * 2 + (i & 1); }
 
+// two fp32 values of adjacent columns -> their hi halves and their lo halves, each pair in 32 bits (first column low)
+template <bool F16>
+__device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+  uint16_t h0, l0, h1, l1;
+  split16<F16>(x0, h0, l0);
+  split16<F16>(x1, h1, l1);
+  hi = h0 | (uint32_t)h1 << 16;
+  lo = l0 | (uint32_t)l1 << 16;
+}
+
+// this lane's 32 bits of the transpose of the warp's 8 x 8 16-bit matrix (same fragment layout)
+__device__ __forceinline__ uint32_t movmatrix_trans(uint32_t x) {
+  uint32_t y;
+  asm volatile("movmatrix.sync.aligned.m8n8.trans.b16 %0, %1;\n" : "=r"(y) : "r"(x));
+  return y;
+}
+
 struct Epi {
   int kind;                 // 0: Y = act(acc + bias) ; 1: D (=|+=) mask * (acc + r1_vec r1_row) ; 2: dW += acc (atomic)
   int M, N, act;            // output rows / columns
@@ -280,31 +296,102 @@ struct Epi {
   int ldo, col_off, Kv;
   const float *mask, *r1_vec, *r1_row;
   int ldmask, accumulate;
+  float* colsum;            // kind 1: += column sums of the output
+  uint16_t *row, *tr;       // output images, row_ks / tr_ks k-steps per row tile
+  int row_ks, tr_ks;
 };
 
-template <bool F16, int PASSES>
-__global__ void __launch_bounds__(256) wg_gemm_kernel(const uint16_t* __restrict__ pa, int a_ks, const uint16_t* __restrict__ pb,
-                                                      int b_ks, int nk_total, int nk_slab, Epi e) {
+// One CTA = one 128 x 128 output tile.  The epilogue writes, each only when its template flag is set: the fp32 output
+// (F32), a row image of the output (rows = output rows, K = output columns) and a transposed image (rows = output
+// columns, K = output rows), with ROWP / TRP passes (3: hi and lo halves, 1: hi only) in the GEMM's 16-bit type.  An
+// image holds the split of the very fp32 value the output gets, zero past M and N, so it is bit-identical to what
+// pack_kernel would make of the fp32 output.  Images and column sums take one slab (gridDim.z == 1) and no accumulate.
+template <bool F16, int PASSES, bool F32, int ROWP, int TRP>
+__global__ void __launch_bounds__(256) wg_gemm_kernel(Opnd a, Opnd b, int nk_total, int nk_slab, Epi e) {
   const int kt0 = blockIdx.z * nk_slab;
   float acc[64];
-  wg_pipeline<F16, PASSES>(acc, pa, a_ks, pb, b_ks, kt0, min(nk_slab, nk_total - kt0));
+  wg_pipeline<F16, PASSES>(acc, a, b, kt0, min(nk_slab, nk_total - kt0));
   const int m0 = blockIdx.y * TM, n0 = blockIdx.x * TN;
 #pragma unroll
   for (int i = 0; i < 64; ++i) {
     const int m = m0 + frag_row(i), n = n0 + frag_col(i);
-    if (m >= e.M || n >= e.N) continue;
+    if (m >= e.M || n >= e.N) {
+      acc[i] = 0.f;
+      continue;
+    }
     if (e.kind == 0) {
       float v = acc[i] + (e.bias ? e.bias[n] : 0.f);
       if (e.act == 1) v = fmaxf(v, 0.f);
-      e.out[(size_t)m * e.ldo + n] = v;
+      if (F32) e.out[(size_t)m * e.ldo + n] = v;
+      acc[i] = v;
     } else if (e.kind == 1) {
       float v = acc[i];
       if (e.r1_vec && n < e.Kv) v = fmaf(e.r1_vec[m], e.r1_row[n], v);
       if (e.mask && !(e.mask[(size_t)m * e.ldmask + n] > 0.f)) v = 0.f;
-      float* d = e.out + (size_t)m * e.ldo + n;
-      *d = e.accumulate ? (*d + v) : v;
-    } else if (n < e.Kv) {
+      if (F32) {
+        float* d = e.out + (size_t)m * e.ldo + n;
+        *d = e.accumulate ? (*d + v) : v;
+      }
+      acc[i] = v;
+    } else if (F32 && n < e.Kv) {
       atomicAdd(e.out + (size_t)m * e.ldo + e.col_off + n, acc[i]);
+    }
+  }
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  if (e.colsum) {               // over the 16 rows of each warp (shuffles), the 8 warps (shared memory), the CTAs (atomics)
+    extern __shared__ __align__(1024) uint8_t smem[];
+    float* red = reinterpret_cast<float*>(smem);      // [8][128], over the drained pipeline stages
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        float s = acc[4 * j + c] + acc[4 * j + 2 + c];
+#pragma unroll
+        for (int o = 4; o < 32; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        if (lane < 4) red[w * TN + 8 * j + 2 * lane + c] = s;
+      }
+    __syncthreads();
+    if (threadIdx.x < TN && n0 + (int)threadIdx.x < e.N) {
+      float s = 0.f;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) s += red[i * TN + threadIdx.x];
+      atomicAdd(e.colsum + n0 + threadIdx.x, s);
+    }
+  }
+  // The fragment of (j, h) is an 8 x 8 block: lane holds its row lane / 4, columns 2 (lane % 4) + {0, 1}.  In an image
+  // that block is one core matrix (sw_off) and the lane's two values are its 32-bit word `lane`: a warp stores 128
+  // contiguous bytes per half.
+  if constexpr (ROWP > 0) {     // image row m, k n: tile (blockIdx.y, n / 32)
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int kt = (n0 >> 5) + (j >> 2);
+      if (kt >= e.row_ks) break;
+      uint16_t* t = e.row + ((size_t)blockIdx.y * e.row_ks + kt) * 2 * TILE_ELEMS;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        uint32_t hi, lo;
+        split2<F16>(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], hi, lo);
+        const int core = (2 * w + h) * (TK / 8) + (j & 3);
+        reinterpret_cast<uint32_t*>(t + core * 64)[lane] = hi;
+        if (ROWP == 3) reinterpret_cast<uint32_t*>(t + TILE_ELEMS + core * 64)[lane] = lo;
+      }
+    }
+  }
+  if constexpr (TRP > 0) {      // image row n, k m: tile (blockIdx.x, m / 32); each block is transposed in registers first
+    const int kt = (m0 >> 5) + (w >> 1);
+    if (kt < e.tr_ks) {
+      uint16_t* t = e.tr + ((size_t)blockIdx.x * e.tr_ks + kt) * 2 * TILE_ELEMS;
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          uint32_t hi, lo;
+          split2<F16>(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], hi, lo);
+          const int core = j * (TK / 8) + 2 * (w & 1) + h;
+          reinterpret_cast<uint32_t*>(t + core * 64)[lane] = movmatrix_trans(hi);
+          if (TRP == 3) reinterpret_cast<uint32_t*>(t + TILE_ELEMS + core * 64)[lane] = movmatrix_trans(lo);
+        }
     }
   }
 }
@@ -316,64 +403,114 @@ static int launch_pack(F f, int rtiles, int ksteps, uint16_t* img, cudaStream_t 
   return SPARF_OK;
 }
 
-// pack A and B, then the pipelined GEMM over grid (B row tiles, A row tiles, slabs of nk_slab k-steps)
-template <bool F16, int PASSES, bool AK, bool BK, class FA, class FB>
-static int run(const TcPrec& p, FA fa, int a_rows, FB fb, int b_rows, int ksteps, int nk_slab, const Epi& e, cudaStream_t st) {
-  const int rta = ceil_div(a_rows, TM), rtb = ceil_div(b_rows, TM);
-  const size_t need = (size_t)std::max(rta, rtb) * ksteps * 2 * TILE_ELEMS;
-  SPARF_REQUIRE(p.pack_a && p.pack_b && need <= p.pack_elems, "tc gemm: operand images need %zu 16-bit elements, have %zu",
-                need, p.pack_elems);
-  int rc = launch_pack<F16, PASSES, AK>(fa, rta, ksteps, p.pack_a, st);
-  if (rc) return rc;
-  rc = launch_pack<F16, PASSES, BK>(fb, rtb, ksteps, p.pack_b, st);
-  if (rc) return rc;
-  SPARF_CHECK_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<F16, PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
-  wg_gemm_kernel<F16, PASSES><<<dim3(rtb, rta, ceil_div(ksteps, nk_slab)), 256, GEMM_SMEM, st>>>(p.pack_a, ksteps, p.pack_b,
-                                                                                               ksteps, ksteps, nk_slab, e);
+template <bool F16, int PASSES, bool F32, int ROWP, int TRP>
+static int launch_gemm(const Opnd& a, int rta, const Opnd& b, int rtb, int ksteps, int nk_slab, const Epi& e, cudaStream_t st) {
+  auto kernel = wg_gemm_kernel<F16, PASSES, F32, ROWP, TRP>;
+  SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
+  kernel<<<dim3(rtb, rta, ceil_div(ksteps, nk_slab)), 256, GEMM_SMEM, st>>>(a, b, ksteps, nk_slab, e);
   SPARF_CHECK_LAUNCH("wg_gemm_kernel");
+  return SPARF_OK;
+}
+
+// pack B into p.pack_b, then the pipelined GEMM over grid (B row tiles, A row tiles, slabs of nk_slab k-steps) with the
+// epilogue outputs e asks for: fp32 (e.out), a row image (row image passes = the GEMM's), a transposed image
+template <bool F16, int PASSES, bool BK, class FB>
+static int run(const TcPrec& p, const Opnd& a, int a_rows, FB fb, int b_rows, int ksteps, int nk_slab, const Epi& e,
+               int row_passes, int tr_passes, cudaStream_t st) {
+  const int rta = ceil_div(a_rows, TM), rtb = ceil_div(b_rows, TM);
+  SPARF_REQUIRE(p.pack_b && (size_t)rtb * ksteps * 2 * TILE_ELEMS <= p.pack_elems,
+                "tc gemm: B operand image needs %zu 16-bit elements, have %zu", (size_t)rtb * ksteps * 2 * TILE_ELEMS,
+                p.pack_elems);
+  int rc = launch_pack<F16, PASSES, BK>(fb, rtb, ksteps, p.pack_b, st);
+  if (rc) return rc;
+  const Opnd b{p.pack_b, nullptr, ksteps, 0};
+  const bool f32 = e.out != nullptr;
+  if (f32 && !row_passes && !tr_passes) return launch_gemm<F16, PASSES, true, 0, 0>(a, rta, b, rtb, ksteps, nk_slab, e, st);
+  if (f32 && row_passes == PASSES && !tr_passes)
+    return launch_gemm<F16, PASSES, true, PASSES, 0>(a, rta, b, rtb, ksteps, nk_slab, e, st);
+  if (!f32 && row_passes == PASSES && tr_passes == 3)
+    return launch_gemm<F16, PASSES, false, PASSES, 3>(a, rta, b, rtb, ksteps, nk_slab, e, st);
+  if (!f32 && row_passes == PASSES && tr_passes == 1)
+    return launch_gemm<F16, PASSES, false, PASSES, 1>(a, rta, b, rtb, ksteps, nk_slab, e, st);
+  SPARF_REQUIRE(false, "tc gemm: no kernel for fp32 output %d, row image %d passes, transposed image %d passes", (int)f32,
+                row_passes, tr_passes);
+}
+
+static Opnd opnd(const TcImage& x, const TcImage& y = TcImage{}) { return Opnd{x.p, y.p, x.ks, y.ks}; }
+
+// the image outputs of an epilogue; they need one slab and no accumulation
+static int set_images(Epi& e, const TcOut& o, int M, int N) {
+  SPARF_REQUIRE(!e.accumulate || (!o.row_passes && !o.tr_passes), "tc gemm: images of an accumulated output");
+  SPARF_REQUIRE(!o.row_passes || (o.row.p && o.row.ks == ceil_div(N, TK)), "tc gemm: row image needs %d k-steps",
+                ceil_div(N, TK));
+  SPARF_REQUIRE(!o.tr_passes || (o.tr.p && o.tr.ks == ceil_div(M, TK)), "tc gemm: transposed image needs %d k-steps",
+                ceil_div(M, TK));
+  e.row = o.row.p; e.row_ks = o.row.ks;
+  e.tr = o.tr.p; e.tr_ks = o.tr.ks;
   return SPARF_OK;
 }
 
 }  // namespace
 
-#define SPARF_WG_RUN(AK, BK, ...)                                              \
-  (p.f16 ? (p.passes == 3 ? run<true, 3, AK, BK>(__VA_ARGS__) : run<true, 1, AK, BK>(__VA_ARGS__))     \
-         : (p.passes == 3 ? run<false, 3, AK, BK>(__VA_ARGS__) : run<false, 1, AK, BK>(__VA_ARGS__)))
+#define SPARF_WG_RUN(BK, ...)                                                                   \
+  (p.f16 ? (p.passes == 3 ? run<true, 3, BK>(__VA_ARGS__) : run<true, 1, BK>(__VA_ARGS__))       \
+         : (p.passes == 3 ? run<false, 3, BK>(__VA_ARGS__) : run<false, 1, BK>(__VA_ARGS__)))
+#define SPARF_WG_PACK(KFAST, ...)                                                                                 \
+  (p.f16 ? (p.passes == 3 ? launch_pack<true, 3, KFAST>(__VA_ARGS__) : launch_pack<true, 1, KFAST>(__VA_ARGS__)) \
+         : (p.passes == 3 ? launch_pack<false, 3, KFAST>(__VA_ARGS__) : launch_pack<false, 1, KFAST>(__VA_ARGS__)))
+
+size_t tc_image_elems(int rows, int cols) { return (size_t)ceil_div(rows, TM) * ceil_div(cols, TK) * 2 * TILE_ELEMS; }
 
 size_t tc_pack_elems(int rows, int ksteps_rows, int cols) {
   // an image of max(rows, cols) rounded to row tiles x ksteps_rows k-steps (callers pass their largest GEMM)
   return (size_t)ceil_div(std::max(rows, cols), TM) * ksteps_rows * 2 * TILE_ELEMS;
 }
 
-int tc_gemm_nt(TcPrec p, int act, int M, int N, const float* X1, int ld1, int K1, int K1v, const float* X2, int ld2, int K2,
-               int K2v, int div2, const float* W, int ldw, int wcol2, const float* bias, float* Y, int ldy, cudaStream_t st) {
-  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && (act == 0 || act == 1), "tc_gemm_nt: passes=%d act=%d", p.passes, act);
-  const int s1 = ceil_div(K1, TK), ks = s1 + (X2 ? ceil_div(K2, TK) : 0);
+int tc_pack_rows(TcPrec p, int M, int K, const float* X, int ldx, int div, TcImage img, cudaStream_t st) {
+  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && img.p && img.ks == ceil_div(K, TK), "tc_pack_rows: passes=%d ks=%d K=%d",
+                p.passes, img.ks, K);
+  return SPARF_WG_PACK(true, Rows{X, ldx, K, div, M}, ceil_div(M, TM), img.ks, img.p, st);
+}
+
+int tc_pack_cols(TcPrec p, int M, int N, const float* X, int ldx, TcImage img, cudaStream_t st) {
+  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && img.p && img.ks == ceil_div(M, TK), "tc_pack_cols: passes=%d ks=%d M=%d",
+                p.passes, img.ks, M);
+  return SPARF_WG_PACK(false, Cols{X, ldx, M, N}, ceil_div(N, TM), img.ks, img.p, st);
+}
+
+int tc_gemm_nt(TcPrec p, int act, int M, int N, TcImage a1, int K1v, TcImage a2, int K2v, const float* W, int ldw, int wcol2,
+               const float* bias, float* Y, int ldy, const TcOut& out, cudaStream_t st) {
+  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && (act == 0 || act == 1) && Y, "tc_gemm_nt: passes=%d act=%d", p.passes, act);
+  const int ks = a1.ks + (a2.p ? a2.ks : 0);
   Epi e{};
   e.kind = 0; e.M = M; e.N = N; e.act = act; e.bias = bias; e.out = Y; e.ldo = ldy;
-  return SPARF_WG_RUN(true, true, p, NtA{X1, X2, ld1, K1, ld2, K2, div2, M, s1}, M, NtB{W, ldw, wcol2, K1v, K2v, N, s1}, N,
-                      ks, ks, e, st);
+  int rc = set_images(e, out, M, N);
+  if (rc) return rc;
+  return SPARF_WG_RUN(true, p, opnd(a1, a2.p ? a2 : TcImage{}), M, NtB{W, ldw, wcol2, K1v, K2v, N, a1.ks}, N, ks, ks, e,
+                      out.row_passes, out.tr_passes, st);
 }
 
-int tc_gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, const float* G, int ldg, const float* W, int ldw, int wcol,
-               const float* mask_src, int ldmask, const float* r1_vec, const float* r1_row, float* D, int ldd, int accumulate,
-               cudaStream_t st) {
-  SPARF_REQUIRE(p.passes == 1 || p.passes == 3, "tc_gemm_nn: passes=%d", p.passes);
-  const int ks = ceil_div(N, TK);
+int tc_gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, TcImage g, const float* W, int ldw, int wcol, const float* mask_src,
+               int ldmask, const float* r1_vec, const float* r1_row, float* D, int ldd, int accumulate, const TcOut& out,
+               float* db, cudaStream_t st) {
+  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && g.ks == ceil_div(N, TK), "tc_gemm_nn: passes=%d ks=%d N=%d", p.passes,
+                g.ks, N);
   Epi e{};
   e.kind = 1; e.M = M; e.N = Kout; e.out = D; e.ldo = ldd; e.Kv = Kv; e.mask = mask_src; e.ldmask = ldmask;
-  e.r1_vec = r1_vec; e.r1_row = r1_row; e.accumulate = accumulate;
-  return SPARF_WG_RUN(true, false, p, NnA{G, ldg, M, N}, M, NnB{W, ldw, wcol, Kv, N}, Kout, ks, ks, e, st);
+  e.r1_vec = r1_vec; e.r1_row = r1_row; e.accumulate = accumulate; e.colsum = db;
+  SPARF_REQUIRE(!db || !accumulate, "tc_gemm_nn: column sums of an accumulated output");
+  int rc = set_images(e, out, M, Kout);
+  if (rc) return rc;
+  return SPARF_WG_RUN(false, p, opnd(g), M, NnB{W, ldw, wcol, Kv, N}, Kout, g.ks, g.ks, e, out.row_passes, out.tr_passes, st);
 }
 
-int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, int rows_per_slab, const float* G, int ldg, const float* X, int ldx,
-               int div, float* dW, int ldw, int wcol, cudaStream_t st) {
-  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && rows_per_slab % TK == 0, "tc_gemm_tn: passes=%d slab=%d", p.passes,
-                rows_per_slab);
-  const int ks = ceil_div(M, TK);
+int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, int rows_per_slab, TcImage gt, const float* X, int ldx, int div,
+               float* dW, int ldw, int wcol, cudaStream_t st) {
+  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && rows_per_slab % TK == 0 && gt.ks == ceil_div(M, TK),
+                "tc_gemm_tn: passes=%d slab=%d ks=%d", p.passes, rows_per_slab, gt.ks);
   Epi e{};
   e.kind = 2; e.M = N; e.N = K; e.out = dW; e.ldo = ldw; e.col_off = wcol; e.Kv = Kv;
-  return SPARF_WG_RUN(false, false, p, TnA{G, ldg, M, N}, N, TnB{X, ldx, div, M, K}, K, ks, rows_per_slab / TK, e, st);
+  return SPARF_WG_RUN(false, p, opnd(gt), N, TnB{X, ldx, div, M, K}, K, gt.ks, rows_per_slab / TK, e, 0, 0, st);
 }
 
 }  // namespace sparf
@@ -381,11 +518,16 @@ int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, int rows_per_slab, const f
 using namespace sparf;
 
 // scratch operand images for the self-tests (diagnostics only: allocated and freed on the stream)
-static int with_images(size_t elems, cudaStream_t st, TcPrec& p) {
+static int alloc_images(size_t elems, cudaStream_t st, TcPrec& p) {
   SPARF_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&p.pack_a), elems * 2, st));
   SPARF_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&p.pack_b), elems * 2, st));
   p.pack_elems = elems;
   return SPARF_OK;
+}
+
+static void free_images(TcPrec& p, cudaStream_t st) {
+  cudaFreeAsync(p.pack_a, st);
+  cudaFreeAsync(p.pack_b, st);
 }
 
 // Exact-integer checks of the operand images, descriptors, the copy ring and the fragment mapping (small integers are
@@ -395,11 +537,12 @@ extern "C" int sparf_tc_selftest(const float* A, const float* B, int32_t K, void
   SPARF_REQUIRE(K % 64 == 0 && K >= 64 && K <= 256, "tc_selftest: K=%d", K);
   cudaStream_t st = (cudaStream_t)stream;
   TcPrec p{false, 1};
-  int rc = with_images(tc_pack_elems(128, K / 32, 128), st, p);
+  int rc = alloc_images(tc_pack_elems(128, K / 32, 128), st, p);
   if (rc) return rc;
-  rc = tc_gemm_nt(p, 0, 128, 128, A, K, K, K, nullptr, 0, 0, 0, 1, B, K, 0, nullptr, D, 128, st);
-  cudaFreeAsync(p.pack_a, st);
-  cudaFreeAsync(p.pack_b, st);
+  const TcImage a{p.pack_a, K / 32};
+  rc = tc_pack_rows(p, 128, K, A, K, 1, a, st);
+  if (!rc) rc = tc_gemm_nt(p, 0, 128, 128, a, K, TcImage{}, 0, B, K, 0, nullptr, D, 128, TcOut{}, st);
+  free_images(p, st);
   return rc;
 }
 
@@ -409,10 +552,45 @@ extern "C" int sparf_tc_selftest_tn(const float* G, const float* X, int32_t rows
   cudaStream_t st = (cudaStream_t)stream;
   SPARF_CHECK_CUDA(cudaMemsetAsync(D, 0, 128 * 128 * sizeof(float), st));
   TcPrec p{false, 1};
-  int rc = with_images(tc_pack_elems(128, rows / 32, 128), st, p);
+  int rc = alloc_images(tc_pack_elems(128, rows / 32, 128), st, p);
   if (rc) return rc;
-  rc = tc_gemm_tn(p, rows, 128, 128, 128, rows, G, 128, X, 128, 1, D, 128, 0, st);
-  cudaFreeAsync(p.pack_a, st);
-  cudaFreeAsync(p.pack_b, st);
+  const TcImage gt{p.pack_a, rows / 32};
+  rc = tc_pack_cols(p, rows, 128, G, 128, gt, st);
+  if (!rc) rc = tc_gemm_tn(p, rows, 128, 128, 128, rows, gt, X, 128, 1, D, 128, 0, st);
+  free_images(p, st);
+  return rc;
+}
+
+// The epilogue images, chained through three 3-pass bf16 GEMMs (exact on small integers):
+//   D = X W1 (X [M,128], W1 [128,96]; the input-gradient GEMM), written only as a row image, a transposed image and its
+//       column sums db[96];
+//   Y = [D | E] W2^T (E [M,40], W2 [128,136]): the row image as the first segment of a two-segment A operand;
+//   Z = D^T X [96,128]: the transposed image as the weight-gradient A operand, over slabs of 64 rows.
+// The image buffers start as NaN, so a k-step past M that is not zero-padded shows in Z.
+extern "C" int sparf_tc_selftest_images(const float* X, const float* W1, const float* E, const float* W2, int32_t M, float* Y,
+                                        float* Z, float* db, sparf_stream_t stream) {
+  SPARF_REQUIRE(M >= 1 && M <= 1024, "tc_selftest_images: M=%d", M);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int N = 128, K = 96, KE = 40;
+  const TcPrec p{false, 3};
+  TcPrec q = p;
+  const TcImage x{nullptr, N / TK}, d{nullptr, K / TK}, e{nullptr, ceil_div(KE, TK)}, dt{nullptr, ceil_div(M, TK)};
+  const size_t nx = tc_image_elems(M, N), nd = tc_image_elems(M, K), ne = tc_image_elems(M, KE), ndt = tc_image_elems(K, M);
+  int rc = alloc_images(nx + nd + ne + ndt + tc_pack_elems(std::max(M, N), ceil_div(K + KE, TK), 0), st, q);
+  if (rc) return rc;
+  TcImage xi = x, di = d, ei = e, dti = dt;
+  xi.p = q.pack_a; di.p = xi.p + nx; ei.p = di.p + nd; dti.p = ei.p + ne;
+  SPARF_CHECK_CUDA(cudaMemsetAsync(q.pack_a, 0xFF, (nx + nd + ne + ndt) * 2, st));
+  SPARF_CHECK_CUDA(cudaMemsetAsync(db, 0, K * sizeof(float), st));
+  SPARF_CHECK_CUDA(cudaMemsetAsync(Z, 0, K * N * sizeof(float), st));
+  TcOut o;
+  o.row = di; o.row_passes = 3;
+  o.tr = dti; o.tr_passes = 3;
+  rc = tc_pack_rows(q, M, N, X, N, 1, xi, st);
+  if (!rc) rc = tc_gemm_nn(q, M, N, K, K, xi, W1, K, 0, nullptr, 0, nullptr, nullptr, nullptr, 0, 0, o, db, st);
+  if (!rc) rc = tc_pack_rows(q, M, KE, E, KE, 1, ei, st);
+  if (!rc) rc = tc_gemm_nt(q, 0, M, 128, di, K, ei, KE, W2, K + KE, K, nullptr, Y, 128, TcOut{}, st);
+  if (!rc) rc = tc_gemm_tn(q, M, K, N, N, 64, dti, X, N, 1, Z, N, 0, st);
+  free_images(q, st);
   return rc;
 }

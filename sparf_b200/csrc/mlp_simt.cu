@@ -242,30 +242,26 @@ __global__ void __launch_bounds__(256) gemm_tn_kernel(int M, int N, int K, int K
   }
 }
 
-// GEMM dispatch: CUDA-core kernels above (passes == 0) or the wgmma kernels of gemm_wgmma.cu
-static int gemm_nt(TcPrec p, int M, int N, const float* X1, int ld1, int K1, int K1v, const float* X2, int ld2, int K2, int K2v,
+// launchers of the CUDA-core GEMMs (the tensor-core engines call gemm_wgmma.cu instead)
+static int gemm_nt(int M, int N, const float* X1, int ld1, int K1, int K1v, const float* X2, int ld2, int K2, int K2v,
                    int div2, const float* W, int ldw, int wcol2, const float* bias, float* Y, int ldy, cudaStream_t st) {
-  if (p.passes) return tc_gemm_nt(p, 1, M, N, X1, ld1, K1, K1v, X2, ld2, K2, K2v, div2, W, ldw, wcol2, bias, Y, ldy, st);
   gemm_nt_kernel<1><<<dim3(ceil_div(N, BN), ceil_div(M, BM)), 256, 0, st>>>(M, N, X1, ld1, K1, K1v, X2, ld2, K2, K2v, div2, W,
                                                                            ldw, wcol2, bias, Y, ldy);
   SPARF_CHECK_LAUNCH("gemm_nt_kernel");
   return SPARF_OK;
 }
 
-static int gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, const float* G, int ldg, const float* W, int ldw, int wcol,
+static int gemm_nn(int M, int N, int Kout, int Kv, const float* G, int ldg, const float* W, int ldw, int wcol,
                    const float* mask_src, int ldmask, const float* r1_vec, const float* r1_row, float* D, int ldd, int accumulate,
                    cudaStream_t st) {
-  if (p.passes)
-    return tc_gemm_nn(p, M, N, Kout, Kv, G, ldg, W, ldw, wcol, mask_src, ldmask, r1_vec, r1_row, D, ldd, accumulate, st);
   gemm_nn_kernel<<<dim3(ceil_div(Kout, BN), ceil_div(M, BM)), 256, 0, st>>>(M, N, Kout, Kv, G, ldg, W, ldw, wcol, mask_src,
                                                                            ldmask, r1_vec, r1_row, D, ldd, accumulate);
   SPARF_CHECK_LAUNCH("gemm_nn_kernel");
   return SPARF_OK;
 }
 
-static int gemm_tn(TcPrec p, int M, int N, int K, int Kv, int rows_per_slab, const float* G, int ldg, const float* X, int ldx,
+static int gemm_tn(int M, int N, int K, int Kv, int rows_per_slab, const float* G, int ldg, const float* X, int ldx,
                    int div, float* dW, int ldw, int wcol, cudaStream_t st) {
-  if (p.passes) return tc_gemm_tn(p, M, N, K, Kv, rows_per_slab, G, ldg, X, ldx, div, dW, ldw, wcol, st);
   gemm_tn_kernel<<<dim3(ceil_div(K, BN), ceil_div(N, BM), ceil_div(M, rows_per_slab)), 256, 0, st>>>(
       M, N, K, Kv, rows_per_slab, G, ldg, X, ldx, div, dW, ldw, wcol);
   SPARF_CHECK_LAUNCH("gemm_tn_kernel");
@@ -533,13 +529,19 @@ struct Carver {
     used += bytes;
     return r;
   }
+  TcImage image(int rows, int cols) {   // operand image of a [rows x cols] matrix
+    return TcImage{reinterpret_cast<uint16_t*>(take((tc_image_elems(rows, cols) + 1) / 2)), ceil_div(cols, 32)};
+  }
 };
 
 // Workspace of one call, per chunk of nrc rays.  mode 0: forward, 1: backward (recomputes the forward), 2: backward from a
-// tape, 3: taped forward (the activations go to the tape).  Tensor-core engines add two operand-image buffers.
+// tape, 3: taped forward (the activations go to the tape).  Tensor-core engines keep their GEMM operands as images: the
+// forward's encodings and ping-pong trunk activations, the backward's ping-pong trunk gradients (a row image for the next
+// input gradient, a transposed one for the weight gradient; no fp32 copy), and two buffers for the operands packed per GEMM.
 struct Ws {
   float *wts, *enc, *denc, *hid, *raw, *rgbv, *G0, *G1, *Genc, *Ghid, *gpre, *graw, *Gdtmp, *Gdenc;
   float* H[SPARF_MAX_TRUNK];
+  TcImage encimg, dencimg, Himg[2], Grow[2], Gtr[2];
   uint16_t *pack_a, *pack_b;
   size_t pack_elems;
 };
@@ -559,15 +561,26 @@ static size_t carve(const SimtDims& d, bool tc, int nrc, int S, int mode, char* 
     for (int l = 0; l < nH; ++l) w.H[l] = cv.take(Mc * d.W);
     for (int l = nH; l < d.nt; ++l) w.H[l] = w.H[l & 1];
   }
-  if (mode == 1 || mode == 2) {
+  if ((mode == 1 || mode == 2) && !tc) {
     w.G0 = cv.take(Mc * d.W);
     w.G1 = cv.take(Mc * d.W);
+  }
+  if (mode == 1 || mode == 2) {
     w.Genc = cv.take(Mc * d.E3p);
     w.Ghid = cv.take(Mc * d.HW);
     w.gpre = cv.take(Mc * 4);
     w.graw = cv.take(Mc);
     w.Gdtmp = cv.take(Mc * d.Evp);
     w.Gdenc = cv.take((size_t)nrc * d.Evp);
+  }
+  if (tc && mode != 2) {
+    w.encimg = cv.image((int)Mc, d.E3p);
+    w.dencimg = cv.image((int)Mc, d.Evp);
+    for (TcImage& h : w.Himg) h = cv.image((int)Mc, d.W);
+  }
+  if (tc && (mode == 1 || mode == 2)) {
+    for (TcImage& g : w.Grow) g = cv.image((int)Mc, d.W);
+    for (TcImage& g : w.Gtr) g = cv.image(d.W, (int)Mc);
   }
   if (tc) {     // largest operand images: [max(Mc, width) x (W + encoding)] forward, [width x Mc] weight gradient
     const int wmax = std::max(std::max(d.W, d.HW), std::max(d.E3p, d.Evp));
@@ -604,10 +617,11 @@ static inline int trunk_ldw(const SimtDims& d, int l) {
 #define LAUNCH_OK(name) SPARF_CHECK_LAUNCH(name)
 
 // forward through the MLP for one chunk.  H: array of nt activation buffers (may alias in pairs when
-// !keep), raw may be NULL.
+// !keep), raw may be NULL.  The tensor-core engines pack the encodings once and chain the trunk layers through the row
+// images their epilogues write (w's image buffers).
 static int simt_chunk_forward(const SparfMLP* mlp, const EnginePrec& ep, const SimtDims& d, int nr, int S, const float* origins,
                               const float* dirs, const float* t, const float* noise, float* wts, float* enc,
-                              float* denc, float** H, float* raw, float* hid, float* sigma, float* rgb,
+                              float* denc, float** H, float* raw, float* hid, float* sigma, float* rgb, const Ws& w,
                               cudaStream_t st) {
   const long long Mc = (long long)nr * S;
   C2F c2f{mlp->use_c2f, mlp->c2f_start, mlp->c2f_range, mlp->progress};
@@ -617,6 +631,11 @@ static int simt_chunk_forward(const SparfMLP* mlp, const EnginePrec& ep, const S
   LAUNCH_OK("encode_xyz_kernel");
   encode_dir_kernel<<<ceil_div((long long)nr * d.Evp, 256), 256, 0, st>>>(nr * d.Evp, mlp->L_view, d.Evp, dirs, wts + 16, denc);
   LAUNCH_OK("encode_dir_kernel");
+  const bool tc = ep.fwd.passes != 0;
+  if (tc) {
+    SPARF_TRY(tc_pack_rows(ep.fwd, (int)Mc, d.E3p, enc, d.E3p, 1, w.encimg, st));
+    SPARF_TRY(tc_pack_rows(ep.fwd, (int)Mc, d.Evp, denc, d.Evp, S, w.dencimg, st));
+  }
   const float* in = enc;
   for (int l = 0; l < d.nt; ++l) {
     const bool last = l == d.nt - 1;
@@ -624,8 +643,16 @@ static int simt_chunk_forward(const SparfMLP* mlp, const EnginePrec& ep, const S
     const float* Wl = mlp->trunk_w[l] + (last ? ldw : 0);  // last layer: row 0 is the density row
     const float* bl = mlp->trunk_b[l] + (last ? 1 : 0);
     const bool sk = l == d.skip;
-    SPARF_TRY(gemm_nt(ep.fwd, (int)Mc, d.W, in, trunk_in_main(d, l), trunk_in_main(d, l), trunk_in_main_valid(d, l),
-                      sk ? enc : nullptr, d.E3p, d.E3p, d.E3, 1, Wl, ldw, d.W, bl, H[l], d.W, st));
+    if (tc) {
+      TcOut o;
+      o.row = w.Himg[l & 1];
+      o.row_passes = ep.fwd.passes;
+      SPARF_TRY(tc_gemm_nt(ep.fwd, 1, (int)Mc, d.W, l == 0 ? w.encimg : w.Himg[(l - 1) & 1], trunk_in_main_valid(d, l),
+                           sk ? w.encimg : TcImage{}, d.E3, Wl, ldw, d.W, bl, H[l], d.W, o, st));
+    } else {
+      SPARF_TRY(gemm_nt((int)Mc, d.W, in, trunk_in_main(d, l), trunk_in_main(d, l), trunk_in_main_valid(d, l),
+                        sk ? enc : nullptr, d.E3p, d.E3p, d.E3, 1, Wl, ldw, d.W, bl, H[l], d.W, st));
+    }
     if (last) {
       rowdot_kernel<0><<<ceil_div(Mc, 8), 256, 0, st>>>(Mc, d.W, in, d.W, mlp->trunk_w[l], ldw, mlp->trunk_b[l], noise, raw, sigma);
       LAUNCH_OK("rowdot_kernel<0>");
@@ -633,8 +660,12 @@ static int simt_chunk_forward(const SparfMLP* mlp, const EnginePrec& ep, const S
     in = H[l];
   }
   {
-    SPARF_TRY(gemm_nt(ep.fwd, (int)Mc, d.HW, H[d.nt - 1], d.W, d.W, d.W, denc, d.Evp, d.Evp, d.Ev, S, mlp->head_w[0],
-                      d.W + d.Ev, d.W, mlp->head_b[0], hid, d.HW, st));
+    if (tc)
+      SPARF_TRY(tc_gemm_nt(ep.fwd, 1, (int)Mc, d.HW, w.Himg[(d.nt - 1) & 1], d.W, w.dencimg, d.Ev, mlp->head_w[0], d.W + d.Ev,
+                           d.W, mlp->head_b[0], hid, d.HW, TcOut{}, st));
+    else
+      SPARF_TRY(gemm_nt((int)Mc, d.HW, H[d.nt - 1], d.W, d.W, d.W, denc, d.Evp, d.Evp, d.Ev, S, mlp->head_w[0], d.W + d.Ev, d.W,
+                        mlp->head_b[0], hid, d.HW, st));
     rowdot_kernel<1><<<ceil_div(Mc, 8), 256, 0, st>>>(Mc, d.HW, hid, d.HW, mlp->head_w[1], d.HW, mlp->head_b[1], nullptr, nullptr, rgb);
     LAUNCH_OK("rowdot_kernel<1>");
   }
@@ -659,7 +690,7 @@ int simt_mlp_forward(const SparfMLP* mlp, int engine, int R, int S, const float*
     int nr = std::min(nrc, R - r0);
     size_t m0 = (size_t)r0 * S;
     rc = simt_chunk_forward(mlp, ep, d, nr, S, origins + (size_t)r0 * 3, dirs + (size_t)r0 * 3, t + m0,
-                            noise ? noise + m0 : nullptr, w.wts, w.enc, w.denc, w.H, nullptr, w.hid, sigma + m0, rgb + m0 * 3, st);
+                            noise ? noise + m0 : nullptr, w.wts, w.enc, w.denc, w.H, nullptr, w.hid, sigma + m0, rgb + m0 * 3, w, st);
     if (rc) return rc;
   }
   return SPARF_OK;
@@ -717,7 +748,7 @@ int simt_mlp_forward_tape(const SparfMLP* mlp, int engine, int R, int S, const f
     for (int l = 0; l < d.nt; ++l) H[l] = tp.H[l] + m0 * d.W;
     rc = simt_chunk_forward(mlp, ep, d, nr, S, origins + (size_t)r0 * 3, dirs + (size_t)r0 * 3, t + m0,
                             noise ? noise + m0 : nullptr, w.wts, tp.enc + m0 * d.E3p, tp.denc + (size_t)r0 * d.Evp, H,
-                            tp.raw + m0, tp.hid + m0 * d.HW, sigma + m0, rgb + m0 * 3, st);
+                            tp.raw + m0, tp.hid + m0 * d.HW, sigma + m0, rgb + m0 * 3, w, st);
     if (rc) return rc;
   }
   return SPARF_OK;
@@ -766,6 +797,7 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
   Ws w;
   carve(d, uses_tc(engine), nrc, S, mode, reinterpret_cast<char*>(workspace), &w);
   const EnginePrec ep = with_images(engine_prec(engine), w);
+  const bool tc = ep.fwd.passes != 0;
   float *wts = w.wts, *enc_w = w.enc, *denc_w = w.denc, *hid_w = w.hid, *raw_w = w.raw, *rgbv_w = w.rgbv;
   float** H_w = w.H;
   Tape tp{};
@@ -792,7 +824,7 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
       for (int l = 0; l < d.nt; ++l) H[l] = tp.H[l] + m0 * d.W;
     } else {
       for (int l = 0; l < d.nt; ++l) H[l] = H_w[l];
-      rc = simt_chunk_forward(mlp, ep, d, nr, S, o_c, d_c, t_c, nz, wts, enc, denc, H, raw, hid, nullptr, rgbv, st);
+      rc = simt_chunk_forward(mlp, ep, d, nr, S, o_c, d_c, t_c, nz, wts, enc, denc, H, raw, hid, nullptr, rgbv, w, st);
       if (rc) return rc;
     }
     const int slab = ep.wgrad.passes ? 512 : 2048;  // rows per wgrad slab (tensor cores: >= 2 waves of CTAs per layer)
@@ -808,13 +840,42 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
     // colour head, layer 0 ([feat | denc] -> HW)
     const int ldw8 = d.W + d.Ev;
     float* feat = H[d.nt - 1];
-    SPARF_TRY(gemm_tn(ep.wgrad, (int)Mc, d.HW, d.W, d.W, slab, Ghid, d.HW, feat, d.W, 1, grad->head_w[0], ldw8, 0, st));
-    SPARF_TRY(gemm_tn(ep.wgrad, (int)Mc, d.HW, d.Evp, d.Ev, slab, Ghid, d.HW, denc, d.Evp, S, grad->head_w[0], ldw8, d.W, st));
+    // tensor cores: the trunk gradients G leave each input-gradient GEMM as images (gout(i) = ping-pong buffer i), with the
+    // bias gradient of the layer that produced them; pack_a holds Ghid's image
+    auto gtr = [&](int i) { return TcImage{w.Gtr[i].p, ceil_div(Mc, 32)}; };   // K = this chunk's rows
+    auto gout = [&](int i) {
+      TcOut o;
+      o.row = w.Grow[i];
+      o.tr = gtr(i);
+      o.row_passes = ep.dgrad.passes;
+      o.tr_passes = ep.wgrad.passes;
+      return o;
+    };
+    const TcImage ghid_t{w.pack_a, ceil_div(Mc, 32)}, ghid{w.pack_a, ceil_div(d.HW, 32)};
+    if (tc) {
+      SPARF_TRY(tc_pack_cols(ep.wgrad, (int)Mc, d.HW, Ghid, d.HW, ghid_t, st));
+      SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.W, d.W, slab, ghid_t, feat, d.W, 1, grad->head_w[0], ldw8, 0, st));
+      SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.Evp, d.Ev, slab, ghid_t, denc, d.Evp, S, grad->head_w[0], ldw8, d.W, st));
+    } else {
+      SPARF_TRY(gemm_tn((int)Mc, d.HW, d.W, d.W, slab, Ghid, d.HW, feat, d.W, 1, grad->head_w[0], ldw8, 0, st));
+      SPARF_TRY(gemm_tn((int)Mc, d.HW, d.Evp, d.Ev, slab, Ghid, d.HW, denc, d.Evp, S, grad->head_w[0], ldw8, d.W, st));
+    }
     colsum_kernel<<<dim3(ceil_div(d.HW, 32), ceil_div(Mc, 1024)), 256, 0, st>>>(Mc, d.HW, 1024, Ghid, d.HW, grad->head_b[0]);
     LAUNCH_OK("colsum_kernel(head)");
-    SPARF_TRY(gemm_nn(ep.dgrad, (int)Mc, d.HW, d.W, d.W, Ghid, d.HW, mlp->head_w[0], ldw8, 0, feat, d.W, nullptr, nullptr, G0, d.W, 0, st));
+    if (tc) {
+      SPARF_TRY(tc_pack_rows(ep.dgrad, (int)Mc, d.HW, Ghid, d.HW, 1, ghid, st));
+      SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.HW, d.W, d.W, ghid, mlp->head_w[0], ldw8, 0, feat, d.W, nullptr, nullptr,
+                           nullptr, 0, 0, gout(0), grad->trunk_b[d.nt - 1] + 1, st));
+    } else {
+      SPARF_TRY(gemm_nn((int)Mc, d.HW, d.W, d.W, Ghid, d.HW, mlp->head_w[0], ldw8, 0, feat, d.W, nullptr, nullptr, G0, d.W, 0, st));
+    }
     if (d_dirs) {
-      SPARF_TRY(gemm_nn(ep.dgrad, (int)Mc, d.HW, d.Evp, d.Ev, Ghid, d.HW, mlp->head_w[0], ldw8, d.W, nullptr, 0, nullptr, nullptr, Gdtmp, d.Evp, 0, st));
+      if (tc)
+        SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.HW, d.Evp, d.Ev, ghid, mlp->head_w[0], ldw8, d.W, nullptr, 0, nullptr, nullptr,
+                             Gdtmp, d.Evp, 0, TcOut{}, nullptr, st));
+      else
+        SPARF_TRY(gemm_nn((int)Mc, d.HW, d.Evp, d.Ev, Ghid, d.HW, mlp->head_w[0], ldw8, d.W, nullptr, 0, nullptr, nullptr, Gdtmp,
+                          d.Evp, 0, st));
       ray_reduce_kernel<<<ceil_div((long long)nr * d.Evp, 256), 256, 0, st>>>(nr, S, d.Evp, Gdtmp, Gdenc);
       LAUNCH_OK("ray_reduce_kernel");
       direnc_bwd_kernel<<<ceil_div(nr, 128), 128, 0, st>>>(nr, mlp->L_view, d.Evp, denc, Gdenc, d_c, d_dirs + (size_t)r0 * 3);
@@ -823,6 +884,7 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
     // trunk, last layer: z = [raw | feat_pre]
     float* G = G0;
     float* Gn = G1;
+    int gi = 0;       // tensor cores: G is image pair gi
     bool genc_written = false;
     for (int l = d.nt - 1; l >= 0; --l) {
       const bool last = l == d.nt - 1;
@@ -832,24 +894,38 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
       const int rowoff = last ? 1 : 0;
       float* dWl = grad->trunk_w[l] + (size_t)rowoff * ldw;
       const float* Wl = mlp->trunk_w[l] + (size_t)rowoff * ldw;
-      SPARF_TRY(gemm_tn(ep.wgrad, (int)Mc, d.W, Kin, Kinv, slab, G, d.W, in, Kin, 1, dWl, ldw, 0, st));
-      if (l == d.skip) SPARF_TRY(gemm_tn(ep.wgrad, (int)Mc, d.W, d.E3p, d.E3, slab, G, d.W, enc, d.E3p, 1, dWl, ldw, d.W, st));
-      colsum_kernel<<<dim3(ceil_div(d.W, 32), ceil_div(Mc, 1024)), 256, 0, st>>>(Mc, d.W, 1024, G, d.W, grad->trunk_b[l] + rowoff);
-      LAUNCH_OK("colsum_kernel(trunk)");
+      if (tc) {
+        SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, Kin, Kinv, slab, gtr(gi), in, Kin, 1, dWl, ldw, 0, st));
+        if (l == d.skip)
+          SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, d.E3p, d.E3, slab, gtr(gi), enc, d.E3p, 1, dWl, ldw, d.W, st));
+      } else {
+        SPARF_TRY(gemm_tn((int)Mc, d.W, Kin, Kinv, slab, G, d.W, in, Kin, 1, dWl, ldw, 0, st));
+        if (l == d.skip) SPARF_TRY(gemm_tn((int)Mc, d.W, d.E3p, d.E3, slab, G, d.W, enc, d.E3p, 1, dWl, ldw, d.W, st));
+        colsum_kernel<<<dim3(ceil_div(d.W, 32), ceil_div(Mc, 1024)), 256, 0, st>>>(Mc, d.W, 1024, G, d.W, grad->trunk_b[l] + rowoff);
+        LAUNCH_OK("colsum_kernel(trunk)");
+      }
       if (last) {
         narrow_wgrad_kernel<1><<<ceil_div(Mc, 512), 128, 0, st>>>(Mc, d.W, 512, graw, 1, in, d.W, grad->trunk_w[l], ldw, grad->trunk_b[l]);
         LAUNCH_OK("narrow_wgrad_kernel<1>");
       }
-      if (l > 0) {
-        SPARF_TRY(gemm_nn(ep.dgrad, (int)Mc, d.W, d.W, d.W, G, d.W, Wl, ldw, 0, in, d.W, last ? graw : nullptr,
+      if (l > 0 && tc) {
+        SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.W, d.W, w.Grow[gi], Wl, ldw, 0, in, d.W, last ? graw : nullptr,
+                             last ? mlp->trunk_w[l] : nullptr, nullptr, 0, 0, gout(gi ^ 1), grad->trunk_b[l - 1], st));
+      } else if (l > 0) {
+        SPARF_TRY(gemm_nn((int)Mc, d.W, d.W, d.W, G, d.W, Wl, ldw, 0, in, d.W, last ? graw : nullptr,
                           last ? mlp->trunk_w[l] : nullptr, Gn, d.W, 0, st));
       }
       if (need_rays && (l == d.skip || l == 0)) {
-        SPARF_TRY(gemm_nn(ep.dgrad, (int)Mc, d.W, d.E3p, d.E3, G, d.W, Wl, ldw, l == 0 ? 0 : d.W, nullptr, 0, nullptr, nullptr, Genc,
-                          d.E3p, genc_written ? 1 : 0, st));
+        if (tc)
+          SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.E3p, d.E3, w.Grow[gi], Wl, ldw, l == 0 ? 0 : d.W, nullptr, 0, nullptr,
+                               nullptr, Genc, d.E3p, genc_written ? 1 : 0, TcOut{}, nullptr, st));
+        else
+          SPARF_TRY(gemm_nn((int)Mc, d.W, d.E3p, d.E3, G, d.W, Wl, ldw, l == 0 ? 0 : d.W, nullptr, 0, nullptr, nullptr, Genc,
+                            d.E3p, genc_written ? 1 : 0, st));
         genc_written = true;
       }
       float* tmp = G; G = Gn; Gn = tmp;
+      gi ^= 1;
     }
     if (need_rays) {
       posenc_bwd_kernel<<<ceil_div(nr, 4), 128, 0, st>>>(nr, S, mlp->L_xyz, d.E3p, enc, Genc, t_c,
