@@ -230,6 +230,10 @@ int sparf_tc_selftest_tn(const float* G, const float* X, int32_t rows, float* D,
  * Z[96,128] = D^T X reads the transposed image.  Exact on small integers. */
 int sparf_tc_selftest_images(const float* X, const float* W1, const float* E, const float* W2, int32_t M, float* Y, float* Z,
                              float* db, sparf_stream_t stream);
+/* The same chain with every GEMM grid capped at max_ctas CTAs (max_ctas <= 0: one per SM, as the engines run), so each
+ * CTA of the persistent GEMM kernel walks several work units and its copy ring wraps across them. */
+int sparf_tc_selftest_persistent(const float* X, const float* W1, const float* E, const float* W2, int32_t M, float* Y,
+                                 float* Z, float* db, int32_t max_ctas, sparf_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -6,10 +6,11 @@
 // adjacent (16 KB).
 //   pack: splits an fp32 operand (with the GEMM's own indexing: transposes, per-ray rows, bounds) into an image; the
 //     weights, the encodings and the colour-head gradient take this path;
-//   gemm: one CTA = two warpgroups = one 128 x 128 output tile; one thread streams the tiles of both operands with
-//     cp.async.bulk into a STAGES-deep ring of shared-memory stages, each completing on its own mbarrier (complete_tx);
-//     both warpgroups wait on the stage's barrier and issue wgmma.m64n128k16 (register accumulators); one MMA group stays
-//     in flight while the stage consumed before it is refilled, so STAGES - 1 tile copies overlap the MMAs.  The
+//   gemm: persistent, one CTA per SM walking 128 x 128 output tiles (the weight gradient: tiles x k-ranges).  A
+//     producer thread streams the tiles of both operands with cp.async.bulk into a STAGES-deep ring of shared-memory
+//     stages that runs on across tiles, each stage completing on its "full" mbarrier (complete_tx); two consumer
+//     warpgroups wait on it, issue wgmma.m64n128k16 (register accumulators) and hand the stage back on its "empty"
+//     mbarrier once the MMAs that read it have retired.  So the next tile's first stages load during an epilogue.  The
 //     epilogue can write the output's own images (row and transposed) for the next GEMMs, so trunk activations and
 //     gradients are never packed from fp32.
 #include <cuda_bf16.h>
@@ -93,9 +94,12 @@ __device__ __forceinline__ void split16(float x, uint16_t& hi, uint16_t& lo) {
 }
 
 constexpr int TILE_BYTES = TILE_ELEMS * 2;        // one 16-bit half of a tile
-constexpr int STAGES = 4;
+constexpr int STAGES = 6;
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;       // A hi, A lo, B hi, B lo
-constexpr int GEMM_SMEM = STAGES * STAGE_BYTES + STAGES * 8;
+constexpr int CONSUMERS = 256;                    // two MMA warpgroups (warps 0-7)
+constexpr int GEMM_THREADS = CONSUMERS + 128;     // + the producer warpgroup (one thread issues the copies)
+constexpr int RED_BYTES = 8 * TN * 4;             // column-sum reduction, [8 warps][128 columns] fp32
+constexpr int GEMM_SMEM = STAGES * STAGE_BYTES + RED_BYTES + 2 * STAGES * 8;
 
 // element i of this thread's share of a [128 x 32] tile: KFAST = consecutive threads along K (operand contiguous in K
 // in global memory), else consecutive threads along the 128 rows
@@ -188,6 +192,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* b, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* b, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(smem_u32(b)), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* b) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(b)) : "memory");
+}
 __device__ __forceinline__ void mbar_wait(uint64_t* b, uint32_t parity) {
   asm volatile("{\n.reg .pred P;\nSPARF_WAIT_%=:\n"
                "mbarrier.try_wait.parity.shared::cta.b64 P, [%0], %1;\n"
@@ -209,38 +216,74 @@ struct Opnd {
   }
 };
 
-// acc[64] of this thread = its fragment of the warpgroup's [64 x 128] block: acc[4 j + 2 h + c] is
-// row 16 warp + lane/4 + 8 h, column 8 j + 2 (lane % 4) + c.  Operands: A row tile blockIdx.y, B row tile blockIdx.x,
-// k-steps [kt0, kt0 + nk).
-template <bool F16, int PASSES>
-__device__ __forceinline__ void wg_pipeline(float (&acc)[64], const Opnd& a, const Opnd& b, int kt0, int nk) {
+struct Epi {
+  int kind;                 // 0: Y = act(acc + bias) ; 1: D (=|+=) mask * (acc + r1_vec r1_row) ; 2: dW += acc (atomic)
+  int M, N, act;            // output rows / columns
+  const float* bias;
+  float* out;
+  int ldo, col_off, Kv;
+  const float *mask, *r1_vec, *r1_row;
+  int ldmask, accumulate;
+  float* colsum;            // kind 1: += column sums of the output
+  uint16_t *row, *tr;       // output images, row_ks / tr_ks k-steps per row tile
+  int row_ks, tr_ks;
+  int pairs;                // N even, out and mask 8-byte aligned with even leading dimensions (kinds 0 and 1)
+};
+
+// The work units of a persistent GEMM: unit u = output tile u % tiles (B row tile t % rtb, A row tile t / rtb: the B
+// tiles of one A row tile are consecutive units, so they read that A row tile from L2 at about the same time) over
+// k-range u / tiles of nsplit, the ranges as even as possible.  CTA c takes units c, c + gridDim.x, ...
+struct Units {
+  int rtb, tiles, nsplit, nk;
+  __device__ void get(int u, int& bx, int& by, int& kt0, int& nku) const {
+    const int t = u % tiles, s = u / tiles;
+    bx = t % rtb;
+    by = t / rtb;
+    kt0 = s * nk / nsplit;
+    nku = (s + 1) * nk / nsplit - kt0;
+  }
+};
+
+// The producer (one thread): the A and B tiles of every k-step of the CTA's units, in order, into a ring of STAGES
+// stages that runs on across units.  Stage s is refilled once the consumers' 8 warps have arrived on empty[s] (the
+// first pass finds every stage free), and completes on full[s] with the copies' bytes.
+template <int PASSES>
+__device__ __forceinline__ void produce(const Opnd& a, const Opnd& b, const Units& w, uint64_t* full, uint64_t* empty) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-  const int tid = threadIdx.x, wg = tid >> 7;
+  const uint32_t bytes = PASSES == 3 ? 2 * TILE_BYTES : TILE_BYTES;
+  int it = 0;
+  for (int u = blockIdx.x; u < w.tiles * w.nsplit; u += gridDim.x) {
+    int bx, by, kt0, nk;
+    w.get(u, bx, by, kt0, nk);
+    for (int j = 0; j < nk; ++j, ++it) {
+      const int s = it % STAGES;
+      mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+      uint8_t* st = smem + s * STAGE_BYTES;
+      mbar_expect_tx(&full[s], 2 * bytes);
+      bulk_g2s(st, a.tile(by, kt0 + j), bytes, &full[s]);
+      bulk_g2s(st + 2 * TILE_BYTES, b.tile(bx, kt0 + j), bytes, &full[s]);
+    }
+  }
+}
+
+// The MMAs of one unit of nk k-steps, ring position it on entry (advanced by nk).  acc[64] of this thread = its
+// fragment of the warpgroup's [64 x 128] block: acc[4 j + 2 h + c] is row 16 warp + lane/4 + 8 h, column
+// 8 j + 2 (lane % 4) + c.  One MMA group stays in flight: each warp releases a stage once the group that read it has
+// retired.
+template <bool F16, int PASSES>
+__device__ __forceinline__ void mma_unit(float (&acc)[64], int nk, int& it, uint64_t* full, uint64_t* empty) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   float acc_lo[PASSES == 3 ? 64 : 1];
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
 #pragma unroll
   for (int i = 0; i < (PASSES == 3 ? 64 : 1); ++i) acc_lo[i] = 0.f;
-  if (tid == 0) {
-    for (int i = 0; i < STAGES; ++i) mbar_init(&full[i], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-  }
-  __syncthreads();
   if (nk <= 0) return;
-  const uint32_t bytes = PASSES == 3 ? 2 * TILE_BYTES : TILE_BYTES;
-  auto issue = [&](int j) {       // k-step j of this CTA -> stage j % STAGES
-    uint8_t* st = smem + (j % STAGES) * STAGE_BYTES;
-    uint64_t* bar = &full[j % STAGES];
-    mbar_expect_tx(bar, 2 * bytes);
-    bulk_g2s(st, a.tile(blockIdx.y, kt0 + j), bytes, bar);
-    bulk_g2s(st + 2 * TILE_BYTES, b.tile(blockIdx.x, kt0 + j), bytes, bar);
-  };
-  if (tid == 0)
-    for (int j = 0; j < STAGES - 1 && j < nk; ++j) issue(j);
-  for (int j = 0; j < nk; ++j) {
-    mbar_wait(&full[j % STAGES], (j / STAGES) & 1);
-    const uint8_t* st = smem + (j % STAGES) * STAGE_BYTES;
+  for (int j = 0; j < nk; ++j, ++it) {
+    const int s = it % STAGES;
+    mbar_wait(&full[s], (it / STAGES) & 1);
+    const uint8_t* st = smem + s * STAGE_BYTES;
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < TK / 16; ++ks) {
@@ -254,11 +297,11 @@ __device__ __forceinline__ void wg_pipeline(float (&acc)[64], const Opnd& a, con
       wgmma_m64n128k16<F16>(acc, ahi, bhi);
     }
     wgmma_commit();
-    wgmma_wait_1();               // the MMAs of k-step j - 1 are done (this warpgroup) ...
-    __syncthreads();              // ... in both warpgroups: its stage is free
-    if (tid == 0 && j + STAGES - 1 < nk) issue(j + STAGES - 1);
+    wgmma_wait_1();               // the MMAs of the previous k-step are done: its stage is free
+    if (j > 0 && lane == 0) mbar_arrive(&empty[(it + STAGES - 1) % STAGES]);
   }
   wgmma_wait_all();
+  if (lane == 0) mbar_arrive(&empty[(it + STAGES - 1) % STAGES]);
   if constexpr (PASSES == 3) {
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] += ldexpf(acc_lo[i], -LO_SHIFT);
@@ -288,60 +331,105 @@ __device__ __forceinline__ uint32_t movmatrix_trans(uint32_t x) {
   return y;
 }
 
-struct Epi {
-  int kind;                 // 0: Y = act(acc + bias) ; 1: D (=|+=) mask * (acc + r1_vec r1_row) ; 2: dW += acc (atomic)
-  int M, N, act;            // output rows / columns
-  const float* bias;
-  float* out;
-  int ldo, col_off, Kv;
-  const float *mask, *r1_vec, *r1_row;
-  int ldmask, accumulate;
-  float* colsum;            // kind 1: += column sums of the output
-  uint16_t *row, *tr;       // output images, row_ks / tr_ks k-steps per row tile
-  int row_ks, tr_ks;
-};
 
-// One CTA = one 128 x 128 output tile.  The epilogue writes, each only when its template flag is set: the fp32 output
-// (F32), a row image of the output (rows = output rows, K = output columns) and a transposed image (rows = output
-// columns, K = output rows), with ROWP / TRP passes (3: hi and lo halves, 1: hi only) in the GEMM's 16-bit type.  An
-// image holds the split of the very fp32 value the output gets, zero past M and N, so it is bit-identical to what
-// pack_kernel would make of the fp32 output.  Images and column sums take one slab (gridDim.z == 1) and no accumulate.
-template <bool F16, int PASSES, bool F32, int ROWP, int TRP>
-__global__ void __launch_bounds__(256) wg_gemm_kernel(Opnd a, Opnd b, int nk_total, int nk_slab, Epi e) {
-  const int kt0 = blockIdx.z * nk_slab;
-  float acc[64];
-  wg_pipeline<F16, PASSES>(acc, a, b, kt0, min(nk_slab, nk_total - kt0));
-  const int m0 = blockIdx.y * TM, n0 = blockIdx.x * TN;
+static bool pair_aligned(const float* p, int ld) { return !p || (!(reinterpret_cast<uintptr_t>(p) & 7) && ld % 2 == 0); }
+
+// columns n, n + 1 of one row (n even; two: column n + 1 exists): one 8-byte access when every such pair of the
+// matrix is 8-byte aligned and complete (PAIRS).  The choice is made once per tile, not per pair: a branch per access
+// would keep the compiler from issuing the tile's loads together.
+template <bool PAIRS>
+__device__ __forceinline__ float2 ld2(const float* p, bool two) {
+  if (PAIRS) return *reinterpret_cast<const float2*>(p);
+  return make_float2(p[0], two ? p[1] : 0.f);
+}
+template <bool PAIRS>
+__device__ __forceinline__ void st2(float* p, float x, float y, bool two) {
+  if (PAIRS) {
+    *reinterpret_cast<float2*>(p) = make_float2(x, y);
+  } else {
+    p[0] = x;
+    if (two) p[1] = y;
+  }
+}
+
+// the consumer warpgroups only (the producer warpgroup never joins)
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;\n" ::"n"(CONSUMERS) : "memory"); }
+
+// The epilogue of output tile (B row tile bx, A row tile by).  It writes, each only when its template flag is set: the
+// fp32 output (F32), a row image of the output (rows = output rows, K = output columns) and a transposed image (rows =
+// output columns, K = output rows), with ROWP / TRP passes (3: hi and lo halves, 1: hi only) in the GEMM's 16-bit type.
+// An image holds the split of the very fp32 value the output gets, zero past M and N, so it is bit-identical to what
+// pack_kernel would make of the fp32 output.  Images and column sums take the full k-range and no accumulate.
+// the fp32 values of the tile (kinds of Epi), stored when F32; acc = the values the images take, 0 past M and N
+template <bool F32, bool PAIRS>
+__device__ __forceinline__ void epilogue_values(float (&acc)[64], int m0, int n0, const Epi e) {
+  // The mask loads come first, in a loop of their own, and leave one bit per value (acc[i] is kept iff bit i of keep).
+  // Issued pair by pair inside the loop below, behind its branches, each would wait out its own memory latency (a mask
+  // tile is 64 KB from HBM).
+  uint64_t keep = ~0ull;
+  if (e.kind == 1 && e.mask) {
 #pragma unroll
-  for (int i = 0; i < 64; ++i) {
-    const int m = m0 + frag_row(i), n = n0 + frag_col(i);
-    if (m >= e.M || n >= e.N) {
-      acc[i] = 0.f;
-      continue;
-    }
-    if (e.kind == 0) {
-      float v = acc[i] + (e.bias ? e.bias[n] : 0.f);
-      if (e.act == 1) v = fmaxf(v, 0.f);
-      if (F32) e.out[(size_t)m * e.ldo + n] = v;
-      acc[i] = v;
-    } else if (e.kind == 1) {
-      float v = acc[i];
-      if (e.r1_vec && n < e.Kv) v = fmaf(e.r1_vec[m], e.r1_row[n], v);
-      if (e.mask && !(e.mask[(size_t)m * e.ldmask + n] > 0.f)) v = 0.f;
-      if (F32) {
-        float* d = e.out + (size_t)m * e.ldo + n;
-        *d = e.accumulate ? (*d + v) : v;
-      }
-      acc[i] = v;
-    } else if (F32 && n < e.Kv) {
-      atomicAdd(e.out + (size_t)m * e.ldo + e.col_off + n, acc[i]);
+    for (int i = 0; i < 64; i += 2) {
+      const int m = m0 + frag_row(i), n = n0 + frag_col(i);
+      const float2 mk = m < e.M && n < e.N ? ld2<PAIRS>(e.mask + (size_t)m * e.ldmask + n, n + 1 < e.N) : make_float2(0.f, 0.f);
+      keep &= ~((uint64_t)!(mk.x > 0.f) << i | (uint64_t)!(mk.y > 0.f) << (i + 1));
     }
   }
+#pragma unroll
+  for (int i = 0; i < 64; i += 2) {     // the pair acc[i], acc[i + 1]: columns n, n + 1 of row m
+    const int m = m0 + frag_row(i), n = n0 + frag_col(i);
+    if (m >= e.M || n >= e.N) {
+      acc[i] = acc[i + 1] = 0.f;
+      continue;
+    }
+    const bool two = n + 1 < e.N;
+    if (e.kind == 0) {
+      // two 4-byte loads: the last trunk layer's bias starts one float into its buffer (after the density row's)
+      const float2 bv = e.bias ? make_float2(e.bias[n], two ? e.bias[n + 1] : 0.f) : make_float2(0.f, 0.f);
+      float v0 = acc[i] + bv.x, v1 = acc[i + 1] + bv.y;
+      if (e.act == 1) {
+        v0 = fmaxf(v0, 0.f);
+        v1 = fmaxf(v1, 0.f);
+      }
+      if (F32) st2<PAIRS>(e.out + (size_t)m * e.ldo + n, v0, v1, two);
+      acc[i] = v0;
+      acc[i + 1] = v1;
+    } else if (e.kind == 1) {
+      float v0 = acc[i], v1 = acc[i + 1];
+      if (e.r1_vec && n < e.Kv) v0 = fmaf(e.r1_vec[m], e.r1_row[n], v0);
+      if (e.r1_vec && two && n + 1 < e.Kv) v1 = fmaf(e.r1_vec[m], e.r1_row[n + 1], v1);
+      if (!(keep >> i & 1)) v0 = 0.f;
+      if (!(keep >> (i + 1) & 1)) v1 = 0.f;
+      if (F32) {
+        float* d = e.out + (size_t)m * e.ldo + n;
+        if (e.accumulate) {
+          const float2 o = ld2<PAIRS>(d, two);
+          st2<PAIRS>(d, o.x + v0, o.y + v1, two);
+        } else {
+          st2<PAIRS>(d, v0, v1, two);
+        }
+      }
+      acc[i] = v0;
+      acc[i + 1] = v1;
+    } else if (F32) {
+      float* d = e.out + (size_t)m * e.ldo + e.col_off + n;
+      if (n < e.Kv) atomicAdd(d, acc[i]);
+      if (two && n + 1 < e.Kv) atomicAdd(d + 1, acc[i + 1]);
+    }
+    if (!two) acc[i + 1] = 0.f;
+  }
+}
+
+template <bool F16, bool F32, int ROWP, int TRP>
+__device__ __forceinline__ void epilogue(float (&acc)[64], int bx, int by, const Epi e) {
+  const int m0 = by * TM, n0 = bx * TN;
+  if (e.pairs) epilogue_values<F32, true>(acc, m0, n0, e);
+  else epilogue_values<F32, false>(acc, m0, n0, e);
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   if (e.colsum) {               // over the 16 rows of each warp (shuffles), the 8 warps (shared memory), the CTAs (atomics)
     extern __shared__ __align__(1024) uint8_t smem[];
-    float* red = reinterpret_cast<float*>(smem);      // [8][128], over the drained pipeline stages
-    __syncthreads();
+    float* red = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [8][128]
+    consumer_sync();            // the previous unit's sums have been read
 #pragma unroll
     for (int j = 0; j < 16; ++j)
 #pragma unroll
@@ -351,7 +439,7 @@ __global__ void __launch_bounds__(256) wg_gemm_kernel(Opnd a, Opnd b, int nk_tot
         for (int o = 4; o < 32; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
         if (lane < 4) red[w * TN + 8 * j + 2 * lane + c] = s;
       }
-    __syncthreads();
+    consumer_sync();
     if (threadIdx.x < TN && n0 + (int)threadIdx.x < e.N) {
       float s = 0.f;
 #pragma unroll
@@ -362,12 +450,12 @@ __global__ void __launch_bounds__(256) wg_gemm_kernel(Opnd a, Opnd b, int nk_tot
   // The fragment of (j, h) is an 8 x 8 block: lane holds its row lane / 4, columns 2 (lane % 4) + {0, 1}.  In an image
   // that block is one core matrix (sw_off) and the lane's two values are its 32-bit word `lane`: a warp stores 128
   // contiguous bytes per half.
-  if constexpr (ROWP > 0) {     // image row m, k n: tile (blockIdx.y, n / 32)
+  if constexpr (ROWP > 0) {     // image row m, k n: tile (by, n / 32)
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       const int kt = (n0 >> 5) + (j >> 2);
       if (kt >= e.row_ks) break;
-      uint16_t* t = e.row + ((size_t)blockIdx.y * e.row_ks + kt) * 2 * TILE_ELEMS;
+      uint16_t* t = e.row + ((size_t)by * e.row_ks + kt) * 2 * TILE_ELEMS;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         uint32_t hi, lo;
@@ -378,10 +466,10 @@ __global__ void __launch_bounds__(256) wg_gemm_kernel(Opnd a, Opnd b, int nk_tot
       }
     }
   }
-  if constexpr (TRP > 0) {      // image row n, k m: tile (blockIdx.x, m / 32); each block is transposed in registers first
+  if constexpr (TRP > 0) {      // image row n, k m: tile (bx, m / 32); each block is transposed in registers first
     const int kt = (m0 >> 5) + (w >> 1);
     if (kt < e.tr_ks) {
-      uint16_t* t = e.tr + ((size_t)blockIdx.x * e.tr_ks + kt) * 2 * TILE_ELEMS;
+      uint16_t* t = e.tr + ((size_t)bx * e.tr_ks + kt) * 2 * TILE_ELEMS;
 #pragma unroll
       for (int j = 0; j < 16; ++j)
 #pragma unroll
@@ -396,6 +484,40 @@ __global__ void __launch_bounds__(256) wg_gemm_kernel(Opnd a, Opnd b, int nk_tot
   }
 }
 
+// Persistent, warp-specialized GEMM: each CTA walks its units (Units); thread 256 streams their tiles into the ring while
+// warps 0-7 (two warpgroups, 64 output rows each) run the MMAs and epilogue of one unit after another, so the next
+// unit's first stages load during an epilogue.  Registers are handed out per warpgroup: the producer warpgroup gives
+// its share back (setmaxnreg), so that the consumers get 232 each (128 x 40 + 256 x 232 <= 64 K) and the epilogue,
+// with its loads issued together, does not spill.
+template <bool F16, int PASSES, bool F32, int ROWP, int TRP>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) wg_gemm_kernel(Opnd a, Opnd b, Units w, Epi e) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + RED_BYTES);
+  uint64_t* empty = full + STAGES;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], CONSUMERS / 32);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+  }
+  __syncthreads();
+  if (threadIdx.x >= CONSUMERS) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (threadIdx.x == CONSUMERS) produce<PASSES>(a, b, w, full, empty);
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  int it = 0;
+  for (int u = blockIdx.x; u < w.tiles * w.nsplit; u += gridDim.x) {
+    int bx, by, kt0, nk;
+    w.get(u, bx, by, kt0, nk);
+    float acc[64];
+    mma_unit<F16, PASSES>(acc, nk, it, full, empty);
+    epilogue<F16, F32, ROWP, TRP>(acc, bx, by, e);
+  }
+}
+
 template <bool F16, int PASSES, bool KFAST, class F>
 static int launch_pack(F f, int rtiles, int ksteps, uint16_t* img, cudaStream_t st) {
   pack_kernel<F16, PASSES, KFAST, F><<<dim3(ksteps, rtiles), 256, 0, st>>>(f, ksteps, img);
@@ -404,18 +526,31 @@ static int launch_pack(F f, int rtiles, int ksteps, uint16_t* img, cudaStream_t 
 }
 
 template <bool F16, int PASSES, bool F32, int ROWP, int TRP>
-static int launch_gemm(const Opnd& a, int rta, const Opnd& b, int rtb, int ksteps, int nk_slab, const Epi& e, cudaStream_t st) {
+static int launch_gemm(const Opnd& a, const Opnd& b, const Units& w, int ctas, const Epi& e, cudaStream_t st) {
   auto kernel = wg_gemm_kernel<F16, PASSES, F32, ROWP, TRP>;
   SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
-  kernel<<<dim3(rtb, rta, ceil_div(ksteps, nk_slab)), 256, GEMM_SMEM, st>>>(a, b, ksteps, nk_slab, e);
+  kernel<<<std::min(w.tiles * w.nsplit, ctas), GEMM_THREADS, GEMM_SMEM, st>>>(a, b, w, e);
   SPARF_CHECK_LAUNCH("wg_gemm_kernel");
   return SPARF_OK;
 }
 
-// pack B into p.pack_b, then the pipelined GEMM over grid (B row tiles, A row tiles, slabs of nk_slab k-steps) with the
-// epilogue outputs e asks for: fp32 (e.out), a row image (row image passes = the GEMM's), a transposed image
+// SMs of the current device, queried once (one CTA of the GEMM kernel fills an SM)
+static int sm_count() {
+  static const int n = [] {
+    int dev = 0, v = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+    return std::max(v, 1);
+  }();
+  return n;
+}
+
+// pack B into p.pack_b, then the persistent GEMM over (B row tiles x A row tiles) output tiles with the epilogue
+// outputs e asks for: fp32 (e.out), a row image (row image passes = the GEMM's), a transposed image.  split_k: each
+// output tile's k-steps are shared out in ceil(CTAs / output tiles) ranges (atomic epilogues only), so every CTA does
+// one long reduction.
 template <bool F16, int PASSES, bool BK, class FB>
-static int run(const TcPrec& p, const Opnd& a, int a_rows, FB fb, int b_rows, int ksteps, int nk_slab, const Epi& e,
+static int run(const TcPrec& p, const Opnd& a, int a_rows, FB fb, int b_rows, int ksteps, bool split_k, const Epi& e,
                int row_passes, int tr_passes, cudaStream_t st) {
   const int rta = ceil_div(a_rows, TM), rtb = ceil_div(b_rows, TM);
   SPARF_REQUIRE(p.pack_b && (size_t)rtb * ksteps * 2 * TILE_ELEMS <= p.pack_elems,
@@ -424,21 +559,21 @@ static int run(const TcPrec& p, const Opnd& a, int a_rows, FB fb, int b_rows, in
   int rc = launch_pack<F16, PASSES, BK>(fb, rtb, ksteps, p.pack_b, st);
   if (rc) return rc;
   const Opnd b{p.pack_b, nullptr, ksteps, 0};
+  const int ctas = p.max_ctas > 0 ? std::min(p.max_ctas, sm_count()) : sm_count();
+  Units w{rtb, rta * rtb, 1, ksteps};
+  if (split_k) w.nsplit = std::max(1, std::min(ksteps, ceil_div(ctas, w.tiles)));
   const bool f32 = e.out != nullptr;
-  if (f32 && !row_passes && !tr_passes) return launch_gemm<F16, PASSES, true, 0, 0>(a, rta, b, rtb, ksteps, nk_slab, e, st);
-  if (f32 && row_passes == PASSES && !tr_passes)
-    return launch_gemm<F16, PASSES, true, PASSES, 0>(a, rta, b, rtb, ksteps, nk_slab, e, st);
-  if (!f32 && row_passes == PASSES && tr_passes == 3)
-    return launch_gemm<F16, PASSES, false, PASSES, 3>(a, rta, b, rtb, ksteps, nk_slab, e, st);
-  if (!f32 && row_passes == PASSES && tr_passes == 1)
-    return launch_gemm<F16, PASSES, false, PASSES, 1>(a, rta, b, rtb, ksteps, nk_slab, e, st);
+  if (f32 && !row_passes && !tr_passes) return launch_gemm<F16, PASSES, true, 0, 0>(a, b, w, ctas, e, st);
+  if (f32 && row_passes == PASSES && !tr_passes) return launch_gemm<F16, PASSES, true, PASSES, 0>(a, b, w, ctas, e, st);
+  if (!f32 && row_passes == PASSES && tr_passes == 3) return launch_gemm<F16, PASSES, false, PASSES, 3>(a, b, w, ctas, e, st);
+  if (!f32 && row_passes == PASSES && tr_passes == 1) return launch_gemm<F16, PASSES, false, PASSES, 1>(a, b, w, ctas, e, st);
   SPARF_REQUIRE(false, "tc gemm: no kernel for fp32 output %d, row image %d passes, transposed image %d passes", (int)f32,
                 row_passes, tr_passes);
 }
 
 static Opnd opnd(const TcImage& x, const TcImage& y = TcImage{}) { return Opnd{x.p, y.p, x.ks, y.ks}; }
 
-// the image outputs of an epilogue; they need one slab and no accumulation
+// the image outputs of an epilogue; they need the full k-range and no accumulation
 static int set_images(Epi& e, const TcOut& o, int M, int N) {
   SPARF_REQUIRE(!e.accumulate || (!o.row_passes && !o.tr_passes), "tc gemm: images of an accumulated output");
   SPARF_REQUIRE(!o.row_passes || (o.row.p && o.row.ks == ceil_div(N, TK)), "tc gemm: row image needs %d k-steps",
@@ -484,9 +619,10 @@ int tc_gemm_nt(TcPrec p, int act, int M, int N, TcImage a1, int K1v, TcImage a2,
   const int ks = a1.ks + (a2.p ? a2.ks : 0);
   Epi e{};
   e.kind = 0; e.M = M; e.N = N; e.act = act; e.bias = bias; e.out = Y; e.ldo = ldy;
+  e.pairs = N % 2 == 0 && pair_aligned(Y, ldy);
   int rc = set_images(e, out, M, N);
   if (rc) return rc;
-  return SPARF_WG_RUN(true, p, opnd(a1, a2.p ? a2 : TcImage{}), M, NtB{W, ldw, wcol2, K1v, K2v, N, a1.ks}, N, ks, ks, e,
+  return SPARF_WG_RUN(true, p, opnd(a1, a2.p ? a2 : TcImage{}), M, NtB{W, ldw, wcol2, K1v, K2v, N, a1.ks}, N, ks, false, e,
                       out.row_passes, out.tr_passes, st);
 }
 
@@ -498,19 +634,19 @@ int tc_gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, TcImage g, const float*
   Epi e{};
   e.kind = 1; e.M = M; e.N = Kout; e.out = D; e.ldo = ldd; e.Kv = Kv; e.mask = mask_src; e.ldmask = ldmask;
   e.r1_vec = r1_vec; e.r1_row = r1_row; e.accumulate = accumulate; e.colsum = db;
+  e.pairs = Kout % 2 == 0 && pair_aligned(D, ldd) && pair_aligned(mask_src, ldmask);
   SPARF_REQUIRE(!db || !accumulate, "tc_gemm_nn: column sums of an accumulated output");
   int rc = set_images(e, out, M, Kout);
   if (rc) return rc;
-  return SPARF_WG_RUN(false, p, opnd(g), M, NnB{W, ldw, wcol, Kv, N}, Kout, g.ks, g.ks, e, out.row_passes, out.tr_passes, st);
+  return SPARF_WG_RUN(false, p, opnd(g), M, NnB{W, ldw, wcol, Kv, N}, Kout, g.ks, false, e, out.row_passes, out.tr_passes, st);
 }
 
-int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, int rows_per_slab, TcImage gt, const float* X, int ldx, int div,
-               float* dW, int ldw, int wcol, cudaStream_t st) {
-  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && rows_per_slab % TK == 0 && gt.ks == ceil_div(M, TK),
-                "tc_gemm_tn: passes=%d slab=%d ks=%d", p.passes, rows_per_slab, gt.ks);
+int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, TcImage gt, const float* X, int ldx, int div, float* dW, int ldw,
+               int wcol, cudaStream_t st) {
+  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && gt.ks == ceil_div(M, TK), "tc_gemm_tn: passes=%d ks=%d", p.passes, gt.ks);
   Epi e{};
   e.kind = 2; e.M = N; e.N = K; e.out = dW; e.ldo = ldw; e.col_off = wcol; e.Kv = Kv;
-  return SPARF_WG_RUN(false, p, opnd(gt), N, TnB{X, ldx, div, M, K}, K, gt.ks, rows_per_slab / TK, e, 0, 0, st);
+  return SPARF_WG_RUN(false, p, opnd(gt), N, TnB{X, ldx, div, M, K}, K, gt.ks, true, e, 0, 0, st);
 }
 
 }  // namespace sparf
@@ -556,7 +692,7 @@ extern "C" int sparf_tc_selftest_tn(const float* G, const float* X, int32_t rows
   if (rc) return rc;
   const TcImage gt{p.pack_a, rows / 32};
   rc = tc_pack_cols(p, rows, 128, G, 128, gt, st);
-  if (!rc) rc = tc_gemm_tn(p, rows, 128, 128, 128, rows, gt, X, 128, 1, D, 128, 0, st);
+  if (!rc) rc = tc_gemm_tn(p, rows, 128, 128, 128, gt, X, 128, 1, D, 128, 0, st);
   free_images(p, st);
   return rc;
 }
@@ -565,15 +701,15 @@ extern "C" int sparf_tc_selftest_tn(const float* G, const float* X, int32_t rows
 //   D = X W1 (X [M,128], W1 [128,96]; the input-gradient GEMM), written only as a row image, a transposed image and its
 //       column sums db[96];
 //   Y = [D | E] W2^T (E [M,40], W2 [128,136]): the row image as the first segment of a two-segment A operand;
-//   Z = D^T X [96,128]: the transposed image as the weight-gradient A operand, over slabs of 64 rows.
-// The image buffers start as NaN, so a k-step past M that is not zero-padded shows in Z.
-extern "C" int sparf_tc_selftest_images(const float* X, const float* W1, const float* E, const float* W2, int32_t M, float* Y,
-                                        float* Z, float* db, sparf_stream_t stream) {
+//   Z = D^T X [96,128]: the transposed image as the weight-gradient A operand, its rows split into k-ranges.
+// The image buffers start as NaN, so a k-step past M that is not zero-padded shows in Z.  max_ctas > 0 caps the GEMM
+// grids (else they take one CTA per SM), so that CTAs take several units and the copy ring wraps across them.
+static int selftest_images(const float* X, const float* W1, const float* E, const float* W2, int M, float* Y, float* Z,
+                           float* db, int max_ctas, cudaStream_t st) {
   SPARF_REQUIRE(M >= 1 && M <= 1024, "tc_selftest_images: M=%d", M);
-  cudaStream_t st = (cudaStream_t)stream;
   const int N = 128, K = 96, KE = 40;
-  const TcPrec p{false, 3};
-  TcPrec q = p;
+  TcPrec q{false, 3};
+  q.max_ctas = max_ctas;
   const TcImage x{nullptr, N / TK}, d{nullptr, K / TK}, e{nullptr, ceil_div(KE, TK)}, dt{nullptr, ceil_div(M, TK)};
   const size_t nx = tc_image_elems(M, N), nd = tc_image_elems(M, K), ne = tc_image_elems(M, KE), ndt = tc_image_elems(K, M);
   int rc = alloc_images(nx + nd + ne + ndt + tc_pack_elems(std::max(M, N), ceil_div(K + KE, TK), 0), st, q);
@@ -590,7 +726,17 @@ extern "C" int sparf_tc_selftest_images(const float* X, const float* W1, const f
   if (!rc) rc = tc_gemm_nn(q, M, N, K, K, xi, W1, K, 0, nullptr, 0, nullptr, nullptr, nullptr, 0, 0, o, db, st);
   if (!rc) rc = tc_pack_rows(q, M, KE, E, KE, 1, ei, st);
   if (!rc) rc = tc_gemm_nt(q, 0, M, 128, di, K, ei, KE, W2, K + KE, K, nullptr, Y, 128, TcOut{}, st);
-  if (!rc) rc = tc_gemm_tn(q, M, K, N, N, 64, dti, X, N, 1, Z, N, 0, st);
+  if (!rc) rc = tc_gemm_tn(q, M, K, N, N, dti, X, N, 1, Z, N, 0, st);
   free_images(q, st);
   return rc;
+}
+
+extern "C" int sparf_tc_selftest_images(const float* X, const float* W1, const float* E, const float* W2, int32_t M, float* Y,
+                                        float* Z, float* db, sparf_stream_t stream) {
+  return selftest_images(X, W1, E, W2, M, Y, Z, db, 0, (cudaStream_t)stream);
+}
+
+extern "C" int sparf_tc_selftest_persistent(const float* X, const float* W1, const float* E, const float* W2, int32_t M,
+                                            float* Y, float* Z, float* db, int32_t max_ctas, sparf_stream_t stream) {
+  return selftest_images(X, W1, E, W2, M, Y, Z, db, max_ctas, (cudaStream_t)stream);
 }

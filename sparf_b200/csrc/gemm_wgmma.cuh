@@ -18,6 +18,7 @@ struct TcPrec {
   uint16_t* pack_a = nullptr;
   uint16_t* pack_b = nullptr;
   size_t pack_elems = 0;
+  int max_ctas = 0;   // > 0: at most this many CTAs per GEMM (self-tests of the persistent loop); else one per SM
 };
 
 // An operand image of a [rows x K] matrix: split 16-bit halves in [128 rows x 32 K] tiles of wgmma's shared-memory
@@ -54,8 +55,9 @@ int tc_gemm_nt(TcPrec p, int act, int M, int N, TcImage a1, int K1v, TcImage a2,
 int tc_gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, TcImage g, const float* W, int ldw, int wcol, const float* mask_src,
                int ldmask, const float* r1_vec, const float* r1_row, float* D, int ldd, int accumulate, const TcOut& out,
                float* db, cudaStream_t st);
-// dW[n][wcol+k] += sum_m G[m][n] X[m/div][k]   (atomic over slabs of rows_per_slab rows), G [M x N] as its transposed image
-int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, int rows_per_slab, TcImage gt, const float* X, int ldx, int div,
-               float* dW, int ldw, int wcol, cudaStream_t st);
+// dW[n][wcol+k] += sum_m G[m][n] X[m/div][k]   (atomic over k-ranges of the rows, about one CTA per SM in all), G [M x N]
+// as its transposed image
+int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, TcImage gt, const float* X, int ldx, int div, float* dW, int ldw,
+               int wcol, cudaStream_t st);
 
 }  // namespace sparf

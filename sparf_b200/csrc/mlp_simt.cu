@@ -827,8 +827,7 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
       rc = simt_chunk_forward(mlp, ep, d, nr, S, o_c, d_c, t_c, nz, wts, enc, denc, H, raw, hid, nullptr, rgbv, w, st);
       if (rc) return rc;
     }
-    const int slab = ep.wgrad.passes ? 512 : 2048;  // rows per wgrad slab (tensor cores: >= 2 waves of CTAs per layer)
-    const int nslab = ceil_div(Mc, slab);
+    const int slab = 2048;  // rows per SIMT wgrad slab (the tensor-core GEMMs choose their own k-ranges)
 
     head_grad_kernel<<<ceil_div(Mc, 256), 256, 0, st>>>(Mc, d_rgb + m0 * 3, rgbv, d_sigma + m0, raw, nullptr, gpre, graw);
     LAUNCH_OK("head_grad_kernel");
@@ -854,8 +853,8 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
     const TcImage ghid_t{w.pack_a, ceil_div(Mc, 32)}, ghid{w.pack_a, ceil_div(d.HW, 32)};
     if (tc) {
       SPARF_TRY(tc_pack_cols(ep.wgrad, (int)Mc, d.HW, Ghid, d.HW, ghid_t, st));
-      SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.W, d.W, slab, ghid_t, feat, d.W, 1, grad->head_w[0], ldw8, 0, st));
-      SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.Evp, d.Ev, slab, ghid_t, denc, d.Evp, S, grad->head_w[0], ldw8, d.W, st));
+      SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.W, d.W, ghid_t, feat, d.W, 1, grad->head_w[0], ldw8, 0, st));
+      SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.Evp, d.Ev, ghid_t, denc, d.Evp, S, grad->head_w[0], ldw8, d.W, st));
     } else {
       SPARF_TRY(gemm_tn((int)Mc, d.HW, d.W, d.W, slab, Ghid, d.HW, feat, d.W, 1, grad->head_w[0], ldw8, 0, st));
       SPARF_TRY(gemm_tn((int)Mc, d.HW, d.Evp, d.Ev, slab, Ghid, d.HW, denc, d.Evp, S, grad->head_w[0], ldw8, d.W, st));
@@ -895,9 +894,9 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
       float* dWl = grad->trunk_w[l] + (size_t)rowoff * ldw;
       const float* Wl = mlp->trunk_w[l] + (size_t)rowoff * ldw;
       if (tc) {
-        SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, Kin, Kinv, slab, gtr(gi), in, Kin, 1, dWl, ldw, 0, st));
+        SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, Kin, Kinv, gtr(gi), in, Kin, 1, dWl, ldw, 0, st));
         if (l == d.skip)
-          SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, d.E3p, d.E3, slab, gtr(gi), enc, d.E3p, 1, dWl, ldw, d.W, st));
+          SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, d.E3p, d.E3, gtr(gi), enc, d.E3p, 1, dWl, ldw, d.W, st));
       } else {
         SPARF_TRY(gemm_tn((int)Mc, d.W, Kin, Kinv, slab, G, d.W, in, Kin, 1, dWl, ldw, 0, st));
         if (l == d.skip) SPARF_TRY(gemm_tn((int)Mc, d.W, d.E3p, d.E3, slab, G, d.W, enc, d.E3p, 1, dWl, ldw, d.W, st));

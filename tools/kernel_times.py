@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel device time of one MLP training step / inference forward (torch.profiler = CUPTI activity records, no
-replay, warm caches).  Usage: [SPARF_KT_ENGINE=tc_3x|tc_3x_w1] [SPARF_KT_NOPOSE=1] python tools/kernel_times.py [R S]"""
+replay, warm caches), and the achieved HBM bandwidth of the wgmma GEMM kernels against the bytes they must move.
+Usage: [SPARF_KT_ENGINE=tc_3x|tc_1x|tc_3x_w1] [SPARF_KT_NOPOSE=1] python tools/kernel_times.py [R S]"""
 import os
 import sys
 from collections import defaultdict
@@ -13,6 +14,45 @@ from torch.profiler import ProfilerActivity, profile
 
 import common
 from sparf_b200 import _lib, ops
+
+HBM_PEAK = 3.35e12      # H100 SXM data sheet, bytes/s
+GEMM_KERNEL = "wg_gemm_kernel"
+# 16-bit passes of the images (forward, input gradient, weight gradient) per tensor-core engine
+PASSES = {"tc_3x": (3, 3, 3), "tc_1x": (1, 1, 1), "tc_3x_w1": (3, 3, 1), "auto": (3, 3, 3)}
+
+
+def gemm_bytes_per_row(spec, passes, backward, pose):
+    """HBM bytes per sample row that the wgmma GEMMs must read and write, counted from the shapes: the A operand images,
+    the weight-gradient GEMMs' B operand images (activation-sized), the fp32 outputs, the epilogue images and the fp32
+    ReLU-mask sources.  The weights' images are small and stay in L2; they are not counted."""
+    pf, pd, pw = passes
+    W, HW, skip, nt = spec.width, spec.head_width, spec.skip_layer, spec.n_trunk
+    E3p, Evp = -(-(3 + 6 * spec.L_xyz) // 8) * 8, -(-(3 + 6 * spec.L_view) // 8) * 8
+
+    def img(cols, p):     # one row of an image: K padded to 32, 2 bytes per half, hi and lo halves when p == 3
+        return -(-cols // 32) * 32 * 2 * (2 if p == 3 else 1)
+
+    # forward: trunk layer l reads its input image (+ enc at the skip layer), writes fp32 H and its row image; the colour
+    # head reads [H | denc] and writes fp32 hid
+    n = sum(img(W if l else E3p, pf) + (img(E3p, pf) if l == skip else 0) + 4 * W + img(W, pf) for l in range(nt))
+    n += img(W, pf) + img(Evp, pf) + 4 * HW
+    if not backward:
+        return n
+    # colour head: two weight-gradient GEMMs (Ghid^T [feat | denc]); the input gradient of feat (mask = feat) as row and
+    # transposed images; with pose gradients the direction-encoding gradient in fp32
+    n += 2 * img(HW, pw) + img(W, pw) + img(Evp, pw)
+    n += img(HW, pd) + 4 * W + img(W, pd) + img(W, pw)
+    if pose:
+        n += img(HW, pd) + 4 * Evp
+    for l in range(nt - 1, -1, -1):
+        n += img(W, pw) + img(W if l else E3p, pw)                      # weight gradient
+        if l == skip:
+            n += img(W, pw) + img(E3p, pw)
+        if l > 0:                                                       # input gradient: G image, mask, two images out
+            n += img(W, pd) + 4 * W + img(W, pd) + img(W, pw)
+        if pose and (l == skip or l == 0):                              # encoding gradient, fp32 (+= at layer 0)
+            n += img(W, pd) + 4 * E3p + (4 * E3p if l == 0 and skip > 0 else 0)
+    return n
 
 
 def main():
@@ -27,7 +67,8 @@ def main():
     d = torch.nn.functional.normalize(torch.randn(R, 3, device="cuda"), dim=-1).requires_grad_(pose)
     t = torch.sort(torch.rand(R, S, device="cuda") * 4 + 1.2, dim=1).values
     spec = ops.MLPSpec()
-    eng = _lib.ENGINES[os.environ.get("SPARF_KT_ENGINE", "tc_3x")]
+    eng_name = os.environ.get("SPARF_KT_ENGINE", "tc_3x")
+    eng = _lib.ENGINES[eng_name]
     gs, gc = torch.randn(R, S, device="cuda"), torch.randn(R, S, 3, device="cuda")
 
     def step():
@@ -40,7 +81,10 @@ def main():
         with torch.no_grad():
             ops.mlp_forward(spec, o, d, t, params, engine=eng)
 
-    for name, fn in (("training step (forward with tape + backward)", step), ("inference forward", infer)):
+    if torch.cuda.is_available():
+        p = torch.cuda.get_device_properties(0)
+        print("device: %s, %d SMs" % (p.name, p.multi_processor_count))
+    for name, fn, bwd in (("training step (forward with tape + backward)", step, True), ("inference forward", infer, False)):
         for _ in range(3):
             fn()
         torch.cuda.synchronize()
@@ -58,6 +102,12 @@ def main():
         print("== %s: %.1f us of kernels per call" % (name, tot))
         for k, v in sorted(agg.items(), key=lambda kv: -kv[1][1]):
             print("  %8.1f us  x%-3d %s" % (v[1] / n, v[0] // n, k[:110]))
+        if eng_name in PASSES:
+            g_us = sum(v[1] for k, v in agg.items() if GEMM_KERNEL in k) / n
+            g_bytes = R * S * gemm_bytes_per_row(spec, PASSES[eng_name], bwd, pose and bwd)
+            print("  GEMM group (%s): %.1f us per call, %.2f GB to move (from shapes), %.0f GB/s = %.1f %% of %.2f TB/s"
+                  % (GEMM_KERNEL, g_us, g_bytes / 1e9, g_bytes / (g_us * 1e-6) / 1e9 if g_us else 0.0,
+                     100 * g_bytes / (g_us * 1e-6) / HBM_PEAK if g_us else 0.0, HBM_PEAK / 1e12))
 
 
 if __name__ == "__main__":
