@@ -139,7 +139,8 @@ int sparf_sample_pdf_merge(int32_t R, int32_t S, int32_t S_fine, float near, flo
  * NeRF.forward_samples (frequency_nerf.py:260-281): x = o + t*d, positional encoding, trunk, softplus
  * density (+ noise[R,S] on the raw value when non-NULL), colour head, sigmoid.
  * Outputs sigma [R,S], rgb [R,S,3].
- * sparf_mlp_workspace_bytes: `backward` = 0 forward call, 1 sparf_mlp_backward (recompute), 2 sparf_mlp_backward_tape.
+ * sparf_mlp_workspace_bytes: `backward` = 0 forward call (sparf_mlp_forward or sparf_mlp_forward_tape), 1
+ * sparf_mlp_backward (recompute), 2 sparf_mlp_backward_tape.
  */
 size_t sparf_mlp_workspace_bytes(const SparfMLP* mlp, int32_t R, int32_t S, int32_t backward, int32_t engine);
 int sparf_mlp_forward(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S, const float* origins,
@@ -234,6 +235,15 @@ int sparf_tc_selftest_images(const float* X, const float* W1, const float* E, co
  * CTA of the persistent GEMM kernel walks several work units and its copy ring wraps across them. */
 int sparf_tc_selftest_persistent(const float* X, const float* W1, const float* E, const float* W2, int32_t M, float* Y,
                                  float* Z, float* db, int32_t max_ctas, sparf_stream_t stream);
+/* The fused colour-head backward of the tensor-core engines against the kernels it replaces, on the same inputs:
+ * d_rgb, rgb [M,3], d_sigma, raw [M], hid [M,HW], W9 [3,HW]; M in [1, 2^20], HW a multiple of 8 in [8, 512].  img gets,
+ * each after a fill with 0xFFFF, four bf16 images (row_passes / tr_passes: 1 or 3, hi only or hi and lo): the fused
+ * kernel's row image of Ghid [M,HW] (ceil(M/128) * ceil(HW/32) * 8192 elements) and its transposed image (ceil(HW/128) *
+ * ceil(M/32) * 8192), then the same two packed from the fp32 Ghid of the old path.  graw [2,M]: the fused kernel's
+ * density gradient, then the old path's.  Both halves must be bit-identical. */
+int sparf_tc_selftest_head(const float* d_rgb, const float* rgb, const float* d_sigma, const float* raw, const float* hid,
+                           const float* W9, int32_t M, int32_t HW, int32_t row_passes, int32_t tr_passes, uint16_t* img,
+                           float* graw, sparf_stream_t stream);
 
 #ifdef __cplusplus
 }

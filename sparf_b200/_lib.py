@@ -62,6 +62,7 @@ _SIGNATURES = {
     "sparf_tc_selftest_tn": (c_int32, [_P, _P, c_int32, _P, _P]),
     "sparf_tc_selftest_images": (c_int32, [_P, _P, _P, _P, c_int32, _P, _P, _P, _P]),
     "sparf_tc_selftest_persistent": (c_int32, [_P, _P, _P, _P, c_int32, _P, _P, _P, c_int32, _P]),
+    "sparf_tc_selftest_head": (c_int32, [_P, _P, _P, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, _P, _P, _P]),
 }
 
 _lib = None

@@ -5,7 +5,8 @@
 // in K 128 B apart = leading byte offset, 8-row groups 512 B apart = stride byte offset), hi and lo halves of a tile
 // adjacent (16 KB).
 //   pack: splits an fp32 operand (with the GEMM's own indexing: transposes, per-ray rows, bounds) into an image; the
-//     weights, the encodings and the colour-head gradient take this path;
+//     weights and the encodings take this path;
+//   head backward: the colour head's narrow layer, whose gradient it writes straight into its two images;
 //   gemm: persistent, one CTA per SM walking 128 x 128 output tiles (the weight gradient: tiles x k-ranges).  A
 //     producer thread streams the tiles of both operands with cp.async.bulk into a STAGES-deep ring of shared-memory
 //     stages that runs on across tiles, each stage completing on its "full" mbarrier (complete_tx); two consumer
@@ -185,6 +186,158 @@ __global__ void __launch_bounds__(256) pack_kernel(F f, int ksteps, uint16_t* __
   for (int i = threadIdx.x; i < NV; i += 256) dst[i] = src[i];
 }
 
+// The colour-head backward of the tensor-core engines, one CTA per 128-row tile (rows m0 + r):
+//   gpre[m][j] = d_rgb[m][j] c (1 - c), c = rgb[m][j];  graw[m] = d_sigma[m] softplus'(raw[m])      (as head_grad_kernel)
+//   Ghid[m][n] = (hid[m][n] > 0) * sum_j gpre[m][j] W9[j][n]                                          (as narrow_dgrad_kernel)
+// Ghid never goes to HBM in fp32: it leaves as its row image (dgrad passes) and its transposed image (wgrad passes),
+// split from the same fp32 values as pack_kernel would split them, zero past M and HW.  Per CTA, one atomic per output:
+// db_hid += the column sums of Ghid, dW9[j] += gpre_j^T hid, db9[j] += sum gpre_j, db_raw += sum graw.
+struct HeadBwd {
+  int M, HW;
+  const float *d_rgb, *rgb, *d_sigma, *raw, *hid, *W9;
+  float* graw;
+  uint16_t *row, *tr;       // images, row_ks = ceil(HW / 32) and tr_ks = ceil(M / 32) k-steps per row tile
+  int row_ks, tr_ks;
+  float *dW9, *db9, *db_hid, *db_raw;
+};
+
+constexpr int HB_LD = TN + 1;       // Ghid tile in shared memory, [128 rows][128 columns + 1]: conflict-free both ways
+constexpr int HEAD_SMEM = (TM * HB_LD + 8 * 16 * 32 + TM * 4 + 3 * TN + 4 * 4) * 4;
+
+// eight consecutive k of one image row -> their bf16 hi halves and lo halves, 16 bytes each
+__device__ __forceinline__ void split8(const float (&v)[8], uint4& hi, uint4& lo) {
+  uint16_t h[8], l[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) split16<false>(v[e], h[e], l[e]);
+  hi = make_uint4(h[0] | (uint32_t)h[1] << 16, h[2] | (uint32_t)h[3] << 16, h[4] | (uint32_t)h[5] << 16, h[6] | (uint32_t)h[7] << 16);
+  lo = make_uint4(l[0] | (uint32_t)l[1] << 16, l[2] | (uint32_t)l[3] << 16, l[4] | (uint32_t)l[5] << 16, l[6] | (uint32_t)l[7] << 16);
+}
+
+template <int ROWP, int TRP>
+__global__ void __launch_bounds__(256) head_bwd_kernel(const HeadBwd p) {
+  extern __shared__ __align__(16) float hsm[];
+  float* V = hsm;                           // [TM][HB_LD] Ghid of this tile's rows, one column block at a time
+  float* red = V + TM * HB_LD;              // [8 warps][16 sums][32 lanes]
+  float* g = red + 8 * 16 * 32;             // [TM][4]: gpre 0..2, graw
+  float* w9 = g + TM * 4;                   // [3][TN]: this column block of W9
+  float* rsum = w9 + 3 * TN;                // [4 warps][4]: sums of gpre 0..2 and graw
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int m0 = blockIdx.x * TM;
+  if (tid < TM) {
+    const int m = m0 + tid;
+    float s[4] = {0.f, 0.f, 0.f, 0.f};
+    if (m < p.M) {
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+        const float c = p.rgb[(size_t)m * 3 + j];
+        s[j] = p.d_rgb[(size_t)m * 3 + j] * c * (1.f - c);
+      }
+      s[3] = p.d_sigma[m] * softplus_grad_f(p.raw[m]);
+      p.graw[m] = s[3];
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) g[tid * 4 + j] = s[j];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s[j] += __shfl_xor_sync(0xffffffffu, s[j], o);
+      if (lane == 0) rsum[warp * 4 + j] = s[j];
+    }
+  }
+  for (int n0 = 0; n0 < p.HW; n0 += TN) {
+    __syncthreads();                        // g and rsum written; the previous column block's V and red read
+    if (n0 == 0 && tid < 4) {
+      const float s = rsum[tid] + rsum[4 + tid] + rsum[8 + tid] + rsum[12 + tid];
+      atomicAdd(tid < 3 ? p.db9 + tid : p.db_raw, s);
+    }
+    for (int i = tid; i < 3 * TN; i += 256) {
+      const int n = n0 + i % TN;
+      w9[i] = n < p.HW ? p.W9[(size_t)(i / TN) * p.HW + n] : 0.f;
+    }
+    __syncthreads();
+    // columns n0 + 4 c4 + q of rows warp + 8 i: hid in 16-byte loads, all issued first
+    const int c4 = lane, n = n0 + 4 * c4;
+    float4 x[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int m = m0 + warp + 8 * i;
+      x[i] = m < p.M && n < p.HW ? *reinterpret_cast<const float4*>(p.hid + (size_t)m * p.HW + n) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    float cs[4] = {0.f, 0.f, 0.f, 0.f}, dw[3][4];
+#pragma unroll
+    for (int j = 0; j < 3; ++j)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) dw[j][q] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int r = warp + 8 * i;
+      const float h[4] = {x[i].x, x[i].y, x[i].z, x[i].w};
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        float v = 0.f;
+#pragma unroll
+        for (int j = 0; j < 3; ++j) v = fmaf(g[r * 4 + j], w9[j * TN + 4 * c4 + q], v);
+        v = h[q] > 0.f ? v : 0.f;
+        V[r * HB_LD + 4 * c4 + q] = v;
+        cs[q] += v;
+#pragma unroll
+        for (int j = 0; j < 3; ++j) dw[j][q] = fmaf(g[r * 4 + j], h[q], dw[j][q]);
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      red[(warp * 16 + q) * 32 + lane] = cs[q];
+#pragma unroll
+      for (int j = 0; j < 3; ++j) red[(warp * 16 + 4 + 4 * j + q) * 32 + lane] = dw[j][q];
+    }
+    __syncthreads();
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {           // sum k of lane l's columns: k = 0..3 Ghid column q = k, 4 + 4 j + q: dW9[j]
+      const int idx = tid + 256 * s, k = idx >> 5, l = idx & 31, col = n0 + 4 * l + (k & 3);
+      float v = 0.f;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) v += red[(w * 16 + k) * 32 + l];
+      if (col < p.HW) atomicAdd(k < 4 ? p.db_hid + col : p.dW9 + (size_t)((k - 4) >> 2) * p.HW + col, v);
+    }
+    // images: 16-byte chunk c of a tile half is row c & 7 of core matrix c >> 3 (eight consecutive k), so consecutive
+    // threads write consecutive 16 bytes
+#pragma unroll
+    for (int kq = 0; kq < 4; ++kq) {
+      const int kt = (n0 >> 5) + kq;      // row image: rows m, k = n
+      if (kt >= p.row_ks) break;
+      uint16_t* t = p.row + ((size_t)blockIdx.x * p.row_ks + kt) * 2 * TILE_ELEMS;
+#pragma unroll
+      for (int s = 0; s < 2; ++s) {
+        const int c = tid + 256 * s, core = c >> 3, r = (core >> 2) * 8 + (c & 7), k = kq * 32 + (core & 3) * 8;
+        float v[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) v[e] = V[r * HB_LD + k + e];
+        uint4 hi, lo;
+        split8(v, hi, lo);
+        reinterpret_cast<uint4*>(t)[c] = hi;
+        if (ROWP == 3) reinterpret_cast<uint4*>(t + TILE_ELEMS)[c] = lo;
+      }
+    }
+#pragma unroll
+    for (int kq = 0; kq < 4; ++kq) {
+      const int kt = blockIdx.x * (TM / TK) + kq;   // transposed image: rows n (row tile n0 / 128), k = m
+      if (kt >= p.tr_ks) break;
+      uint16_t* t = p.tr + ((size_t)(n0 / TN) * p.tr_ks + kt) * 2 * TILE_ELEMS;
+#pragma unroll
+      for (int s = 0; s < 2; ++s) {
+        const int c = tid + 256 * s, core = c >> 3, r = (core >> 2) * 8 + (c & 7), k = kq * 32 + (core & 3) * 8;
+        float v[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) v[e] = V[(k + e) * HB_LD + r];
+        uint4 hi, lo;
+        split8(v, hi, lo);
+        reinterpret_cast<uint4*>(t)[c] = hi;
+        if (TRP == 3) reinterpret_cast<uint4*>(t + TILE_ELEMS)[c] = lo;
+      }
+    }
+  }
+}
+
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 __device__ __forceinline__ void mbar_init(uint64_t* b, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(smem_u32(b)), "r"(count) : "memory");
@@ -225,7 +378,8 @@ struct Epi {
   const float *mask, *r1_vec, *r1_row;
   int ldmask, accumulate;
   float* colsum;            // kind 1: += column sums of the output
-  uint16_t *row, *tr;       // output images, row_ks / tr_ks k-steps per row tile
+  float* r1_wgrad;          // kind 1 with mask and r1_vec: += sum_m r1_vec[m] mask[m][n] (the density row's gradient)
+  uint16_t *row, *tr;      // output images, row_ks / tr_ks k-steps per row tile
   int row_ks, tr_ks;
   int pairs;                // N even, out and mask 8-byte aligned with even leading dimensions (kinds 0 and 1)
 };
@@ -355,6 +509,32 @@ __device__ __forceinline__ void st2(float* p, float x, float y, bool two) {
 // the consumer warpgroups only (the producer warpgroup never joins)
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;\n" ::"n"(CONSUMERS) : "memory"); }
 
+// dst[n0 + c] += column c of the tile summed over its rows, from part[2 j + c'] = this thread's share of column
+// 8 j + 2 (lane % 4) + c' (its two rows): over the 16 rows of each warp (shuffles), the 8 warps (the 4 KB of shared
+// memory after the ring), the CTAs (one atomic per column)
+__device__ __forceinline__ void tile_colsum(const float (&part)[32], int n0, int N, float* dst) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  float* red = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [8][128]
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  consumer_sync();              // the previous sums have been read
+#pragma unroll
+  for (int j = 0; j < 16; ++j)
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      float s = part[2 * j + c];
+#pragma unroll
+      for (int o = 4; o < 32; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      if (lane < 4) red[w * TN + 8 * j + 2 * lane + c] = s;
+    }
+  consumer_sync();
+  if (threadIdx.x < TN && n0 + (int)threadIdx.x < N) {
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) s += red[i * TN + threadIdx.x];
+    atomicAdd(dst + n0 + threadIdx.x, s);
+  }
+}
+
 // The epilogue of output tile (B row tile bx, A row tile by).  It writes, each only when its template flag is set: the
 // fp32 output (F32), a row image of the output (rows = output rows, K = output columns) and a transposed image (rows =
 // output columns, K = output rows), with ROWP / TRP passes (3: hi and lo halves, 1: hi only) in the GEMM's 16-bit type.
@@ -366,13 +546,32 @@ __device__ __forceinline__ void epilogue_values(float (&acc)[64], int m0, int n0
   // The mask loads come first, in a loop of their own, and leave one bit per value (acc[i] is kept iff bit i of keep).
   // Issued pair by pair inside the loop below, behind its branches, each would wait out its own memory latency (a mask
   // tile is 64 KB from HBM).
+  // The density row's weight gradient (r1_wgrad) is summed from the same mask values: there the mask source is the
+  // layer's input.  Only the input-gradient GEMMs that write images (no fp32 output) carry that code; it would change
+  // how the compiler builds the other instantiations' epilogues.
   uint64_t keep = ~0ull;
   if (e.kind == 1 && e.mask) {
+    float rv[2] = {0.f, 0.f}, part[32];
+    if constexpr (!F32) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = m0 + frag_row(2 * h);
+        if (e.r1_wgrad && m < e.M) rv[h] = e.r1_vec[m];
+      }
+    }
 #pragma unroll
     for (int i = 0; i < 64; i += 2) {
       const int m = m0 + frag_row(i), n = n0 + frag_col(i);
       const float2 mk = m < e.M && n < e.N ? ld2<PAIRS>(e.mask + (size_t)m * e.ldmask + n, n + 1 < e.N) : make_float2(0.f, 0.f);
       keep &= ~((uint64_t)!(mk.x > 0.f) << i | (uint64_t)!(mk.y > 0.f) << (i + 1));
+      if constexpr (!F32) {
+        const int h = (i >> 1) & 1, p = 2 * (i >> 2);
+        part[p] = h ? fmaf(rv[1], mk.x, part[p]) : rv[0] * mk.x;
+        part[p + 1] = h ? fmaf(rv[1], mk.y, part[p + 1]) : rv[0] * mk.y;
+      }
+    }
+    if constexpr (!F32) {
+      if (e.r1_wgrad) tile_colsum(part, n0, e.N, e.r1_wgrad);
     }
   }
 #pragma unroll
@@ -426,26 +625,13 @@ __device__ __forceinline__ void epilogue(float (&acc)[64], int bx, int by, const
   if (e.pairs) epilogue_values<F32, true>(acc, m0, n0, e);
   else epilogue_values<F32, false>(acc, m0, n0, e);
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  if (e.colsum) {               // over the 16 rows of each warp (shuffles), the 8 warps (shared memory), the CTAs (atomics)
-    extern __shared__ __align__(1024) uint8_t smem[];
-    float* red = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [8][128]
-    consumer_sync();            // the previous unit's sums have been read
+  if (e.colsum) {
+    float part[32];
 #pragma unroll
     for (int j = 0; j < 16; ++j)
 #pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        float s = acc[4 * j + c] + acc[4 * j + 2 + c];
-#pragma unroll
-        for (int o = 4; o < 32; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        if (lane < 4) red[w * TN + 8 * j + 2 * lane + c] = s;
-      }
-    consumer_sync();
-    if (threadIdx.x < TN && n0 + (int)threadIdx.x < e.N) {
-      float s = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) s += red[i * TN + threadIdx.x];
-      atomicAdd(e.colsum + n0 + threadIdx.x, s);
-    }
+      for (int c = 0; c < 2; ++c) part[2 * j + c] = acc[4 * j + c] + acc[4 * j + 2 + c];
+    tile_colsum(part, n0, e.N, e.colsum);
   }
   // The fragment of (j, h) is an 8 x 8 block: lane holds its row lane / 4, columns 2 (lane % 4) + {0, 1}.  In an image
   // that block is one core matrix (sw_off) and the lane's two values are its 32-bit word `lane`: a warp stores 128
@@ -547,8 +733,8 @@ static int sm_count() {
 
 // pack B into p.pack_b, then the persistent GEMM over (B row tiles x A row tiles) output tiles with the epilogue
 // outputs e asks for: fp32 (e.out), a row image (row image passes = the GEMM's), a transposed image.  split_k: each
-// output tile's k-steps are shared out in ceil(CTAs / output tiles) ranges (atomic epilogues only), so every CTA does
-// one long reduction.
+// output tile's k-steps are shared out in ceil(CTAs / output tiles) ranges per 32 768 rows (atomic epilogues only), so
+// every CTA does one long reduction per 32 768 rows.
 template <bool F16, int PASSES, bool BK, class FB>
 static int run(const TcPrec& p, const Opnd& a, int a_rows, FB fb, int b_rows, int ksteps, bool split_k, const Epi& e,
                int row_passes, int tr_passes, cudaStream_t st) {
@@ -561,7 +747,9 @@ static int run(const TcPrec& p, const Opnd& a, int a_rows, FB fb, int b_rows, in
   const Opnd b{p.pack_b, nullptr, ksteps, 0};
   const int ctas = p.max_ctas > 0 ? std::min(p.max_ctas, sm_count()) : sm_count();
   Units w{rtb, rta * rtb, 1, ksteps};
-  if (split_k) w.nsplit = std::max(1, std::min(ksteps, ceil_div(ctas, w.tiles)));
+  // about ceil(CTAs / output tiles) ranges per 1024 k-steps (32 768 rows): no accumulator chain gets longer than at
+  // 32 768 rows, whatever the chunk size, so the rounding of the sums does not grow with it
+  if (split_k) w.nsplit = std::max(1, std::min(ksteps, ceil_div(ctas, w.tiles) * ceil_div(ksteps, 1024)));
   const bool f32 = e.out != nullptr;
   if (f32 && !row_passes && !tr_passes) return launch_gemm<F16, PASSES, true, 0, 0>(a, b, w, ctas, e, st);
   if (f32 && row_passes == PASSES && !tr_passes) return launch_gemm<F16, PASSES, true, PASSES, 0>(a, b, w, ctas, e, st);
@@ -628,12 +816,13 @@ int tc_gemm_nt(TcPrec p, int act, int M, int N, TcImage a1, int K1v, TcImage a2,
 
 int tc_gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, TcImage g, const float* W, int ldw, int wcol, const float* mask_src,
                int ldmask, const float* r1_vec, const float* r1_row, float* D, int ldd, int accumulate, const TcOut& out,
-               float* db, cudaStream_t st) {
+               float* db, float* r1_wgrad, cudaStream_t st) {
   SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && g.ks == ceil_div(N, TK), "tc_gemm_nn: passes=%d ks=%d N=%d", p.passes,
                 g.ks, N);
+  SPARF_REQUIRE(!r1_wgrad || (mask_src && r1_vec && !D), "tc_gemm_nn: r1_wgrad needs the mask source, r1_vec, no fp32 D");
   Epi e{};
   e.kind = 1; e.M = M; e.N = Kout; e.out = D; e.ldo = ldd; e.Kv = Kv; e.mask = mask_src; e.ldmask = ldmask;
-  e.r1_vec = r1_vec; e.r1_row = r1_row; e.accumulate = accumulate; e.colsum = db;
+  e.r1_vec = r1_vec; e.r1_row = r1_row; e.accumulate = accumulate; e.colsum = db; e.r1_wgrad = r1_wgrad;
   e.pairs = Kout % 2 == 0 && pair_aligned(D, ldd) && pair_aligned(mask_src, ldmask);
   SPARF_REQUIRE(!db || !accumulate, "tc_gemm_nn: column sums of an accumulated output");
   int rc = set_images(e, out, M, Kout);
@@ -647,6 +836,30 @@ int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, TcImage gt, const float* X
   Epi e{};
   e.kind = 2; e.M = N; e.N = K; e.out = dW; e.ldo = ldw; e.col_off = wcol; e.Kv = Kv;
   return SPARF_WG_RUN(false, p, opnd(gt), N, TnB{X, ldx, div, M, K}, K, gt.ks, true, e, 0, 0, st);
+}
+
+template <int ROWP, int TRP>
+static int launch_head_bwd(const HeadBwd& h, cudaStream_t st) {
+  auto kernel = head_bwd_kernel<ROWP, TRP>;
+  SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HEAD_SMEM));
+  kernel<<<ceil_div(h.M, TM), 256, HEAD_SMEM, st>>>(h);
+  SPARF_CHECK_LAUNCH("head_bwd_kernel");
+  return SPARF_OK;
+}
+
+int tc_head_backward(TcPrec dg, TcPrec wg, int M, int HW, const float* d_rgb, const float* rgb, const float* d_sigma,
+                     const float* raw, const float* hid, const float* W9, float* graw, TcImage row, TcImage tr, float* dW9,
+                     float* db9, float* db_hid, float* db_raw, cudaStream_t st) {
+  SPARF_REQUIRE(!dg.f16 && !wg.f16 && (dg.passes == 1 || dg.passes == 3) && (wg.passes == 1 || wg.passes == 3),
+                "tc_head_backward: bf16 1- or 3-pass images only");
+  SPARF_REQUIRE(M >= 1 && HW % 4 == 0 && !(reinterpret_cast<uintptr_t>(hid) & 15), "tc_head_backward: M=%d HW=%d", M, HW);
+  SPARF_REQUIRE(row.p && row.ks == ceil_div(HW, TK) && tr.p && tr.ks == ceil_div(M, TK),
+                "tc_head_backward: images need %d and %d k-steps", ceil_div(HW, TK), ceil_div(M, TK));
+  const HeadBwd h{M, HW, d_rgb, rgb, d_sigma, raw, hid, W9, graw, row.p, tr.p, row.ks, tr.ks, dW9, db9, db_hid, db_raw};
+  if (dg.passes == 3 && wg.passes == 3) return launch_head_bwd<3, 3>(h, st);
+  if (dg.passes == 3 && wg.passes == 1) return launch_head_bwd<3, 1>(h, st);
+  if (dg.passes == 1 && wg.passes == 1) return launch_head_bwd<1, 1>(h, st);
+  SPARF_REQUIRE(false, "tc_head_backward: no kernel for %d-pass row and %d-pass transposed images", dg.passes, wg.passes);
 }
 
 }  // namespace sparf
@@ -723,7 +936,7 @@ static int selftest_images(const float* X, const float* W1, const float* E, cons
   o.row = di; o.row_passes = 3;
   o.tr = dti; o.tr_passes = 3;
   rc = tc_pack_rows(q, M, N, X, N, 1, xi, st);
-  if (!rc) rc = tc_gemm_nn(q, M, N, K, K, xi, W1, K, 0, nullptr, 0, nullptr, nullptr, nullptr, 0, 0, o, db, st);
+  if (!rc) rc = tc_gemm_nn(q, M, N, K, K, xi, W1, K, 0, nullptr, 0, nullptr, nullptr, nullptr, 0, 0, o, db, nullptr, st);
   if (!rc) rc = tc_pack_rows(q, M, KE, E, KE, 1, ei, st);
   if (!rc) rc = tc_gemm_nt(q, 0, M, 128, di, K, ei, KE, W2, K + KE, K, nullptr, Y, 128, TcOut{}, st);
   if (!rc) rc = tc_gemm_tn(q, M, K, N, N, dti, X, N, 1, Z, N, 0, st);

@@ -14,7 +14,7 @@ struct TcPrec {
   bool f16;     // fp16 halves (forward: 11-bit mantissas) or bf16 halves (gradients: fp32 exponent range)
   int passes;   // 3 or 1; 0 = CUDA-core FFMA kernels instead of tensor cores
   // caller-owned buffer of pack_elems 16-bit elements for the packed B operand (tensor cores only); pack_a, as large,
-  // is the caller's scratch image for A operands that no epilogue writes
+  // is the self-tests' scratch image for A operands
   uint16_t* pack_a = nullptr;
   uint16_t* pack_b = nullptr;
   size_t pack_elems = 0;
@@ -51,13 +51,24 @@ int tc_pack_cols(TcPrec p, int M, int N, const float* X, int ldx, TcImage img, c
 int tc_gemm_nt(TcPrec p, int act, int M, int N, TcImage a1, int K1v, TcImage a2, int K2v, const float* W, int ldw, int wcol2,
                const float* bias, float* Y, int ldy, const TcOut& out, cudaStream_t st);
 // D[m][k] = mask(m,k) * ( sum_n G[m][n] W[n][wcol+k] + r1_vec[m]*r1_row[k] )   (= or +=), G [M x N] as its row image.
-// D may be NULL when out writes images; db (may be NULL) += the column sums of D.
+// D may be NULL when out writes images; db (may be NULL) += the column sums of D; r1_wgrad (may be NULL; needs mask_src
+// and r1_vec) += sum_m r1_vec[m] mask_src[m][k], the weight gradient of the rank-1 row when mask_src is the layer input.
 int tc_gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, TcImage g, const float* W, int ldw, int wcol, const float* mask_src,
                int ldmask, const float* r1_vec, const float* r1_row, float* D, int ldd, int accumulate, const TcOut& out,
-               float* db, cudaStream_t st);
-// dW[n][wcol+k] += sum_m G[m][n] X[m/div][k]   (atomic over k-ranges of the rows, about one CTA per SM in all), G [M x N]
+               float* db, float* r1_wgrad, cudaStream_t st);
+// dW[n][wcol+k] += sum_m G[m][n] X[m/div][k]   (atomic over k-ranges of the rows, about one per SM per 32 768 rows), G [M x N]
 // as its transposed image
 int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, TcImage gt, const float* X, int ldx, int div, float* dW, int ldw,
                int wcol, cudaStream_t st);
+
+// The colour-head backward in one kernel (bf16 images): from the upstream d_rgb [M,3], d_sigma [M], the forward's rgb
+// [M,3], raw [M] (softplus argument) and hid [M,HW], and the head's output layer W9 [3,HW]:
+//   graw[m] = d_sigma[m] softplus'(raw[m]);  gpre[m][j] = d_rgb[m][j] rgb (1 - rgb);  Ghid = (hid > 0) * gpre W9,
+// Ghid written only as its row image (dg passes) and its transposed image (wg passes), bit-identical to tc_pack_rows /
+// tc_pack_cols of the fp32 Ghid; and dW9 [3,HW] += gpre^T hid, db9[3] += sum gpre, db_hid[HW] += the column sums of
+// Ghid, db_raw[0] += sum graw.
+int tc_head_backward(TcPrec dg, TcPrec wg, int M, int HW, const float* d_rgb, const float* rgb, const float* d_sigma,
+                     const float* raw, const float* hid, const float* W9, float* graw, TcImage row, TcImage tr, float* dW9,
+                     float* db9, float* db_hid, float* db_raw, cudaStream_t st);
 
 }  // namespace sparf

@@ -513,9 +513,11 @@ int simt_validate(const SparfMLP* mlp) {
   return SPARF_OK;
 }
 
-// rows handled per chunk (whole rays)
-static int chunk_rays(int S, int backward) {
-  int rows = backward ? 32768 : 65536;
+// Rays per chunk, by workspace mode (see carve): the recompute backward keeps every trunk activation of its chunk, so it
+// takes the smallest chunks; the taped passes keep only a chunk's images and gradients (about 1 GB at 131072 rows of the
+// default net) and take the largest, so that weight packs, GEMM ramp-ups and small kernels repeat as seldom as possible.
+static int chunk_rays(int S, int mode) {
+  const int rows = mode == 1 ? 32768 : mode == 0 ? 65536 : 131072;
   int n = rows / S;
   return n < 1 ? 1 : n;
 }
@@ -537,12 +539,13 @@ struct Carver {
 // Workspace of one call, per chunk of nrc rays.  mode 0: forward, 1: backward (recomputes the forward), 2: backward from a
 // tape, 3: taped forward (the activations go to the tape).  Tensor-core engines keep their GEMM operands as images: the
 // forward's encodings and ping-pong trunk activations, the backward's ping-pong trunk gradients (a row image for the next
-// input gradient, a transposed one for the weight gradient; no fp32 copy), and two buffers for the operands packed per GEMM.
+// input gradient, a transposed one for the weight gradient; no fp32 copy), the colour-head gradient's two images (no fp32
+// copy either), and a buffer for the weight operand packed per GEMM.
 struct Ws {
   float *wts, *enc, *denc, *hid, *raw, *rgbv, *G0, *G1, *Genc, *Ghid, *gpre, *graw, *Gdtmp, *Gdenc;
   float* H[SPARF_MAX_TRUNK];
-  TcImage encimg, dencimg, Himg[2], Grow[2], Gtr[2];
-  uint16_t *pack_a, *pack_b;
+  TcImage encimg, dencimg, Himg[2], Grow[2], Gtr[2], ghid_row, ghid_tr;
+  uint16_t* pack_b;
   size_t pack_elems;
 };
 
@@ -567,8 +570,10 @@ static size_t carve(const SimtDims& d, bool tc, int nrc, int S, int mode, char* 
   }
   if (mode == 1 || mode == 2) {
     w.Genc = cv.take(Mc * d.E3p);
-    w.Ghid = cv.take(Mc * d.HW);
-    w.gpre = cv.take(Mc * 4);
+    if (!tc) {
+      w.Ghid = cv.take(Mc * d.HW);
+      w.gpre = cv.take(Mc * 4);
+    }
     w.graw = cv.take(Mc);
     w.Gdtmp = cv.take(Mc * d.Evp);
     w.Gdenc = cv.take((size_t)nrc * d.Evp);
@@ -581,12 +586,13 @@ static size_t carve(const SimtDims& d, bool tc, int nrc, int S, int mode, char* 
   if (tc && (mode == 1 || mode == 2)) {
     for (TcImage& g : w.Grow) g = cv.image((int)Mc, d.W);
     for (TcImage& g : w.Gtr) g = cv.image(d.W, (int)Mc);
+    w.ghid_row = cv.image((int)Mc, d.HW);
+    w.ghid_tr = cv.image(d.HW, (int)Mc);
   }
   if (tc) {     // largest operand images: [max(Mc, width) x (W + encoding)] forward, [width x Mc] weight gradient
     const int wmax = std::max(std::max(d.W, d.HW), std::max(d.E3p, d.Evp));
     w.pack_elems = std::max(tc_pack_elems((int)Mc, ceil_div(wmax, 32) + ceil_div(std::max(d.E3p, d.Evp), 32), wmax),
                             tc_pack_elems(wmax, ceil_div((long long)Mc, 32), 0));
-    w.pack_a = reinterpret_cast<uint16_t*>(cv.take((w.pack_elems + 1) / 2));
     w.pack_b = reinterpret_cast<uint16_t*>(cv.take((w.pack_elems + 1) / 2));
   }
   if (out) *out = w;
@@ -595,13 +601,16 @@ static size_t carve(const SimtDims& d, bool tc, int nrc, int S, int mode, char* 
 
 static bool uses_tc(int engine) { return engine_prec(engine).fwd.passes != 0; }
 
+// mode 0 is the size a forward call is given, taped or not: the larger of modes 0 and 3
 size_t simt_workspace_bytes(const SparfMLP* mlp, int R, int S, int mode, int engine) {
-  return carve(simt_dims(mlp), uses_tc(engine), std::min(R, chunk_rays(S, mode == 1 || mode == 2)), S, mode, nullptr, nullptr);
+  auto bytes = [&](int md) {
+    return carve(simt_dims(mlp), uses_tc(engine), std::min(R, chunk_rays(S, md)), S, md, nullptr, nullptr);
+  };
+  return mode == 0 ? std::max(bytes(0), bytes(3)) : bytes(mode);
 }
 
 static EnginePrec with_images(EnginePrec ep, const Ws& w) {
   for (TcPrec* p : {&ep.fwd, &ep.dgrad, &ep.wgrad}) {
-    p->pack_a = w.pack_a;
     p->pack_b = w.pack_b;
     p->pack_elems = w.pack_elems;
   }
@@ -737,7 +746,7 @@ int simt_mlp_forward_tape(const SparfMLP* mlp, int engine, int R, int S, const f
   }
   Tape tp;
   tape_layout(d, R, S, reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(tape), 256)), &tp);
-  const int nrc = std::min(R, chunk_rays(S, 0));
+  const int nrc = std::min(R, chunk_rays(S, 3));
   Ws w;
   carve(d, uses_tc(engine), nrc, S, 3, reinterpret_cast<char*>(workspace), &w);
   const EnginePrec ep = with_images(engine_prec(engine), w);
@@ -793,7 +802,7 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
   }
   SimtDims d = simt_dims(mlp);
   const bool need_rays = d_origins != nullptr || d_dirs != nullptr;
-  const int nrc = std::min(R, chunk_rays(S, 1));
+  const int nrc = std::min(R, chunk_rays(S, mode));
   Ws w;
   carve(d, uses_tc(engine), nrc, S, mode, reinterpret_cast<char*>(workspace), &w);
   const EnginePrec ep = with_images(engine_prec(engine), w);
@@ -829,18 +838,10 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
     }
     const int slab = 2048;  // rows per SIMT wgrad slab (the tensor-core GEMMs choose their own k-ranges)
 
-    head_grad_kernel<<<ceil_div(Mc, 256), 256, 0, st>>>(Mc, d_rgb + m0 * 3, rgbv, d_sigma + m0, raw, nullptr, gpre, graw);
-    LAUNCH_OK("head_grad_kernel");
-    // colour head, layer 1 (HW -> 3)
-    narrow_wgrad_kernel<3><<<ceil_div(Mc, 512), 128, 0, st>>>(Mc, d.HW, 512, gpre, 4, hid, d.HW, grad->head_w[1], d.HW, grad->head_b[1]);
-    LAUNCH_OK("narrow_wgrad_kernel<3>");
-    narrow_dgrad_kernel<<<ceil_div(Mc * d.HW, 256), 256, 0, st>>>(Mc * d.HW, d.HW, gpre, mlp->head_w[1], d.HW, hid, Ghid);
-    LAUNCH_OK("narrow_dgrad_kernel");
-    // colour head, layer 0 ([feat | denc] -> HW)
     const int ldw8 = d.W + d.Ev;
     float* feat = H[d.nt - 1];
     // tensor cores: the trunk gradients G leave each input-gradient GEMM as images (gout(i) = ping-pong buffer i), with the
-    // bias gradient of the layer that produced them; pack_a holds Ghid's image
+    // bias gradient of the layer that produced them; the colour-head gradient Ghid leaves tc_head_backward as images
     auto gtr = [&](int i) { return TcImage{w.Gtr[i].p, ceil_div(Mc, 32)}; };   // K = this chunk's rows
     auto gout = [&](int i) {
       TcOut o;
@@ -850,28 +851,36 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
       o.tr_passes = ep.wgrad.passes;
       return o;
     };
-    const TcImage ghid_t{w.pack_a, ceil_div(Mc, 32)}, ghid{w.pack_a, ceil_div(d.HW, 32)};
+    const TcImage ghid_t{w.ghid_tr.p, ceil_div(Mc, 32)}, ghid = w.ghid_row;
     if (tc) {
-      SPARF_TRY(tc_pack_cols(ep.wgrad, (int)Mc, d.HW, Ghid, d.HW, ghid_t, st));
+      // colour head, layer 1 (HW -> 3) and the head's gradients: one kernel, Ghid as images; layer 0 ([feat | denc] -> HW)
+      SPARF_TRY(tc_head_backward(ep.dgrad, ep.wgrad, (int)Mc, d.HW, d_rgb + m0 * 3, rgbv, d_sigma + m0, raw, hid, mlp->head_w[1],
+                                 graw, ghid, ghid_t, grad->head_w[1], grad->head_b[1], grad->head_b[0], grad->trunk_b[d.nt - 1],
+                                 st));
       SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.W, d.W, ghid_t, feat, d.W, 1, grad->head_w[0], ldw8, 0, st));
       SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.Evp, d.Ev, ghid_t, denc, d.Evp, S, grad->head_w[0], ldw8, d.W, st));
+      SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.HW, d.W, d.W, ghid, mlp->head_w[0], ldw8, 0, feat, d.W, nullptr, nullptr,
+                           nullptr, 0, 0, gout(0), grad->trunk_b[d.nt - 1] + 1, nullptr, st));
     } else {
+      head_grad_kernel<<<ceil_div(Mc, 256), 256, 0, st>>>(Mc, d_rgb + m0 * 3, rgbv, d_sigma + m0, raw, nullptr, gpre, graw);
+      LAUNCH_OK("head_grad_kernel");
+      // colour head, layer 1 (HW -> 3)
+      narrow_wgrad_kernel<3><<<ceil_div(Mc, 512), 128, 0, st>>>(Mc, d.HW, 512, gpre, 4, hid, d.HW, grad->head_w[1], d.HW,
+                                                                 grad->head_b[1]);
+      LAUNCH_OK("narrow_wgrad_kernel<3>");
+      narrow_dgrad_kernel<<<ceil_div(Mc * d.HW, 256), 256, 0, st>>>(Mc * d.HW, d.HW, gpre, mlp->head_w[1], d.HW, hid, Ghid);
+      LAUNCH_OK("narrow_dgrad_kernel");
+      // colour head, layer 0 ([feat | denc] -> HW)
       SPARF_TRY(gemm_tn((int)Mc, d.HW, d.W, d.W, slab, Ghid, d.HW, feat, d.W, 1, grad->head_w[0], ldw8, 0, st));
       SPARF_TRY(gemm_tn((int)Mc, d.HW, d.Evp, d.Ev, slab, Ghid, d.HW, denc, d.Evp, S, grad->head_w[0], ldw8, d.W, st));
-    }
-    colsum_kernel<<<dim3(ceil_div(d.HW, 32), ceil_div(Mc, 1024)), 256, 0, st>>>(Mc, d.HW, 1024, Ghid, d.HW, grad->head_b[0]);
-    LAUNCH_OK("colsum_kernel(head)");
-    if (tc) {
-      SPARF_TRY(tc_pack_rows(ep.dgrad, (int)Mc, d.HW, Ghid, d.HW, 1, ghid, st));
-      SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.HW, d.W, d.W, ghid, mlp->head_w[0], ldw8, 0, feat, d.W, nullptr, nullptr,
-                           nullptr, 0, 0, gout(0), grad->trunk_b[d.nt - 1] + 1, st));
-    } else {
+      colsum_kernel<<<dim3(ceil_div(d.HW, 32), ceil_div(Mc, 1024)), 256, 0, st>>>(Mc, d.HW, 1024, Ghid, d.HW, grad->head_b[0]);
+      LAUNCH_OK("colsum_kernel(head)");
       SPARF_TRY(gemm_nn((int)Mc, d.HW, d.W, d.W, Ghid, d.HW, mlp->head_w[0], ldw8, 0, feat, d.W, nullptr, nullptr, G0, d.W, 0, st));
     }
     if (d_dirs) {
       if (tc)
         SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.HW, d.Evp, d.Ev, ghid, mlp->head_w[0], ldw8, d.W, nullptr, 0, nullptr, nullptr,
-                             Gdtmp, d.Evp, 0, TcOut{}, nullptr, st));
+                             Gdtmp, d.Evp, 0, TcOut{}, nullptr, nullptr, st));
       else
         SPARF_TRY(gemm_nn((int)Mc, d.HW, d.Evp, d.Ev, Ghid, d.HW, mlp->head_w[0], ldw8, d.W, nullptr, 0, nullptr, nullptr, Gdtmp,
                           d.Evp, 0, st));
@@ -903,13 +912,14 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
         colsum_kernel<<<dim3(ceil_div(d.W, 32), ceil_div(Mc, 1024)), 256, 0, st>>>(Mc, d.W, 1024, G, d.W, grad->trunk_b[l] + rowoff);
         LAUNCH_OK("colsum_kernel(trunk)");
       }
-      if (last) {
+      if (last && !tc) {
         narrow_wgrad_kernel<1><<<ceil_div(Mc, 512), 128, 0, st>>>(Mc, d.W, 512, graw, 1, in, d.W, grad->trunk_w[l], ldw, grad->trunk_b[l]);
         LAUNCH_OK("narrow_wgrad_kernel<1>");
       }
-      if (l > 0 && tc) {
+      if (l > 0 && tc) {        // last layer: its epilogue also sums the density row's weight gradient (bias: tc_head_backward)
         SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.W, d.W, w.Grow[gi], Wl, ldw, 0, in, d.W, last ? graw : nullptr,
-                             last ? mlp->trunk_w[l] : nullptr, nullptr, 0, 0, gout(gi ^ 1), grad->trunk_b[l - 1], st));
+                             last ? mlp->trunk_w[l] : nullptr, nullptr, 0, 0, gout(gi ^ 1), grad->trunk_b[l - 1],
+                             last ? grad->trunk_w[l] : nullptr, st));
       } else if (l > 0) {
         SPARF_TRY(gemm_nn((int)Mc, d.W, d.W, d.W, G, d.W, Wl, ldw, 0, in, d.W, last ? graw : nullptr,
                           last ? mlp->trunk_w[l] : nullptr, Gn, d.W, 0, st));
@@ -917,7 +927,7 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
       if (need_rays && (l == d.skip || l == 0)) {
         if (tc)
           SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.E3p, d.E3, w.Grow[gi], Wl, ldw, l == 0 ? 0 : d.W, nullptr, 0, nullptr,
-                               nullptr, Genc, d.E3p, genc_written ? 1 : 0, TcOut{}, nullptr, st));
+                               nullptr, Genc, d.E3p, genc_written ? 1 : 0, TcOut{}, nullptr, nullptr, st));
         else
           SPARF_TRY(gemm_nn((int)Mc, d.W, d.E3p, d.E3, G, d.W, Wl, ldw, l == 0 ? 0 : d.W, nullptr, 0, nullptr, nullptr, Genc,
                             d.E3p, genc_written ? 1 : 0, st));
@@ -936,4 +946,40 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
   return SPARF_OK;
 }
 
+// tc_head_backward and the path it replaced (head_grad_kernel, narrow_dgrad_kernel's fp32 Ghid, then tc_pack_rows /
+// tc_pack_cols) on the same inputs; scratch = Ghid [M x HW], gpre [M x 4], the fused kernel's sums [4 HW + 4]
+static int selftest_head(const float* d_rgb, const float* rgb, const float* d_sigma, const float* raw, const float* hid,
+                         const float* W9, int M, int HW, TcPrec dg, TcPrec wg, uint16_t* img, float* graw, float* scratch,
+                         cudaStream_t st) {
+  const size_t nrow = tc_image_elems(M, HW), ntr = tc_image_elems(HW, M);
+  const TcImage row{img, ceil_div(HW, 32)}, tr{img + nrow, ceil_div(M, 32)};
+  const TcImage row_ref{img + nrow + ntr, row.ks}, tr_ref{img + 2 * nrow + ntr, tr.ks};
+  float *Ghid = scratch, *gpre = Ghid + (size_t)M * HW, *sums = gpre + (size_t)M * 4;
+  SPARF_CHECK_CUDA(cudaMemsetAsync(img, 0xFF, 2 * (nrow + ntr) * sizeof(uint16_t), st));
+  SPARF_CHECK_CUDA(cudaMemsetAsync(sums, 0, (4 * HW + 4) * sizeof(float), st));
+  SPARF_TRY(tc_head_backward(dg, wg, M, HW, d_rgb, rgb, d_sigma, raw, hid, W9, graw, row, tr, sums, sums + 3 * HW,
+                             sums + 3 * HW + 3, sums + 4 * HW + 3, st));
+  head_grad_kernel<<<ceil_div(M, 256), 256, 0, st>>>(M, d_rgb, rgb, d_sigma, raw, nullptr, gpre, graw + M);
+  LAUNCH_OK("head_grad_kernel");
+  narrow_dgrad_kernel<<<ceil_div((long long)M * HW, 256), 256, 0, st>>>((long long)M * HW, HW, gpre, W9, HW, hid, Ghid);
+  LAUNCH_OK("narrow_dgrad_kernel");
+  SPARF_TRY(tc_pack_rows(dg, M, HW, Ghid, HW, 1, row_ref, st));
+  return tc_pack_cols(wg, M, HW, Ghid, HW, tr_ref, st);
+}
+
 }  // namespace sparf
+
+using namespace sparf;
+
+extern "C" int sparf_tc_selftest_head(const float* d_rgb, const float* rgb, const float* d_sigma, const float* raw,
+                                      const float* hid, const float* W9, int32_t M, int32_t HW, int32_t row_passes,
+                                      int32_t tr_passes, uint16_t* img, float* graw, sparf_stream_t stream) {
+  SPARF_REQUIRE(M >= 1 && M <= (1 << 20) && HW >= 8 && HW <= 512 && HW % 8 == 0, "tc_selftest_head: M=%d HW=%d", M, HW);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* scratch = nullptr;
+  SPARF_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch), ((size_t)M * (HW + 4) + 4 * HW + 4) * sizeof(float), st));
+  const int rc = selftest_head(d_rgb, rgb, d_sigma, raw, hid, W9, M, HW, TcPrec{false, row_passes}, TcPrec{false, tr_passes},
+                               img, graw, scratch, st);
+  cudaFreeAsync(scratch, st);
+  return rc;
+}
