@@ -169,6 +169,23 @@ int sparf_mlp_backward_tape(const SparfMLP* mlp, int32_t engine, int32_t R, int3
                             float* d_dirs, void* tape, size_t tape_bytes, void* workspace, size_t workspace_bytes,
                             sparf_stream_t stream);
 
+/* ---------------------------------------------------------------- density queries
+ * NeRF.compute_raw_density (frequency_nerf.py:149-170): the trunk alone at M arbitrary points [M,3] (x = p; no view
+ * direction, no colour head).  Outputs raw [M], the density row before the softplus, without noise, and, when feat is
+ * not NULL, feat [M,width] = relu of the last trunk layer's feature rows.  The BARF mask applies as in the MLP entry
+ * points.  These calls read no head tensor: SparfMLP.head_* and SparfMLPGrad.head_* may be NULL.  M may exceed 2^31;
+ * M = 0 is a no-op.  Engines as for the MLP (AUTO: TC_3X on sm_90, else SIMT_FP32).
+ * sparf_density_workspace_bytes: `backward` = 0 sparf_density_forward, 1 sparf_density_backward.  A forward without
+ * feat skips the last layer's feature GEMM (the density row reads the layer below). */
+size_t sparf_density_workspace_bytes(const SparfMLP* mlp, int64_t M, int32_t backward, int32_t engine);
+int sparf_density_forward(const SparfMLP* mlp, int32_t engine, int64_t M, const float* points, float* raw, float* feat,
+                          void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+/* Backward of the above (recomputes the forward).  d_raw [M] and d_feat [M,width] may each be NULL (a zero gradient).
+ * Trunk parameter gradients (+=) into grad's trunk fields and, when non-NULL, d_points [M,3] (+=). */
+int sparf_density_backward(const SparfMLP* mlp, int32_t engine, int64_t M, const float* points, const float* d_raw,
+                           const float* d_feat, const SparfMLPGrad* grad, float* d_points, void* workspace,
+                           size_t workspace_bytes, sparf_stream_t stream);
+
 /* ---------------------------------------------------------------- compositing
  * NeRF.composite (frequency_nerf.py:283-343).  Outputs: rgb_map [R,3], depth/opacity/depth_var/rgb_var
  * [R], weights [R,S], all_cumulated [R] (= T at sample S-2).  white_bg: rgb += 1 - opacity.
@@ -244,6 +261,14 @@ int sparf_tc_selftest_persistent(const float* X, const float* W1, const float* E
 int sparf_tc_selftest_head(const float* d_rgb, const float* rgb, const float* d_sigma, const float* raw, const float* hid,
                            const float* W9, int32_t M, int32_t HW, int32_t row_passes, int32_t tr_passes, uint16_t* img,
                            float* graw, sparf_stream_t stream);
+/* The density backward's last-layer kernel of the tensor-core engines against masking in fp32, packing and summing, on
+ * the same inputs: d_raw [M], d_feat, feat [M,W]; M in [1, 2^20], W a multiple of 8 in [8, 512].  img gets, each after
+ * a fill with 0xFFFF, four bf16 images (row_passes / tr_passes: 1 or 3): the kernel's row image of G = (feat > 0) *
+ * d_feat (ceil(M/128) * ceil(W/32) * 8192 elements) and its transposed image (ceil(W/128) * ceil(M/32) * 8192), then
+ * the same two packed from the fp32 G.  sums [2, W+1] (zeroed first): the kernel's sum of d_raw and column sums of G,
+ * then colsum_kernel's.  The images must be bit-identical; the sums are where the inputs sum exactly in any order. */
+int sparf_tc_selftest_featgrad(const float* d_raw, const float* d_feat, const float* feat, int32_t M, int32_t W,
+                               int32_t row_passes, int32_t tr_passes, uint16_t* img, float* sums, sparf_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -51,6 +51,10 @@ _SIGNATURES = {
                                          _P, c_size_t, _P]),
     "sparf_mlp_backward_tape": (c_int32, [POINTER(SparfMLP), c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, _P, _P,
                                           POINTER(SparfMLPGrad), _P, _P, _P, c_size_t, _P, c_size_t, _P]),
+    "sparf_density_workspace_bytes": (c_size_t, [POINTER(SparfMLP), c_int64, c_int32, c_int32]),
+    "sparf_density_forward": (c_int32, [POINTER(SparfMLP), c_int32, c_int64, _P, _P, _P, _P, c_size_t, _P]),
+    "sparf_density_backward": (c_int32, [POINTER(SparfMLP), c_int32, c_int64, _P, _P, _P, POINTER(SparfMLPGrad), _P, _P,
+                                         c_size_t, _P]),
     "sparf_composite_forward": (c_int32, [c_int32, c_int32, _P, _P, _P, _P, c_int32, _P, _P, _P, _P, _P, _P, _P, _P]),
     "sparf_composite_backward": (c_int32, [c_int32, c_int32, _P, _P, _P, _P, c_int32, _P, _P, _P, _P, _P, _P, _P, _P]),
     "sparf_huber2_fwd_bwd": (c_int32, [c_int64, _P, _P, c_float, _P, _P, _P]),
@@ -63,6 +67,7 @@ _SIGNATURES = {
     "sparf_tc_selftest_images": (c_int32, [_P, _P, _P, _P, c_int32, _P, _P, _P, _P]),
     "sparf_tc_selftest_persistent": (c_int32, [_P, _P, _P, _P, c_int32, _P, _P, _P, c_int32, _P]),
     "sparf_tc_selftest_head": (c_int32, [_P, _P, _P, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, _P, _P, _P]),
+    "sparf_tc_selftest_featgrad": (c_int32, [_P, _P, _P, c_int32, c_int32, c_int32, c_int32, _P, _P, _P]),
 }
 
 _lib = None

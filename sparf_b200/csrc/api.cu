@@ -97,6 +97,42 @@ extern "C" int sparf_mlp_backward(const SparfMLP* mlp, int32_t engine, int32_t R
                            workspace_bytes, (cudaStream_t)stream);
 }
 
+// ---------------------------------------------------------------- density queries: the trunk alone at arbitrary points
+extern "C" size_t sparf_density_workspace_bytes(const SparfMLP* mlp, int64_t M, int32_t backward, int32_t engine) {
+  if (!mlp || M <= 0) return 0;
+  const int e = resolve_engine(mlp, engine);
+  if (e < 0 || backward < 0 || backward > 1) return 0;
+  return simt_density_workspace_bytes(mlp, M, backward, e);
+}
+
+extern "C" int sparf_density_forward(const SparfMLP* mlp, int32_t engine, int64_t M, const float* points, float* raw,
+                                     float* feat, void* workspace, size_t workspace_bytes, sparf_stream_t stream) {
+  SPARF_REQUIRE(mlp && M >= 0, "density_forward: bad arguments");
+  if (M == 0) return SPARF_OK;
+  SPARF_REQUIRE(points && raw, "density_forward: NULL tensor");
+  const int e = resolve_engine(mlp, engine);
+  if (e < 0) {
+    set_error("density_forward: engine %d not available in this build", engine);
+    return SPARF_ERR_UNSUPPORTED;
+  }
+  return simt_density_forward(mlp, e, M, points, raw, feat, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int sparf_density_backward(const SparfMLP* mlp, int32_t engine, int64_t M, const float* points, const float* d_raw,
+                                      const float* d_feat, const SparfMLPGrad* grad, float* d_points, void* workspace,
+                                      size_t workspace_bytes, sparf_stream_t stream) {
+  SPARF_REQUIRE(mlp && M >= 0, "density_backward: bad arguments");
+  if (M == 0) return SPARF_OK;
+  SPARF_REQUIRE(points && grad, "density_backward: NULL tensor");
+  const int e = resolve_engine(mlp, engine);
+  if (e < 0) {
+    set_error("density_backward: engine %d not available in this build", engine);
+    return SPARF_ERR_UNSUPPORTED;
+  }
+  return simt_density_backward(mlp, e, M, points, d_raw, d_feat, grad, d_points, workspace, workspace_bytes,
+                               (cudaStream_t)stream);
+}
+
 // ---------------------------------------------------------------- tape variants: the training forward keeps what the
 // backward needs, so that the backward does not recompute the forward
 extern "C" size_t sparf_mlp_tape_bytes(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S) {

@@ -7,6 +7,7 @@
 //   pack: splits an fp32 operand (with the GEMM's own indexing: transposes, per-ray rows, bounds) into an image; the
 //     weights and the encodings take this path;
 //   head backward: the colour head's narrow layer, whose gradient it writes straight into its two images;
+//   feature backward: the last trunk layer's gradient of a density query, (feat > 0) * d_feat, likewise;
 //   gemm: persistent, one CTA per SM walking 128 x 128 output tiles (the weight gradient: tiles x k-ranges).  A
 //     producer thread streams the tiles of both operands with cp.async.bulk into a STAGES-deep ring of shared-memory
 //     stages that runs on across tiles, each stage completing on its "full" mbarrier (complete_tx); two consumer
@@ -213,6 +214,50 @@ __device__ __forceinline__ void split8(const float (&v)[8], uint4& hi, uint4& lo
   lo = make_uint4(l[0] | (uint32_t)l[1] << 16, l[2] | (uint32_t)l[3] << 16, l[4] | (uint32_t)l[5] << 16, l[6] | (uint32_t)l[7] << 16);
 }
 
+// The images of the column block n0 of a 128-row tile (rows blockIdx.x * 128 + r) whose fp32 values are in V
+// [TM][HB_LD]: row image (rows m, k = n, ROWP passes) and transposed image (rows n, k = m, TRP passes).  16-byte chunk c
+// of a tile half is row c & 7 of core matrix c >> 3 (eight consecutive k), so consecutive threads write consecutive 16
+// bytes.
+template <int ROWP, int TRP>
+__device__ __forceinline__ void store_block_images(const float* V, int n0, uint16_t* row, int row_ks, uint16_t* tr,
+                                                   int tr_ks) {
+  const int tid = threadIdx.x;
+#pragma unroll
+  for (int kq = 0; kq < 4; ++kq) {
+    const int kt = (n0 >> 5) + kq;      // row image: rows m, k = n
+    if (kt >= row_ks) break;
+    uint16_t* t = row + ((size_t)blockIdx.x * row_ks + kt) * 2 * TILE_ELEMS;
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      const int c = tid + 256 * s, core = c >> 3, r = (core >> 2) * 8 + (c & 7), k = kq * 32 + (core & 3) * 8;
+      float v[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) v[e] = V[r * HB_LD + k + e];
+      uint4 hi, lo;
+      split8(v, hi, lo);
+      reinterpret_cast<uint4*>(t)[c] = hi;
+      if (ROWP == 3) reinterpret_cast<uint4*>(t + TILE_ELEMS)[c] = lo;
+    }
+  }
+#pragma unroll
+  for (int kq = 0; kq < 4; ++kq) {
+    const int kt = blockIdx.x * (TM / TK) + kq;   // transposed image: rows n (row tile n0 / 128), k = m
+    if (kt >= tr_ks) break;
+    uint16_t* t = tr + ((size_t)(n0 / TN) * tr_ks + kt) * 2 * TILE_ELEMS;
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      const int c = tid + 256 * s, core = c >> 3, r = (core >> 2) * 8 + (c & 7), k = kq * 32 + (core & 3) * 8;
+      float v[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) v[e] = V[(k + e) * HB_LD + r];
+      uint4 hi, lo;
+      split8(v, hi, lo);
+      reinterpret_cast<uint4*>(t)[c] = hi;
+      if (TRP == 3) reinterpret_cast<uint4*>(t + TILE_ELEMS)[c] = lo;
+    }
+  }
+}
+
 template <int ROWP, int TRP>
 __global__ void __launch_bounds__(256) head_bwd_kernel(const HeadBwd p) {
   extern __shared__ __align__(16) float hsm[];
@@ -299,42 +344,79 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(const HeadBwd p) {
       for (int w = 0; w < 8; ++w) v += red[(w * 16 + k) * 32 + l];
       if (col < p.HW) atomicAdd(k < 4 ? p.db_hid + col : p.dW9 + (size_t)((k - 4) >> 2) * p.HW + col, v);
     }
-    // images: 16-byte chunk c of a tile half is row c & 7 of core matrix c >> 3 (eight consecutive k), so consecutive
-    // threads write consecutive 16 bytes
+    store_block_images<ROWP, TRP>(V, n0, p.row, p.row_ks, p.tr, p.tr_ks);
+  }
+}
+
+// The last trunk layer's gradient when the caller gives it (sparf_density_backward), one CTA per 128-row tile:
+//   G[m][n] = (feat[m][n] > 0) * d_feat[m][n]      (d_feat NULL: G = 0)
+// G leaves only as its row image (dgrad passes) and its transposed image (wgrad passes), split from the same fp32 values
+// as pack_kernel would split them, zero past M and W.  Per CTA, one atomic per output: db_feat += the column sums of G,
+// db_raw[0] += sum d_raw (d_raw may be NULL).
+struct FeatBwd {
+  int M, W;
+  const float *d_raw, *d_feat, *feat;
+  uint16_t *row, *tr;
+  int row_ks, tr_ks;
+  float *db_raw, *db_feat;
+  bool vec;                 // d_feat 16-byte aligned: 16-byte loads
+};
+
+constexpr int FEAT_SMEM = (TM * HB_LD + 8 * 4 * 32 + 4) * 4;
+
+template <int ROWP, int TRP>
+__global__ void __launch_bounds__(256) feat_bwd_kernel(const FeatBwd p) {
+  extern __shared__ __align__(16) float fsm[];
+  float* V = fsm;                           // [TM][HB_LD] G of this tile's rows, one column block at a time
+  float* red = V + TM * HB_LD;              // [8 warps][4 columns per lane][32 lanes]
+  float* rsum = red + 8 * 4 * 32;           // [4 warps]: sums of d_raw
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int m0 = blockIdx.x * TM;
+  if (p.d_raw && tid < TM) {
+    float s = m0 + tid < p.M ? p.d_raw[m0 + tid] : 0.f;
 #pragma unroll
-    for (int kq = 0; kq < 4; ++kq) {
-      const int kt = (n0 >> 5) + kq;      // row image: rows m, k = n
-      if (kt >= p.row_ks) break;
-      uint16_t* t = p.row + ((size_t)blockIdx.x * p.row_ks + kt) * 2 * TILE_ELEMS;
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) rsum[warp] = s;
+  }
+  for (int n0 = 0; n0 < p.W; n0 += TN) {
+    __syncthreads();                        // rsum written; the previous column block's V and red read
+    if (n0 == 0 && tid == 0 && p.d_raw) atomicAdd(p.db_raw, rsum[0] + rsum[1] + rsum[2] + rsum[3]);
+    // columns n0 + 4 c4 + q of rows warp + 8 i, all loads issued first
+    const int c4 = lane, n = n0 + 4 * c4;
+    float4 x[16], g[16];
 #pragma unroll
-      for (int s = 0; s < 2; ++s) {
-        const int c = tid + 256 * s, core = c >> 3, r = (core >> 2) * 8 + (c & 7), k = kq * 32 + (core & 3) * 8;
-        float v[8];
+    for (int i = 0; i < 16; ++i) {
+      const int m = m0 + warp + 8 * i;
+      const bool in = p.d_feat && m < p.M && n < p.W;
+      const size_t o = (size_t)m * p.W + n;
+      x[i] = in ? *reinterpret_cast<const float4*>(p.feat + o) : make_float4(0.f, 0.f, 0.f, 0.f);
+      g[i] = !in ? make_float4(0.f, 0.f, 0.f, 0.f)
+                 : p.vec ? *reinterpret_cast<const float4*>(p.d_feat + o)
+                         : make_float4(p.d_feat[o], p.d_feat[o + 1], p.d_feat[o + 2], p.d_feat[o + 3]);
+    }
+    float cs[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-        for (int e = 0; e < 8; ++e) v[e] = V[r * HB_LD + k + e];
-        uint4 hi, lo;
-        split8(v, hi, lo);
-        reinterpret_cast<uint4*>(t)[c] = hi;
-        if (ROWP == 3) reinterpret_cast<uint4*>(t + TILE_ELEMS)[c] = lo;
+    for (int i = 0; i < 16; ++i) {
+      const int r = warp + 8 * i;
+      const float h[4] = {x[i].x, x[i].y, x[i].z, x[i].w}, d[4] = {g[i].x, g[i].y, g[i].z, g[i].w};
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const float v = h[q] > 0.f ? d[q] : 0.f;
+        V[r * HB_LD + 4 * c4 + q] = v;
+        cs[q] += v;
       }
     }
 #pragma unroll
-    for (int kq = 0; kq < 4; ++kq) {
-      const int kt = blockIdx.x * (TM / TK) + kq;   // transposed image: rows n (row tile n0 / 128), k = m
-      if (kt >= p.tr_ks) break;
-      uint16_t* t = p.tr + ((size_t)(n0 / TN) * p.tr_ks + kt) * 2 * TILE_ELEMS;
+    for (int q = 0; q < 4; ++q) red[(warp * 4 + q) * 32 + lane] = cs[q];
+    __syncthreads();
+    if (p.d_feat && tid < TM) {             // column n0 + 4 l + q, q = tid / 32, l = tid % 32
+      const int q = tid >> 5, col = n0 + 4 * lane + q;
+      float v = 0.f;
 #pragma unroll
-      for (int s = 0; s < 2; ++s) {
-        const int c = tid + 256 * s, core = c >> 3, r = (core >> 2) * 8 + (c & 7), k = kq * 32 + (core & 3) * 8;
-        float v[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) v[e] = V[(k + e) * HB_LD + r];
-        uint4 hi, lo;
-        split8(v, hi, lo);
-        reinterpret_cast<uint4*>(t)[c] = hi;
-        if (TRP == 3) reinterpret_cast<uint4*>(t + TILE_ELEMS)[c] = lo;
-      }
+      for (int w = 0; w < 8; ++w) v += red[(w * 4 + q) * 32 + lane];
+      if (col < p.W) atomicAdd(p.db_feat + col, v);
     }
+    store_block_images<ROWP, TRP>(V, n0, p.row, p.row_ks, p.tr, p.tr_ks);
   }
 }
 
@@ -860,6 +942,31 @@ int tc_head_backward(TcPrec dg, TcPrec wg, int M, int HW, const float* d_rgb, co
   if (dg.passes == 3 && wg.passes == 1) return launch_head_bwd<3, 1>(h, st);
   if (dg.passes == 1 && wg.passes == 1) return launch_head_bwd<1, 1>(h, st);
   SPARF_REQUIRE(false, "tc_head_backward: no kernel for %d-pass row and %d-pass transposed images", dg.passes, wg.passes);
+}
+
+template <int ROWP, int TRP>
+static int launch_feat_bwd(const FeatBwd& f, cudaStream_t st) {
+  auto kernel = feat_bwd_kernel<ROWP, TRP>;
+  SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FEAT_SMEM));
+  kernel<<<ceil_div(f.M, TM), 256, FEAT_SMEM, st>>>(f);
+  SPARF_CHECK_LAUNCH("feat_bwd_kernel");
+  return SPARF_OK;
+}
+
+int tc_feat_backward(TcPrec dg, TcPrec wg, int M, int W, const float* d_raw, const float* d_feat, const float* feat,
+                     TcImage row, TcImage tr, float* db_raw, float* db_feat, cudaStream_t st) {
+  SPARF_REQUIRE(!dg.f16 && !wg.f16 && (dg.passes == 1 || dg.passes == 3) && (wg.passes == 1 || wg.passes == 3),
+                "tc_feat_backward: bf16 1- or 3-pass images only");
+  SPARF_REQUIRE(M >= 1 && W % 4 == 0 && (!d_feat || (feat && !(reinterpret_cast<uintptr_t>(feat) & 15))),
+                "tc_feat_backward: M=%d W=%d", M, W);
+  SPARF_REQUIRE(row.p && row.ks == ceil_div(W, TK) && tr.p && tr.ks == ceil_div(M, TK),
+                "tc_feat_backward: images need %d and %d k-steps", ceil_div(W, TK), ceil_div(M, TK));
+  const FeatBwd f{M, W, d_raw, d_feat, feat, row.p, tr.p, row.ks, tr.ks, db_raw, db_feat,
+                  !(reinterpret_cast<uintptr_t>(d_feat) & 15)};
+  if (dg.passes == 3 && wg.passes == 3) return launch_feat_bwd<3, 3>(f, st);
+  if (dg.passes == 3 && wg.passes == 1) return launch_feat_bwd<3, 1>(f, st);
+  if (dg.passes == 1 && wg.passes == 1) return launch_feat_bwd<1, 1>(f, st);
+  SPARF_REQUIRE(false, "tc_feat_backward: no kernel for %d-pass row and %d-pass transposed images", dg.passes, wg.passes);
 }
 
 }  // namespace sparf

@@ -71,4 +71,11 @@ int tc_head_backward(TcPrec dg, TcPrec wg, int M, int HW, const float* d_rgb, co
                      const float* raw, const float* hid, const float* W9, float* graw, TcImage row, TcImage tr, float* dW9,
                      float* db9, float* db_hid, float* db_raw, cudaStream_t st);
 
+// The last trunk layer's gradient from the caller's d_raw [M] and d_feat [M,W] (each may be NULL: a zero gradient) and
+// the recomputed features feat [M,W] (16-byte aligned; may be NULL when d_feat is):  G = (feat > 0) * d_feat, written only
+// as its row image (dg passes) and its transposed image (wg passes), bit-identical to tc_pack_rows / tc_pack_cols of the
+// fp32 G; and db_feat[W] += the column sums of G, db_raw[0] += sum d_raw.
+int tc_feat_backward(TcPrec dg, TcPrec wg, int M, int W, const float* d_raw, const float* d_feat, const float* feat,
+                     TcImage row, TcImage tr, float* db_raw, float* db_feat, cudaStream_t st);
+
 }  // namespace sparf

@@ -4,6 +4,7 @@
 //     arithmetic, fp32 accumulate): the exact engine and the on-device cross-check of the tensor-core engines.
 //   SPARF_ENGINE_TC_3X / TC_1X / TC_3X_W1: the same orchestration with every wide GEMM on Hopper tensor cores
 //     (gemm_wgmma.cu); encoders, narrow layers and reductions are the shared CUDA-core kernels below.
+// The density queries (sparf_density_*) run the same trunk code at arbitrary points, without the colour head.
 //
 // Reference: NeRF.compute_raw_density / NeRF.forward (source/models/frequency_nerf.py:149-227),
 // FrequencyEmbedder (:47-69), positional_encoding (:229-258).
@@ -12,6 +13,12 @@
 #include "common.cuh"
 #include "gemm_wgmma.cuh"
 #include "mlp_simt.cuh"
+
+#define SPARF_TRY(expr)      \
+  do {                       \
+    int _rc = (expr);        \
+    if (_rc) return _rc;     \
+  } while (0)
 
 namespace sparf {
 
@@ -25,6 +32,7 @@ __global__ void c2f_weights_kernel(C2F c, int L_xyz, int L_view, float* __restri
 }
 
 // enc[m][0:3] = x = o + t*d ; enc[m][3 + c*2L + {0,L} + j] = w_j * {sin,cos}(x_c * 2^j pi) ; zero pad to E3p
+// dirs == NULL: the origins are the points themselves, x = o (S = 1; the value o + 0*d takes)
 __global__ void encode_xyz_kernel(long long total, int S, int L, int E3p, const float* __restrict__ origins,
                                   const float* __restrict__ dirs, const float* __restrict__ t,
                                   const float* __restrict__ wts, float* __restrict__ enc) {
@@ -36,7 +44,7 @@ __global__ void encode_xyz_kernel(long long total, int S, int L, int E3p, const 
   float val = 0.f;
   if (col < 3 + 6 * L) {
     int c = col < 3 ? col : (col - 3) / (2 * L);
-    float x = add_rn(origins[r * 3 + c], mul_rn(dirs[r * 3 + c], t[m]));  // camera.py:433-435
+    float x = dirs ? add_rn(origins[r * 3 + c], mul_rn(dirs[r * 3 + c], t[m])) : origins[r * 3 + c];  // camera.py:433-435
     if (col < 3) {
       val = x;
     } else {
@@ -268,12 +276,6 @@ static int gemm_tn(int M, int N, int K, int Kv, int rows_per_slab, const float* 
   return SPARF_OK;
 }
 
-#define SPARF_TRY(expr)      \
-  do {                       \
-    int _rc = (expr);        \
-    if (_rc) return _rc;     \
-  } while (0)
-
 EnginePrec engine_prec(int engine) {
   const TcPrec fp32{false, 0}, f16x3{true, 3}, f16x1{true, 1}, bf16x3{false, 3}, bf16x1{false, 1};
   switch (engine) {
@@ -398,6 +400,14 @@ __global__ void colsum_kernel(long long M, int N, int rows_per_block, const floa
   }
 }
 
+// G[i] = (feat[i] > 0) * d_feat[i]: the last trunk layer's gradient when the caller gives it (density backward)
+__global__ void relu_mask_kernel(long long total, const float* __restrict__ feat, const float* __restrict__ d_feat,
+                                 float* __restrict__ G) {
+  long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  G[idx] = feat[idx] > 0.f ? d_feat[idx] : 0.f;
+}
+
 // out[r][c] = sum_{k<S} in[(r*S+k)][c]
 __global__ void ray_reduce_kernel(int nrays, int S, int C, const float* __restrict__ in, float* __restrict__ out) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -410,6 +420,7 @@ __global__ void ray_reduce_kernel(int nrays, int S, int C, const float* __restri
 
 // positional-encoding backward + reduction over the ray:  d_o += sum_k g_x ; d_d += sum_k t_k g_x
 // d/dx [w sin(f x)] = f * (w cos(f x)) = f * enc_cos ; d/dx [w cos(f x)] = -f * enc_sin.  One warp per ray.
+// t == NULL (with d_d == NULL): the encoding of points (encode_xyz_kernel without dirs), d_o = the points' gradient.
 __global__ void posenc_bwd_kernel(int nrays, int S, int L, int E3p, const float* __restrict__ enc,
                                   const float* __restrict__ Genc, const float* __restrict__ t,
                                   float* __restrict__ d_o, float* __restrict__ d_d) {
@@ -421,7 +432,7 @@ __global__ void posenc_bwd_kernel(int nrays, int S, int L, int E3p, const float*
     size_t m = (size_t)r * S + k;
     const float* e = enc + m * E3p;
     const float* g = Genc + m * E3p;
-    float tk = t[m];
+    float tk = t ? t[m] : 0.f;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       float gx = g[c];
@@ -498,17 +509,22 @@ SimtDims simt_dims(const SparfMLP* mlp) {
   return d;
 }
 
-int simt_validate(const SparfMLP* mlp) {
+int simt_validate_trunk(const SparfMLP* mlp) {
   SPARF_REQUIRE(mlp != nullptr, "mlp is NULL");
   SPARF_REQUIRE(mlp->n_trunk >= 2 && mlp->n_trunk <= SPARF_MAX_TRUNK, "n_trunk=%d unsupported", mlp->n_trunk);
-  SPARF_REQUIRE(mlp->width % 8 == 0 && mlp->width >= 8 && mlp->head_width % 8 == 0 && mlp->head_width >= 8,
-                "width=%d / head_width=%d must be multiples of 8", mlp->width, mlp->head_width);
+  SPARF_REQUIRE(mlp->width % 8 == 0 && mlp->width >= 8, "width=%d must be a multiple of 8", mlp->width);
   SPARF_REQUIRE(mlp->L_xyz >= 1 && mlp->L_xyz <= SPARF_MAX_L && mlp->L_view >= 1 && mlp->L_view <= SPARF_MAX_L,
                 "L_xyz=%d / L_view=%d unsupported", mlp->L_xyz, mlp->L_view);
   SPARF_REQUIRE(mlp->skip_layer < mlp->n_trunk && mlp->skip_layer != 0, "skip_layer=%d unsupported", mlp->skip_layer);
   SPARF_REQUIRE(!mlp->use_c2f || mlp->progress, "use_c2f needs the progress pointer");
   for (int i = 0; i < mlp->n_trunk; ++i)
     SPARF_REQUIRE(mlp->trunk_w[i] && mlp->trunk_b[i], "trunk layer %d has NULL tensors", i);
+  return SPARF_OK;
+}
+
+int simt_validate(const SparfMLP* mlp) {
+  SPARF_TRY(simt_validate_trunk(mlp));
+  SPARF_REQUIRE(mlp->head_width % 8 == 0 && mlp->head_width >= 8, "head_width=%d must be a multiple of 8", mlp->head_width);
   SPARF_REQUIRE(mlp->head_w[0] && mlp->head_b[0] && mlp->head_w[1] && mlp->head_b[1], "head has NULL tensors");
   return SPARF_OK;
 }
@@ -540,7 +556,8 @@ struct Carver {
 // tape, 3: taped forward (the activations go to the tape).  Tensor-core engines keep their GEMM operands as images: the
 // forward's encodings and ping-pong trunk activations, the backward's ping-pong trunk gradients (a row image for the next
 // input gradient, a transposed one for the weight gradient; no fp32 copy), the colour-head gradient's two images (no fp32
-// copy either), and a buffer for the weight operand packed per GEMM.
+// copy either), and a buffer for the weight operand packed per GEMM.  head = false (density calls, S = 1): no colour-head
+// or view-direction buffer.
 struct Ws {
   float *wts, *enc, *denc, *hid, *raw, *rgbv, *G0, *G1, *Genc, *Ghid, *gpre, *graw, *Gdtmp, *Gdenc;
   float* H[SPARF_MAX_TRUNK];
@@ -549,17 +566,19 @@ struct Ws {
   size_t pack_elems;
 };
 
-static size_t carve(const SimtDims& d, bool tc, int nrc, int S, int mode, char* base, Ws* out) {
+static size_t carve(const SimtDims& d, bool tc, int nrc, int S, int mode, bool head, char* base, Ws* out) {
   const size_t Mc = (size_t)nrc * S;
   Carver cv{base, 0, 0};
   Ws w{};
   w.wts = cv.take(32);
   if (mode == 0 || mode == 1) {
     w.enc = cv.take(Mc * d.E3p);
-    w.denc = cv.take((size_t)nrc * d.Evp);
-    w.hid = cv.take(Mc * d.HW);
-    w.raw = cv.take(Mc);
-    w.rgbv = cv.take(Mc * 3);
+    if (head) {
+      w.denc = cv.take((size_t)nrc * d.Evp);
+      w.hid = cv.take(Mc * d.HW);
+      w.raw = cv.take(Mc);
+      w.rgbv = cv.take(Mc * 3);
+    }
     const int nH = mode == 0 ? 2 : d.nt;            // the forward ping-pongs, the backward keeps every layer
     for (int l = 0; l < nH; ++l) w.H[l] = cv.take(Mc * d.W);
     for (int l = nH; l < d.nt; ++l) w.H[l] = w.H[l & 1];
@@ -570,28 +589,33 @@ static size_t carve(const SimtDims& d, bool tc, int nrc, int S, int mode, char* 
   }
   if (mode == 1 || mode == 2) {
     w.Genc = cv.take(Mc * d.E3p);
-    if (!tc) {
+    if (!tc && head) {
       w.Ghid = cv.take(Mc * d.HW);
       w.gpre = cv.take(Mc * 4);
     }
-    w.graw = cv.take(Mc);
-    w.Gdtmp = cv.take(Mc * d.Evp);
-    w.Gdenc = cv.take((size_t)nrc * d.Evp);
+    if (head) {
+      w.graw = cv.take(Mc);
+      w.Gdtmp = cv.take(Mc * d.Evp);
+      w.Gdenc = cv.take((size_t)nrc * d.Evp);
+    }
   }
   if (tc && mode != 2) {
     w.encimg = cv.image((int)Mc, d.E3p);
-    w.dencimg = cv.image((int)Mc, d.Evp);
+    if (head) w.dencimg = cv.image((int)Mc, d.Evp);
     for (TcImage& h : w.Himg) h = cv.image((int)Mc, d.W);
   }
   if (tc && (mode == 1 || mode == 2)) {
     for (TcImage& g : w.Grow) g = cv.image((int)Mc, d.W);
     for (TcImage& g : w.Gtr) g = cv.image(d.W, (int)Mc);
-    w.ghid_row = cv.image((int)Mc, d.HW);
-    w.ghid_tr = cv.image(d.HW, (int)Mc);
+    if (head) {
+      w.ghid_row = cv.image((int)Mc, d.HW);
+      w.ghid_tr = cv.image(d.HW, (int)Mc);
+    }
   }
   if (tc) {     // largest operand images: [max(Mc, width) x (W + encoding)] forward, [width x Mc] weight gradient
-    const int wmax = std::max(std::max(d.W, d.HW), std::max(d.E3p, d.Evp));
-    w.pack_elems = std::max(tc_pack_elems((int)Mc, ceil_div(wmax, 32) + ceil_div(std::max(d.E3p, d.Evp), 32), wmax),
+    const int HW = head ? d.HW : 0, Evp = head ? d.Evp : 0;
+    const int wmax = std::max(std::max(d.W, HW), std::max(d.E3p, Evp));
+    w.pack_elems = std::max(tc_pack_elems((int)Mc, ceil_div(wmax, 32) + ceil_div(std::max(d.E3p, Evp), 32), wmax),
                             tc_pack_elems(wmax, ceil_div((long long)Mc, 32), 0));
     w.pack_b = reinterpret_cast<uint16_t*>(cv.take((w.pack_elems + 1) / 2));
   }
@@ -604,7 +628,7 @@ static bool uses_tc(int engine) { return engine_prec(engine).fwd.passes != 0; }
 // mode 0 is the size a forward call is given, taped or not: the larger of modes 0 and 3
 size_t simt_workspace_bytes(const SparfMLP* mlp, int R, int S, int mode, int engine) {
   auto bytes = [&](int md) {
-    return carve(simt_dims(mlp), uses_tc(engine), std::min(R, chunk_rays(S, md)), S, md, nullptr, nullptr);
+    return carve(simt_dims(mlp), uses_tc(engine), std::min(R, chunk_rays(S, md)), S, md, true, nullptr, nullptr);
   };
   return mode == 0 ? std::max(bytes(0), bytes(3)) : bytes(mode);
 }
@@ -625,26 +649,28 @@ static inline int trunk_ldw(const SimtDims& d, int l) {
 
 #define LAUNCH_OK(name) SPARF_CHECK_LAUNCH(name)
 
-// forward through the MLP for one chunk.  H: array of nt activation buffers (may alias in pairs when
-// !keep), raw may be NULL.  The tensor-core engines pack the encodings once and chain the trunk layers through the row
-// images their epilogues write (w's image buffers).
-static int simt_chunk_forward(const SparfMLP* mlp, const EnginePrec& ep, const SimtDims& d, int nr, int S, const float* origins,
-                              const float* dirs, const float* t, const float* noise, float* wts, float* enc,
-                              float* denc, float** H, float* raw, float* hid, float* sigma, float* rgb, const Ws& w,
-                              cudaStream_t st) {
-  const long long Mc = (long long)nr * S;
+// c2f weights and the point encoding of one chunk of Mc rows (rows r * S + k; dirs == NULL: origins are the points,
+// S = 1), and on the tensor cores its operand image
+static int chunk_encode_xyz(const SparfMLP* mlp, const EnginePrec& ep, const SimtDims& d, long long Mc, int S,
+                            const float* origins, const float* dirs, const float* t, float* wts, float* enc, const Ws& w,
+                            cudaStream_t st) {
   C2F c2f{mlp->use_c2f, mlp->c2f_start, mlp->c2f_range, mlp->progress};
   c2f_weights_kernel<<<1, 32, 0, st>>>(c2f, mlp->L_xyz, mlp->L_view, wts);
   LAUNCH_OK("c2f_weights_kernel");
   encode_xyz_kernel<<<ceil_div(Mc * d.E3p, 256), 256, 0, st>>>(Mc * d.E3p, S, mlp->L_xyz, d.E3p, origins, dirs, t, wts, enc);
   LAUNCH_OK("encode_xyz_kernel");
-  encode_dir_kernel<<<ceil_div((long long)nr * d.Evp, 256), 256, 0, st>>>(nr * d.Evp, mlp->L_view, d.Evp, dirs, wts + 16, denc);
-  LAUNCH_OK("encode_dir_kernel");
+  if (ep.fwd.passes != 0) SPARF_TRY(tc_pack_rows(ep.fwd, (int)Mc, d.E3p, enc, d.E3p, 1, w.encimg, st));
+  return SPARF_OK;
+}
+
+// trunk layers 0 ... nt-1 of one chunk from its encoding.  H: array of nt activation buffers (may alias in pairs when
+// !keep); H[nt-1] == NULL skips the last layer's feature GEMM (the density row reads H[nt-2] only).  raw (the softplus
+// argument, noise added) and sigma may be NULL; both NULL skips the density row.  The tensor-core engines chain the
+// layers through the row images their epilogues write (w's image buffers); last_image: the last layer's too (the colour
+// head reads it).
+static int chunk_trunk(const SparfMLP* mlp, const EnginePrec& ep, const SimtDims& d, long long Mc, const float* enc,
+                       float** H, const float* noise, float* raw, float* sigma, bool last_image, const Ws& w, cudaStream_t st) {
   const bool tc = ep.fwd.passes != 0;
-  if (tc) {
-    SPARF_TRY(tc_pack_rows(ep.fwd, (int)Mc, d.E3p, enc, d.E3p, 1, w.encimg, st));
-    SPARF_TRY(tc_pack_rows(ep.fwd, (int)Mc, d.Evp, denc, d.Evp, S, w.dencimg, st));
-  }
   const float* in = enc;
   for (int l = 0; l < d.nt; ++l) {
     const bool last = l == d.nt - 1;
@@ -652,22 +678,40 @@ static int simt_chunk_forward(const SparfMLP* mlp, const EnginePrec& ep, const S
     const float* Wl = mlp->trunk_w[l] + (last ? ldw : 0);  // last layer: row 0 is the density row
     const float* bl = mlp->trunk_b[l] + (last ? 1 : 0);
     const bool sk = l == d.skip;
-    if (tc) {
+    if (tc && H[l]) {
       TcOut o;
-      o.row = w.Himg[l & 1];
-      o.row_passes = ep.fwd.passes;
+      if (!last || last_image) {
+        o.row = w.Himg[l & 1];
+        o.row_passes = ep.fwd.passes;
+      }
       SPARF_TRY(tc_gemm_nt(ep.fwd, 1, (int)Mc, d.W, l == 0 ? w.encimg : w.Himg[(l - 1) & 1], trunk_in_main_valid(d, l),
                            sk ? w.encimg : TcImage{}, d.E3, Wl, ldw, d.W, bl, H[l], d.W, o, st));
-    } else {
+    } else if (H[l]) {
       SPARF_TRY(gemm_nt((int)Mc, d.W, in, trunk_in_main(d, l), trunk_in_main(d, l), trunk_in_main_valid(d, l),
                         sk ? enc : nullptr, d.E3p, d.E3p, d.E3, 1, Wl, ldw, d.W, bl, H[l], d.W, st));
     }
-    if (last) {
+    if (last && (raw || sigma)) {
       rowdot_kernel<0><<<ceil_div(Mc, 8), 256, 0, st>>>(Mc, d.W, in, d.W, mlp->trunk_w[l], ldw, mlp->trunk_b[l], noise, raw, sigma);
       LAUNCH_OK("rowdot_kernel<0>");
     }
     in = H[l];
   }
+  return SPARF_OK;
+}
+
+// forward through the MLP for one chunk.  H: array of nt activation buffers (may alias in pairs when
+// !keep), raw may be NULL.  The tensor-core engines pack the encodings once.
+static int simt_chunk_forward(const SparfMLP* mlp, const EnginePrec& ep, const SimtDims& d, int nr, int S, const float* origins,
+                              const float* dirs, const float* t, const float* noise, float* wts, float* enc,
+                              float* denc, float** H, float* raw, float* hid, float* sigma, float* rgb, const Ws& w,
+                              cudaStream_t st) {
+  const long long Mc = (long long)nr * S;
+  SPARF_TRY(chunk_encode_xyz(mlp, ep, d, Mc, S, origins, dirs, t, wts, enc, w, st));
+  encode_dir_kernel<<<ceil_div((long long)nr * d.Evp, 256), 256, 0, st>>>(nr * d.Evp, mlp->L_view, d.Evp, dirs, wts + 16, denc);
+  LAUNCH_OK("encode_dir_kernel");
+  const bool tc = ep.fwd.passes != 0;
+  if (tc) SPARF_TRY(tc_pack_rows(ep.fwd, (int)Mc, d.Evp, denc, d.Evp, S, w.dencimg, st));
+  SPARF_TRY(chunk_trunk(mlp, ep, d, Mc, enc, H, noise, raw, sigma, true, w, st));
   {
     if (tc)
       SPARF_TRY(tc_gemm_nt(ep.fwd, 1, (int)Mc, d.HW, w.Himg[(d.nt - 1) & 1], d.W, w.dencimg, d.Ev, mlp->head_w[0], d.W + d.Ev,
@@ -693,7 +737,7 @@ int simt_mlp_forward(const SparfMLP* mlp, int engine, int R, int S, const float*
   SimtDims d = simt_dims(mlp);
   const int nrc = std::min(R, chunk_rays(S, 0));
   Ws w;
-  carve(d, uses_tc(engine), nrc, S, 0, reinterpret_cast<char*>(workspace), &w);
+  carve(d, uses_tc(engine), nrc, S, 0, true, reinterpret_cast<char*>(workspace), &w);
   const EnginePrec ep = with_images(engine_prec(engine), w);
   for (int r0 = 0; r0 < R; r0 += nrc) {
     int nr = std::min(nrc, R - r0);
@@ -748,7 +792,7 @@ int simt_mlp_forward_tape(const SparfMLP* mlp, int engine, int R, int S, const f
   tape_layout(d, R, S, reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(tape), 256)), &tp);
   const int nrc = std::min(R, chunk_rays(S, 3));
   Ws w;
-  carve(d, uses_tc(engine), nrc, S, 3, reinterpret_cast<char*>(workspace), &w);
+  carve(d, uses_tc(engine), nrc, S, 3, true, reinterpret_cast<char*>(workspace), &w);
   const EnginePrec ep = with_images(engine_prec(engine), w);
   for (int r0 = 0; r0 < R; r0 += nrc) {       // chunk by chunk, straight into the tape
     const int nr = std::min(nrc, R - r0);
@@ -759,6 +803,79 @@ int simt_mlp_forward_tape(const SparfMLP* mlp, int engine, int R, int S, const f
                             noise ? noise + m0 : nullptr, w.wts, tp.enc + m0 * d.E3p, tp.denc + (size_t)r0 * d.Evp, H,
                             tp.raw + m0, tp.hid + m0 * d.HW, sigma + m0, rgb + m0 * 3, w, st);
     if (rc) return rc;
+  }
+  return SPARF_OK;
+}
+
+constexpr int kSimtSlab = 2048;   // rows per SIMT wgrad slab (the tensor-core GEMMs choose their own k-ranges)
+
+// tensor cores: the trunk gradients G leave each input-gradient GEMM as images, in ping-pong buffer i: a row image (the
+// next input gradient's A operand) and a transposed one (K = this chunk's Mc rows; the weight gradient's A operand)
+static TcImage grad_tr(const Ws& w, int i, long long Mc) { return TcImage{w.Gtr[i].p, ceil_div(Mc, 32)}; }
+static TcOut grad_images(const Ws& w, const EnginePrec& ep, int i, long long Mc) {
+  TcOut o;
+  o.row = w.Grow[i];
+  o.tr = grad_tr(w, i, Mc);
+  o.row_passes = ep.dgrad.passes;
+  o.tr_passes = ep.wgrad.passes;
+  return o;
+}
+
+// Backward through trunk layers nt-1 ... 0 of one chunk of Mc rows, from the gradient of the last layer's features
+// (SIMT: w.G0 in fp32; tensor cores: image pair 0) and of its density row, graw (may be NULL: zero).  H: the chunk's
+// nt-1 first trunk activations, enc its encoding.  Parameter gradients +=, the encoding's gradient into w.Genc when
+// enc_grad.  The last layer's bias gradient is the caller's: on the tensor cores the kernel that made image pair 0 adds
+// it; SIMT adds the column sums of G0 here (and sum graw with the density row's weights).
+static int trunk_backward(const SparfMLP* mlp, const EnginePrec& ep, const SimtDims& d, const Ws& w, long long Mc,
+                          const float* enc, float* const* H, const float* graw, const SparfMLPGrad* grad, bool enc_grad,
+                          cudaStream_t st) {
+  const bool tc = ep.fwd.passes != 0;
+  float* G = w.G0;
+  float* Gn = w.G1;
+  int gi = 0;       // tensor cores: G is image pair gi
+  bool genc_written = false;
+  for (int l = d.nt - 1; l >= 0; --l) {
+    const bool last = l == d.nt - 1;
+    const bool r1 = last && graw;       // the density row's rank-1 term: z = [raw | feat_pre]
+    const int ldw = trunk_ldw(d, l);
+    const float* in = l == 0 ? enc : H[l - 1];
+    const int Kin = trunk_in_main(d, l), Kinv = trunk_in_main_valid(d, l);
+    const int rowoff = last ? 1 : 0;
+    float* dWl = grad->trunk_w[l] + (size_t)rowoff * ldw;
+    const float* Wl = mlp->trunk_w[l] + (size_t)rowoff * ldw;
+    if (tc) {
+      SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, Kin, Kinv, grad_tr(w, gi, Mc), in, Kin, 1, dWl, ldw, 0, st));
+      if (l == d.skip)
+        SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, d.E3p, d.E3, grad_tr(w, gi, Mc), enc, d.E3p, 1, dWl, ldw, d.W, st));
+    } else {
+      SPARF_TRY(gemm_tn((int)Mc, d.W, Kin, Kinv, kSimtSlab, G, d.W, in, Kin, 1, dWl, ldw, 0, st));
+      if (l == d.skip) SPARF_TRY(gemm_tn((int)Mc, d.W, d.E3p, d.E3, kSimtSlab, G, d.W, enc, d.E3p, 1, dWl, ldw, d.W, st));
+      colsum_kernel<<<dim3(ceil_div(d.W, 32), ceil_div(Mc, 1024)), 256, 0, st>>>(Mc, d.W, 1024, G, d.W, grad->trunk_b[l] + rowoff);
+      LAUNCH_OK("colsum_kernel(trunk)");
+    }
+    if (r1 && !tc) {
+      narrow_wgrad_kernel<1><<<ceil_div(Mc, 512), 128, 0, st>>>(Mc, d.W, 512, graw, 1, in, d.W, grad->trunk_w[l], ldw, grad->trunk_b[l]);
+      LAUNCH_OK("narrow_wgrad_kernel<1>");
+    }
+    if (l > 0 && tc) {        // last layer: its epilogue also sums the density row's weight gradient
+      SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.W, d.W, w.Grow[gi], Wl, ldw, 0, in, d.W, r1 ? graw : nullptr,
+                           r1 ? mlp->trunk_w[l] : nullptr, nullptr, 0, 0, grad_images(w, ep, gi ^ 1, Mc), grad->trunk_b[l - 1],
+                           r1 ? grad->trunk_w[l] : nullptr, st));
+    } else if (l > 0) {
+      SPARF_TRY(gemm_nn((int)Mc, d.W, d.W, d.W, G, d.W, Wl, ldw, 0, in, d.W, r1 ? graw : nullptr,
+                        r1 ? mlp->trunk_w[l] : nullptr, Gn, d.W, 0, st));
+    }
+    if (enc_grad && (l == d.skip || l == 0)) {
+      if (tc)
+        SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.E3p, d.E3, w.Grow[gi], Wl, ldw, l == 0 ? 0 : d.W, nullptr, 0, nullptr,
+                             nullptr, w.Genc, d.E3p, genc_written ? 1 : 0, TcOut{}, nullptr, nullptr, st));
+      else
+        SPARF_TRY(gemm_nn((int)Mc, d.W, d.E3p, d.E3, G, d.W, Wl, ldw, l == 0 ? 0 : d.W, nullptr, 0, nullptr, nullptr, w.Genc,
+                          d.E3p, genc_written ? 1 : 0, st));
+      genc_written = true;
+    }
+    float* tmp = G; G = Gn; Gn = tmp;
+    gi ^= 1;
   }
   return SPARF_OK;
 }
@@ -804,14 +921,14 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
   const bool need_rays = d_origins != nullptr || d_dirs != nullptr;
   const int nrc = std::min(R, chunk_rays(S, mode));
   Ws w;
-  carve(d, uses_tc(engine), nrc, S, mode, reinterpret_cast<char*>(workspace), &w);
+  carve(d, uses_tc(engine), nrc, S, mode, true, reinterpret_cast<char*>(workspace), &w);
   const EnginePrec ep = with_images(engine_prec(engine), w);
   const bool tc = ep.fwd.passes != 0;
   float *wts = w.wts, *enc_w = w.enc, *denc_w = w.denc, *hid_w = w.hid, *raw_w = w.raw, *rgbv_w = w.rgbv;
   float** H_w = w.H;
   Tape tp{};
   if (tape) tape_layout(d, R, S, reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(tape), 256)), &tp);
-  float *G0 = w.G0, *G1 = w.G1, *Genc = w.Genc, *Ghid = w.Ghid, *gpre = w.gpre, *graw = w.graw, *Gdtmp = w.Gdtmp,
+  float *G0 = w.G0, *Ghid = w.Ghid, *gpre = w.gpre, *graw = w.graw, *Gdtmp = w.Gdtmp,
         *Gdenc = w.Gdenc;
 
   for (int r0 = 0; r0 < R; r0 += nrc) {
@@ -836,21 +953,10 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
       rc = simt_chunk_forward(mlp, ep, d, nr, S, o_c, d_c, t_c, nz, wts, enc, denc, H, raw, hid, nullptr, rgbv, w, st);
       if (rc) return rc;
     }
-    const int slab = 2048;  // rows per SIMT wgrad slab (the tensor-core GEMMs choose their own k-ranges)
-
     const int ldw8 = d.W + d.Ev;
     float* feat = H[d.nt - 1];
     // tensor cores: the trunk gradients G leave each input-gradient GEMM as images (gout(i) = ping-pong buffer i), with the
     // bias gradient of the layer that produced them; the colour-head gradient Ghid leaves tc_head_backward as images
-    auto gtr = [&](int i) { return TcImage{w.Gtr[i].p, ceil_div(Mc, 32)}; };   // K = this chunk's rows
-    auto gout = [&](int i) {
-      TcOut o;
-      o.row = w.Grow[i];
-      o.tr = gtr(i);
-      o.row_passes = ep.dgrad.passes;
-      o.tr_passes = ep.wgrad.passes;
-      return o;
-    };
     const TcImage ghid_t{w.ghid_tr.p, ceil_div(Mc, 32)}, ghid = w.ghid_row;
     if (tc) {
       // colour head, layer 1 (HW -> 3) and the head's gradients: one kernel, Ghid as images; layer 0 ([feat | denc] -> HW)
@@ -860,7 +966,7 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
       SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.W, d.W, ghid_t, feat, d.W, 1, grad->head_w[0], ldw8, 0, st));
       SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.Evp, d.Ev, ghid_t, denc, d.Evp, S, grad->head_w[0], ldw8, d.W, st));
       SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.HW, d.W, d.W, ghid, mlp->head_w[0], ldw8, 0, feat, d.W, nullptr, nullptr,
-                           nullptr, 0, 0, gout(0), grad->trunk_b[d.nt - 1] + 1, nullptr, st));
+                           nullptr, 0, 0, grad_images(w, ep, 0, Mc), grad->trunk_b[d.nt - 1] + 1, nullptr, st));
     } else {
       head_grad_kernel<<<ceil_div(Mc, 256), 256, 0, st>>>(Mc, d_rgb + m0 * 3, rgbv, d_sigma + m0, raw, nullptr, gpre, graw);
       LAUNCH_OK("head_grad_kernel");
@@ -871,8 +977,8 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
       narrow_dgrad_kernel<<<ceil_div(Mc * d.HW, 256), 256, 0, st>>>(Mc * d.HW, d.HW, gpre, mlp->head_w[1], d.HW, hid, Ghid);
       LAUNCH_OK("narrow_dgrad_kernel");
       // colour head, layer 0 ([feat | denc] -> HW)
-      SPARF_TRY(gemm_tn((int)Mc, d.HW, d.W, d.W, slab, Ghid, d.HW, feat, d.W, 1, grad->head_w[0], ldw8, 0, st));
-      SPARF_TRY(gemm_tn((int)Mc, d.HW, d.Evp, d.Ev, slab, Ghid, d.HW, denc, d.Evp, S, grad->head_w[0], ldw8, d.W, st));
+      SPARF_TRY(gemm_tn((int)Mc, d.HW, d.W, d.W, kSimtSlab, Ghid, d.HW, feat, d.W, 1, grad->head_w[0], ldw8, 0, st));
+      SPARF_TRY(gemm_tn((int)Mc, d.HW, d.Evp, d.Ev, kSimtSlab, Ghid, d.HW, denc, d.Evp, S, grad->head_w[0], ldw8, d.W, st));
       colsum_kernel<<<dim3(ceil_div(d.HW, 32), ceil_div(Mc, 1024)), 256, 0, st>>>(Mc, d.HW, 1024, Ghid, d.HW, grad->head_b[0]);
       LAUNCH_OK("colsum_kernel(head)");
       SPARF_TRY(gemm_nn((int)Mc, d.HW, d.W, d.W, Ghid, d.HW, mlp->head_w[0], ldw8, 0, feat, d.W, nullptr, nullptr, G0, d.W, 0, st));
@@ -889,61 +995,115 @@ static int mlp_backward_impl(const SparfMLP* mlp, int engine, int R, int S, cons
       direnc_bwd_kernel<<<ceil_div(nr, 128), 128, 0, st>>>(nr, mlp->L_view, d.Evp, denc, Gdenc, d_c, d_dirs + (size_t)r0 * 3);
       LAUNCH_OK("direnc_bwd_kernel");
     }
-    // trunk, last layer: z = [raw | feat_pre]
-    float* G = G0;
-    float* Gn = G1;
-    int gi = 0;       // tensor cores: G is image pair gi
-    bool genc_written = false;
-    for (int l = d.nt - 1; l >= 0; --l) {
-      const bool last = l == d.nt - 1;
-      const int ldw = trunk_ldw(d, l);
-      const float* in = l == 0 ? enc : H[l - 1];
-      const int Kin = trunk_in_main(d, l), Kinv = trunk_in_main_valid(d, l);
-      const int rowoff = last ? 1 : 0;
-      float* dWl = grad->trunk_w[l] + (size_t)rowoff * ldw;
-      const float* Wl = mlp->trunk_w[l] + (size_t)rowoff * ldw;
-      if (tc) {
-        SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, Kin, Kinv, gtr(gi), in, Kin, 1, dWl, ldw, 0, st));
-        if (l == d.skip)
-          SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, d.E3p, d.E3, gtr(gi), enc, d.E3p, 1, dWl, ldw, d.W, st));
-      } else {
-        SPARF_TRY(gemm_tn((int)Mc, d.W, Kin, Kinv, slab, G, d.W, in, Kin, 1, dWl, ldw, 0, st));
-        if (l == d.skip) SPARF_TRY(gemm_tn((int)Mc, d.W, d.E3p, d.E3, slab, G, d.W, enc, d.E3p, 1, dWl, ldw, d.W, st));
-        colsum_kernel<<<dim3(ceil_div(d.W, 32), ceil_div(Mc, 1024)), 256, 0, st>>>(Mc, d.W, 1024, G, d.W, grad->trunk_b[l] + rowoff);
-        LAUNCH_OK("colsum_kernel(trunk)");
-      }
-      if (last && !tc) {
-        narrow_wgrad_kernel<1><<<ceil_div(Mc, 512), 128, 0, st>>>(Mc, d.W, 512, graw, 1, in, d.W, grad->trunk_w[l], ldw, grad->trunk_b[l]);
-        LAUNCH_OK("narrow_wgrad_kernel<1>");
-      }
-      if (l > 0 && tc) {        // last layer: its epilogue also sums the density row's weight gradient (bias: tc_head_backward)
-        SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.W, d.W, w.Grow[gi], Wl, ldw, 0, in, d.W, last ? graw : nullptr,
-                             last ? mlp->trunk_w[l] : nullptr, nullptr, 0, 0, gout(gi ^ 1), grad->trunk_b[l - 1],
-                             last ? grad->trunk_w[l] : nullptr, st));
-      } else if (l > 0) {
-        SPARF_TRY(gemm_nn((int)Mc, d.W, d.W, d.W, G, d.W, Wl, ldw, 0, in, d.W, last ? graw : nullptr,
-                          last ? mlp->trunk_w[l] : nullptr, Gn, d.W, 0, st));
-      }
-      if (need_rays && (l == d.skip || l == 0)) {
-        if (tc)
-          SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.E3p, d.E3, w.Grow[gi], Wl, ldw, l == 0 ? 0 : d.W, nullptr, 0, nullptr,
-                               nullptr, Genc, d.E3p, genc_written ? 1 : 0, TcOut{}, nullptr, nullptr, st));
-        else
-          SPARF_TRY(gemm_nn((int)Mc, d.W, d.E3p, d.E3, G, d.W, Wl, ldw, l == 0 ? 0 : d.W, nullptr, 0, nullptr, nullptr, Genc,
-                            d.E3p, genc_written ? 1 : 0, st));
-        genc_written = true;
-      }
-      float* tmp = G; G = Gn; Gn = tmp;
-      gi ^= 1;
-    }
+    SPARF_TRY(trunk_backward(mlp, ep, d, w, Mc, enc, H, graw, grad, need_rays, st));
     if (need_rays) {
-      posenc_bwd_kernel<<<ceil_div(nr, 4), 128, 0, st>>>(nr, S, mlp->L_xyz, d.E3p, enc, Genc, t_c,
+      posenc_bwd_kernel<<<ceil_div(nr, 4), 128, 0, st>>>(nr, S, mlp->L_xyz, d.E3p, enc, w.Genc, t_c,
                                                         d_origins ? d_origins + (size_t)r0 * 3 : nullptr,
                                                         d_dirs ? d_dirs + (size_t)r0 * 3 : nullptr);
       LAUNCH_OK("posenc_bwd_kernel");
     }
   }
   return SPARF_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// density queries: the trunk alone at arbitrary points (NeRF.compute_raw_density), rows = points (S = 1), in chunks of
+// the forward's (mode 0) or the recompute backward's (mode 1) rows, without the colour head's buffers
+// ------------------------------------------------------------------------------------------------
+size_t simt_density_workspace_bytes(const SparfMLP* mlp, long long M, int mode, int engine) {
+  return carve(simt_dims(mlp), uses_tc(engine), (int)std::min<long long>(M, chunk_rays(1, mode)), 1, mode, false, nullptr,
+               nullptr);
+}
+
+int simt_density_forward(const SparfMLP* mlp, int engine, long long M, const float* points, float* raw, float* feat,
+                         void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  SPARF_TRY(simt_validate_trunk(mlp));
+  const size_t need = simt_density_workspace_bytes(mlp, M, 0, engine);
+  if (workspace_bytes < need) {
+    set_error("density_forward: workspace %zu < %zu bytes", workspace_bytes, need);
+    return SPARF_ERR_WORKSPACE;
+  }
+  const SimtDims d = simt_dims(mlp);
+  const int nrc = (int)std::min<long long>(M, chunk_rays(1, 0));
+  Ws w;
+  carve(d, uses_tc(engine), nrc, 1, 0, false, reinterpret_cast<char*>(workspace), &w);
+  const EnginePrec ep = with_images(engine_prec(engine), w);
+  for (long long p0 = 0; p0 < M; p0 += nrc) {
+    const int n = (int)std::min<long long>(nrc, M - p0);
+    float* H[SPARF_MAX_TRUNK];
+    for (int l = 0; l < d.nt; ++l) H[l] = w.H[l];
+    H[d.nt - 1] = feat ? feat + (size_t)p0 * d.W : nullptr;     // the features go straight to the caller, or nowhere
+    SPARF_TRY(chunk_encode_xyz(mlp, ep, d, n, 1, points + (size_t)p0 * 3, nullptr, nullptr, w.wts, w.enc, w, st));
+    SPARF_TRY(chunk_trunk(mlp, ep, d, n, w.enc, H, nullptr, raw + p0, nullptr, false, w, st));
+  }
+  return SPARF_OK;
+}
+
+// recomputes the forward per chunk, then the last layer's gradient from the caller's (tensor cores: tc_feat_backward,
+// straight into image pair 0; SIMT: the masked d_feat in G0) and the trunk backward with d_raw as the density row's
+int simt_density_backward(const SparfMLP* mlp, int engine, long long M, const float* points, const float* d_raw,
+                          const float* d_feat, const SparfMLPGrad* grad, float* d_points, void* workspace,
+                          size_t workspace_bytes, cudaStream_t st) {
+  SPARF_TRY(simt_validate_trunk(mlp));
+  SPARF_REQUIRE(grad != nullptr, "density_backward: grad is NULL");
+  const size_t need = simt_density_workspace_bytes(mlp, M, 1, engine);
+  if (workspace_bytes < need) {
+    set_error("density_backward: workspace %zu < %zu bytes", workspace_bytes, need);
+    return SPARF_ERR_WORKSPACE;
+  }
+  const SimtDims d = simt_dims(mlp);
+  const int nrc = (int)std::min<long long>(M, chunk_rays(1, 1));
+  Ws w;
+  carve(d, uses_tc(engine), nrc, 1, 1, false, reinterpret_cast<char*>(workspace), &w);
+  const EnginePrec ep = with_images(engine_prec(engine), w);
+  const bool tc = ep.fwd.passes != 0;
+  float* db = grad->trunk_b[d.nt - 1];
+  for (long long p0 = 0; p0 < M; p0 += nrc) {
+    const int n = (int)std::min<long long>(nrc, M - p0);
+    const float* dr = d_raw ? d_raw + p0 : nullptr;
+    const float* df = d_feat ? d_feat + (size_t)p0 * d.W : nullptr;
+    float* H[SPARF_MAX_TRUNK];
+    for (int l = 0; l < d.nt; ++l) H[l] = w.H[l];
+    if (!df) H[d.nt - 1] = nullptr;   // the features are needed only as the mask of d_feat
+    SPARF_TRY(chunk_encode_xyz(mlp, ep, d, n, 1, points + (size_t)p0 * 3, nullptr, nullptr, w.wts, w.enc, w, st));
+    SPARF_TRY(chunk_trunk(mlp, ep, d, n, w.enc, H, nullptr, nullptr, nullptr, false, w, st));
+    if (tc) {
+      SPARF_TRY(tc_feat_backward(ep.dgrad, ep.wgrad, n, d.W, dr, df, H[d.nt - 1], w.Grow[0], grad_tr(w, 0, n), db, db + 1, st));
+    } else if (df) {
+      relu_mask_kernel<<<ceil_div((long long)n * d.W, 256), 256, 0, st>>>((long long)n * d.W, H[d.nt - 1], df, w.G0);
+      LAUNCH_OK("relu_mask_kernel");
+    } else {
+      SPARF_CHECK_CUDA(cudaMemsetAsync(w.G0, 0, (size_t)n * d.W * sizeof(float), st));
+    }
+    SPARF_TRY(trunk_backward(mlp, ep, d, w, n, w.enc, H, dr, grad, d_points != nullptr, st));
+    if (d_points) {
+      posenc_bwd_kernel<<<ceil_div(n, 4), 128, 0, st>>>(n, 1, mlp->L_xyz, d.E3p, w.enc, w.Genc, nullptr,
+                                                       d_points + (size_t)p0 * 3, nullptr);
+      LAUNCH_OK("posenc_bwd_kernel");
+    }
+  }
+  return SPARF_OK;
+}
+
+// tc_feat_backward and the path it stands for (relu_mask_kernel's fp32 G, then tc_pack_rows / tc_pack_cols and
+// colsum_kernel) on the same inputs; scratch = G [M x W]
+static int selftest_featgrad(const float* d_raw, const float* d_feat, const float* feat, int M, int W, TcPrec dg, TcPrec wg,
+                             uint16_t* img, float* sums, float* scratch, cudaStream_t st) {
+  const size_t nrow = tc_image_elems(M, W), ntr = tc_image_elems(W, M);
+  const TcImage row{img, ceil_div(W, 32)}, tr{img + nrow, ceil_div(M, 32)};
+  const TcImage row_ref{img + nrow + ntr, row.ks}, tr_ref{img + 2 * nrow + ntr, tr.ks};
+  float* ref = sums + W + 1;
+  SPARF_CHECK_CUDA(cudaMemsetAsync(img, 0xFF, 2 * (nrow + ntr) * sizeof(uint16_t), st));
+  SPARF_CHECK_CUDA(cudaMemsetAsync(sums, 0, 2 * (W + 1) * sizeof(float), st));
+  SPARF_TRY(tc_feat_backward(dg, wg, M, W, d_raw, d_feat, feat, row, tr, sums, sums + 1, st));
+  relu_mask_kernel<<<ceil_div((long long)M * W, 256), 256, 0, st>>>((long long)M * W, feat, d_feat, scratch);
+  LAUNCH_OK("relu_mask_kernel");
+  colsum_kernel<<<dim3(ceil_div(W, 32), ceil_div(M, 1024)), 256, 0, st>>>(M, W, 1024, scratch, W, ref + 1);
+  LAUNCH_OK("colsum_kernel");
+  colsum_kernel<<<dim3(1, ceil_div(M, 1024)), 256, 0, st>>>(M, 1, 1024, d_raw, 1, ref);
+  LAUNCH_OK("colsum_kernel");
+  SPARF_TRY(tc_pack_rows(dg, M, W, scratch, W, 1, row_ref, st));
+  return tc_pack_cols(wg, M, W, scratch, W, tr_ref, st);
 }
 
 // tc_head_backward and the path it replaced (head_grad_kernel, narrow_dgrad_kernel's fp32 Ghid, then tc_pack_rows /
@@ -980,6 +1140,20 @@ extern "C" int sparf_tc_selftest_head(const float* d_rgb, const float* rgb, cons
   SPARF_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch), ((size_t)M * (HW + 4) + 4 * HW + 4) * sizeof(float), st));
   const int rc = selftest_head(d_rgb, rgb, d_sigma, raw, hid, W9, M, HW, TcPrec{false, row_passes}, TcPrec{false, tr_passes},
                                img, graw, scratch, st);
+  cudaFreeAsync(scratch, st);
+  return rc;
+}
+
+extern "C" int sparf_tc_selftest_featgrad(const float* d_raw, const float* d_feat, const float* feat, int32_t M, int32_t W,
+                                          int32_t row_passes, int32_t tr_passes, uint16_t* img, float* sums,
+                                          sparf_stream_t stream) {
+  SPARF_REQUIRE(M >= 1 && M <= (1 << 20) && W >= 8 && W <= 512 && W % 8 == 0, "tc_selftest_featgrad: M=%d W=%d", M, W);
+  SPARF_REQUIRE(d_raw && d_feat && feat && img && sums, "tc_selftest_featgrad: NULL tensor");
+  cudaStream_t st = (cudaStream_t)stream;
+  float* scratch = nullptr;
+  SPARF_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch), (size_t)M * W * sizeof(float), st));
+  const int rc = selftest_featgrad(d_raw, d_feat, feat, M, W, TcPrec{false, row_passes}, TcPrec{false, tr_passes}, img, sums,
+                                   scratch, st);
   cudaFreeAsync(scratch, st);
   return rc;
 }

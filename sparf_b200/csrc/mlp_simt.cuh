@@ -16,6 +16,8 @@ struct EnginePrec {
 EnginePrec engine_prec(int engine);
 
 SimtDims simt_dims(const SparfMLP* mlp);
+// the trunk's fields (density calls); simt_validate: these and the colour head's (MLP calls)
+int simt_validate_trunk(const SparfMLP* mlp);
 int simt_validate(const SparfMLP* mlp);
 // mode 0: forward, 1: backward (recompute), 2: backward from a tape, 3: taped forward
 size_t simt_workspace_bytes(const SparfMLP* mlp, int R, int S, int mode, int engine);
@@ -33,5 +35,12 @@ int simt_mlp_backward_tape(const SparfMLP* mlp, int engine, int R, int S, const 
 int simt_mlp_backward(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs, const float* t,
                       const float* noise, const float* d_sigma, const float* d_rgb, const SparfMLPGrad* grad,
                       float* d_origins, float* d_dirs, void* workspace, size_t workspace_bytes, cudaStream_t st);
+// trunk-only density queries at M points: mode 0 forward, 1 backward (recomputes the forward)
+size_t simt_density_workspace_bytes(const SparfMLP* mlp, long long M, int mode, int engine);
+int simt_density_forward(const SparfMLP* mlp, int engine, long long M, const float* points, float* raw, float* feat,
+                         void* workspace, size_t workspace_bytes, cudaStream_t st);
+int simt_density_backward(const SparfMLP* mlp, int engine, long long M, const float* points, const float* d_raw,
+                          const float* d_feat, const SparfMLPGrad* grad, float* d_points, void* workspace,
+                          size_t workspace_bytes, cudaStream_t st);
 
 }  // namespace sparf

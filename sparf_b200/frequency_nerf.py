@@ -159,8 +159,15 @@ class NeRF(nn.Module):
         is accepted for signature compatibility (the kernel implements the log-sampled, pi-scaled embedder)."""
         return ops.posenc(input, L, barf_c2f=opt.barf_c2f, progress=self.progress)
 
-    def compute_raw_density(self, opt, points_3D_samples, embedder_pts):  # pragma: no cover
-        raise NotImplementedError("fused into the sparf_b200 MLP kernels (csrc/): use forward()/forward_samples()")
+    def compute_raw_density(self, opt, points_3D_samples: torch.Tensor, embedder_pts=None):
+        """The trunk alone at points [..., 3] (frequency_nerf.py:149-170) -> (raw_density [...] before the softplus, no noise;
+        feat [..., width] after the ReLU).  Differentiable w.r.t. the points (normals = -grad of the density) and the
+        trunk's parameters.  `embedder_pts` is accepted for signature compatibility (the kernel implements the
+        log-sampled, pi-scaled embedder).  For density grids without the features: ops.density_forward(..., features=False)."""
+        shape = points_3D_samples.shape[:-1]
+        raw, feat = ops.density_forward(self._spec(), points_3D_samples, self.kernel_params()[:2 * len(self.mlp_feat)],
+                                        progress=self.progress)
+        return raw.view(shape), feat.view(*shape, feat.shape[-1])
 
     def composite(self, opt, ray: torch.Tensor, pred_dict: Dict[str, Any], depth_samples: torch.Tensor) -> Dict[str, Any]:
         """Volume-rendering quadrature (frequency_nerf.py:283-343) on the kernel; adds rgb, rgb_var, depth,

@@ -124,7 +124,8 @@ class MLPSpec:
         return 2 * self.n_trunk + 4
 
     def fill(self, params: Sequence[torch.Tensor], progress: Optional[torch.Tensor]) -> Tuple[SparfMLP, list]:
-        """params = [trunk_w0, trunk_b0, ..., head_w0, head_b0, head_w1, head_b1] (nn.Linear tensors)."""
+        """params = [trunk_w0, trunk_b0, ..., head_w0, head_b0, head_w1, head_b1] (nn.Linear tensors); the trunk's 2 n_trunk
+        alone leave the head pointers NULL (density calls)."""
         keep = [_f32c(p.detach()) for p in params]
         m = SparfMLP()
         m.n_trunk, m.width, m.head_width, m.skip_layer = self.n_trunk, self.width, self.head_width, self.skip_layer
@@ -144,8 +145,9 @@ class MLPSpec:
             m.trunk_w[i] = keep[2 * i].data_ptr()
             m.trunk_b[i] = keep[2 * i + 1].data_ptr()
         o = 2 * self.n_trunk
-        m.head_w[0], m.head_b[0] = keep[o].data_ptr(), keep[o + 1].data_ptr()
-        m.head_w[1], m.head_b[1] = keep[o + 2].data_ptr(), keep[o + 3].data_ptr()
+        if len(params) > o:
+            m.head_w[0], m.head_b[0] = keep[o].data_ptr(), keep[o + 1].data_ptr()
+            m.head_w[1], m.head_b[1] = keep[o + 2].data_ptr(), keep[o + 3].data_ptr()
         return m, keep
 
     def grad_struct(self, grads: Sequence[torch.Tensor]) -> SparfMLPGrad:
@@ -154,8 +156,9 @@ class MLPSpec:
             g.trunk_w[i] = grads[2 * i].data_ptr()
             g.trunk_b[i] = grads[2 * i + 1].data_ptr()
         o = 2 * self.n_trunk
-        g.head_w[0], g.head_b[0] = grads[o].data_ptr(), grads[o + 1].data_ptr()
-        g.head_w[1], g.head_b[1] = grads[o + 2].data_ptr(), grads[o + 3].data_ptr()
+        if len(grads) > o:
+            g.head_w[0], g.head_b[0] = grads[o].data_ptr(), grads[o + 1].data_ptr()
+            g.head_w[1], g.head_b[1] = grads[o + 2].data_ptr(), grads[o + 3].data_ptr()
         return g
 
 
@@ -236,17 +239,7 @@ class MLPFunction(torch.autograd.Function):
         g_sigma = _f32c(g_sigma) if g_sigma is not None else torch.zeros(R, S, device=t.device)
         g_rgb = _f32c(g_rgb) if g_rgb is not None else torch.zeros(R, S, 3, device=t.device)
         m, keep = spec.fill(params, ctx.progress)
-        inplace = ctx.param_refs is not None and all(
-            p.grad is not None and p.grad.is_contiguous() and p.grad.dtype == torch.float32 for p in ctx.param_refs)
-        if inplace:
-            grads = [p.grad for p in ctx.param_refs]
-        else:
-            sizes = [p.numel() for p in params]
-            flat = torch.zeros(sum(sizes), device=t.device, dtype=torch.float32)
-            grads, o = [], 0
-            for p, n in zip(params, sizes):
-                grads.append(flat[o:o + n].view(p.shape))
-                o += n
+        grads, ret = _param_grads(ctx, params, t.device)
         gs = spec.grad_struct(grads)
         need_o, need_d = ctx.needs_input_grad[3], ctx.needs_input_grad[4]
         d_o = torch.zeros_like(origins) if (need_o or need_d) else None
@@ -264,9 +257,7 @@ class MLPFunction(torch.autograd.Function):
                 check(L.sparf_mlp_backward(ctypes.byref(m), ctx.engine, R, S, _ptr(origins), _ptr(dirs), _ptr(t),
                                            _ptr(ctx.noise), _ptr(g_sigma), _ptr(g_rgb), ctypes.byref(gs), _ptr(d_o),
                                            _ptr(d_d), _ptr(ws), ws.numel(), _stream()), "mlp_backward")
-        if inplace:
-            grads = [None] * len(grads)
-        return (None, None, None, d_o if need_o else None, d_d if need_d else None, None, None, None, *grads)
+        return (None, None, None, d_o if need_o else None, d_d if need_d else None, None, None, None, *ret)
 
 
 def mlp_forward(spec: MLPSpec, origins, dirs, t, params: Sequence[torch.Tensor], *, noise=None, progress=None,
@@ -274,6 +265,85 @@ def mlp_forward(spec: MLPSpec, origins, dirs, t, params: Sequence[torch.Tensor],
     """origins/dirs [R,3], t [R,S] -> (sigma [R,S], rgb [R,S,3]); differentiable w.r.t. origins, dirs, params."""
     eng = get_engine() if engine is None else engine
     return MLPFunction.apply(spec, eng, torch.is_grad_enabled(), origins, dirs, t, noise, progress, *params)
+
+
+def _param_grads(ctx, params, device):
+    """Gradient destinations of a backward: the parameters' own `.grad` when the forward opted in and every one exists
+    (then autograd gets None), else fresh zeroed tensors in one flat buffer.  -> (grads for the C ABI, grads to return)."""
+    inplace = ctx.param_refs is not None and all(
+        p.grad is not None and p.grad.is_contiguous() and p.grad.dtype == torch.float32 for p in ctx.param_refs)
+    if inplace:
+        return [p.grad for p in ctx.param_refs], [None] * len(params)
+    sizes = [p.numel() for p in params]
+    flat = torch.zeros(sum(sizes), device=device, dtype=torch.float32)
+    grads, o = [], 0
+    for p, n in zip(params, sizes):
+        grads.append(flat[o:o + n].view(p.shape))
+        o += n
+    return grads, grads
+
+
+# ------------------------------------------------------------------------------------------------
+# density queries: raw, feat = NeRF.compute_raw_density(points)
+# ------------------------------------------------------------------------------------------------
+class DensityFunction(torch.autograd.Function):
+    @staticmethod
+    @_on_tensor_device
+    def forward(ctx, spec: MLPSpec, engine: int, grad_mode: bool, features: bool, points, progress, *trunk_params):
+        L = _lib.lib()
+        pts = _f32c(points).reshape(-1, 3)
+        M = pts.shape[0]
+        m, keep = spec.fill(trunk_params, progress)
+        raw = torch.empty(M, device=pts.device, dtype=torch.float32)
+        feat = torch.empty(M, spec.width, device=pts.device, dtype=torch.float32) if features else None
+        ws = _workspace(L.sparf_density_workspace_bytes(ctypes.byref(m), M, 0, engine), pts.device)
+        EVALS["fwd"] += M
+        with _timed("density_forward"):
+            check(L.sparf_density_forward(ctypes.byref(m), engine, M, _ptr(pts), _ptr(raw), _ptr(feat), _ptr(ws), ws.numel(),
+                                          _stream()), "density_forward")
+        ctx.set_materialize_grads(False)     # an output nobody differentiated arrives as None and goes to the ABI as NULL
+        ctx.spec, ctx.engine, ctx.progress = spec, engine, progress
+        ctx.points_shape = points.shape
+        ctx.saved = grad_mode and (ctx.needs_input_grad[4] or any(ctx.needs_input_grad[6:]))
+        if ctx.saved:
+            ctx.param_refs = trunk_params if (ACCUMULATE_INTO_PARAM_GRAD[0] or
+                                              all(getattr(p, "_sparf_inplace_grad", False) for p in trunk_params)) else None
+            ctx.save_for_backward(pts, *trunk_params)
+        return raw, feat
+
+    @staticmethod
+    @_on_tensor_device
+    def backward(ctx, g_raw, g_feat):
+        if not ctx.saved or (g_raw is None and g_feat is None):    # (only `progress` asked for a gradient)
+            return (None,) * (6 + 2 * ctx.spec.n_trunk)
+        L = _lib.lib()
+        pts, *params = ctx.saved_tensors
+        M = pts.shape[0]
+        EVALS["bwd"] += M
+        g_raw = _f32c(g_raw) if g_raw is not None else None
+        g_feat = _f32c(g_feat) if g_feat is not None else None
+        m, keep = ctx.spec.fill(params, ctx.progress)
+        grads, ret = _param_grads(ctx, params, pts.device)
+        gs = ctx.spec.grad_struct(grads)
+        d_pts = torch.zeros_like(pts) if ctx.needs_input_grad[4] else None
+        ws = _workspace(L.sparf_density_workspace_bytes(ctypes.byref(m), M, 1, ctx.engine), pts.device)
+        with _timed("density_backward"):
+            check(L.sparf_density_backward(ctypes.byref(m), ctx.engine, M, _ptr(pts), _ptr(g_raw), _ptr(g_feat), ctypes.byref(gs),
+                                           _ptr(d_pts), _ptr(ws), ws.numel(), _stream()), "density_backward")
+        d_pts = d_pts.view(ctx.points_shape) if d_pts is not None else None
+        ret = [g if need else None for g, need in zip(ret, ctx.needs_input_grad[6:])]
+        return (None, None, None, None, d_pts, None, *ret)
+
+
+def density_forward(spec: MLPSpec, points, trunk_params: Sequence[torch.Tensor], progress=None, engine: Optional[int] = None,
+                    features: bool = True):
+    """The trunk alone at points [..., 3] (NeRF.compute_raw_density, frequency_nerf.py:149-170) -> (raw [M], feat [M, width]),
+    M = points.numel() / 3: raw = the density row before the softplus (no noise), feat = relu of the last layer's features;
+    features=False returns feat = None and skips the feature GEMM of the last layer (density grids).  trunk_params =
+    [trunk_w0, trunk_b0, ...] (2 n_trunk tensors).  Differentiable w.r.t. the points and trunk_params."""
+    eng = get_engine() if engine is None else engine
+    assert len(trunk_params) == 2 * spec.n_trunk, "density_forward takes the trunk's 2 * n_trunk tensors"
+    return DensityFunction.apply(spec, eng, torch.is_grad_enabled(), bool(features), points, progress, *trunk_params)
 
 
 # ------------------------------------------------------------------------------------------------
