@@ -186,6 +186,39 @@ int sparf_density_backward(const SparfMLP* mlp, int32_t engine, int64_t M, const
                            const float* d_feat, const SparfMLPGrad* grad, float* d_points, void* workspace,
                            size_t workspace_bytes, sparf_stream_t stream);
 
+/* ---------------------------------------------------------------- marching cubes
+ * A triangle mesh of the iso-surface of a dense fp32 volume vol [nx][ny][nz] (row-major, k fastest), in index space,
+ * vertex-deduplicated: what mcubes.marching_cubes(volume, iso) returns, computed on the device.  Mesh extraction from a
+ * density grid (BARF's extract_mesh over opt.trimesh; sparf_b200/mesh.py).
+ *   inside:    vol >= iso (NaN is outside).  Cell (i,j,k), i < nx-1, j < ny-1, k < nz-1, has case index
+ *              sum over corners c of inside(corner c) << c, corner c at offset (c & 1, (c >> 1) & 1, (c >> 2) & 1).
+ *   vertices:  one per crossing lattice edge (one end inside, one outside), owned by its lower end p and its axis a, at
+ *              p + s e_a with s = (iso - vol[p]) / (vol[p + e_a] - vol[p]) in fp32; the coordinate along a is
+ *              float(p_a) + s, the others are exact.  Ordered by (linear index of p, a).
+ *   triangles: cells in linear order, each cell's triangles in table order; int64 vertex ids.  (v1 - v0) x (v2 - v0)
+ *              points from the inside toward the outside.  Where no lattice point on the volume's border is inside, the
+ *              mesh is closed and consistently oriented: every undirected edge lies in exactly two triangles, once in
+ *              each direction.
+ * Deterministic (identical bytes on every run).  Non-finite values cause no out-of-bounds access; only the mesh near
+ * them is unspecified.  Every extent must be >= 2 (SPARF_ERR_INVALID otherwise).
+ * Two calls on one stream with one workspace: sparf_mcubes_count writes totals [2] = {V, F} (device int64) and leaves
+ * per-point offsets in the workspace; sparf_mcubes_emit, enqueued after it on the same stream with the same volume, iso
+ * and workspace, reads them and writes verts [V,3] fp32 and faces [F,3] int64.  The caller reads the totals to size
+ * the outputs.  Neither call synchronises; both are capturable.  Workspace: 8 B per lattice point + 16 B per 2048
+ * points (0 for an invalid extent). */
+#define SPARF_MCUBES_MAX_TRIS 5
+size_t sparf_mcubes_workspace_bytes(int64_t nx, int64_t ny, int64_t nz);
+int sparf_mcubes_count(const float* vol, int64_t nx, int64_t ny, int64_t nz, float iso, int64_t* totals, void* workspace,
+                       size_t workspace_bytes, sparf_stream_t stream);
+int sparf_mcubes_emit(const float* vol, int64_t nx, int64_t ny, int64_t nz, float iso, float* verts, int64_t* faces,
+                      void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+/* Host only: the case table, table [256][3 * SPARF_MCUBES_MAX_TRIS] (host int8).  Row c lists the triangles of case c
+ * as cell-edge ids, three per triangle, padded with -1.  Edge e = 4a + m runs along axis a from the corner whose
+ * offsets along the two other axes b < b' are (m & 1, m >> 1); its vertex is owned by that corner.  The table is
+ * generated from one rule per cube face (sparf_b200/csrc/mcubes_table.py): inside corners never connect across a face,
+ * so two cells sharing a face cut it the same way. */
+int sparf_mcubes_table(int8_t* table);
+
 /* ---------------------------------------------------------------- compositing
  * NeRF.composite (frequency_nerf.py:283-343).  Outputs: rgb_map [R,3], depth/opacity/depth_var/rgb_var
  * [R], weights [R,S], all_cumulated [R] (= T at sample S-2).  white_bg: rgb += 1 - opacity.

@@ -9,6 +9,7 @@ from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_size_t, c_voi
 from . import build as _build
 
 MAX_TRUNK = 12
+MCUBES_MAX_TRIS = 5     # SPARF_MCUBES_MAX_TRIS: a row of the marching-cubes case table holds 3 * 5 edge ids
 
 ENGINE_AUTO, ENGINE_SIMT_FP32, ENGINE_TC_3X, ENGINE_TC_1X, ENGINE_TC_3X_W1 = 0, 1, 2, 3, 4
 ENGINES = {"auto": 0, "simt_fp32": 1, "tc_3x": 2, "tc_1x": 3, "tc_3x_w1": 4}
@@ -55,7 +56,11 @@ _SIGNATURES = {
     "sparf_density_forward": (c_int32, [POINTER(SparfMLP), c_int32, c_int64, _P, _P, _P, _P, c_size_t, _P]),
     "sparf_density_backward": (c_int32, [POINTER(SparfMLP), c_int32, c_int64, _P, _P, _P, POINTER(SparfMLPGrad), _P, _P,
                                          c_size_t, _P]),
-    "sparf_composite_forward": (c_int32, [c_int32, c_int32, _P, _P, _P, _P, c_int32, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "sparf_mcubes_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64]),
+    "sparf_mcubes_count": (c_int32, [_P, c_int64, c_int64, c_int64, c_float, _P, _P, c_size_t, _P]),
+    "sparf_mcubes_emit": (c_int32, [_P, c_int64, c_int64, c_int64, c_float, _P, _P, _P, c_size_t, _P]),
+    "sparf_mcubes_table": (c_int32, [_P]),
+    "sparf_composite_forward":(c_int32, [c_int32, c_int32, _P, _P, _P, _P, c_int32, _P, _P, _P, _P, _P, _P, _P, _P]),
     "sparf_composite_backward": (c_int32, [c_int32, c_int32, _P, _P, _P, _P, c_int32, _P, _P, _P, _P, _P, _P, _P, _P]),
     "sparf_huber2_fwd_bwd": (c_int32, [c_int64, _P, _P, c_float, _P, _P, _P]),
     "sparf_posenc_forward": (c_int32, [c_int64, c_int32, c_int32, _P, c_int32, c_float, c_float, _P, _P, _P]),

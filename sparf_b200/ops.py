@@ -347,6 +347,31 @@ def density_forward(spec: MLPSpec, points, trunk_params: Sequence[torch.Tensor],
 
 
 # ------------------------------------------------------------------------------------------------
+# marching cubes (no gradient)
+# ------------------------------------------------------------------------------------------------
+@torch.no_grad()
+@_on_tensor_device
+def marching_cubes(vol, iso: float):
+    """Iso-surface of a dense volume vol [nx, ny, nz] (inside: vol >= iso) -> (verts [V, 3] fp32 in index space, faces
+    [F, 3] int64), on vol's device; the semantics of mcubes.marching_cubes, specified in include/sparf_b200.h.  One
+    device-to-host copy: the two totals that size the outputs.  Not differentiable."""
+    L = _lib.lib()
+    v = _f32c(vol)
+    assert v.dim() == 3, "marching_cubes takes a 3-D volume"
+    nx, ny, nz = v.shape
+    ws = torch.empty(max(L.sparf_mcubes_workspace_bytes(nx, ny, nz), 1), dtype=torch.uint8, device=v.device)
+    totals = torch.empty(2, dtype=torch.int64, device=v.device)
+    check(L.sparf_mcubes_count(_ptr(v), nx, ny, nz, float(iso), _ptr(totals), _ptr(ws), ws.numel(), _stream()),
+          "mcubes_count")
+    n_verts, n_faces = totals.tolist()
+    verts = torch.empty(n_verts, 3, device=v.device, dtype=torch.float32)
+    faces = torch.empty(n_faces, 3, device=v.device, dtype=torch.int64)
+    check(L.sparf_mcubes_emit(_ptr(v), nx, ny, nz, float(iso), _ptr(verts), _ptr(faces), _ptr(ws), ws.numel(), _stream()),
+          "mcubes_emit")
+    return verts, faces
+
+
+# ------------------------------------------------------------------------------------------------
 # compositing
 # ------------------------------------------------------------------------------------------------
 class CompositeFunction(torch.autograd.Function):
