@@ -41,11 +41,25 @@ extern unsigned long long g_launch_count;
     }                                            \
   } while (0)
 
+// returns the status of a call that fails with a nonzero SPARF_ERR_*
+#define SPARF_TRY(expr)      \
+  do {                       \
+    int _rc = (expr);        \
+    if (_rc) return _rc;     \
+  } while (0)
+
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 // number of SMs of the current device (cached)
 int num_sms();
+
+// the MLP engines that run their wide GEMMs on the tensor cores (gemm_wgmma.cu)
+static inline bool is_tc(int engine) {
+  return engine == SPARF_ENGINE_TC_3X || engine == SPARF_ENGINE_TC_1X || engine == SPARF_ENGINE_TC_3X_W1;
+}
+// the engine an MLP or density call runs on: AUTO resolved, -1 when the engine is not available on this device
+int resolve_engine(int engine);
 
 // ---- arithmetic that must round exactly like the reference's separate fp32 torch ops (no FMA
 // contraction): the 2^9*pi positional-encoding band amplifies a 1-ulp difference in x by ~1e3.
@@ -63,8 +77,7 @@ __device__ __forceinline__ float sigmoid_f(float z) { return 1.f / (1.f + expf(-
 
 // BARF coarse-to-fine weight of frequency band j (frequency_nerf.py:248-253), fp32 op-for-op:
 //   alpha = (progress - start) / (end - start) * L ; w = (1 - cos(pi * clamp(alpha - j, 0, 1))) / 2
-__device__ __forceinline__ float c2f_weight(float progress, float start, float inv_den /*unused*/, float den,
-                                            int L, int j) {
+__device__ __forceinline__ float c2f_weight(float progress, float start, float den, int L, int j) {
   float alpha = mul_rn(__fdiv_rn(__fsub_rn(progress, start), den), (float)L);
   float x = fminf(fmaxf(__fsub_rn(alpha, (float)j), 0.f), 1.f);
   float c = cosf(mul_rn(x, 3.14159274101257324f));
@@ -79,7 +92,7 @@ struct C2F {
 
 __device__ __forceinline__ float band_weight(const C2F& c, int L, int j) {
   if (!c.enabled) return 1.f;
-  return c2f_weight(*c.progress, c.start, 0.f, c.den, L, j);
+  return c2f_weight(*c.progress, c.start, c.den, L, j);
 }
 
 // frequency of band j: 2^j * float(pi) (exact scaling of the fp32 constant), frequency_nerf.py:52

@@ -802,17 +802,6 @@ static int launch_gemm(const Opnd& a, const Opnd& b, const Units& w, int ctas, c
   return SPARF_OK;
 }
 
-// SMs of the current device, queried once (one CTA of the GEMM kernel fills an SM)
-static int sm_count() {
-  static const int n = [] {
-    int dev = 0, v = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    return std::max(v, 1);
-  }();
-  return n;
-}
-
 // pack B into p.pack_b, then the persistent GEMM over (B row tiles x A row tiles) output tiles with the epilogue
 // outputs e asks for: fp32 (e.out), a row image (row image passes = the GEMM's), a transposed image.  split_k: each
 // output tile's k-steps are shared out in ceil(CTAs / output tiles) ranges per 32 768 rows (atomic epilogues only), so
@@ -824,10 +813,9 @@ static int run(const TcPrec& p, const Opnd& a, int a_rows, FB fb, int b_rows, in
   SPARF_REQUIRE(p.pack_b && (size_t)rtb * ksteps * 2 * TILE_ELEMS <= p.pack_elems,
                 "tc gemm: B operand image needs %zu 16-bit elements, have %zu", (size_t)rtb * ksteps * 2 * TILE_ELEMS,
                 p.pack_elems);
-  int rc = launch_pack<F16, PASSES, BK>(fb, rtb, ksteps, p.pack_b, st);
-  if (rc) return rc;
+  SPARF_TRY((launch_pack<F16, PASSES, BK>(fb, rtb, ksteps, p.pack_b, st)));
   const Opnd b{p.pack_b, nullptr, ksteps, 0};
-  const int ctas = p.max_ctas > 0 ? std::min(p.max_ctas, sm_count()) : sm_count();
+  const int ctas = p.max_ctas > 0 ? std::min(p.max_ctas, num_sms()) : num_sms();   // one CTA fills an SM
   Units w{rtb, rta * rtb, 1, ksteps};
   // about ceil(CTAs / output tiles) ranges per 1024 k-steps (32 768 rows): no accumulator chain gets longer than at
   // 32 768 rows, whatever the chunk size, so the rounding of the sums does not grow with it
@@ -890,8 +878,7 @@ int tc_gemm_nt(TcPrec p, int act, int M, int N, TcImage a1, int K1v, TcImage a2,
   Epi e{};
   e.kind = 0; e.M = M; e.N = N; e.act = act; e.bias = bias; e.out = Y; e.ldo = ldy;
   e.pairs = N % 2 == 0 && pair_aligned(Y, ldy);
-  int rc = set_images(e, out, M, N);
-  if (rc) return rc;
+  SPARF_TRY(set_images(e, out, M, N));
   return SPARF_WG_RUN(true, p, opnd(a1, a2.p ? a2 : TcImage{}), M, NtB{W, ldw, wcol2, K1v, K2v, N, a1.ks}, N, ks, false, e,
                       out.row_passes, out.tr_passes, st);
 }
@@ -907,8 +894,7 @@ int tc_gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, TcImage g, const float*
   e.r1_vec = r1_vec; e.r1_row = r1_row; e.accumulate = accumulate; e.colsum = db; e.r1_wgrad = r1_wgrad;
   e.pairs = Kout % 2 == 0 && pair_aligned(D, ldd) && pair_aligned(mask_src, ldmask);
   SPARF_REQUIRE(!db || !accumulate, "tc_gemm_nn: column sums of an accumulated output");
-  int rc = set_images(e, out, M, Kout);
-  if (rc) return rc;
+  SPARF_TRY(set_images(e, out, M, Kout));
   return SPARF_WG_RUN(false, p, opnd(g), M, NnB{W, ldw, wcol, Kv, N}, Kout, g.ks, false, e, out.row_passes, out.tr_passes, st);
 }
 
@@ -993,10 +979,9 @@ extern "C" int sparf_tc_selftest(const float* A, const float* B, int32_t K, void
   SPARF_REQUIRE(K % 64 == 0 && K >= 64 && K <= 256, "tc_selftest: K=%d", K);
   cudaStream_t st = (cudaStream_t)stream;
   TcPrec p{false, 1};
-  int rc = alloc_images(tc_pack_elems(128, K / 32, 128), st, p);
-  if (rc) return rc;
+  SPARF_TRY(alloc_images(tc_pack_elems(128, K / 32, 128), st, p));
   const TcImage a{p.pack_a, K / 32};
-  rc = tc_pack_rows(p, 128, K, A, K, 1, a, st);
+  int rc = tc_pack_rows(p, 128, K, A, K, 1, a, st);
   if (!rc) rc = tc_gemm_nt(p, 0, 128, 128, a, K, TcImage{}, 0, B, K, 0, nullptr, D, 128, TcOut{}, st);
   free_images(p, st);
   return rc;
@@ -1008,10 +993,9 @@ extern "C" int sparf_tc_selftest_tn(const float* G, const float* X, int32_t rows
   cudaStream_t st = (cudaStream_t)stream;
   SPARF_CHECK_CUDA(cudaMemsetAsync(D, 0, 128 * 128 * sizeof(float), st));
   TcPrec p{false, 1};
-  int rc = alloc_images(tc_pack_elems(128, rows / 32, 128), st, p);
-  if (rc) return rc;
+  SPARF_TRY(alloc_images(tc_pack_elems(128, rows / 32, 128), st, p));
   const TcImage gt{p.pack_a, rows / 32};
-  rc = tc_pack_cols(p, rows, 128, G, 128, gt, st);
+  int rc = tc_pack_cols(p, rows, 128, G, 128, gt, st);
   if (!rc) rc = tc_gemm_tn(p, rows, 128, 128, 128, gt, X, 128, 1, D, 128, 0, st);
   free_images(p, st);
   return rc;
@@ -1032,8 +1016,7 @@ static int selftest_images(const float* X, const float* W1, const float* E, cons
   q.max_ctas = max_ctas;
   const TcImage x{nullptr, N / TK}, d{nullptr, K / TK}, e{nullptr, ceil_div(KE, TK)}, dt{nullptr, ceil_div(M, TK)};
   const size_t nx = tc_image_elems(M, N), nd = tc_image_elems(M, K), ne = tc_image_elems(M, KE), ndt = tc_image_elems(K, M);
-  int rc = alloc_images(nx + nd + ne + ndt + tc_pack_elems(std::max(M, N), ceil_div(K + KE, TK), 0), st, q);
-  if (rc) return rc;
+  SPARF_TRY(alloc_images(nx + nd + ne + ndt + tc_pack_elems(std::max(M, N), ceil_div(K + KE, TK), 0), st, q));
   TcImage xi = x, di = d, ei = e, dti = dt;
   xi.p = q.pack_a; di.p = xi.p + nx; ei.p = di.p + nd; dti.p = ei.p + ne;
   SPARF_CHECK_CUDA(cudaMemsetAsync(q.pack_a, 0xFF, (nx + nd + ne + ndt) * 2, st));
@@ -1042,7 +1025,7 @@ static int selftest_images(const float* X, const float* W1, const float* E, cons
   TcOut o;
   o.row = di; o.row_passes = 3;
   o.tr = dti; o.tr_passes = 3;
-  rc = tc_pack_rows(q, M, N, X, N, 1, xi, st);
+  int rc = tc_pack_rows(q, M, N, X, N, 1, xi, st);
   if (!rc) rc = tc_gemm_nn(q, M, N, K, K, xi, W1, K, 0, nullptr, 0, nullptr, nullptr, nullptr, 0, 0, o, db, nullptr, st);
   if (!rc) rc = tc_pack_rows(q, M, KE, E, KE, 1, ei, st);
   if (!rc) rc = tc_gemm_nt(q, 0, M, 128, di, K, ei, KE, W2, K + KE, K, nullptr, Y, 128, TcOut{}, st);

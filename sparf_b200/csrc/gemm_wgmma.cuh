@@ -1,5 +1,5 @@
 // Hopper (sm_90a) tensor-core GEMMs of the layer-by-layer MLP engine: the same three contractions as the CUDA-core
-// FFMA kernels of mlp_simt.cu (NT forward, NN input gradient, TN weight gradient, same epilogues), on wgmma with 16-bit
+// FFMA kernels of mlp.cu (NT forward, NN input gradient, TN weight gradient, same epilogues), on wgmma with 16-bit
 // operands and fp32 accumulation.  passes = 3 splits both fp32 operands into (hi, lo) 16-bit halves and accumulates
 // x_lo*w_hi + x_hi*w_lo (in a second accumulator) + x_hi*w_hi (fp32-level products); passes = 1 multiplies the hi halves only.
 //
