@@ -219,6 +219,37 @@ int sparf_mcubes_emit(const float* vol, int64_t nx, int64_t ny, int64_t nz, floa
  * so two cells sharing a face cut it the same way. */
 int sparf_mcubes_table(int8_t* table);
 
+/* ---------------------------------------------------------------- occupancy grid
+ * Empty-space skipping for inference renders (sparf_b200/occupancy.py): a bitfield over the box [r0, r1]^3 split into
+ * res^3 cells, built from the density lattice sigma [res+1]^3 of mesh.density_grid (lattice point (a,b,c) at
+ * linspace(r0, r1, res+1)[a, b, c], axis 0 = x, c fastest), and a per-sample lookup that compacts the samples a render
+ * must evaluate into the inputs of sparf_mlp_forward.
+ *   cells:   cell (i,j,k) has linear index (i*res + j)*res + k and is bit idx & 31 of word idx >> 5 of
+ *            bits [ceil(res^3 / 32)] (uint32).  Bits past res^3 in the last word are 0.
+ *   build:   a cell is occupied iff a lattice point within one cell of it, indices [c-1, c+2] on each axis clipped to
+ *            [0, res], has sigma >= thres or NaN: the corners of the cell and of its 26 neighbours (dilation radius 1).
+ *   lookup:  sample (r,k) is at x = o[r] + t[r,k] * d[r] per axis in the fp32 op order of the MLP encoder
+ *            (__fadd_rn(o, __fmul_rn(d, t))); u = __fmul_rn(__fdiv_rn(__fsub_rn(x, r0), __fsub_rn(r1, r0)), res).
+ *            The sample is KEPT if any u is NaN, < 0 or >= res (outside the box: always evaluated) or if cell
+ *            ((int)u_x, (int)u_y, (int)u_z) is occupied; otherwise it is skipped.
+ * sparf_occupancy_build writes bits; it needs no workspace.  1 <= res <= 4096.
+ * Compaction: two calls on one stream with one workspace (sparf_occupancy_workspace_bytes(R, S): 4 B per 4 samples + 8 B
+ * per 2048 samples, 0 for invalid sizes).  sparf_occupancy_count reads origins, dirs [R,3], t [R,S] and the bits, and
+ * writes K (device int64) = the number of kept samples, leaving tile-local offsets in the workspace.
+ * sparf_occupancy_emit, enqueued after it with the same arguments and workspace, writes for the kept samples, in
+ * increasing order of r*S + k: sample_idx [K] (int64, r*S + k), origins_k, dirs_k [K,3] (the ray's o and d) and t_k [K]
+ * (t[r,k]): sparf_mlp_forward with R = K, S = 1 on them evaluates exactly the kept samples.  The caller reads K to size
+ * the outputs.  R * S may exceed 2^31 (offsets are 64-bit); R = 0 gives K = 0.  No atomics: the output is
+ * deterministic.  Neither call synchronises; both are capturable. */
+int sparf_occupancy_build(const float* sigma, int32_t res, float thres, uint32_t* bits, sparf_stream_t stream);
+size_t sparf_occupancy_workspace_bytes(int64_t R, int32_t S);
+int sparf_occupancy_count(int64_t R, int32_t S, const float* origins, const float* dirs, const float* t,
+                          const uint32_t* bits, int32_t res, float r0, float r1, int64_t* K, void* workspace,
+                          size_t workspace_bytes, sparf_stream_t stream);
+int sparf_occupancy_emit(int64_t R, int32_t S, const float* origins, const float* dirs, const float* t,
+                         const uint32_t* bits, int32_t res, float r0, float r1, int64_t* sample_idx, float* origins_k,
+                         float* dirs_k, float* t_k, void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+
 /* ---------------------------------------------------------------- compositing
  * NeRF.composite (frequency_nerf.py:283-343).  Outputs: rgb_map [R,3], depth/opacity/depth_var/rgb_var
  * [R], weights [R,S], all_cumulated [R] (= T at sample S-2).  white_bg: rgb += 1 - opacity.

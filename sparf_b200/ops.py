@@ -372,6 +372,50 @@ def marching_cubes(vol, iso: float):
 
 
 # ------------------------------------------------------------------------------------------------
+# occupancy grid (no gradient)
+# ------------------------------------------------------------------------------------------------
+@torch.no_grad()
+@_on_tensor_device
+def occupancy_build(sigma, thres: float):
+    """Density lattice sigma [res+1]^3 -> occupancy bits [ceil(res^3 / 32)] (int32 storage of the uint32 words): cell
+    (i,j,k) is occupied iff a lattice point with indices in [c-1, c+2] per axis has sigma >= thres or NaN (semantics in
+    include/sparf_b200.h)."""
+    L = _lib.lib()
+    s = _f32c(sigma)
+    assert s.dim() == 3 and s.shape[0] == s.shape[1] == s.shape[2] >= 2, "occupancy_build takes a [res+1]^3 lattice"
+    res = s.shape[0] - 1
+    bits = torch.empty((res ** 3 + 31) // 32, dtype=torch.int32, device=s.device)
+    check(L.sparf_occupancy_build(_ptr(s), res, float(thres), _ptr(bits), _stream()), "occupancy_build")
+    return bits
+
+
+@torch.no_grad()
+@_on_tensor_device
+def occupancy_compact(bits, res: int, range, origins, dirs, t):
+    """The samples x = o + t d (origins, dirs [R,3], t [R,S]) an occupancy grid keeps -> (sample_idx [K] int64 = r * S + k,
+    origins_k [K,3], dirs_k [K,3], t_k [K,1]) in increasing sample order: the inputs of mlp_forward for exactly the kept
+    samples.  One device-to-host copy (K).  Not differentiable."""
+    L = _lib.lib()
+    o, d, tt = _f32c(origins), _f32c(dirs), _f32c(t)
+    R, S = tt.shape
+    assert o.shape == (R, 3) and d.shape == (R, 3)
+    assert bits.dtype == torch.int32 and bits.is_contiguous() and bits.numel() == (res ** 3 + 31) // 32
+    r0, r1 = float(range[0]), float(range[1])
+    dev = tt.device
+    ws = _workspace(L.sparf_occupancy_workspace_bytes(R, S), dev)
+    K = torch.empty((), dtype=torch.int64, device=dev)
+    args = (R, S, _ptr(o), _ptr(d), _ptr(tt), _ptr(bits), int(res), r0, r1)
+    check(L.sparf_occupancy_count(*args, _ptr(K), _ptr(ws), ws.numel(), _stream()), "occupancy_count")
+    k = int(K.item())
+    sample_idx = torch.empty(k, dtype=torch.int64, device=dev)
+    o_k, d_k = torch.empty(k, 3, device=dev), torch.empty(k, 3, device=dev)
+    t_k = torch.empty(k, 1, device=dev)
+    check(L.sparf_occupancy_emit(*args, _ptr(sample_idx), _ptr(o_k), _ptr(d_k), _ptr(t_k), _ptr(ws), ws.numel(), _stream()),
+          "occupancy_emit")
+    return sample_idx, o_k, d_k, t_k
+
+
+# ------------------------------------------------------------------------------------------------
 # compositing
 # ------------------------------------------------------------------------------------------------
 class CompositeFunction(torch.autograd.Function):

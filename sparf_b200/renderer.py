@@ -180,16 +180,32 @@ class Graph(torch.nn.Module):
             cache[n] = torch.arange(start=0, end=n, device=self.device)
         return cache[n]
 
+    # ---------------------------------------------------------------------------- occupancy grids
+    def set_occupancy(self, grid, grid_fine=None):
+        """Attach occupancy grids (sparf_b200.occupancy.OccupancyGrid) to the coarse and the fine network; None detaches.
+        `render` then skips the samples a network's grid marks empty, but only in val / eval / test mode with gradients
+        off: every other call renders densely.  Without a fine grid the fine pass stays dense."""
+        self._occupancy = (grid, grid_fine)
+
+    def _forward_samples(self, nerf, which, opt, center, ray, depth_samples, mode):
+        """nerf.forward_samples, or occupancy.forward_samples when grid `which` (0 coarse, 1 fine) applies"""
+        grid = getattr(self, "_occupancy", (None, None))[which]
+        if grid is not None and mode in ("val", "eval", "test") and not torch.is_grad_enabled():
+            from . import occupancy
+            return occupancy.forward_samples(nerf, grid, center, ray, depth_samples)
+        return nerf.forward_samples(opt, center, ray, depth_samples, embedder_pts=self.embedder_pts,
+                                    embedder_view=self.embedder_view, mode=mode)
+
     # ---------------------------------------------------------------------------- core
     def render(self, opt, pose, H, W, intr, pixels=None, ray_idx=None, depth_range=None, iter=None, mode=None):
-        """Coarse pass + optional hierarchical fine pass (renderer.py:250-345)."""
+        """Coarse pass + optional hierarchical fine pass (renderer.py:250-345).  With an occupancy grid attached
+        (set_occupancy), val / eval / test renders without gradients skip the samples it marks empty."""
         batch_size = len(pose)
         center, ray = self._rays(pose, intr, H, W, pixels, ray_idx)          # [B,N,3]
         pred = edict(origins=center, viewdirs=ray)
         depth_samples = self.sample_depth(opt, batch_size, num_rays=ray.shape[1], n_samples=opt.nerf.sample_intvs,
                                           H=H, W=W, depth_range=depth_range, mode=mode)   # [B,N,S,1]
-        pred_coarse = self.nerf.forward_samples(opt, center, ray, depth_samples, embedder_pts=self.embedder_pts,
-                                                embedder_view=self.embedder_view, mode=mode)
+        pred_coarse = self._forward_samples(self.nerf, 0, opt, center, ray, depth_samples, mode)
         pred_coarse["t"] = depth_samples
         pred_coarse = self.nerf.composite(opt, ray, pred_coarse, depth_samples)
         pred.update(pred_coarse)
@@ -198,8 +214,7 @@ class Graph(torch.nn.Module):
                 det = mode not in ["train", "test-optim"] or (not opt.nerf.sample_stratified)
                 depth_all = self._resample_and_merge(opt, pred_coarse["weights"][..., 0], depth_samples[..., 0],
                                                      depth_range, det)           # [B,N,S+Sf,1]
-            pred_fine = self.nerf_fine.forward_samples(opt, center, ray, depth_all, embedder_pts=self.embedder_pts,
-                                                       embedder_view=self.embedder_view, mode=mode)
+            pred_fine = self._forward_samples(self.nerf_fine, 1, opt, center, ray, depth_all, mode)
             pred_fine["t"] = depth_all
             pred_fine = self.nerf_fine.composite(opt, ray, pred_fine, depth_all)
             pred.update({k + "_fine": v for k, v in pred_fine.items()})
