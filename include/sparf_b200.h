@@ -250,6 +250,40 @@ int sparf_occupancy_emit(int64_t R, int32_t S, const float* origins, const float
                          const uint32_t* bits, int32_t res, float r0, float r1, int64_t* sample_idx, float* origins_k,
                          float* dirs_k, float* t_k, void* workspace, size_t workspace_bytes, sparf_stream_t stream);
 
+/* ---------------------------------------------------------------- early ray termination
+ * Inference renders stop evaluating a ray once it is opaque (sparf_b200/termination.py).  A pass's S samples per ray
+ * are split into windows [k0, min(k0 + window, S)), k0 = 0, window, 2*window, ...; every ray is alive in the first.
+ * A window evaluates (the MLP) the samples of the alive rays, and with an occupancy grid only those the grid keeps;
+ * every other sample counts as sigma = 0, rgb = 0.  After each window every alive ray r adds the window's optical
+ * depth to its running tau[r] (fp32, 0 at the start), sequentially in k, each op rounded to nearest (no contraction):
+ *   len  = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)))   (d = dirs[r])
+ *   gap  = k + 1 < S ? __fsub_rn(t[r,k+1], t[r,k]) : 1e10f
+ *   tau  = __fadd_rn(tau, __fmul_rn(sigma[r,k], __fmul_rn(gap, len)))
+ * with sigma [R,S] the pass's output so far (0 at every skipped sample, so 0 * inf gives a NaN tau).  The ray dies
+ * when tau > tau_max, where tau_max = fp32(-ln eps) is computed by the caller (eps = 0: +inf, nothing dies); a NaN
+ * tau keeps the ray alive.  A dead ray's later samples are all skipped.  The composite of such a pass differs from the
+ * dense one (same t) only by the mass behind a transmittance exp(-tau) < eps: |d opacity| < eps, |d rgb| < eps (2 eps
+ * with an opaque background), |d depth| < eps * max t, up to the composite's own fp32 rounding.
+ * Compaction of one window: sparf_termination_count / _emit, the two-call contract of sparf_occupancy_count / _emit
+ * (same outputs, in increasing order of r*S + k, one workspace) over the samples k in [k0, k1) of the rays with
+ * alive[r] != 0 (uint8 [R]; NULL = all alive).  bits = NULL: no grid (res, r0, r1 ignored); otherwise a sample must
+ * also be KEPT by the occupancy lookup above.  Workspace: sparf_termination_workspace_bytes(R, k1 - k0) (the
+ * occupancy workspace of R x (k1 - k0) samples; 0 for invalid sizes).  0 <= k0 < k1 <= S.
+ * sparf_termination_update: for each ray with alive[r] != 0, adds the samples k in [k0, k1) to tau [R] (in / out) as
+ * above and clears alive[r] when tau > tau_max.  Rays with alive[r] == 0 are untouched.
+ * No atomics; none of the calls synchronises.  A render's loop over the windows reads K once per window on the host,
+ * so that loop cannot be captured into a CUDA graph. */
+size_t sparf_termination_workspace_bytes(int64_t R, int32_t window);
+int sparf_termination_count(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins, const float* dirs,
+                            const float* t, const uint8_t* alive, const uint32_t* bits, int32_t res, float r0, float r1,
+                            int64_t* K, void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+int sparf_termination_emit(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins, const float* dirs,
+                           const float* t, const uint8_t* alive, const uint32_t* bits, int32_t res, float r0, float r1,
+                           int64_t* sample_idx, float* origins_k, float* dirs_k, float* t_k, void* workspace,
+                           size_t workspace_bytes, sparf_stream_t stream);
+int sparf_termination_update(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* sigma, const float* t,
+                             const float* dirs, float tau_max, float* tau, uint8_t* alive, sparf_stream_t stream);
+
 /* ---------------------------------------------------------------- compositing
  * NeRF.composite (frequency_nerf.py:283-343).  Outputs: rgb_map [R,3], depth/opacity/depth_var/rgb_var
  * [R], weights [R,S], all_cumulated [R] (= T at sample S-2).  white_bg: rgb += 1 - opacity.

@@ -416,6 +416,54 @@ def occupancy_compact(bits, res: int, range, origins, dirs, t):
 
 
 # ------------------------------------------------------------------------------------------------
+# early ray termination (no gradient)
+# ------------------------------------------------------------------------------------------------
+@torch.no_grad()
+@_on_tensor_device
+def termination_compact(origins, dirs, t, k0: int, k1: int, alive=None, bits=None, res: int = 0, range=None):
+    """The samples k in [k0, k1) of the rays with alive[r] != 0 (uint8 [R]; None = every ray) of origins, dirs [R,3],
+    t [R,S], and with occupancy bits (res, range as in occupancy_compact) only those the grid keeps -> (sample_idx [K]
+    int64 = r * S + k, origins_k [K,3], dirs_k [K,3], t_k [K,1]) in increasing sample order.  One device-to-host copy
+    (K).  Not differentiable."""
+    L = _lib.lib()
+    o, d, tt = _f32c(origins), _f32c(dirs), _f32c(t)
+    R, S = tt.shape
+    assert o.shape == (R, 3) and d.shape == (R, 3)
+    assert alive is None or (alive.dtype == torch.uint8 and alive.is_contiguous() and alive.shape == (R,))
+    r0, r1 = (0.0, 1.0) if bits is None else (float(range[0]), float(range[1]))
+    if bits is not None:
+        assert bits.dtype == torch.int32 and bits.is_contiguous() and bits.numel() == (res ** 3 + 31) // 32
+    dev = tt.device
+    ws = _workspace(L.sparf_termination_workspace_bytes(R, k1 - k0), dev)
+    K = torch.empty((), dtype=torch.int64, device=dev)
+    args = (R, S, int(k0), int(k1), _ptr(o), _ptr(d), _ptr(tt), _ptr(alive), _ptr(bits), int(res), r0, r1)
+    check(L.sparf_termination_count(*args, _ptr(K), _ptr(ws), ws.numel(), _stream()), "termination_count")
+    k = int(K.item())
+    sample_idx = torch.empty(k, dtype=torch.int64, device=dev)
+    o_k, d_k = torch.empty(k, 3, device=dev), torch.empty(k, 3, device=dev)
+    t_k = torch.empty(k, 1, device=dev)
+    check(L.sparf_termination_emit(*args, _ptr(sample_idx), _ptr(o_k), _ptr(d_k), _ptr(t_k), _ptr(ws), ws.numel(),
+                                   _stream()), "termination_emit")
+    return sample_idx, o_k, d_k, t_k
+
+
+@torch.no_grad()
+@_on_tensor_device
+def termination_update(sigma, t, dirs, k0: int, k1: int, tau_max: float, tau, alive):
+    """In place, for every ray with alive[r] != 0: tau[r] += the optical depth of its samples k in [k0, k1) (sigma, t
+    [R,S], dirs [R,3]; op order in include/sparf_b200.h), then alive[r] = 0 when tau[r] > tau_max.  tau: float32 [R],
+    alive: uint8 [R], both contiguous."""
+    L = _lib.lib()
+    s, tt, d = _f32c(sigma), _f32c(t), _f32c(dirs)
+    R, S = tt.shape
+    assert s.shape == (R, S) and d.shape == (R, 3)
+    assert tau.dtype == torch.float32 and tau.is_contiguous() and tau.shape == (R,)
+    assert alive.dtype == torch.uint8 and alive.is_contiguous() and alive.shape == (R,)
+    check(L.sparf_termination_update(R, S, int(k0), int(k1), _ptr(s), _ptr(tt), _ptr(d), float(tau_max), _ptr(tau),
+                                     _ptr(alive), _stream()), "termination_update")
+
+
+# ------------------------------------------------------------------------------------------------
 # compositing
 # ------------------------------------------------------------------------------------------------
 class CompositeFunction(torch.autograd.Function):

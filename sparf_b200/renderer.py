@@ -187,10 +187,25 @@ class Graph(torch.nn.Module):
         off: every other call renders densely.  Without a fine grid the fine pass stays dense."""
         self._occupancy = (grid, grid_fine)
 
+    def set_early_termination(self, eps=1e-4, window=16):
+        """Stop evaluating a ray once its transmittance is below eps (sparf_b200.termination), checked every `window`
+        samples, in the coarse and the fine pass and on top of any occupancy grid; None detaches.  Like the grids it
+        applies only in val / eval / test mode with gradients off."""
+        if eps is None:
+            self._termination = None
+            return
+        assert 0 <= eps < 1 and int(window) == window >= 1, (eps, window)
+        self._termination = (float(eps), int(window))
+
     def _forward_samples(self, nerf, which, opt, center, ray, depth_samples, mode):
-        """nerf.forward_samples, or occupancy.forward_samples when grid `which` (0 coarse, 1 fine) applies"""
+        """nerf.forward_samples, or in val / eval / test mode without gradients termination.forward_samples when early
+        termination is set, occupancy.forward_samples when only grid `which` (0 coarse, 1 fine) is attached"""
         grid = getattr(self, "_occupancy", (None, None))[which]
-        if grid is not None and mode in ("val", "eval", "test") and not torch.is_grad_enabled():
+        term = getattr(self, "_termination", None)
+        if (grid is not None or term is not None) and mode in ("val", "eval", "test") and not torch.is_grad_enabled():
+            if term is not None:
+                from . import termination
+                return termination.forward_samples(nerf, grid, *term, center, ray, depth_samples)
             from . import occupancy
             return occupancy.forward_samples(nerf, grid, center, ray, depth_samples)
         return nerf.forward_samples(opt, center, ray, depth_samples, embedder_pts=self.embedder_pts,
@@ -199,7 +214,8 @@ class Graph(torch.nn.Module):
     # ---------------------------------------------------------------------------- core
     def render(self, opt, pose, H, W, intr, pixels=None, ray_idx=None, depth_range=None, iter=None, mode=None):
         """Coarse pass + optional hierarchical fine pass (renderer.py:250-345).  With an occupancy grid attached
-        (set_occupancy), val / eval / test renders without gradients skip the samples it marks empty."""
+        (set_occupancy), val / eval / test renders without gradients skip the samples it marks empty; with early
+        termination set (set_early_termination), they also skip the samples behind an opaque point of the ray."""
         batch_size = len(pose)
         center, ray = self._rays(pose, intr, H, W, pixels, ray_idx)          # [B,N,3]
         pred = edict(origins=center, viewdirs=ray)
