@@ -367,6 +367,21 @@ int sparf_tc_selftest_head(const float* d_rgb, const float* rgb, const float* d_
  * then colsum_kernel's.  The images must be bit-identical; the sums are where the inputs sum exactly in any order. */
 int sparf_tc_selftest_featgrad(const float* d_raw, const float* d_feat, const float* feat, int32_t M, int32_t W,
                                int32_t row_passes, int32_t tr_passes, uint16_t* img, float* sums, sparf_stream_t stream);
+/* The weight-gradient GEMM as the engines run it, with the ReLU mask bits its operand pack writes: dW[N,K] (zeroed
+ * first) gets sum_m G[m][n] X[m / div][k] for k < Kv (0 elsewhere), with G [M,N] fp32 packed as its transposed bf16 image and both
+ * operands split in `passes` (1 or 3) passes; X has rows of ldx >= K floats.  bits (may be NULL) [M, ceil(K/32)] gets
+ * bit k % 32 of word k / 32 of row m = (X[m / div][k] > 0).  M in [1, 2^20], N and K in [1, 512], div >= 1; max_ctas > 0
+ * caps the grid (else one CTA per SM). */
+int sparf_tc_selftest_wgrad(const float* G, const float* X, int32_t M, int32_t N, int32_t K, int32_t Kv, int32_t ldx,
+                            int32_t div, int32_t passes, int32_t max_ctas, float* dW, uint32_t* bits, sparf_stream_t stream);
+/* The input-gradient GEMM's two ReLU masks against each other, 3-pass bf16: D = (X > 0) * (G W), G [M,N], W [N,K],
+ * X [M,K] fp32 row-major, written only as its row and transposed images, once with the fp32 mask X and once with the
+ * bits of X > 0 that the weight-gradient GEMM G^T X writes.  img gets, after a fill with 0xFFFF, the fp32-mask run's
+ * row image (ceil(M/128) * ceil(K/32) * 8192 elements) and transposed image (ceil(K/128) * ceil(M/32) * 8192), then the
+ * bit-mask run's two; they must be bit-identical.  M in [1, 2^20], N in [1, 512], K even in [2, 512]; max_ctas > 0
+ * caps the grids. */
+int sparf_tc_selftest_mask_bits(const float* G, const float* W, const float* X, int32_t M, int32_t N, int32_t K,
+                                int32_t max_ctas, uint16_t* img, sparf_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -84,6 +84,9 @@ _SIGNATURES = {
     "sparf_tc_selftest_persistent": (c_int32, [_P, _P, _P, _P, c_int32, _P, _P, _P, c_int32, _P]),
     "sparf_tc_selftest_head": (c_int32, [_P, _P, _P, _P, _P, _P, c_int32, c_int32, c_int32, c_int32, _P, _P, _P]),
     "sparf_tc_selftest_featgrad": (c_int32, [_P, _P, _P, c_int32, c_int32, c_int32, c_int32, _P, _P, _P]),
+    "sparf_tc_selftest_wgrad": (c_int32, [_P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                          _P, _P, _P]),
+    "sparf_tc_selftest_mask_bits": (c_int32, [_P, _P, _P, c_int32, c_int32, c_int32, c_int32, _P, _P]),
 }
 
 _lib = None

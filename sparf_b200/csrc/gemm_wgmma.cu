@@ -19,6 +19,7 @@
 #include <cuda_fp16.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "gemm_wgmma.cuh"
 
@@ -147,9 +148,13 @@ struct Cols {   // X[m][n] as rows n, contraction over m
     return (m < M && n < N) ? X[(size_t)m * ldx + n] : 0.f;
   }
 };
-struct TnB {    // X[m / div][k] as rows k, contraction over m
+// X[m / div][k] as rows k, contraction over m.  bits (may be NULL): pack_kernel also writes bits[m][k >> 5] bit k & 31
+// = X[m / div][k] > 0 (kw = ceil(K / 32) words per row), the ReLU mask of the same layer's input gradient.
+struct TnB {
   const float* X;
   int ldx, div, M, K;
+  uint32_t* bits;
+  int kw;
   __device__ float operator()(int kt, int k, int mm) const {
     const int m = kt * TK + mm;
     return (m < M && k < K) ? X[(size_t)(m / div) * ldx + k] : 0.f;
@@ -168,6 +173,21 @@ __global__ void __launch_bounds__(256) pack_kernel(F f, int ksteps, uint16_t* __
     int r, k;
     tile_pos<KFAST>(i, r, k);
     v[i] = f(kt, rt * TM + r, k);
+  }
+  if constexpr (std::is_same<F, TnB>::value) {
+    // warp w holds rows r = 32 (w % 4) + lane (one bit word) of k-columns mm = w / 4 + 2 i: a ballot per i makes word
+    // (m = kt * 32 + mm, rt * 4 + w % 4), which lane i stores; every word is written by one block
+    if (f.bits) {
+      const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+      uint32_t word = 0;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const uint32_t b = __ballot_sync(0xffffffffu, v[i] > 0.f);
+        if (lane == i) word = b;
+      }
+      const int m = kt * TK + (w >> 2) + 2 * lane, c = rt * (TM / 32) + (w & 3);
+      if (lane < 16 && m < f.M && c < f.kw) f.bits[(size_t)m * f.kw + c] = word;
+    }
   }
 #pragma unroll
   for (int i = 0; i < 16; ++i) {
@@ -457,13 +477,20 @@ struct Epi {
   const float* bias;
   float* out;
   int ldo, col_off, Kv;
-  const float *mask, *r1_vec, *r1_row;
+  union {
+    const float* mask;          // kind 1, ldbits == 0: keep = mask[m][n] > 0
+    const uint32_t* mask_bits;  // kind 1, ldbits > 0: keep = bit n & 31 of word [m][n >> 5], ldbits words per row
+  };
+  const float *r1_vec, *r1_row;
   int ldmask, accumulate;
   float* colsum;            // kind 1: += column sums of the output
   float* r1_wgrad;          // kind 1 with mask and r1_vec: += sum_m r1_vec[m] mask[m][n] (the density row's gradient)
   uint16_t *row, *tr;      // output images, row_ks / tr_ks k-steps per row tile
   int row_ks, tr_ks;
   int pairs;                // N even, out and mask 8-byte aligned with even leading dimensions (kinds 0 and 1)
+  // Last, in what was padding: the kernels' code is sensitive to the size of this parameter (a larger Epi made ptxas
+  // build the forward GEMM's epilogue differently, and that GEMM ran about 10 % slower).
+  int ldbits;
 };
 
 // The work units of a persistent GEMM: unit u = output tile u % tiles (B row tile t % rtb, A row tile t / rtb: the B
@@ -632,7 +659,29 @@ __device__ __forceinline__ void epilogue_values(float (&acc)[64], int m0, int n0
   // layer's input.  Only the input-gradient GEMMs that write images (no fp32 output) carry that code; it would change
   // how the compiler builds the other instantiations' epilogues.
   uint64_t keep = ~0ull;
-  if (e.kind == 1 && e.mask) {
+  if (!F32 && e.kind == 1 && e.ldbits > 0) {
+    // the same bits as one word per 32 columns: this thread's two rows of the tile's four words (2 KB per tile).  Like
+    // r1_wgrad, only the image-writing input gradients carry this code, so that the other instantiations keep theirs.
+    uint32_t wd[2][TN / 32];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = m0 + frag_row(2 * h);
+#pragma unroll
+      for (int q = 0; q < TN / 32; ++q) {
+        const int c = (n0 >> 5) + q;
+        wd[h][q] = m < e.M && c < e.ldbits ? e.mask_bits[(size_t)m * e.ldbits + c] : 0u;
+      }
+    }
+    keep = 0;
+#pragma unroll
+    for (int i = 0; i < 64; i += 2) {     // columns n0 + 8 j + 2 (lane % 4) + {0, 1}, j = i / 4
+      const int j = i >> 2, b = 8 * (j & 3) + 2 * (threadIdx.x & 3);
+      keep |= (uint64_t)(wd[(i >> 1) & 1][j >> 2] >> b & 3u) << i;
+    }
+  } else if (e.kind == 1 && e.mask) {
+    // e.mask shares its storage with e.mask_bits: this branch may read it as fp32 only because a bit mask never reaches
+    // it.  The branch above takes every bit mask of the !F32 instantiations, and tc_gemm_nn refuses a bit mask with an
+    // fp32 output D, so the F32 instantiations are never given one.
     float rv[2] = {0.f, 0.f}, part[32];
     if constexpr (!F32) {
 #pragma unroll
@@ -884,13 +933,19 @@ int tc_gemm_nt(TcPrec p, int act, int M, int N, TcImage a1, int K1v, TcImage a2,
 }
 
 int tc_gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, TcImage g, const float* W, int ldw, int wcol, const float* mask_src,
-               int ldmask, const float* r1_vec, const float* r1_row, float* D, int ldd, int accumulate, const TcOut& out,
-               float* db, float* r1_wgrad, cudaStream_t st) {
+               int ldmask, const uint32_t* mask_bits, const float* r1_vec, const float* r1_row, float* D, int ldd,
+               int accumulate, const TcOut& out, float* db, float* r1_wgrad, cudaStream_t st) {
   SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && g.ks == ceil_div(N, TK), "tc_gemm_nn: passes=%d ks=%d N=%d", p.passes,
                 g.ks, N);
   SPARF_REQUIRE(!r1_wgrad || (mask_src && r1_vec && !D), "tc_gemm_nn: r1_wgrad needs the mask source, r1_vec, no fp32 D");
+  SPARF_REQUIRE(!mask_src || !mask_bits, "tc_gemm_nn: an fp32 mask or a bit mask, not both");
+  SPARF_REQUIRE(!mask_bits || !D, "tc_gemm_nn: a bit mask needs image outputs only (no fp32 D)");
   Epi e{};
   e.kind = 1; e.M = M; e.N = Kout; e.out = D; e.ldo = ldd; e.Kv = Kv; e.mask = mask_src; e.ldmask = ldmask;
+  if (mask_bits) {
+    e.mask_bits = mask_bits;
+    e.ldbits = ceil_div(Kout, 32);
+  }
   e.r1_vec = r1_vec; e.r1_row = r1_row; e.accumulate = accumulate; e.colsum = db; e.r1_wgrad = r1_wgrad;
   e.pairs = Kout % 2 == 0 && pair_aligned(D, ldd) && pair_aligned(mask_src, ldmask);
   SPARF_REQUIRE(!db || !accumulate, "tc_gemm_nn: column sums of an accumulated output");
@@ -899,11 +954,11 @@ int tc_gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, TcImage g, const float*
 }
 
 int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, TcImage gt, const float* X, int ldx, int div, float* dW, int ldw,
-               int wcol, cudaStream_t st) {
+               int wcol, uint32_t* bits, cudaStream_t st) {
   SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && gt.ks == ceil_div(M, TK), "tc_gemm_tn: passes=%d ks=%d", p.passes, gt.ks);
   Epi e{};
   e.kind = 2; e.M = N; e.N = K; e.out = dW; e.ldo = ldw; e.col_off = wcol; e.Kv = Kv;
-  return SPARF_WG_RUN(false, p, opnd(gt), N, TnB{X, ldx, div, M, K}, K, gt.ks, true, e, 0, 0, st);
+  return SPARF_WG_RUN(false, p, opnd(gt), N, TnB{X, ldx, div, M, K, bits, ceil_div(K, 32)}, K, gt.ks, true, e, 0, 0, st);
 }
 
 template <int ROWP, int TRP>
@@ -996,7 +1051,7 @@ extern "C" int sparf_tc_selftest_tn(const float* G, const float* X, int32_t rows
   SPARF_TRY(alloc_images(tc_pack_elems(128, rows / 32, 128), st, p));
   const TcImage gt{p.pack_a, rows / 32};
   int rc = tc_pack_cols(p, rows, 128, G, 128, gt, st);
-  if (!rc) rc = tc_gemm_tn(p, rows, 128, 128, 128, gt, X, 128, 1, D, 128, 0, st);
+  if (!rc) rc = tc_gemm_tn(p, rows, 128, 128, 128, gt, X, 128, 1, D, 128, 0, nullptr, st);
   free_images(p, st);
   return rc;
 }
@@ -1026,10 +1081,11 @@ static int selftest_images(const float* X, const float* W1, const float* E, cons
   o.row = di; o.row_passes = 3;
   o.tr = dti; o.tr_passes = 3;
   int rc = tc_pack_rows(q, M, N, X, N, 1, xi, st);
-  if (!rc) rc = tc_gemm_nn(q, M, N, K, K, xi, W1, K, 0, nullptr, 0, nullptr, nullptr, nullptr, 0, 0, o, db, nullptr, st);
+  if (!rc)
+    rc = tc_gemm_nn(q, M, N, K, K, xi, W1, K, 0, nullptr, 0, nullptr, nullptr, nullptr, nullptr, 0, 0, o, db, nullptr, st);
   if (!rc) rc = tc_pack_rows(q, M, KE, E, KE, 1, ei, st);
   if (!rc) rc = tc_gemm_nt(q, 0, M, 128, di, K, ei, KE, W2, K + KE, K, nullptr, Y, 128, TcOut{}, st);
-  if (!rc) rc = tc_gemm_tn(q, M, K, N, N, dti, X, N, 1, Z, N, 0, st);
+  if (!rc) rc = tc_gemm_tn(q, M, K, N, N, dti, X, N, 1, Z, N, 0, nullptr, st);
   free_images(q, st);
   return rc;
 }
@@ -1037,6 +1093,62 @@ static int selftest_images(const float* X, const float* W1, const float* E, cons
 extern "C" int sparf_tc_selftest_images(const float* X, const float* W1, const float* E, const float* W2, int32_t M, float* Y,
                                         float* Z, float* db, sparf_stream_t stream) {
   return selftest_images(X, W1, E, W2, M, Y, Z, db, 0, (cudaStream_t)stream);
+}
+
+extern "C" int sparf_tc_selftest_wgrad(const float* G, const float* X, int32_t M, int32_t N, int32_t K, int32_t Kv, int32_t ldx,
+                                       int32_t div, int32_t passes, int32_t max_ctas, float* dW, uint32_t* bits,
+                                       sparf_stream_t stream) {
+  SPARF_REQUIRE(M >= 1 && M <= (1 << 20) && N >= 1 && N <= 512 && K >= 1 && K <= 512 && Kv >= 0 && Kv <= K && ldx >= K &&
+                    div >= 1 && (passes == 1 || passes == 3),
+                "tc_selftest_wgrad: M=%d N=%d K=%d Kv=%d ldx=%d div=%d passes=%d", M, N, K, Kv, ldx, div, passes);
+  SPARF_REQUIRE(G && X && dW, "tc_selftest_wgrad: NULL tensor");
+  cudaStream_t st = (cudaStream_t)stream;
+  SPARF_CHECK_CUDA(cudaMemsetAsync(dW, 0, (size_t)N * K * sizeof(float), st));
+  TcPrec p{false, passes};
+  p.max_ctas = max_ctas;
+  SPARF_TRY(alloc_images(std::max(tc_image_elems(N, M), tc_pack_elems(K, ceil_div(M, TK), 0)), st, p));
+  const TcImage gt{p.pack_a, ceil_div(M, TK)};
+  int rc = tc_pack_cols(p, M, N, G, N, gt, st);
+  if (!rc) rc = tc_gemm_tn(p, M, N, K, Kv, gt, X, ldx, div, dW, K, 0, bits, st);
+  free_images(p, st);
+  return rc;
+}
+
+extern "C" int sparf_tc_selftest_mask_bits(const float* G, const float* W, const float* X, int32_t M, int32_t N, int32_t K,
+                                           int32_t max_ctas, uint16_t* img, sparf_stream_t stream) {
+  SPARF_REQUIRE(M >= 1 && M <= (1 << 20) && N >= 1 && N <= 512 && K >= 2 && K <= 512 && K % 2 == 0,
+                "tc_selftest_mask_bits: M=%d N=%d K=%d", M, N, K);
+  SPARF_REQUIRE(G && W && X && img, "tc_selftest_mask_bits: NULL tensor");
+  cudaStream_t st = (cudaStream_t)stream;
+  TcPrec p{false, 3};
+  p.max_ctas = max_ctas;
+  const size_t ng = tc_image_elems(M, N), ngt = tc_image_elems(N, M);
+  const size_t nrow = tc_image_elems(M, K), ntr = tc_image_elems(K, M);
+  SPARF_TRY(alloc_images(ng + ngt + tc_pack_elems(K, ceil_div(M, TK) + ceil_div(N, TK), 0), st, p));
+  uint32_t* bits = nullptr;
+  float* dW = nullptr;
+  const size_t nbits = (size_t)M * ceil_div(K, 32);
+  SPARF_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&bits), nbits * 4 + (size_t)N * K * sizeof(float), st));
+  dW = reinterpret_cast<float*>(bits + nbits);
+  SPARF_CHECK_CUDA(cudaMemsetAsync(dW, 0, (size_t)N * K * sizeof(float), st));
+  SPARF_CHECK_CUDA(cudaMemsetAsync(img, 0xFF, 2 * (nrow + ntr) * sizeof(uint16_t), st));
+  const TcImage g{p.pack_a, ceil_div(N, TK)}, gt{p.pack_a + ng, ceil_div(M, TK)};
+  TcOut o[2];
+  for (int i = 0; i < 2; ++i) {
+    o[i].row = TcImage{img + i * (nrow + ntr), ceil_div(K, TK)};
+    o[i].tr = TcImage{img + i * (nrow + ntr) + nrow, ceil_div(M, TK)};
+    o[i].row_passes = o[i].tr_passes = 3;
+  }
+  int rc = tc_pack_rows(p, M, N, G, N, 1, g, st);
+  if (!rc) rc = tc_pack_cols(p, M, N, G, N, gt, st);
+  if (!rc) rc = tc_gemm_tn(p, M, N, K, K, gt, X, K, 1, dW, K, 0, bits, st);
+  if (!rc)
+    rc = tc_gemm_nn(p, M, N, K, K, g, W, K, 0, X, K, nullptr, nullptr, nullptr, nullptr, 0, 0, o[0], nullptr, nullptr, st);
+  if (!rc)
+    rc = tc_gemm_nn(p, M, N, K, K, g, W, K, 0, nullptr, 0, bits, nullptr, nullptr, nullptr, 0, 0, o[1], nullptr, nullptr, st);
+  cudaFreeAsync(bits, st);
+  free_images(p, st);
+  return rc;
 }
 
 extern "C" int sparf_tc_selftest_persistent(const float* X, const float* W1, const float* E, const float* W2, int32_t M,

@@ -4,7 +4,8 @@
 // x_lo*w_hi + x_hi*w_lo (in a second accumulator) + x_hi*w_hi (fp32-level products); passes = 1 multiplies the hi halves only.
 //
 // The activation / gradient operand (A) is given as an operand image: either the image a GEMM epilogue wrote of its
-// output, or one packed from fp32 (tc_pack_rows / tc_pack_cols).  The weight operand (B) is packed by each call.
+// output, or one packed from fp32 (tc_pack_rows / tc_pack_cols).  The B operand (a weight, or the weight gradient's
+// activation) is packed by each call.
 #pragma once
 #include "common.cuh"
 
@@ -37,7 +38,7 @@ struct TcOut {
 
 // 16-bit elements of the image of a [rows x cols] matrix
 size_t tc_image_elems(int rows, int cols);
-// 16-bit elements of one B operand image buffer for GEMMs whose operands have at most max(rows, cols) rows and ksteps
+// 16-bit elements of one B operand image buffer for GEMMs whose B operands have at most max(rows, cols) rows and ksteps
 // 32-wide k-steps
 size_t tc_pack_elems(int rows, int ksteps, int cols);
 
@@ -51,15 +52,18 @@ int tc_pack_cols(TcPrec p, int M, int N, const float* X, int ldx, TcImage img, c
 int tc_gemm_nt(TcPrec p, int act, int M, int N, TcImage a1, int K1v, TcImage a2, int K2v, const float* W, int ldw, int wcol2,
                const float* bias, float* Y, int ldy, const TcOut& out, cudaStream_t st);
 // D[m][k] = mask(m,k) * ( sum_n G[m][n] W[n][wcol+k] + r1_vec[m]*r1_row[k] )   (= or +=), G [M x N] as its row image.
-// D may be NULL when out writes images; db (may be NULL) += the column sums of D; r1_wgrad (may be NULL; needs mask_src
-// and r1_vec) += sum_m r1_vec[m] mask_src[m][k], the weight gradient of the rank-1 row when mask_src is the layer input.
+// mask(m,k) = mask_src[m][k] > 0, or bit k & 31 of mask_bits[m][k >> 5] (ceil(Kout / 32) words per row, as tc_gemm_tn
+// writes them; only with D NULL), or 1 when both are NULL.  D may be NULL when out writes images; db (may be NULL) +=
+// the column sums of D; r1_wgrad (may be NULL; needs mask_src and r1_vec) += sum_m r1_vec[m] mask_src[m][k], the weight
+// gradient of the rank-1 row when mask_src is the layer input.
 int tc_gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, TcImage g, const float* W, int ldw, int wcol, const float* mask_src,
-               int ldmask, const float* r1_vec, const float* r1_row, float* D, int ldd, int accumulate, const TcOut& out,
-               float* db, float* r1_wgrad, cudaStream_t st);
+               int ldmask, const uint32_t* mask_bits, const float* r1_vec, const float* r1_row, float* D, int ldd,
+               int accumulate, const TcOut& out, float* db, float* r1_wgrad, cudaStream_t st);
 // dW[n][wcol+k] += sum_m G[m][n] X[m/div][k]   (atomic over k-ranges of the rows, about one per SM per 32 768 rows), G [M x N]
-// as its transposed image
+// as its transposed image.  bits (may be NULL) [M x ceil(K / 32)]: bit k & 31 of word [m][k >> 5] = X[m/div][k] > 0, the
+// ReLU mask of the input gradient of the layer whose input X is, written while X is packed.
 int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, TcImage gt, const float* X, int ldx, int div, float* dW, int ldw,
-               int wcol, cudaStream_t st);
+               int wcol, uint32_t* bits, cudaStream_t st);
 
 // The colour-head backward in one kernel (bf16 images): from the upstream d_rgb [M,3], d_sigma [M], the forward's rgb
 // [M,3], raw [M] (softplus argument) and hid [M,HW], and the head's output layer W9 [3,HW]:

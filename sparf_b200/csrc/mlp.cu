@@ -599,12 +599,14 @@ static Tape tape_chunk(const Tape& t, const MlpDims& d, int r0, int S) {
 // Workspace of one call, per chunk of nrc rays.  Tensor-core engines keep their GEMM operands as images: the forward's
 // encodings and ping-pong trunk activations, the backward's ping-pong trunk gradients (a row image for the next input
 // gradient, a transposed one for the weight gradient; no fp32 copy), the colour-head gradient's two images (no fp32 copy
-// either), and a buffer for the weight operand packed per GEMM.  head = false (density calls, S = 1): no colour-head or
+// either), the ReLU mask bits of one layer input (written by its weight-gradient GEMM, read by its input-gradient GEMM),
+// and a buffer for the B operand packed per GEMM.  head = false (density calls, S = 1): no colour-head or
 // view-direction buffer.
 struct Ws {
   float *wts, *rgbv, *G0, *G1, *Genc, *Ghid, *gpre, *graw, *Gdtmp, *Gdenc;
   Tape act;     // the forward's activations of one chunk (forward and recompute backward)
   TcImage encimg, dencimg, Himg[2], Grow[2], Gtr[2], ghid_row, ghid_tr;
+  uint32_t* mask_bits;   // [Mc x ceil(W / 32)]
   uint16_t* pack_b;
   size_t pack_elems;
 };
@@ -656,12 +658,13 @@ static size_t carve(const MlpDims& d, bool tc, int nrc, int S, Pass pass, bool h
       w.ghid_row = cv.image((int)Mc, d.HW);
       w.ghid_tr = cv.image(d.HW, (int)Mc);
     }
+    w.mask_bits = reinterpret_cast<uint32_t*>(cv.take(Mc * ceil_div(d.W, 32)));
   }
-  if (tc) {     // largest operand images: [max(Mc, width) x (W + encoding)] forward, [width x Mc] weight gradient
+  if (tc) {     // largest B operand images: a weight [width x (W + encoding)], the weight gradient's [width x Mc]
     const int HW = head ? d.HW : 0, Evp = head ? d.Evp : 0;
     const int wmax = std::max(std::max(d.W, HW), std::max(d.E3p, Evp));
-    w.pack_elems = std::max(tc_pack_elems((int)Mc, ceil_div(wmax, 32) + ceil_div(std::max(d.E3p, Evp), 32), wmax),
-                            tc_pack_elems(wmax, ceil_div((long long)Mc, 32), 0));
+    w.pack_elems = tc_pack_elems(wmax, ceil_div(wmax, 32) + ceil_div(std::max(d.E3p, Evp), 32), 0);
+    if (bwd) w.pack_elems = std::max(w.pack_elems, tc_pack_elems(wmax, ceil_div((long long)Mc, 32), 0));
     w.pack_b = reinterpret_cast<uint16_t*>(cv.take((w.pack_elems + 1) / 2));
   }
   if (out) *out = w;
@@ -878,13 +881,14 @@ static int head_backward_tc(const SparfMLP* mlp, const Call& c, long long Mc, in
   const TcImage ghid_t{w.ghid_tr.p, ceil_div(Mc, 32)}, ghid = w.ghid_row;
   SPARF_TRY(tc_head_backward(ep.dgrad, ep.wgrad, (int)Mc, d.HW, d_rgb, rgbv, d_sigma, v.raw, v.hid, mlp->head_w[1], w.graw, ghid,
                              ghid_t, grad->head_w[1], grad->head_b[1], grad->head_b[0], grad->trunk_b[d.nt - 1], st));
-  SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.W, d.W, ghid_t, feat, d.W, 1, grad->head_w[0], ldw8, 0, st));
-  SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.Evp, d.Ev, ghid_t, v.denc, d.Evp, S, grad->head_w[0], ldw8, d.W, st));
-  SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.HW, d.W, d.W, ghid, mlp->head_w[0], ldw8, 0, feat, d.W, nullptr, nullptr, nullptr, 0,
-                       0, grad_images(c, 0, Mc), grad->trunk_b[d.nt - 1] + 1, nullptr, st));
+  // the weight gradient of feat writes its ReLU mask bits, the input gradient of feat reads them
+  SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.W, d.W, ghid_t, feat, d.W, 1, grad->head_w[0], ldw8, 0, w.mask_bits, st));
+  SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.HW, d.Evp, d.Ev, ghid_t, v.denc, d.Evp, S, grad->head_w[0], ldw8, d.W, nullptr, st));
+  SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.HW, d.W, d.W, ghid, mlp->head_w[0], ldw8, 0, nullptr, 0, w.mask_bits, nullptr,
+                       nullptr, nullptr, 0, 0, grad_images(c, 0, Mc), grad->trunk_b[d.nt - 1] + 1, nullptr, st));
   if (dir_grad)
     SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.HW, d.Evp, d.Ev, ghid, mlp->head_w[0], ldw8, d.W, nullptr, 0, nullptr, nullptr,
-                         w.Gdtmp, d.Evp, 0, TcOut{}, nullptr, nullptr, st));
+                         nullptr, w.Gdtmp, d.Evp, 0, TcOut{}, nullptr, nullptr, st));
   return SPARF_OK;
 }
 
@@ -945,16 +949,20 @@ static int trunk_backward_tc(const SparfMLP* mlp, const Call& c, long long Mc, c
     const int rowoff = last ? 1 : 0;
     float* dWl = grad->trunk_w[l] + (size_t)rowoff * ldw;
     const float* Wl = mlp->trunk_w[l] + (size_t)rowoff * ldw;
-    SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, Kin, Kinv, grad_tr(c.w, gi, Mc), in, Kin, 1, dWl, ldw, 0, st));
+    // The input gradient's ReLU mask is H_{l-1} > 0: as bits that the weight gradient writes while it reads H_{l-1} anyway,
+    // except with the density row's rank-1 term, whose weight gradient (r1_wgrad) the epilogue sums from the fp32 values
+    // of H_{l-1}: that layer reads them as its mask.
+    uint32_t* bits = l > 0 && !r1 ? c.w.mask_bits : nullptr;
+    SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, Kin, Kinv, grad_tr(c.w, gi, Mc), in, Kin, 1, dWl, ldw, 0, bits, st));
     if (l == d.skip)
-      SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, d.E3p, d.E3, grad_tr(c.w, gi, Mc), enc, d.E3p, 1, dWl, ldw, d.W, st));
+      SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, d.E3p, d.E3, grad_tr(c.w, gi, Mc), enc, d.E3p, 1, dWl, ldw, d.W, nullptr, st));
     if (l > 0)
-      SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.W, d.W, c.w.Grow[gi], Wl, ldw, 0, in, d.W, r1 ? graw : nullptr,
-                           r1 ? mlp->trunk_w[l] : nullptr, nullptr, 0, 0, grad_images(c, gi ^ 1, Mc), grad->trunk_b[l - 1],
-                           r1 ? grad->trunk_w[l] : nullptr, st));
+      SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.W, d.W, c.w.Grow[gi], Wl, ldw, 0, bits ? nullptr : in, d.W, bits,
+                           r1 ? graw : nullptr, r1 ? mlp->trunk_w[l] : nullptr, nullptr, 0, 0, grad_images(c, gi ^ 1, Mc),
+                           grad->trunk_b[l - 1], r1 ? grad->trunk_w[l] : nullptr, st));
     if (enc_grad && (l == d.skip || l == 0)) {
       SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.E3p, d.E3, c.w.Grow[gi], Wl, ldw, l == 0 ? 0 : d.W, nullptr, 0, nullptr,
-                           nullptr, c.w.Genc, d.E3p, genc_written ? 1 : 0, TcOut{}, nullptr, nullptr, st));
+                           nullptr, nullptr, c.w.Genc, d.E3p, genc_written ? 1 : 0, TcOut{}, nullptr, nullptr, st));
       genc_written = true;
     }
     gi ^= 1;

@@ -23,8 +23,10 @@ PASSES = {"tc_3x": (3, 3, 3), "tc_1x": (1, 1, 1), "tc_3x_w1": (3, 3, 1), "auto":
 
 def gemm_bytes_per_row(spec, passes, backward, pose):
     """HBM bytes per sample row that the wgmma GEMMs must read and write, counted from the shapes: the A operand images,
-    the weight-gradient GEMMs' B operand images (activation-sized), the fp32 outputs, the epilogue images and the fp32
-    ReLU-mask sources.  The weights' images are small and stay in L2; they are not counted."""
+    the weight-gradient GEMMs' B operand images (activation-sized), the fp32 outputs, the epilogue images and the ReLU
+    masks (bits, 1/8 byte per value, written by the weight gradient's operand pack; fp32 at the last trunk layer, whose
+    epilogue sums the density row's weight gradient from the values).  The weights' images are small and stay in L2;
+    they are not counted."""
     pf, pd, pw = passes
     W, HW, skip, nt = spec.width, spec.head_width, spec.skip_layer, spec.n_trunk
     E3p, Evp = -(-(3 + 6 * spec.L_xyz) // 8) * 8, -(-(3 + 6 * spec.L_view) // 8) * 8
@@ -41,7 +43,7 @@ def gemm_bytes_per_row(spec, passes, backward, pose):
     # colour head: two weight-gradient GEMMs (Ghid^T [feat | denc]); the input gradient of feat (mask = feat) as row and
     # transposed images; with pose gradients the direction-encoding gradient in fp32
     n += 2 * img(HW, pw) + img(W, pw) + img(Evp, pw)
-    n += img(HW, pd) + 4 * W + img(W, pd) + img(W, pw)
+    n += img(HW, pd) + W / 8 + img(W, pd) + img(W, pw)
     if pose:
         n += img(HW, pd) + 4 * Evp
     for l in range(nt - 1, -1, -1):
@@ -49,7 +51,7 @@ def gemm_bytes_per_row(spec, passes, backward, pose):
         if l == skip:
             n += img(W, pw) + img(E3p, pw)
         if l > 0:                                                       # input gradient: G image, mask, two images out
-            n += img(W, pd) + 4 * W + img(W, pd) + img(W, pw)
+            n += img(W, pd) + (4 * W if l == nt - 1 else W / 8) + img(W, pd) + img(W, pw)
         if pose and (l == skip or l == 0):                              # encoding gradient, fp32 (+= at layer 0)
             n += img(W, pd) + 4 * E3p + (4 * E3p if l == 0 and skip > 0 else 0)
     return n
