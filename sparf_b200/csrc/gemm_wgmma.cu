@@ -14,7 +14,9 @@
 //     warpgroups wait on it, issue wgmma.m64n128k16 (register accumulators) and hand the stage back on its "empty"
 //     mbarrier once the MMAs that read it have retired.  So the next tile's first stages load during an epilogue.  The
 //     epilogue can write the output's own images (row and transposed) for the next GEMMs, so trunk activations and
-//     gradients are never packed from fp32.
+//     gradients are never packed from fp32;
+//   staged weight-gradient gemm: the same walk, ring and MMAs, with B read as fp32 rows by bulk copies and split in
+//     shared memory by a fourth (converter) warpgroup, so the weight gradient's activation operand is never packed.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -532,9 +534,11 @@ __device__ __forceinline__ void produce(const Opnd& a, const Opnd& b, const Unit
 // The MMAs of one unit of nk k-steps, ring position it on entry (advanced by nk).  acc[64] of this thread = its
 // fragment of the warpgroup's [64 x 128] block: acc[4 j + 2 h + c] is row 16 warp + lane/4 + 8 h, column
 // 8 j + 2 (lane % 4) + c.  One MMA group stays in flight: each warp releases a stage once the group that read it has
-// retired.
-template <bool F16, int PASSES>
-__device__ __forceinline__ void mma_unit(float (&acc)[64], int nk, int& it, uint64_t* full, uint64_t* empty) {
+// retired.  CONV (the staged weight-gradient GEMM): a stage is ready once its copies are complete (full) and its B
+// operand has been split in place (conv).
+template <bool F16, int PASSES, bool CONV = false>
+__device__ __forceinline__ void mma_unit(float (&acc)[64], int nk, int& it, uint64_t* full, uint64_t* empty,
+                                         uint64_t* conv = nullptr) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   float acc_lo[PASSES == 3 ? 64 : 1];
@@ -546,6 +550,7 @@ __device__ __forceinline__ void mma_unit(float (&acc)[64], int nk, int& it, uint
   for (int j = 0; j < nk; ++j, ++it) {
     const int s = it % STAGES;
     mbar_wait(&full[s], (it / STAGES) & 1);
+    if constexpr (CONV) mbar_wait(&conv[s], (it / STAGES) & 1);
     const uint8_t* st = smem + s * STAGE_BYTES;
     wgmma_fence();
 #pragma unroll
@@ -835,6 +840,161 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) wg_gemm_kernel(Opnd a, Opnd b
   }
 }
 
+// The weight gradient's B operand straight from fp32, X[m / div][k] as rows k, contraction over m (TnB's values): X 16-byte
+// aligned, ldx and K multiples of 4 floats, so that every row of a k-step is one bulk copy.  bits (may be NULL) as TnB.
+struct Staged {
+  const float* X;
+  int ldx, div, M, K;
+  uint32_t* bits;
+  int kw;
+};
+
+constexpr int STAGED_THREADS = CONSUMERS + 256;   // + the converter warpgroup (8-11) + the producer warpgroup (12-15)
+constexpr int STAGED_SMEM = STAGES * STAGE_BYTES + 3 * STAGES * 8;
+
+// split8 with the lo half's scaling by 2^LO_SHIFT as a multiply: the same bytes (the scaling of the residual is exact,
+// it overflows to the same infinity, and NaN stays NaN), without the special-case code of ldexpf, which made up most of
+// the converter's instructions
+__device__ __forceinline__ void split8_mul(const float (&v)[8], uint4& hi, uint4& lo) {
+  uint16_t h[8], l[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    const __nv_bfloat16 b = __float2bfloat16_rn(v[e]);
+    h[e] = __bfloat16_as_ushort(b);
+    l[e] = __bfloat16_as_ushort(__float2bfloat16_rn((v[e] - __bfloat162float(b)) * (float)(1 << LO_SHIFT)));
+  }
+  hi = make_uint4(h[0] | (uint32_t)h[1] << 16, h[2] | (uint32_t)h[3] << 16, h[4] | (uint32_t)h[5] << 16, h[6] | (uint32_t)h[7] << 16);
+  lo = make_uint4(l[0] | (uint32_t)l[1] << 16, l[2] | (uint32_t)l[3] << 16, l[4] | (uint32_t)l[5] << 16, l[6] | (uint32_t)l[7] << 16);
+}
+
+__device__ __forceinline__ void converter_sync() { asm volatile("bar.sync 2, 128;\n" ::: "memory"); }
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
+
+// The producer warp: per k-step, the A tile with one copy and the 32 rows m of B (X[m / div][128 bx, 128 bx + 128) in
+// fp32, 512 bytes per row at most) with one copy per lane, into the stage's 16 KB of B halves.  Rows at or past M are not
+// copied and the bytes past K of a row not written; the converter never reads either.
+template <int PASSES>
+__device__ __forceinline__ void produce_staged(const Opnd& a, const Staged& x, const Units& w, uint64_t* full,
+                                               uint64_t* empty) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int lane = threadIdx.x & 31;
+  const uint32_t abytes = PASSES == 3 ? 2 * TILE_BYTES : TILE_BYTES;
+  int it = 0;
+  for (int u = blockIdx.x; u < w.tiles * w.nsplit; u += gridDim.x) {
+    int bx, by, kt0, nk;
+    w.get(u, bx, by, kt0, nk);
+    const int k0 = bx * TM;
+    const uint32_t rbytes = 4 * min(TM, x.K - k0);
+    for (int j = 0; j < nk; ++j, ++it) {
+      const int s = it % STAGES, m0 = (kt0 + j) * TK;
+      mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+      uint8_t* st = smem + s * STAGE_BYTES;
+      if (lane == 0) {
+        mbar_expect_tx(&full[s], abytes + min(TK, x.M - m0) * rbytes);
+        bulk_g2s(st, a.tile(by, kt0 + j), abytes, &full[s]);
+      }
+      __syncwarp();             // the expected bytes are set before any row copy can complete
+      const int m = m0 + lane;
+      if (m < x.M) bulk_g2s(st + 2 * TILE_BYTES + lane * (TM * 4), x.X + (size_t)(m / x.div) * x.ldx + k0, rbytes, &full[s]);
+    }
+  }
+}
+
+// The converter warpgroup: thread t takes column k = 128 bx + t of a staged k-step, reads its 32 values m (lane = k: no
+// bank conflicts), zero at or past M and K, and once the warpgroup has read the whole tile writes them in place as the
+// K-major image pack_kernel<TnB> makes (four 16-byte core-matrix rows per half), then hands the stage to the consumers
+// on conv[s].  Its warps also write the ReLU bits of units with by == 0 (one per (bx, k-step)): a ballot per row m.
+template <int PASSES>
+__device__ __forceinline__ void convert_staged(const Staged& x, const Units& w, uint64_t* full, uint64_t* conv) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int t = threadIdx.x - CONSUMERS, lane = t & 31;
+  int it = 0;
+  for (int u = blockIdx.x; u < w.tiles * w.nsplit; u += gridDim.x) {
+    int bx, by, kt0, nk;
+    w.get(u, bx, by, kt0, nk);
+    const bool kin = bx * TM + t < x.K, bits = x.bits && by == 0;
+    const int bword = bx * (TM / 32) + (t >> 5);
+    for (int j = 0; j < nk; ++j, ++it) {
+      const int s = it % STAGES, m0 = (kt0 + j) * TK;
+      mbar_wait(&full[s], (it / STAGES) & 1);
+      uint8_t* st = smem + s * STAGE_BYTES + 2 * TILE_BYTES;
+      const float* src = reinterpret_cast<const float*>(st);
+      float v[TK];
+      if (kin && m0 + TK <= x.M) {
+#pragma unroll
+        for (int r = 0; r < TK; ++r) v[r] = src[r * TM + t];
+      } else {
+#pragma unroll
+        for (int r = 0; r < TK; ++r) v[r] = kin && m0 + r < x.M ? src[r * TM + t] : 0.f;
+      }
+      if (bits) {
+        uint32_t word = 0;
+#pragma unroll
+        for (int r = 0; r < TK; ++r) {
+          const uint32_t b = __ballot_sync(0xffffffffu, v[r] > 0.f);
+          if (lane == r) word = b;
+        }
+        if (m0 + lane < x.M && bword < x.kw) x.bits[(size_t)(m0 + lane) * x.kw + bword] = word;
+      }
+      converter_sync();         // the whole tile has been read before it is overwritten
+      uint16_t* img = reinterpret_cast<uint16_t*>(st);
+#pragma unroll
+      for (int o = 0; o < TK / 8; ++o) {
+        float e8[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) e8[e] = v[8 * o + e];
+        uint4 hi, lo;
+        split8_mul(e8, hi, lo);
+        const int off = sw_off(t, 8 * o);
+        *reinterpret_cast<uint4*>(img + off) = hi;
+        if (PASSES == 3) *reinterpret_cast<uint4*>(img + TILE_ELEMS + off) = lo;
+      }
+      fence_proxy_async();      // the image is visible to the MMAs; the reads above precede the stage's next copies
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&conv[s]);
+    }
+  }
+}
+
+// The weight-gradient GEMM dW += G^T X with B read as fp32 (Staged): wg_gemm_kernel's units, ring, MMAs and atomic
+// epilogue, with a fourth warpgroup that splits each stage's B in place between its copies and its MMAs, so no pack
+// kernel writes and no GEMM reads an image of X.  Registers: producer 40, converter 64, consumers 200 (<= 64 K).
+template <int PASSES>
+__global__ void __launch_bounds__(STAGED_THREADS, 1) wg_gemm_staged_kernel(Opnd a, Staged x, Units w, Epi e) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+  uint64_t* empty = full + STAGES;
+  uint64_t* conv = empty + STAGES;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], CONSUMERS / 32);
+      mbar_init(&conv[i], 4);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+  }
+  __syncthreads();
+  if (threadIdx.x >= CONSUMERS + 128) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (threadIdx.x < CONSUMERS + 128 + 32) produce_staged<PASSES>(a, x, w, full, empty);
+    return;
+  }
+  if (threadIdx.x >= CONSUMERS) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 64;\n" ::: "memory");
+    convert_staged<PASSES>(x, w, full, conv);
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 200;\n" ::: "memory");
+  int it = 0;
+  for (int u = blockIdx.x; u < w.tiles * w.nsplit; u += gridDim.x) {
+    int bx, by, kt0, nk;
+    w.get(u, bx, by, kt0, nk);
+    float acc[64];
+    mma_unit<false, PASSES, true>(acc, nk, it, full, empty, conv);
+    epilogue<false, true, 0, 0>(acc, bx, by, e);
+  }
+}
+
 template <bool F16, int PASSES, bool KFAST, class F>
 static int launch_pack(F f, int rtiles, int ksteps, uint16_t* img, cudaStream_t st) {
   pack_kernel<F16, PASSES, KFAST, F><<<dim3(ksteps, rtiles), 256, 0, st>>>(f, ksteps, img);
@@ -851,10 +1011,20 @@ static int launch_gemm(const Opnd& a, const Opnd& b, const Units& w, int ctas, c
   return SPARF_OK;
 }
 
-// pack B into p.pack_b, then the persistent GEMM over (B row tiles x A row tiles) output tiles with the epilogue
-// outputs e asks for: fp32 (e.out), a row image (row image passes = the GEMM's), a transposed image.  split_k: each
-// output tile's k-steps are shared out in ceil(CTAs / output tiles) ranges per 32 768 rows (atomic epilogues only), so
-// every CTA does one long reduction per 32 768 rows.
+static int gemm_ctas(const TcPrec& p) { return p.max_ctas > 0 ? std::min(p.max_ctas, num_sms()) : num_sms(); }  // one CTA fills an SM
+
+// The units of a GEMM over (B row tiles x A row tiles) output tiles.  split_k: each output tile's k-steps are shared out
+// in about ceil(CTAs / output tiles) ranges per 1024 k-steps (32 768 rows; atomic epilogues only), so every CTA does one
+// long reduction per 32 768 rows: no accumulator chain gets longer than at 32 768 rows, whatever the chunk size, so the
+// rounding of the sums does not grow with it.
+static Units gemm_units(int rta, int rtb, int ksteps, bool split_k, int ctas) {
+  Units w{rtb, rta * rtb, 1, ksteps};
+  if (split_k) w.nsplit = std::max(1, std::min(ksteps, ceil_div(ctas, w.tiles) * ceil_div(ksteps, 1024)));
+  return w;
+}
+
+// pack B into p.pack_b, then the persistent GEMM over its units (gemm_units) with the epilogue outputs e asks for: fp32
+// (e.out), a row image (row image passes = the GEMM's), a transposed image
 template <bool F16, int PASSES, bool BK, class FB>
 static int run(const TcPrec& p, const Opnd& a, int a_rows, FB fb, int b_rows, int ksteps, bool split_k, const Epi& e,
                int row_passes, int tr_passes, cudaStream_t st) {
@@ -864,11 +1034,8 @@ static int run(const TcPrec& p, const Opnd& a, int a_rows, FB fb, int b_rows, in
                 p.pack_elems);
   SPARF_TRY((launch_pack<F16, PASSES, BK>(fb, rtb, ksteps, p.pack_b, st)));
   const Opnd b{p.pack_b, nullptr, ksteps, 0};
-  const int ctas = p.max_ctas > 0 ? std::min(p.max_ctas, num_sms()) : num_sms();   // one CTA fills an SM
-  Units w{rtb, rta * rtb, 1, ksteps};
-  // about ceil(CTAs / output tiles) ranges per 1024 k-steps (32 768 rows): no accumulator chain gets longer than at
-  // 32 768 rows, whatever the chunk size, so the rounding of the sums does not grow with it
-  if (split_k) w.nsplit = std::max(1, std::min(ksteps, ceil_div(ctas, w.tiles) * ceil_div(ksteps, 1024)));
+  const int ctas = gemm_ctas(p);
+  const Units w = gemm_units(rta, rtb, ksteps, split_k, ctas);
   const bool f32 = e.out != nullptr;
   if (f32 && !row_passes && !tr_passes) return launch_gemm<F16, PASSES, true, 0, 0>(a, b, w, ctas, e, st);
   if (f32 && row_passes == PASSES && !tr_passes) return launch_gemm<F16, PASSES, true, PASSES, 0>(a, b, w, ctas, e, st);
@@ -876,6 +1043,18 @@ static int run(const TcPrec& p, const Opnd& a, int a_rows, FB fb, int b_rows, in
   if (!f32 && row_passes == PASSES && tr_passes == 1) return launch_gemm<F16, PASSES, false, PASSES, 1>(a, b, w, ctas, e, st);
   SPARF_REQUIRE(false, "tc gemm: no kernel for fp32 output %d, row image %d passes, transposed image %d passes", (int)f32,
                 row_passes, tr_passes);
+}
+
+// the weight-gradient GEMM with B = x read as fp32 (no pack), N output rows, over the k-steps of gt
+template <int PASSES>
+static int run_staged(const TcPrec& p, const Opnd& gt, int N, const Staged& x, int ksteps, const Epi& e, cudaStream_t st) {
+  const int ctas = gemm_ctas(p);
+  const Units w = gemm_units(ceil_div(N, TM), ceil_div(x.K, TM), ksteps, true, ctas);
+  auto kernel = wg_gemm_staged_kernel<PASSES>;
+  SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, STAGED_SMEM));
+  kernel<<<std::min(w.tiles * w.nsplit, ctas), STAGED_THREADS, STAGED_SMEM, st>>>(gt, x, w, e);
+  SPARF_CHECK_LAUNCH("wg_gemm_staged_kernel");
+  return SPARF_OK;
 }
 
 static Opnd opnd(const TcImage& x, const TcImage& y = TcImage{}) { return Opnd{x.p, y.p, x.ks, y.ks}; }
@@ -958,6 +1137,12 @@ int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, TcImage gt, const float* X
   SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && gt.ks == ceil_div(M, TK), "tc_gemm_tn: passes=%d ks=%d", p.passes, gt.ks);
   Epi e{};
   e.kind = 2; e.M = N; e.N = K; e.out = dW; e.ldo = ldw; e.col_off = wcol; e.Kv = Kv;
+  // rows of X that bulk copies can read (16-byte aligned), which every engine call has: B is split inside the GEMM
+  if (!(reinterpret_cast<uintptr_t>(X) & 15) && ldx % 4 == 0 && K % 4 == 0) {
+    SPARF_REQUIRE(!p.f16, "tc_gemm_tn: bf16 halves only");
+    const Staged x{X, ldx, div, M, K, bits, ceil_div(K, 32)};
+    return p.passes == 3 ? run_staged<3>(p, opnd(gt), N, x, gt.ks, e, st) : run_staged<1>(p, opnd(gt), N, x, gt.ks, e, st);
+  }
   return SPARF_WG_RUN(false, p, opnd(gt), N, TnB{X, ldx, div, M, K, bits, ceil_div(K, 32)}, K, gt.ks, true, e, 0, 0, st);
 }
 

@@ -4,8 +4,8 @@
 // x_lo*w_hi + x_hi*w_lo (in a second accumulator) + x_hi*w_hi (fp32-level products); passes = 1 multiplies the hi halves only.
 //
 // The activation / gradient operand (A) is given as an operand image: either the image a GEMM epilogue wrote of its
-// output, or one packed from fp32 (tc_pack_rows / tc_pack_cols).  The B operand (a weight, or the weight gradient's
-// activation) is packed by each call.
+// output, or one packed from fp32 (tc_pack_rows / tc_pack_cols).  The B operand (a weight) is packed by each call; the
+// weight gradient's activation operand is read as fp32 and split inside the GEMM.
 #pragma once
 #include "common.cuh"
 
@@ -61,7 +61,9 @@ int tc_gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, TcImage g, const float*
                int accumulate, const TcOut& out, float* db, float* r1_wgrad, cudaStream_t st);
 // dW[n][wcol+k] += sum_m G[m][n] X[m/div][k]   (atomic over k-ranges of the rows, about one per SM per 32 768 rows), G [M x N]
 // as its transposed image.  bits (may be NULL) [M x ceil(K / 32)]: bit k & 31 of word [m][k >> 5] = X[m/div][k] > 0, the
-// ReLU mask of the input gradient of the layer whose input X is, written while X is packed.
+// ReLU mask of the input gradient of the layer whose input X is, written while X is split.  X is read as fp32 inside the
+// GEMM when X is 16-byte aligned and ldx and K are multiples of 4 (bf16 only); otherwise it is packed into p.pack_b
+// first ([ceil(K / 128) * 128 x ceil(M / 32) * 32] image).
 int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, TcImage gt, const float* X, int ldx, int div, float* dW, int ldw,
                int wcol, uint32_t* bits, cudaStream_t st);
 

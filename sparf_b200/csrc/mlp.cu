@@ -600,7 +600,7 @@ static Tape tape_chunk(const Tape& t, const MlpDims& d, int r0, int S) {
 // encodings and ping-pong trunk activations, the backward's ping-pong trunk gradients (a row image for the next input
 // gradient, a transposed one for the weight gradient; no fp32 copy), the colour-head gradient's two images (no fp32 copy
 // either), the ReLU mask bits of one layer input (written by its weight-gradient GEMM, read by its input-gradient GEMM),
-// and a buffer for the B operand packed per GEMM.  head = false (density calls, S = 1): no colour-head or
+// and a buffer for the weight operand packed per GEMM.  head = false (density calls, S = 1): no colour-head or
 // view-direction buffer.
 struct Ws {
   float *wts, *rgbv, *G0, *G1, *Genc, *Ghid, *gpre, *graw, *Gdtmp, *Gdenc;
@@ -660,11 +660,10 @@ static size_t carve(const MlpDims& d, bool tc, int nrc, int S, Pass pass, bool h
     }
     w.mask_bits = reinterpret_cast<uint32_t*>(cv.take(Mc * ceil_div(d.W, 32)));
   }
-  if (tc) {     // largest B operand images: a weight [width x (W + encoding)], the weight gradient's [width x Mc]
+  if (tc) {     // largest B operand image: a weight [width x (W + encoding)] (the weight gradients read theirs as fp32)
     const int HW = head ? d.HW : 0, Evp = head ? d.Evp : 0;
     const int wmax = std::max(std::max(d.W, HW), std::max(d.E3p, Evp));
     w.pack_elems = tc_pack_elems(wmax, ceil_div(wmax, 32) + ceil_div(std::max(d.E3p, Evp), 32), 0);
-    if (bwd) w.pack_elems = std::max(w.pack_elems, tc_pack_elems(wmax, ceil_div((long long)Mc, 32), 0));
     w.pack_b = reinterpret_cast<uint16_t*>(cv.take((w.pack_elems + 1) / 2));
   }
   if (out) *out = w;

@@ -16,17 +16,17 @@ import common
 from sparf_b200 import _lib, ops
 
 HBM_PEAK = 3.35e12      # H100 SXM data sheet, bytes/s
-GEMM_KERNEL = "wg_gemm_kernel"
+GEMM_KERNELS = ("wg_gemm_kernel", "wg_gemm_staged_kernel")
 # 16-bit passes of the images (forward, input gradient, weight gradient) per tensor-core engine
 PASSES = {"tc_3x": (3, 3, 3), "tc_1x": (1, 1, 1), "tc_3x_w1": (3, 3, 1), "auto": (3, 3, 3)}
 
 
 def gemm_bytes_per_row(spec, passes, backward, pose):
     """HBM bytes per sample row that the wgmma GEMMs must read and write, counted from the shapes: the A operand images,
-    the weight-gradient GEMMs' B operand images (activation-sized), the fp32 outputs, the epilogue images and the ReLU
-    masks (bits, 1/8 byte per value, written by the weight gradient's operand pack; fp32 at the last trunk layer, whose
-    epilogue sums the density row's weight gradient from the values).  The weights' images are small and stay in L2;
-    they are not counted."""
+    the weight-gradient GEMMs' B operands (the activations, read as fp32 and split inside the GEMM), the fp32 outputs,
+    the epilogue images and the ReLU masks (bits, 1/8 byte per value, written by the weight-gradient GEMM; fp32 at the
+    last trunk layer, whose epilogue sums the density row's weight gradient from the values).  The weights' images are
+    small and stay in L2; they are not counted."""
     pf, pd, pw = passes
     W, HW, skip, nt = spec.width, spec.head_width, spec.skip_layer, spec.n_trunk
     E3p, Evp = -(-(3 + 6 * spec.L_xyz) // 8) * 8, -(-(3 + 6 * spec.L_view) // 8) * 8
@@ -42,14 +42,14 @@ def gemm_bytes_per_row(spec, passes, backward, pose):
         return n
     # colour head: two weight-gradient GEMMs (Ghid^T [feat | denc]); the input gradient of feat (mask = feat) as row and
     # transposed images; with pose gradients the direction-encoding gradient in fp32
-    n += 2 * img(HW, pw) + img(W, pw) + img(Evp, pw)
+    n += 2 * img(HW, pw) + 4 * W + 4 * Evp
     n += img(HW, pd) + W / 8 + img(W, pd) + img(W, pw)
     if pose:
         n += img(HW, pd) + 4 * Evp
     for l in range(nt - 1, -1, -1):
-        n += img(W, pw) + img(W if l else E3p, pw)                      # weight gradient
+        n += img(W, pw) + 4 * (W if l else E3p)                         # weight gradient
         if l == skip:
-            n += img(W, pw) + img(E3p, pw)
+            n += img(W, pw) + 4 * E3p
         if l > 0:                                                       # input gradient: G image, mask, two images out
             n += img(W, pd) + (4 * W if l == nt - 1 else W / 8) + img(W, pd) + img(W, pw)
         if pose and (l == skip or l == 0):                              # encoding gradient, fp32 (+= at layer 0)
@@ -105,10 +105,10 @@ def main():
         for k, v in sorted(agg.items(), key=lambda kv: -kv[1][1]):
             print("  %8.1f us  x%-3d %s" % (v[1] / n, v[0] // n, k[:110]))
         if eng_name in PASSES:
-            g_us = sum(v[1] for k, v in agg.items() if GEMM_KERNEL in k) / n
+            g_us = sum(v[1] for k, v in agg.items() if any(g in k for g in GEMM_KERNELS)) / n
             g_bytes = R * S * gemm_bytes_per_row(spec, PASSES[eng_name], bwd, pose and bwd)
             print("  GEMM group (%s): %.1f us per call, %.2f GB to move (from shapes), %.0f GB/s = %.1f %% of %.2f TB/s"
-                  % (GEMM_KERNEL, g_us, g_bytes / 1e9, g_bytes / (g_us * 1e-6) / 1e9 if g_us else 0.0,
+                  % (" + ".join(GEMM_KERNELS), g_us, g_bytes / 1e9, g_bytes / (g_us * 1e-6) / 1e9 if g_us else 0.0,
                      100 * g_bytes / (g_us * 1e-6) / HBM_PEAK if g_us else 0.0, HBM_PEAK / 1e12))
 
 
