@@ -284,6 +284,40 @@ int sparf_termination_emit(int64_t R, int32_t S, int32_t k0, int32_t k1, const f
 int sparf_termination_update(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* sigma, const float* t,
                              const float* dirs, float tau_max, float* tau, uint8_t* alive, sparf_stream_t stream);
 
+/* ---------------------------------------------------------------- contracted occupancy grid
+ * An occupancy grid over all of space for inverse-depth and unbounded scenes (sparf_b200/occupancy.py with
+ * contraction = (center, radius)): the world is mapped (mip-NeRF 360's contraction, in the inf-norm) into the cube
+ * [-2, 2]^3, and the grid's res^3 cells split that cube.  center[3] and radius (fp32) set the map; the cells and bits
+ * are laid out as the box grid's above.
+ *   lookup:  sample (r,k), every op rounded to nearest (no contraction into FMAs), per axis a:
+ *              x_a = __fadd_rn(o_a, __fmul_rn(d_a, t))              (the MLP encoder's x, as in the box lookup)
+ *              y_a = __fdiv_rn(__fsub_rn(x_a, c_a), radius),  m = max_a |y_a|
+ *              v_a = y_a if m <= 1, else __fmul_rn(__fmul_rn(y_a, q), __fsub_rn(2, q)) with q = __fdiv_rn(1, m)
+ *              u_a = __fmul_rn(__fmul_rn(__fadd_rn(v_a, 2), 0.25f), (float)res)
+ *            The sample is KEPT if any u_a is NaN or outside [0, res), or if cell ((int)u_x, (int)u_y, (int)u_z) is
+ *            occupied; otherwise it is skipped.  Infinite or NaN coordinates give a NaN u: kept.  For m > 2^24,
+ *            __fsub_rn(2, q) rounds to 2, so u can reach exactly res: kept as well.
+ *   build:   the lattice axis is linspace(-2, 2, res+1) in fp32 (mesh.lattice_axis).  Lattice point v with
+ *            n = ||v||_inf < 2 stands for the world point center + radius * y, y = v for n <= 1 and v / (n (2 - n))
+ *            beyond (the inverse of the lookup's map); sigma there is the softplus of sparf_density_forward, as in
+ *            mesh.density_grid.  Points with n = 2 lie at infinity and are not evaluated: their sigma is NaN.  The
+ *            unchanged sparf_occupancy_build (dilation 1, NaN occupied) then writes the bits, so the outer two-cell
+ *            shell (a cell index 0, 1, res-2 or res-1 on some axis) is always occupied: samples with
+ *            ||x - center||_inf >= radius / (2 - (2 - 8 / res)) = radius * res / 8 (res >= 8) are always evaluated.
+ * Compaction of one window: sparf_contracted_count / _emit, the two-call contract of sparf_termination_count / _emit
+ * (same outputs in increasing order of r*S + k, same workspace, sparf_termination_workspace_bytes(R, k1 - k0);
+ * 0 <= k0 < k1 <= S; alive NULL = all alive) with the contracted lookup in place of the box lookup.  With alive = NULL,
+ * k0 = 0 and k1 = S it is the plain grid compaction.  bits is required (when R > 0), 1 <= res <= 4096, center is a
+ * host float[3] of finite values read during the call, radius is finite and > 0.  No atomics; neither call
+ * synchronises. */
+int sparf_contracted_count(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins, const float* dirs,
+                           const float* t, const uint8_t* alive, const uint32_t* bits, int32_t res, const float* center,
+                           float radius, int64_t* K, void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+int sparf_contracted_emit(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins, const float* dirs,
+                          const float* t, const uint8_t* alive, const uint32_t* bits, int32_t res, const float* center,
+                          float radius, int64_t* sample_idx, float* origins_k, float* dirs_k, float* t_k,
+                          void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+
 /* ---------------------------------------------------------------- compositing
  * NeRF.composite (frequency_nerf.py:283-343).  Outputs: rgb_map [R,3], depth/opacity/depth_var/rgb_var
  * [R], weights [R,S], all_cumulated [R] (= T at sample S-2).  white_bg: rgb += 1 - opacity.

@@ -71,6 +71,10 @@ _SIGNATURES = {
     "sparf_termination_emit": (c_int32, [c_int64, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, c_int32, c_float, c_float,
                                          _P, _P, _P, _P, _P, c_size_t, _P]),
     "sparf_termination_update": (c_int32, [c_int64, c_int32, c_int32, c_int32, _P, _P, _P, c_float, _P, _P, _P]),
+    "sparf_contracted_count": (c_int32, [c_int64, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, c_int32, POINTER(c_float),
+                                         c_float, _P, _P, c_size_t, _P]),
+    "sparf_contracted_emit": (c_int32, [c_int64, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, c_int32, POINTER(c_float),
+                                        c_float, _P, _P, _P, _P, _P, c_size_t, _P]),
     "sparf_composite_forward":(c_int32, [c_int32, c_int32, _P, _P, _P, _P, c_int32, _P, _P, _P, _P, _P, _P, _P, _P]),
     "sparf_composite_backward": (c_int32, [c_int32, c_int32, _P, _P, _P, _P, c_int32, _P, _P, _P, _P, _P, _P, _P, _P]),
     "sparf_huber2_fwd_bwd": (c_int32, [c_int64, _P, _P, c_float, _P, _P, _P]),

@@ -1,5 +1,6 @@
 // The sample compaction shared by the occupancy grid (occupancy.cu) and early ray termination (termination.cu): the
-// occupancy lookup, a block scan, the tile-total scan and the workspace layout of a count / scan / emit over n samples.
+// occupancy lookups (box and contracted), a block scan, the tile-total scan and the workspace layout of a count / scan /
+// emit over n samples.
 //   count: 4 consecutive samples per thread; a block scan writes each thread's tile-local offset and each 2048-sample
 //          tile writes its total;
 //   scan:  one CTA turns the tile totals into 64-bit tile bases and writes K;
@@ -32,6 +33,42 @@ struct Lookup {
       const float x = add_rn(__ldg(o + 3 * r + a), mul_rn(__ldg(d + 3 * r + a), tm));   // encode_xyz_kernel's x
       const float u = __fmul_rn(__fdiv_rn(__fsub_rn(x, r0), __fsub_rn(r1, r0)), fres);
       if (!(u >= 0.f && u < fres)) return true;                                           // outside or NaN
+      cell = cell * res + (int)u;
+    }
+    return __ldg(bits + (cell >> 5)) >> (cell & 31) & 1u;
+  }
+};
+
+// The contracted grid's lookup (include/sparf_b200.h): y = (x - center) / radius, v = y where ||y||_inf <= 1 and
+// y / m * (2 - 1 / m) with m = ||y||_inf beyond, so every finite x lands in the cube [-2, 2]^3 of res^3 cells.
+struct ContractedLookup {
+  const float *o, *d, *t;
+  const uint32_t* bits;
+  int S, res;
+  float c0, c1, c2, radius, fres;
+  // sample m is evaluated: a u outside [0, res) (NaN, infinite or |v| rounded to 2) or an occupied cell
+  __device__ __forceinline__ bool kept(long long m) const {
+    const long long r = m / S;
+    const float tm = __ldg(t + m);
+    const float c[3] = {c0, c1, c2};
+    float v[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      const float x = add_rn(__ldg(o + 3 * r + a), mul_rn(__ldg(d + 3 * r + a), tm));   // encode_xyz_kernel's x
+      v[a] = __fdiv_rn(__fsub_rn(x, c[a]), radius);
+    }
+    // fmaxf drops a NaN |y_a|, but that axis's u is NaN on either branch, so the sample is kept all the same
+    const float n = fmaxf(fmaxf(fabsf(v[0]), fabsf(v[1])), fabsf(v[2]));
+    if (n > 1.f) {
+      const float q = __fdiv_rn(1.f, n), s = __fsub_rn(2.f, q);
+#pragma unroll
+      for (int a = 0; a < 3; ++a) v[a] = __fmul_rn(__fmul_rn(v[a], q), s);
+    }
+    long long cell = 0;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      const float u = __fmul_rn(__fmul_rn(__fadd_rn(v[a], 2.f), 0.25f), fres);
+      if (!(u >= 0.f && u < fres)) return true;                                           // NaN, inf or u = res
       cell = cell * res + (int)u;
     }
     return __ldg(bits + (cell >> 5)) >> (cell & 31) & 1u;
@@ -117,6 +154,11 @@ size_t carve(int64_t R, int32_t S, void* ws, Carve* c) {
 Lookup make_lookup(int64_t R, int32_t S, const float* origins, const float* dirs, const float* t, const uint32_t* bits,
                    int32_t res, float r0, float r1) {
   return Lookup{origins, dirs, t, bits, (long long)R * S, S, res, r0, r1, (float)res};
+}
+
+ContractedLookup make_contracted_lookup(int32_t S, const float* origins, const float* dirs, const float* t,
+                                        const uint32_t* bits, int32_t res, const float* center, float radius) {
+  return ContractedLookup{origins, dirs, t, bits, S, res, center[0], center[1], center[2], radius, (float)res};
 }
 
 }  // namespace

@@ -1,10 +1,14 @@
 // Early ray termination for inference renders: the samples of one window [k0, k1) of every ray are evaluated while the
 // ray is alive, and a ray dies once the optical depth tau it has accumulated shows it opaque (tau > tau_max).
 //   count / scan / emit: the compaction of occupancy.cu (compaction.cuh) over the R * (k1 - k0) window samples; kept =
-//          alive[r] (NULL: every ray) and, with a grid, the occupancy lookup.  Output in increasing order of r * S + k;
+//          alive[r] (NULL: every ray) and, with a grid, the occupancy lookup: the box grid's (sparf_termination_*) or
+//          the contracted grid's (sparf_contracted_*, which with alive = NULL and [0, S) is the plain grid
+//          compaction).  The kernels are templated on the lookup.  Output in increasing order of r * S + k;
 //   update: one thread per alive ray adds the window's sd_k = sigma_k * (gap_k * len) to tau in sample order, with
 //          explicit rounding (include/sparf_b200.h states the op order), and clears alive[r] when tau > tau_max.
 // Deterministic (no atomics).  Workspace: that of a compaction over R * (k1 - k0) samples.
+#include <cmath>
+
 #include "compaction.cuh"
 
 namespace sparf {
@@ -12,8 +16,10 @@ namespace {
 
 constexpr int kUpdateThreads = 256;
 
+// Lk: Lookup (the box grid) or ContractedLookup (the contracted grid)
+template <class Lk>
 struct Window {
-  Lookup Q;               // o, d, t [R,S]; Q.bits NULL = no grid
+  Lk Q;                   // o, d, t [R,S]; Q.bits NULL = no grid
   const uint8_t* alive;   // [R]; NULL = every ray alive
   long long n;            // R * W
   int W, k0;
@@ -24,7 +30,8 @@ struct Window {
   }
 };
 
-__global__ void __launch_bounds__(kOcThreads) termination_count_kernel(Window Wn, uint32_t* __restrict__ local,
+template <class Lk>
+__global__ void __launch_bounds__(kOcThreads) termination_count_kernel(Window<Lk> Wn, uint32_t* __restrict__ local,
                                                                        long long* __restrict__ tiles) {
   const long long m0 = (long long)blockIdx.x * kOcTile + (long long)threadIdx.x * kOcItems;
   int c = 0;
@@ -42,7 +49,8 @@ __global__ void __launch_bounds__(kScanThreads) termination_scan_kernel(long lon
   scan_tiles(tiles, ntiles, K);
 }
 
-__global__ void __launch_bounds__(kOcThreads) termination_emit_kernel(Window Wn, const uint32_t* __restrict__ local,
+template <class Lk>
+__global__ void __launch_bounds__(kOcThreads) termination_emit_kernel(Window<Lk> Wn, const uint32_t* __restrict__ local,
                                                                       const long long* __restrict__ tiles,
                                                                       int64_t* __restrict__ sample_idx,
                                                                       float* __restrict__ origins_k,
@@ -101,16 +109,15 @@ extern "C" size_t sparf_termination_workspace_bytes(int64_t R, int32_t window) {
   return sizes_ok(R, window) ? carve(R, window, nullptr, nullptr) : 0;
 }
 
-// the checks and the workspace carve count and emit share; *ok = false for R == 0 (nothing to launch)
-static int termination_setup(const char* name, int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins,
-                             const float* dirs, const float* t, const uint8_t* alive, const uint32_t* bits, int32_t res,
-                             float r0, float r1, void* workspace, size_t workspace_bytes, Window* wn, Carve* c) {
+// the checks and the workspace carve count and emit share, with the grid's own checks (grid_ok) after the sizes'; fills
+// every field of *wn but the lookup.  R == 0 returns before the pointers are checked (nothing to launch)
+template <class Lk, class GridCheck>
+static int window_setup(const char* name, int64_t R, int32_t S, int32_t k0, int32_t k1, GridCheck grid_ok,
+                        const float* origins, const float* dirs, const float* t, const uint8_t* alive, void* workspace,
+                        size_t workspace_bytes, Window<Lk>* wn, Carve* c) {
   SPARF_REQUIRE(sizes_ok(R, S), "%s: R %lld, S %d (R >= 0, S >= 1, R * S <= 2^58)", name, (long long)R, (int)S);
   SPARF_REQUIRE(window_ok(S, k0, k1), "%s: window [%d, %d) of S %d (0 <= k0 < k1 <= S)", name, (int)k0, (int)k1, (int)S);
-  if (bits) {
-    SPARF_REQUIRE(res_ok(res), "%s: res %d (1 ... 4096)", name, (int)res);
-    SPARF_REQUIRE(r1 > r0, "%s: empty box [%g, %g]", name, (double)r0, (double)r1);
-  }
+  SPARF_TRY(grid_ok());
   if (R == 0) return SPARF_OK;
   SPARF_REQUIRE(origins && dirs && t && workspace, "%s: NULL pointer", name);
   const size_t need = carve(R, k1 - k0, workspace, c);
@@ -119,21 +126,16 @@ static int termination_setup(const char* name, int64_t R, int32_t S, int32_t k0,
     return SPARF_ERR_WORKSPACE;
   }
   SPARF_REQUIRE(c->ntiles < (1ll << 31), "%s: too many samples", name);
-  *wn = Window{make_lookup(R, S, origins, dirs, t, bits, bits ? res : 1, r0, r1), alive, (long long)R * (k1 - k0),
-               k1 - k0, k0};
+  wn->alive = alive;
+  wn->n = (long long)R * (k1 - k0);
+  wn->W = k1 - k0;
+  wn->k0 = k0;
   return SPARF_OK;
 }
 
-extern "C" int sparf_termination_count(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins,
-                                       const float* dirs, const float* t, const uint8_t* alive, const uint32_t* bits,
-                                       int32_t res, float r0, float r1, int64_t* K, void* workspace,
-                                       size_t workspace_bytes, sparf_stream_t stream) {
-  SPARF_REQUIRE(K, "termination_count: NULL pointer");
-  Window wn;
-  Carve c;
-  SPARF_TRY(termination_setup("termination_count", R, S, k0, k1, origins, dirs, t, alive, bits, res, r0, r1, workspace,
-                              workspace_bytes, &wn, &c));
-  cudaStream_t s = (cudaStream_t)stream;
+// count: K = 0 for R == 0, else the count and scan kernels
+template <class Lk>
+static int launch_count(int64_t R, const Window<Lk>& wn, const Carve& c, int64_t* K, cudaStream_t s) {
   if (R == 0) {
     SPARF_CHECK_CUDA(cudaMemsetAsync(K, 0, sizeof(int64_t), s));
     return SPARF_OK;
@@ -145,20 +147,99 @@ extern "C" int sparf_termination_count(int64_t R, int32_t S, int32_t k0, int32_t
   return SPARF_OK;
 }
 
+template <class Lk>
+static int launch_emit(int64_t R, const Window<Lk>& wn, const Carve& c, int64_t* sample_idx, float* origins_k,
+                       float* dirs_k, float* t_k, cudaStream_t s) {
+  if (R == 0) return SPARF_OK;
+  termination_emit_kernel<<<(unsigned)c.ntiles, kOcThreads, 0, s>>>(wn, c.local, c.tiles, sample_idx, origins_k, dirs_k,
+                                                                   t_k);
+  SPARF_CHECK_LAUNCH("termination_emit_kernel");
+  return SPARF_OK;
+}
+
+// the box grid's window (bits NULL: no grid)
+static int termination_setup(const char* name, int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins,
+                             const float* dirs, const float* t, const uint8_t* alive, const uint32_t* bits, int32_t res,
+                             float r0, float r1, void* workspace, size_t workspace_bytes, Window<Lookup>* wn, Carve* c) {
+  auto grid_ok = [&]() -> int {
+    if (bits) {
+      SPARF_REQUIRE(res_ok(res), "%s: res %d (1 ... 4096)", name, (int)res);
+      SPARF_REQUIRE(r1 > r0, "%s: empty box [%g, %g]", name, (double)r0, (double)r1);
+    }
+    return SPARF_OK;
+  };
+  SPARF_TRY(window_setup(name, R, S, k0, k1, grid_ok, origins, dirs, t, alive, workspace, workspace_bytes, wn, c));
+  if (R > 0) wn->Q = make_lookup(R, S, origins, dirs, t, bits, bits ? res : 1, r0, r1);
+  return SPARF_OK;
+}
+
+// the contracted grid's window (bits required; center: host float[3])
+static int contracted_setup(const char* name, int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins,
+                            const float* dirs, const float* t, const uint8_t* alive, const uint32_t* bits, int32_t res,
+                            const float* center, float radius, void* workspace, size_t workspace_bytes,
+                            Window<ContractedLookup>* wn, Carve* c) {
+  auto grid_ok = [&]() -> int {
+    SPARF_REQUIRE(res_ok(res), "%s: res %d (1 ... 4096)", name, (int)res);
+    SPARF_REQUIRE(center, "%s: NULL center", name);
+    SPARF_REQUIRE(std::isfinite(center[0]) && std::isfinite(center[1]) && std::isfinite(center[2]),
+                  "%s: center (%g, %g, %g) is not finite", name, (double)center[0], (double)center[1],
+                  (double)center[2]);
+    SPARF_REQUIRE(radius > 0.f && std::isfinite(radius), "%s: radius %g (finite, > 0)", name, (double)radius);
+    return SPARF_OK;
+  };
+  SPARF_TRY(window_setup(name, R, S, k0, k1, grid_ok, origins, dirs, t, alive, workspace, workspace_bytes, wn, c));
+  if (R == 0) return SPARF_OK;
+  SPARF_REQUIRE(bits, "%s: NULL bits", name);
+  wn->Q = make_contracted_lookup(S, origins, dirs, t, bits, res, center, radius);
+  return SPARF_OK;
+}
+
+extern "C" int sparf_termination_count(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins,
+                                       const float* dirs, const float* t, const uint8_t* alive, const uint32_t* bits,
+                                       int32_t res, float r0, float r1, int64_t* K, void* workspace,
+                                       size_t workspace_bytes, sparf_stream_t stream) {
+  SPARF_REQUIRE(K, "termination_count: NULL pointer");
+  Window<Lookup> wn;
+  Carve c;
+  SPARF_TRY(termination_setup("termination_count", R, S, k0, k1, origins, dirs, t, alive, bits, res, r0, r1, workspace,
+                              workspace_bytes, &wn, &c));
+  return launch_count(R, wn, c, K, (cudaStream_t)stream);
+}
+
 extern "C" int sparf_termination_emit(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins,
                                       const float* dirs, const float* t, const uint8_t* alive, const uint32_t* bits,
                                       int32_t res, float r0, float r1, int64_t* sample_idx, float* origins_k,
                                       float* dirs_k, float* t_k, void* workspace, size_t workspace_bytes,
                                       sparf_stream_t stream) {
-  Window wn;
+  Window<Lookup> wn;
   Carve c;
   SPARF_TRY(termination_setup("termination_emit", R, S, k0, k1, origins, dirs, t, alive, bits, res, r0, r1, workspace,
                               workspace_bytes, &wn, &c));
-  if (R == 0) return SPARF_OK;
-  termination_emit_kernel<<<(unsigned)c.ntiles, kOcThreads, 0, (cudaStream_t)stream>>>(wn, c.local, c.tiles, sample_idx,
-                                                                                      origins_k, dirs_k, t_k);
-  SPARF_CHECK_LAUNCH("termination_emit_kernel");
-  return SPARF_OK;
+  return launch_emit(R, wn, c, sample_idx, origins_k, dirs_k, t_k, (cudaStream_t)stream);
+}
+
+extern "C" int sparf_contracted_count(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins,
+                                      const float* dirs, const float* t, const uint8_t* alive, const uint32_t* bits,
+                                      int32_t res, const float* center, float radius, int64_t* K, void* workspace,
+                                      size_t workspace_bytes, sparf_stream_t stream) {
+  SPARF_REQUIRE(K, "contracted_count: NULL pointer");
+  Window<ContractedLookup> wn;
+  Carve c;
+  SPARF_TRY(contracted_setup("contracted_count", R, S, k0, k1, origins, dirs, t, alive, bits, res, center, radius,
+                             workspace, workspace_bytes, &wn, &c));
+  return launch_count(R, wn, c, K, (cudaStream_t)stream);
+}
+
+extern "C" int sparf_contracted_emit(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins,
+                                     const float* dirs, const float* t, const uint8_t* alive, const uint32_t* bits,
+                                     int32_t res, const float* center, float radius, int64_t* sample_idx,
+                                     float* origins_k, float* dirs_k, float* t_k, void* workspace,
+                                     size_t workspace_bytes, sparf_stream_t stream) {
+  Window<ContractedLookup> wn;
+  Carve c;
+  SPARF_TRY(contracted_setup("contracted_emit", R, S, k0, k1, origins, dirs, t, alive, bits, res, center, radius,
+                             workspace, workspace_bytes, &wn, &c));
+  return launch_emit(R, wn, c, sample_idx, origins_k, dirs_k, t_k, (cudaStream_t)stream);
 }
 
 extern "C" int sparf_termination_update(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* sigma,

@@ -59,15 +59,31 @@ def density_grid(opt, nerf, res=None, range=None, engine=None) -> torch.Tensor:
     where opt has none).  The reference's trimesh.chunk_size is a memory setting of its PyTorch evaluation and is not
     used: the slabs and the kernels' own chunking bound the memory here.  engine: None = the current ops engine."""
     res, rng, _ = trimesh_settings(opt, res, range)
+    return lattice_density(nerf, lattice_axis(res, rng), engine=engine)
+
+
+@torch.no_grad()
+def lattice_density(nerf, axis: torch.Tensor, engine=None, warp=None) -> torch.Tensor:
+    """sigma [n, n, n] (n = axis.numel()) on nerf's device: softplus of the raw density (ops.density_forward,
+    features=False; no noise, the BARF mask at nerf.progress) at the lattice points of lattice_slabs(axis), slab by slab.
+    warp: None (the lattice points are world points), or a map of one slab's lattice points [P, 3] to (world points
+    [P, 3], a bool [P] mask of the points that are not evaluated and get sigma = NaN, or None)."""
     dev = nerf.progress.device
-    t = lattice_axis(res, rng).to(dev)
-    n = res + 1
+    t = axis.to(dev)
+    n = t.numel()
     sigma = torch.empty(n, n, n, device=dev, dtype=torch.float32)
     spec, trunk = nerf._spec(), _trunk(nerf)
     for i0, pts in lattice_slabs(t, max(1, SLAB_POINTS // (n * n))):
+        rows = pts.shape[0] // (n * n)
+        skip = None
+        if warp is not None:
+            pts, skip = warp(pts)
         raw, _ = ops.density_forward(spec, pts, trunk, progress=nerf.progress.detach(), engine=_engine(engine),
                                      features=False)
-        sigma[i0:i0 + pts.shape[0] // (n * n)] = torch.nn.functional.softplus(raw).view(-1, n, n)
+        s = torch.nn.functional.softplus(raw)
+        if skip is not None:
+            s = s.masked_fill(skip.view(s.shape), float("nan"))
+        sigma[i0:i0 + rows] = s.view(-1, n, n)
     return sigma
 
 

@@ -9,26 +9,53 @@
 A sample is skipped when it lies inside the box in a cell none of whose lattice points within one cell has σ >= thres;
 its σ and rgb are then 0, and every other sample is evaluated exactly as the dense render evaluates it (semantics in
 include/sparf_b200.h).  A grid is a snapshot of the network when it was built: rebuild it after the weights change.
-Samples outside the box are always evaluated, so scenes whose samples mostly lie outside it (inverse-depth LLFF) gain
-little.
+Samples outside the box are always evaluated.  For scenes whose samples mostly lie outside any box (inverse-depth LLFF,
+rooms seen from the inside) build a contracted grid instead, which covers all of space:
+
+    grid = occupancy.build_grid(opt, graph.nerf, contraction=(center, radius))
+
+Its lookup maps a point x to y = (x - center) / radius and, where m = ||y||_inf > 1, on to y / m * (2 - 1 / m)
+(mip-NeRF 360's contraction in the inf-norm), into the cube [-2, 2]^3; the grid's cells split that cube.  The cells are
+uniform in the linear region ||y||_inf <= 1.  Beyond it they grow like m^2: they are uniform in 1 / m, which is how
+inverse-depth sampling spaces its samples.
+
+Choosing center and radius: put the cameras and the near bound inside the linear region.  The LLFF loader scales a
+forward-facing scene so that its nearest bound is about 1.33, and the samples start at t = 1 from cameras near the
+origin.  center = the mean camera centre and radius = 1.33 (or the cameras' spread, if that is larger) then put the
+first quarter of every ray, where inverse depth crowds its samples, in the linear region, and space the cells beyond it
+like the samples.  Indoors (Replica), center the grid on the room and pick radius so that the walls lie inside or just
+past the linear region.  Lattice points at infinity (on the cube's faces) are never evaluated and count as occupied, so
+the outer two-cell shell, beyond ||x - center||_inf = radius * res / 8, is always kept.  Conservativeness is weaker in
+the stretched outer cells than in the linear region: there one cell spans a long stretch of world space between its
+lattice points.
 """
 from __future__ import annotations
 
+import math
+
+import numpy as np
 import torch
 
 from . import mesh, ops
 
 _POPCOUNT = [bin(i).count("1") for i in range(256)]
+CONTRACTED_RANGE = (-2.0, 2.0)      # the cube the contraction maps space into
 
 
 class OccupancyGrid:
     """bits [ceil(res^3 / 32)] (int32 storage of uint32 words; cell (i,j,k) is bit idx & 31 of word idx >> 5, idx =
-    (i*res + j)*res + k) over the box [r0, r1]^3 split into res^3 cells, built at density threshold thres."""
+    (i*res + j)*res + k) over the box [r0, r1]^3 split into res^3 cells, built at density threshold thres.
+    contraction: None (a box grid over world space), or (center (3 floats), radius) for a contracted grid, whose cells
+    split the contracted cube: range is then CONTRACTED_RANGE.  center and radius are kept as fp32 values."""
 
-    def __init__(self, bits: torch.Tensor, res: int, range, thres: float):
+    def __init__(self, bits: torch.Tensor, res: int, range, thres: float, contraction=None):
         assert bits.dtype == torch.int32 and bits.numel() == (res ** 3 + 31) // 32
         self.bits, self.res, self.thres = bits.contiguous(), int(res), float(thres)
         self.range = (float(range[0]), float(range[1]))
+        self.contraction = None
+        if contraction is not None:
+            assert self.range == CONTRACTED_RANGE, "a contracted grid covers the cube [-2, 2]^3"
+            self.contraction = _as_contraction(contraction)
 
     def occupied_fraction(self) -> float:
         """occupied cells / res^3"""
@@ -36,25 +63,67 @@ class OccupancyGrid:
         return table[self.bits.view(torch.uint8).long()].sum().item() / self.res ** 3
 
 
+def _as_contraction(contraction):
+    """((cx, cy, cz), radius) as python floats holding fp32 values; finite, radius > 0"""
+    center, radius = contraction
+    c = tuple(float(np.float32(v)) for v in (center.tolist() if torch.is_tensor(center) else center))
+    r = float(np.float32(radius))
+    assert len(c) == 3 and all(math.isfinite(v) for v in c + (r,)) and r > 0, contraction
+    return c, r
+
+
+def contracted_warp(center, radius):
+    """The lattice map of a contracted grid's build (mesh.lattice_density's warp).  A lattice point v of the contracted
+    cube (fp32 [P, 3]) with n = ||v||_inf < 2 goes to the world point center + radius * y, where y = v for n <= 1 and
+    y = v / (n (2 - n)) beyond, the inverse of the lookup's map.  This is computed in fp64 and rounded once to fp32.
+    Points with n >= 2 lie at infinity: they are not evaluated, and their σ is NaN."""
+    center, radius = _as_contraction((center, radius))
+
+    def warp(v):
+        v = v.double()
+        n = v.abs().amax(-1, keepdim=True)
+        far = n[:, 0] >= 2
+        den = torch.where((n <= 1) | far[:, None], torch.ones_like(n), n * (2 - n))
+        c = torch.tensor(center, dtype=torch.float64, device=v.device)
+        x = torch.where(far[:, None], c, c + radius * (v / den))
+        return x.float(), far
+
+    return warp
+
+
 @torch.no_grad()
-def build_grid(opt, nerf, res=None, range=None, thres=0.01, engine=None) -> OccupancyGrid:
+def build_grid(opt, nerf, res=None, range=None, thres=0.01, engine=None, contraction=None) -> OccupancyGrid:
     """The occupancy grid of one network (graph.nerf or graph.nerf_fine) at its current weights and nerf.progress: σ on
     the lattice of opt.trimesh (res and range default to it, as in mesh.density_grid), then ops.occupancy_build at
-    thres.  engine: None = the current ops engine."""
-    res, rng, _ = mesh.trimesh_settings(opt, res, range)
-    sigma = mesh.density_grid(opt, nerf, res=res, range=rng, engine=engine)
-    return OccupancyGrid(ops.occupancy_build(sigma, thres), res, rng, thres)
+    thres.  contraction = (center, radius) builds a contracted grid over all of space instead (module docstring): σ at
+    the world points (contracted_warp) of the lattice linspace(-2, 2, res + 1)^3, evaluated slab by slab as
+    mesh.density_grid does, NaN at infinity, then the same ops.occupancy_build.  range must then be None.
+    engine: None = the current ops engine."""
+    if contraction is None:
+        res, rng, _ = mesh.trimesh_settings(opt, res, range)
+        sigma = mesh.density_grid(opt, nerf, res=res, range=rng, engine=engine)
+        return OccupancyGrid(ops.occupancy_build(sigma, thres), res, rng, thres)
+    assert range is None, "a contracted grid covers the cube [-2, 2]^3 of the contracted space"
+    res = mesh.trimesh_settings(opt, res)[0]
+    contraction = _as_contraction(contraction)
+    sigma = mesh.lattice_density(nerf, mesh.lattice_axis(res, CONTRACTED_RANGE), engine=engine,
+                                 warp=contracted_warp(*contraction))
+    return OccupancyGrid(ops.occupancy_build(sigma, thres), res, CONTRACTED_RANGE, thres, contraction)
 
 
 @torch.no_grad()
 def forward_samples(nerf, grid: OccupancyGrid, center, ray, depth_samples) -> dict:
     """NeRF.forward_samples (no noise) with the samples the grid skips set to σ = 0, rgb = 0: center, ray [B,N,3];
-    depth_samples [B,N,S,1] -> dict(rgb_samples [B,N,S,3], density_samples [B,N,S]).  The kept samples go through
-    ops.mlp_forward as one-sample rays (o, d, t), which evaluates each of them exactly as the dense call does."""
+    depth_samples [B,N,S,1] -> dict(rgb_samples [B,N,S,3], density_samples [B,N,S]).  The kept samples (by the box or
+    the contracted lookup, after the grid's kind) go through ops.mlp_forward as one-sample rays (o, d, t), which
+    evaluates each of them exactly as the dense call does."""
     B, N, S = depth_samples.shape[:3]
     M = B * N * S
-    idx, o_k, d_k, t_k = ops.occupancy_compact(grid.bits, grid.res, grid.range, center.reshape(B * N, 3),
-                                               ray.reshape(B * N, 3), depth_samples.reshape(B * N, S))
+    o, d, t = center.reshape(B * N, 3), ray.reshape(B * N, 3), depth_samples.reshape(B * N, S)
+    if grid.contraction is None:
+        idx, o_k, d_k, t_k = ops.occupancy_compact(grid.bits, grid.res, grid.range, o, d, t)
+    else:
+        idx, o_k, d_k, t_k = ops.contracted_compact(o, d, t, 0, S, None, grid.bits, grid.res, *grid.contraction)
     sigma = torch.zeros(M, device=depth_samples.device)
     rgb = torch.zeros(M, 3, device=depth_samples.device)
     if idx.numel():

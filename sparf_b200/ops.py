@@ -449,6 +449,35 @@ def termination_compact(origins, dirs, t, k0: int, k1: int, alive=None, bits=Non
 
 @torch.no_grad()
 @_on_tensor_device
+def contracted_compact(origins, dirs, t, k0: int, k1: int, alive, bits, res: int, center, radius: float):
+    """termination_compact with a contracted occupancy grid in place of the box grid: the samples k in [k0, k1) of the
+    rays with alive[r] != 0 (None = every ray) that the contracted grid (bits over [-2, 2]^3 in res^3 cells; center
+    (3 floats), radius: the contraction, include/sparf_b200.h) keeps -> (sample_idx [K] int64 = r * S + k, origins_k
+    [K,3], dirs_k [K,3], t_k [K,1]) in increasing sample order.  k0 = 0, k1 = S, alive = None: the plain grid
+    compaction.  One device-to-host copy (K).  Not differentiable."""
+    L = _lib.lib()
+    o, d, tt = _f32c(origins), _f32c(dirs), _f32c(t)
+    R, S = tt.shape
+    assert o.shape == (R, 3) and d.shape == (R, 3)
+    assert alive is None or (alive.dtype == torch.uint8 and alive.is_contiguous() and alive.shape == (R,))
+    assert bits.dtype == torch.int32 and bits.is_contiguous() and bits.numel() == (res ** 3 + 31) // 32
+    c = (ctypes.c_float * 3)(*[float(v) for v in center])
+    dev = tt.device
+    ws = _workspace(L.sparf_termination_workspace_bytes(R, k1 - k0), dev)
+    K = torch.empty((), dtype=torch.int64, device=dev)
+    args = (R, S, int(k0), int(k1), _ptr(o), _ptr(d), _ptr(tt), _ptr(alive), _ptr(bits), int(res), c, float(radius))
+    check(L.sparf_contracted_count(*args, _ptr(K), _ptr(ws), ws.numel(), _stream()), "contracted_count")
+    k = int(K.item())
+    sample_idx = torch.empty(k, dtype=torch.int64, device=dev)
+    o_k, d_k = torch.empty(k, 3, device=dev), torch.empty(k, 3, device=dev)
+    t_k = torch.empty(k, 1, device=dev)
+    check(L.sparf_contracted_emit(*args, _ptr(sample_idx), _ptr(o_k), _ptr(d_k), _ptr(t_k), _ptr(ws), ws.numel(),
+                                  _stream()), "contracted_emit")
+    return sample_idx, o_k, d_k, t_k
+
+
+@torch.no_grad()
+@_on_tensor_device
 def termination_update(sigma, t, dirs, k0: int, k1: int, tau_max: float, tau, alive):
     """In place, for every ray with alive[r] != 0: tau[r] += the optical depth of its samples k in [k0, k1) (sigma, t
     [R,S], dirs [R,3]; op order in include/sparf_b200.h), then alive[r] = 0 when tau[r] > tau_max.  tau: float32 [R],

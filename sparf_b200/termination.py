@@ -12,7 +12,8 @@ dense render evaluates it (semantics in include/sparf_b200.h).  The composite th
 opacity and rgb (2 eps with an opaque background) and by less than eps * max t in depth; the fine pass's samples
 move with the coarse weights, so its error is not bounded.  Each window reads its sample count on the host, so a render
 on this path cannot be captured into a CUDA graph.  Scenes whose rays mostly turn opaque gain; soft or small objects
-and inverse-depth sampling, which crowds the samples in front of the surface, gain little.
+gain little, and so does inverse-depth sampling alone, which crowds the samples in front of the surface.  A contracted
+occupancy grid (sparf_b200.occupancy) skips those front samples, and termination on top of it skips the ones behind.
 """
 from __future__ import annotations
 
@@ -31,8 +32,8 @@ def tau_max(eps: float) -> float:
 
 @torch.no_grad()
 def forward_samples(nerf, grid, eps: float, window: int, center, ray, depth_samples) -> dict:
-    """NeRF.forward_samples (no noise) with the samples of terminated rays, and those the occupancy grid (or None)
-    skips, set to σ = 0, rgb = 0: center, ray [B,N,3]; depth_samples [B,N,S,1] -> dict(rgb_samples [B,N,S,3],
+    """NeRF.forward_samples (no noise) with the samples of terminated rays, and those the occupancy grid (box or
+    contracted; or None) skips, set to σ = 0, rgb = 0: center, ray [B,N,3]; depth_samples [B,N,S,1] -> dict(rgb_samples [B,N,S,3],
     density_samples [B,N,S]).  The evaluated samples go through ops.mlp_forward as one-sample rays (o, d, t)."""
     B, N, S = depth_samples.shape[:3]
     R = B * N
@@ -43,10 +44,14 @@ def forward_samples(nerf, grid, eps: float, window: int, center, ray, depth_samp
     alive = torch.ones(R, dtype=torch.uint8, device=dev)
     tau = torch.zeros(R, device=dev)
     limit = tau_max(eps)
-    grid_args = dict(bits=grid.bits, res=grid.res, range=grid.range) if grid is not None else {}
+    if grid is not None and grid.contraction is not None:
+        compact = lambda k0, k1: ops.contracted_compact(o, d, t, k0, k1, alive, grid.bits, grid.res, *grid.contraction)
+    else:
+        grid_args = dict(bits=grid.bits, res=grid.res, range=grid.range) if grid is not None else {}
+        compact = lambda k0, k1: ops.termination_compact(o, d, t, k0, k1, alive, **grid_args)
     for k0 in range(0, S, window):
         k1 = min(k0 + window, S)
-        idx, o_k, d_k, t_k = ops.termination_compact(o, d, t, k0, k1, alive, **grid_args)
+        idx, o_k, d_k, t_k = compact(k0, k1)
         if idx.numel():            # an empty window (every ray dead, or the grid skips it all) may precede a full one
             sigma_k, rgb_k = ops.mlp_forward(nerf._spec(), o_k, d_k, t_k, nerf.kernel_params(), progress=nerf.progress)
             sigma.view(-1).index_copy_(0, idx, sigma_k.view(-1))
