@@ -168,6 +168,42 @@ int sparf_mlp_backward_tape(const SparfMLP* mlp, int32_t engine, int32_t R, int3
                             const float* d_sigma, const float* d_rgb, const SparfMLPGrad* grad, float* d_origins,
                             float* d_dirs, void* tape, size_t tape_bytes, void* workspace, size_t workspace_bytes,
                             sparf_stream_t stream);
+/* The taped pair with a row count read on the device, for passes over the samples an occupancy grid keeps, whose count
+ * the host never reads (sparf_occupancy_count writes it to device memory), so that a training step stays one CUDA graph.
+ * The arguments are those of the taped pair, with R = C a capacity that sizes the tape (sparf_mlp_tape_bytes(C, 1)),
+ * the workspace (sparf_mlp_workspace_bytes(C, 1, 0 or 2)) and the chunk loop, and rows (device int64) = K, the rows
+ * processed; K > C counts as C, K < 0 as 0.  S must be 1 (one-sample rays, the compaction's layout) and the engine
+ * TC_3X, TC_1X or TC_3X_W1 (AUTO resolving to one of them); otherwise SPARF_ERR_UNSUPPORTED or SPARF_ERR_INVALID.
+ *   - sigma, rgb, d_origins and d_dirs have the bits of the taped pair called with R = K on rows [0, K); the parameter
+ *     gradients agree up to the order of their float atomics (each GEMM unit's partial sums are the same);
+ *   - rows [K, C) of the inputs (origins, dirs, t, noise, sigma, rgb, d_sigma, d_rgb) are never read, and the same rows
+ *     of the outputs (sigma, rgb, d_origins, d_dirs) never written;
+ *   - every kernel processes min(chunk rows, K - chunk start) rows; a chunk wholly past K costs one launch per kernel
+ *     that returns at once.  The weight-gradient GEMMs split their k-ranges in the kernel from K, as the host splits
+ *     them from R in the taped pair.
+ * The tape is left for sparf_mlp_backward_tape_rows with the same rows, which must hold the same K. */
+int sparf_mlp_forward_tape_rows(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S, const int64_t* rows,
+                                const float* origins, const float* dirs, const float* t, const float* noise, float* sigma,
+                                float* rgb, void* tape, size_t tape_bytes, void* workspace, size_t workspace_bytes,
+                                sparf_stream_t stream);
+int sparf_mlp_backward_tape_rows(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S, const int64_t* rows,
+                                 const float* origins, const float* dirs, const float* t, const float* sigma,
+                                 const float* rgb, const float* d_sigma, const float* d_rgb, const SparfMLPGrad* grad,
+                                 float* d_origins, float* d_dirs, void* tape, size_t tape_bytes, void* workspace,
+                                 size_t workspace_bytes, sparf_stream_t stream);
+/* Moving rows between a dense [.., width] layout and the compacted one of a grid pass (kept sample k < K is dense row
+ * sample_idx[k], increasing, as sparf_occupancy_emit / sparf_contracted_emit write it), reading K (device int64) on the
+ * device; C is the capacity of the compacted buffers, width in [1, 4].  No atomics, no synchronisation.
+ *   scatter: dst[sample_idx[k]] = src[k] (the caller zeroes the skipped rows of dst);
+ *   gather:  dst[k] = src[sample_idx[k]] (rows [K, C) of dst are not written);
+ *   ray_sum: dst[r] (written, r < R) = the sum over the kept rows k of ray r (sample_idx[k] / S == r) of src[k], added
+ *            in increasing k from 0: the per-ray gradients of origins and dirs from the per-sample ones. */
+int sparf_compact_scatter(int64_t C, const int64_t* K, const int64_t* sample_idx, int32_t width, const float* src,
+                          float* dst, sparf_stream_t stream);
+int sparf_compact_gather(int64_t C, const int64_t* K, const int64_t* sample_idx, int32_t width, const float* src,
+                         float* dst, sparf_stream_t stream);
+int sparf_compact_ray_sum(int64_t R, int32_t S, int64_t C, const int64_t* K, const int64_t* sample_idx, int32_t width,
+                          const float* src, float* dst, sparf_stream_t stream);
 
 /* ---------------------------------------------------------------- density queries
  * NeRF.compute_raw_density (frequency_nerf.py:149-170): the trunk alone at M arbitrary points [M,3] (x = p; no view

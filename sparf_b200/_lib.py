@@ -52,6 +52,13 @@ _SIGNATURES = {
                                          _P, c_size_t, _P]),
     "sparf_mlp_backward_tape": (c_int32, [POINTER(SparfMLP), c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, _P, _P,
                                           POINTER(SparfMLPGrad), _P, _P, _P, c_size_t, _P, c_size_t, _P]),
+    "sparf_mlp_forward_tape_rows": (c_int32, [POINTER(SparfMLP), c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, _P, _P, _P,
+                                              c_size_t, _P, c_size_t, _P]),
+    "sparf_mlp_backward_tape_rows": (c_int32, [POINTER(SparfMLP), c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, _P, _P, _P,
+                                               POINTER(SparfMLPGrad), _P, _P, _P, c_size_t, _P, c_size_t, _P]),
+    "sparf_compact_scatter": (c_int32, [c_int64, _P, _P, c_int32, _P, _P, _P]),
+    "sparf_compact_gather": (c_int32, [c_int64, _P, _P, c_int32, _P, _P, _P]),
+    "sparf_compact_ray_sum": (c_int32, [c_int64, c_int32, c_int64, _P, _P, c_int32, _P, _P, _P]),
     "sparf_density_workspace_bytes": (c_size_t, [POINTER(SparfMLP), c_int64, c_int32, c_int32]),
     "sparf_density_forward": (c_int32, [POINTER(SparfMLP), c_int32, c_int64, _P, _P, _P, _P, c_size_t, _P]),
     "sparf_density_backward": (c_int32, [POINTER(SparfMLP), c_int32, c_int64, _P, _P, _P, POINTER(SparfMLPGrad), _P, _P,

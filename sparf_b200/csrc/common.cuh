@@ -51,6 +51,23 @@ extern unsigned long long g_launch_count;
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// A row count read on the device (the *_rows MLP entry points): of the cap rows a kernel is sized for, starting at row
+// m0 of the call, it processes min(cap, max(0, *rows - m0)).  Kernels take it behind a template flag DYN; without it
+// they process cap rows and never touch `rows`.
+struct RowCount {
+  const int64_t* rows;
+  long long m0;
+};
+template <bool DYN>
+__device__ __forceinline__ long long live_rows(long long cap, const RowCount& rc) {
+  if constexpr (DYN) {
+    const long long k = *rc.rows - rc.m0;
+    return k < 0 ? 0 : (k < cap ? k : cap);
+  } else {
+    return cap;
+  }
+}
+
 // number of SMs of the current device (cached)
 int num_sms();
 

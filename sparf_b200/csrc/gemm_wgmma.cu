@@ -165,10 +165,15 @@ struct TnB {
 
 // image tile (row tile rt, k-step kt) at ((rt * ksteps + kt) * 2 + half) * TILE_ELEMS.  Loads follow the operand's
 // contiguous dimension (KFAST); the split tile is assembled in shared memory and leaves in 16-byte vectors.
-template <bool F16, int PASSES, bool KFAST, class F>
-__global__ void __launch_bounds__(256) pack_kernel(F f, int ksteps, uint16_t* __restrict__ img) {
+// DYN (Rows only): f.M is a capacity, of which live_rows rows are packed; row tiles past them are not written.
+template <bool F16, int PASSES, bool KFAST, class F, bool DYN = false>
+__global__ void __launch_bounds__(256) pack_kernel(F f, int ksteps, uint16_t* __restrict__ img, RowCount rc) {
   __shared__ __align__(16) uint16_t t[2 * TILE_ELEMS];
   const int kt = blockIdx.x, rt = blockIdx.y;
+  if constexpr (DYN) {
+    f.M = (int)live_rows<true>(f.M, rc);
+    if (rt * TM >= f.M) return;
+  }
   float v[16];
 #pragma unroll
   for (int i = 0; i < 16; ++i) {     // all loads first
@@ -280,8 +285,9 @@ __device__ __forceinline__ void store_block_images(const float* V, int n0, uint1
   }
 }
 
-template <int ROWP, int TRP>
-__global__ void __launch_bounds__(256) head_bwd_kernel(const HeadBwd p) {
+// DYN: p.M is a capacity, of which live_rows rows are processed; CTAs past them return at once.
+template <int ROWP, int TRP, bool DYN = false>
+__global__ void __launch_bounds__(256) head_bwd_kernel(const HeadBwd p, RowCount rc) {
   extern __shared__ __align__(16) float hsm[];
   float* V = hsm;                           // [TM][HB_LD] Ghid of this tile's rows, one column block at a time
   float* red = V + TM * HB_LD;              // [8 warps][16 sums][32 lanes]
@@ -290,10 +296,12 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(const HeadBwd p) {
   float* rsum = w9 + 3 * TN;                // [4 warps][4]: sums of gpre 0..2 and graw
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int m0 = blockIdx.x * TM;
+  const int M = (int)live_rows<DYN>(p.M, rc);
+  if (DYN && m0 >= M) return;
   if (tid < TM) {
     const int m = m0 + tid;
     float s[4] = {0.f, 0.f, 0.f, 0.f};
-    if (m < p.M) {
+    if (m < M) {
 #pragma unroll
       for (int j = 0; j < 3; ++j) {
         const float c = p.rgb[(size_t)m * 3 + j];
@@ -328,7 +336,7 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(const HeadBwd p) {
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
       const int m = m0 + warp + 8 * i;
-      x[i] = m < p.M && n < p.HW ? *reinterpret_cast<const float4*>(p.hid + (size_t)m * p.HW + n) : make_float4(0.f, 0.f, 0.f, 0.f);
+      x[i] = m < M && n < p.HW ? *reinterpret_cast<const float4*>(p.hid + (size_t)m * p.HW + n) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
     float cs[4] = {0.f, 0.f, 0.f, 0.f}, dw[3][4];
 #pragma unroll
@@ -811,9 +819,16 @@ __device__ __forceinline__ void epilogue(float (&acc)[64], int bx, int by, const
 // unit's first stages load during an epilogue.  Registers are handed out per warpgroup: the producer warpgroup gives
 // its share back (setmaxnreg), so that the consumers get 232 each (128 x 40 + 256 x 232 <= 64 K) and the epilogue,
 // with its loads issued together, does not spill.
-template <bool F16, int PASSES, bool F32, int ROWP, int TRP>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) wg_gemm_kernel(Opnd a, Opnd b, Units w, Epi e) {
+// DYN (output tiles only, nsplit = 1): e.M is a capacity, of which live_rows rows are computed; the units of A row
+// tiles past them are skipped.
+template <bool F16, int PASSES, bool F32, int ROWP, int TRP, bool DYN = false>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) wg_gemm_kernel(Opnd a, Opnd b, Units w, Epi e, RowCount rc) {
   extern __shared__ __align__(1024) uint8_t smem[];
+  if constexpr (DYN) {
+    e.M = (int)live_rows<true>(e.M, rc);
+    if (e.M == 0) return;
+    w.tiles = (e.M + TM - 1) / TM * w.rtb;
+  }
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + RED_BYTES);
   uint64_t* empty = full + STAGES;
   if (threadIdx.x == 0) {
@@ -959,9 +974,18 @@ __device__ __forceinline__ void convert_staged(const Staged& x, const Units& w, 
 // The weight-gradient GEMM dW += G^T X with B read as fp32 (Staged): wg_gemm_kernel's units, ring, MMAs and atomic
 // epilogue, with a fourth warpgroup that splits each stage's B in place between its copies and its MMAs, so no pack
 // kernel writes and no GEMM reads an image of X.  Registers: producer 40, converter 64, consumers 200 (<= 64 K).
-template <int PASSES>
-__global__ void __launch_bounds__(STAGED_THREADS, 1) wg_gemm_staged_kernel(Opnd a, Staged x, Units w, Epi e) {
+// DYN: x.M is a capacity, of which live_rows rows are summed; the k-range split is gemm_units' for that count, computed
+// here from ctas (the CTAs gemm_units was given).
+template <int PASSES, bool DYN = false>
+__global__ void __launch_bounds__(STAGED_THREADS, 1) wg_gemm_staged_kernel(Opnd a, Staged x, Units w, Epi e, RowCount rc,
+                                                                           int ctas) {
   extern __shared__ __align__(1024) uint8_t smem[];
+  if constexpr (DYN) {
+    x.M = (int)live_rows<true>(x.M, rc);
+    if (x.M == 0) return;
+    w.nk = (x.M + TK - 1) / TK;
+    w.nsplit = max(1, min(w.nk, (ctas + w.tiles - 1) / w.tiles * ((w.nk + 1023) / 1024)));
+  }
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty = full + STAGES;
   uint64_t* conv = empty + STAGES;
@@ -995,18 +1019,18 @@ __global__ void __launch_bounds__(STAGED_THREADS, 1) wg_gemm_staged_kernel(Opnd 
   }
 }
 
-template <bool F16, int PASSES, bool KFAST, class F>
-static int launch_pack(F f, int rtiles, int ksteps, uint16_t* img, cudaStream_t st) {
-  pack_kernel<F16, PASSES, KFAST, F><<<dim3(ksteps, rtiles), 256, 0, st>>>(f, ksteps, img);
+template <bool F16, int PASSES, bool KFAST, class F, bool DYN = false>
+static int launch_pack(F f, int rtiles, int ksteps, uint16_t* img, cudaStream_t st, RowCount rc = {nullptr, 0}) {
+  pack_kernel<F16, PASSES, KFAST, F, DYN><<<dim3(ksteps, rtiles), 256, 0, st>>>(f, ksteps, img, rc);
   SPARF_CHECK_LAUNCH("pack_kernel");
   return SPARF_OK;
 }
 
 template <bool F16, int PASSES, bool F32, int ROWP, int TRP>
-static int launch_gemm(const Opnd& a, const Opnd& b, const Units& w, int ctas, const Epi& e, cudaStream_t st) {
-  auto kernel = wg_gemm_kernel<F16, PASSES, F32, ROWP, TRP>;
+static int launch_gemm(const Opnd& a, const Opnd& b, const Units& w, int ctas, const Epi& e, RowCount rc, cudaStream_t st) {
+  auto kernel = rc.rows ? wg_gemm_kernel<F16, PASSES, F32, ROWP, TRP, true> : wg_gemm_kernel<F16, PASSES, F32, ROWP, TRP>;
   SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
-  kernel<<<std::min(w.tiles * w.nsplit, ctas), GEMM_THREADS, GEMM_SMEM, st>>>(a, b, w, e);
+  kernel<<<std::min(w.tiles * w.nsplit, ctas), GEMM_THREADS, GEMM_SMEM, st>>>(a, b, w, e, rc);
   SPARF_CHECK_LAUNCH("wg_gemm_kernel");
   return SPARF_OK;
 }
@@ -1037,10 +1061,12 @@ static int run(const TcPrec& p, const Opnd& a, int a_rows, FB fb, int b_rows, in
   const int ctas = gemm_ctas(p);
   const Units w = gemm_units(rta, rtb, ksteps, split_k, ctas);
   const bool f32 = e.out != nullptr;
-  if (f32 && !row_passes && !tr_passes) return launch_gemm<F16, PASSES, true, 0, 0>(a, b, w, ctas, e, st);
-  if (f32 && row_passes == PASSES && !tr_passes) return launch_gemm<F16, PASSES, true, PASSES, 0>(a, b, w, ctas, e, st);
-  if (!f32 && row_passes == PASSES && tr_passes == 3) return launch_gemm<F16, PASSES, false, PASSES, 3>(a, b, w, ctas, e, st);
-  if (!f32 && row_passes == PASSES && tr_passes == 1) return launch_gemm<F16, PASSES, false, PASSES, 1>(a, b, w, ctas, e, st);
+  const RowCount rc = p.rows;
+  SPARF_REQUIRE(!rc.rows || !split_k, "tc gemm: a device row count needs the staged weight-gradient GEMM");
+  if (f32 && !row_passes && !tr_passes) return launch_gemm<F16, PASSES, true, 0, 0>(a, b, w, ctas, e, rc, st);
+  if (f32 && row_passes == PASSES && !tr_passes) return launch_gemm<F16, PASSES, true, PASSES, 0>(a, b, w, ctas, e, rc, st);
+  if (!f32 && row_passes == PASSES && tr_passes == 3) return launch_gemm<F16, PASSES, false, PASSES, 3>(a, b, w, ctas, e, rc, st);
+  if (!f32 && row_passes == PASSES && tr_passes == 1) return launch_gemm<F16, PASSES, false, PASSES, 1>(a, b, w, ctas, e, rc, st);
   SPARF_REQUIRE(false, "tc gemm: no kernel for fp32 output %d, row image %d passes, transposed image %d passes", (int)f32,
                 row_passes, tr_passes);
 }
@@ -1050,9 +1076,9 @@ template <int PASSES>
 static int run_staged(const TcPrec& p, const Opnd& gt, int N, const Staged& x, int ksteps, const Epi& e, cudaStream_t st) {
   const int ctas = gemm_ctas(p);
   const Units w = gemm_units(ceil_div(N, TM), ceil_div(x.K, TM), ksteps, true, ctas);
-  auto kernel = wg_gemm_staged_kernel<PASSES>;
+  auto kernel = p.rows.rows ? wg_gemm_staged_kernel<PASSES, true> : wg_gemm_staged_kernel<PASSES>;
   SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, STAGED_SMEM));
-  kernel<<<std::min(w.tiles * w.nsplit, ctas), STAGED_THREADS, STAGED_SMEM, st>>>(gt, x, w, e);
+  kernel<<<std::min(w.tiles * w.nsplit, ctas), STAGED_THREADS, STAGED_SMEM, st>>>(gt, x, w, e, p.rows, ctas);
   SPARF_CHECK_LAUNCH("wg_gemm_staged_kernel");
   return SPARF_OK;
 }
@@ -1090,6 +1116,13 @@ size_t tc_pack_elems(int rows, int ksteps_rows, int cols) {
 int tc_pack_rows(TcPrec p, int M, int K, const float* X, int ldx, int div, TcImage img, cudaStream_t st) {
   SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && img.p && img.ks == ceil_div(K, TK), "tc_pack_rows: passes=%d ks=%d K=%d",
                 p.passes, img.ks, K);
+  if (p.rows.rows) {
+    const Rows f{X, ldx, K, div, M};
+    return p.f16 ? (p.passes == 3 ? launch_pack<true, 3, true, Rows, true>(f, ceil_div(M, TM), img.ks, img.p, st, p.rows)
+                                  : launch_pack<true, 1, true, Rows, true>(f, ceil_div(M, TM), img.ks, img.p, st, p.rows))
+                 : (p.passes == 3 ? launch_pack<false, 3, true, Rows, true>(f, ceil_div(M, TM), img.ks, img.p, st, p.rows)
+                                  : launch_pack<false, 1, true, Rows, true>(f, ceil_div(M, TM), img.ks, img.p, st, p.rows));
+  }
   return SPARF_WG_PACK(true, Rows{X, ldx, K, div, M}, ceil_div(M, TM), img.ks, img.p, st);
 }
 
@@ -1143,14 +1176,15 @@ int tc_gemm_tn(TcPrec p, int M, int N, int K, int Kv, TcImage gt, const float* X
     const Staged x{X, ldx, div, M, K, bits, ceil_div(K, 32)};
     return p.passes == 3 ? run_staged<3>(p, opnd(gt), N, x, gt.ks, e, st) : run_staged<1>(p, opnd(gt), N, x, gt.ks, e, st);
   }
+  SPARF_REQUIRE(!p.rows.rows, "tc_gemm_tn: a device row count needs X 16-byte aligned with ldx and K multiples of 4");
   return SPARF_WG_RUN(false, p, opnd(gt), N, TnB{X, ldx, div, M, K, bits, ceil_div(K, 32)}, K, gt.ks, true, e, 0, 0, st);
 }
 
 template <int ROWP, int TRP>
-static int launch_head_bwd(const HeadBwd& h, cudaStream_t st) {
-  auto kernel = head_bwd_kernel<ROWP, TRP>;
+static int launch_head_bwd(const HeadBwd& h, RowCount rc, cudaStream_t st) {
+  auto kernel = rc.rows ? head_bwd_kernel<ROWP, TRP, true> : head_bwd_kernel<ROWP, TRP>;
   SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HEAD_SMEM));
-  kernel<<<ceil_div(h.M, TM), 256, HEAD_SMEM, st>>>(h);
+  kernel<<<ceil_div(h.M, TM), 256, HEAD_SMEM, st>>>(h, rc);
   SPARF_CHECK_LAUNCH("head_bwd_kernel");
   return SPARF_OK;
 }
@@ -1164,9 +1198,9 @@ int tc_head_backward(TcPrec dg, TcPrec wg, int M, int HW, const float* d_rgb, co
   SPARF_REQUIRE(row.p && row.ks == ceil_div(HW, TK) && tr.p && tr.ks == ceil_div(M, TK),
                 "tc_head_backward: images need %d and %d k-steps", ceil_div(HW, TK), ceil_div(M, TK));
   const HeadBwd h{M, HW, d_rgb, rgb, d_sigma, raw, hid, W9, graw, row.p, tr.p, row.ks, tr.ks, dW9, db9, db_hid, db_raw};
-  if (dg.passes == 3 && wg.passes == 3) return launch_head_bwd<3, 3>(h, st);
-  if (dg.passes == 3 && wg.passes == 1) return launch_head_bwd<3, 1>(h, st);
-  if (dg.passes == 1 && wg.passes == 1) return launch_head_bwd<1, 1>(h, st);
+  if (dg.passes == 3 && wg.passes == 3) return launch_head_bwd<3, 3>(h, dg.rows, st);
+  if (dg.passes == 3 && wg.passes == 1) return launch_head_bwd<3, 1>(h, dg.rows, st);
+  if (dg.passes == 1 && wg.passes == 1) return launch_head_bwd<1, 1>(h, dg.rows, st);
   SPARF_REQUIRE(false, "tc_head_backward: no kernel for %d-pass row and %d-pass transposed images", dg.passes, wg.passes);
 }
 

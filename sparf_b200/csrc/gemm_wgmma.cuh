@@ -20,6 +20,10 @@ struct TcPrec {
   uint16_t* pack_b = nullptr;
   size_t pack_elems = 0;
   int max_ctas = 0;   // > 0: at most this many CTAs per GEMM (self-tests of the persistent loop); else one per SM
+  // rows.rows != NULL: the row count M of a call (the rows of A and of an NT / NN output, the contraction of a TN) is a
+  // capacity, of which the kernels process min(M, max(0, *rows.rows - rows.m0)) rows, read on the device.  The TN
+  // GEMM's k-range split is then computed in the kernel from that count, as the host computes it from M.
+  RowCount rows{nullptr, 0};
 };
 
 // An operand image of a [rows x K] matrix: split 16-bit halves in [128 rows x 32 K] tiles of wgmma's shared-memory

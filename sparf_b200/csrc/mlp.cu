@@ -27,11 +27,13 @@ __global__ void c2f_weights_kernel(C2F c, int L_xyz, int L_view, float* __restri
 
 // enc[m][0:3] = x = o + t*d ; enc[m][3 + c*2L + {0,L} + j] = w_j * {sin,cos}(x_c * 2^j pi) ; zero pad to E3p
 // dirs == NULL: the origins are the points themselves, x = o (S = 1; the value o + 0*d takes)
+// DYN (S = 1): total / E3p rows is a capacity, of which live_rows are encoded (the same for every kernel below with DYN)
+template <bool DYN = false>
 __global__ void encode_xyz_kernel(long long total, int S, int L, int E3p, const float* __restrict__ origins,
                                   const float* __restrict__ dirs, const float* __restrict__ t,
-                                  const float* __restrict__ wts, float* __restrict__ enc) {
+                                  const float* __restrict__ wts, float* __restrict__ enc, RowCount rc) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= total) return;
+  if (idx >= (DYN ? live_rows<DYN>(total / E3p, rc) * E3p : total)) return;
   int col = (int)(idx % E3p);
   long long m = idx / E3p;
   long long r = m / S;
@@ -53,10 +55,11 @@ __global__ void encode_xyz_kernel(long long total, int S, int L, int E3p, const 
 }
 
 // per-ray view-direction encoding: unit = d / max(|d|, 1e-12) (F.normalize), same layout as above
+template <bool DYN = false>
 __global__ void encode_dir_kernel(int total, int L, int Evp, const float* __restrict__ dirs,
-                                  const float* __restrict__ wts_view, float* __restrict__ denc) {
+                                  const float* __restrict__ wts_view, float* __restrict__ denc, RowCount rc) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= total) return;
+  if (idx >= (DYN ? (int)live_rows<DYN>(total / Evp, rc) * Evp : total)) return;
   int col = idx % Evp, r = idx / Evp;
   float val = 0.f;
   if (col < 3 + 6 * L) {
@@ -289,13 +292,13 @@ static EnginePrec engine_prec(int engine) {
 // ------------------------------------------------------------------------------------------------
 // MODE 0: density row:  raw = X.W[0] + b ; z = raw + noise ; raw_out[m] = z ; sigma[m] = softplus(z)
 // MODE 1: colour head:  rgb[m][j] = sigmoid(X.W[j] + b[j]), j < 3
-template <int MODE>
+template <int MODE, bool DYN = false>
 __global__ void rowdot_kernel(long long M, int K, const float* __restrict__ X, int ldx, const float* __restrict__ W,
                               int ldw, const float* __restrict__ bias, const float* __restrict__ noise,
-                              float* __restrict__ raw_out, float* __restrict__ out) {
+                              float* __restrict__ raw_out, float* __restrict__ out, RowCount rc) {
   const int lane = threadIdx.x & 31;
   long long m = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (m >= M) return;
+  if (m >= live_rows<DYN>(M, rc)) return;
   constexpr int NS = MODE == 0 ? 1 : 3;
   float acc[NS];
 #pragma unroll
@@ -405,9 +408,11 @@ __global__ void relu_mask_kernel(long long total, const float* __restrict__ feat
 }
 
 // out[r][c] = sum_{k<S} in[(r*S+k)][c]
-__global__ void ray_reduce_kernel(int nrays, int S, int C, const float* __restrict__ in, float* __restrict__ out) {
+template <bool DYN = false>
+__global__ void ray_reduce_kernel(int nrays, int S, int C, const float* __restrict__ in, float* __restrict__ out,
+                                  RowCount rc) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= nrays * C) return;
+  if (idx >= (int)live_rows<DYN>(nrays, rc) * C) return;
   int c = idx % C, r = idx / C;
   float acc = 0.f;
   for (int k = 0; k < S; ++k) acc += in[((size_t)r * S + k) * C + c];
@@ -417,12 +422,13 @@ __global__ void ray_reduce_kernel(int nrays, int S, int C, const float* __restri
 // positional-encoding backward + reduction over the ray:  d_o += sum_k g_x ; d_d += sum_k t_k g_x
 // d/dx [w sin(f x)] = f * (w cos(f x)) = f * enc_cos ; d/dx [w cos(f x)] = -f * enc_sin.  One warp per ray.
 // t == NULL (with d_d == NULL): the encoding of points (encode_xyz_kernel without dirs), d_o = the points' gradient.
+template <bool DYN = false>
 __global__ void posenc_bwd_kernel(int nrays, int S, int L, int E3p, const float* __restrict__ enc,
                                   const float* __restrict__ Genc, const float* __restrict__ t,
-                                  float* __restrict__ d_o, float* __restrict__ d_d) {
+                                  float* __restrict__ d_o, float* __restrict__ d_d, RowCount rc) {
   const int lane = threadIdx.x & 31;
   int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (r >= nrays) return;
+  if (r >= (int)live_rows<DYN>(nrays, rc)) return;
   float so[3] = {0.f, 0.f, 0.f}, sd[3] = {0.f, 0.f, 0.f};
   for (int k = lane; k < S; k += 32) {
     size_t m = (size_t)r * S + k;
@@ -459,11 +465,12 @@ __global__ void posenc_bwd_kernel(int nrays, int S, int L, int E3p, const float*
 }
 
 // view-direction encoding backward: g_unit from Gdenc, then through unit = d/|d|
+template <bool DYN = false>
 __global__ void direnc_bwd_kernel(int nrays, int L, int Evp, const float* __restrict__ denc,
                                   const float* __restrict__ Gdenc, const float* __restrict__ dirs,
-                                  float* __restrict__ d_d) {
+                                  float* __restrict__ d_d, RowCount rc) {
   int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= nrays) return;
+  if (r >= (int)live_rows<DYN>(nrays, rc)) return;
   const float* e = denc + (size_t)r * Evp;
   const float* g = Gdenc + (size_t)r * Evp;
   float gu[3];
@@ -688,6 +695,14 @@ struct Call {
   Ws w;             // the workspace, carved for one chunk
   EnginePrec ep;    // with the workspace's buffer for packed weights
   Tape tape;        // the whole batch's tape (taped passes)
+  RowCount rc{nullptr, 0};   // rc.rows != NULL (the *_rows calls, S = 1): the rows are a capacity, *rc.rows live
+
+  // the chunk starting at row m0: the kernels' and GEMMs' live rows are counted from there
+  void at(long long m0) {
+    if (!rc.rows) return;
+    rc.m0 = m0;
+    for (TcPrec* p : {&ep.fwd, &ep.dgrad, &ep.wgrad}) p->rows = rc;
+  }
 };
 
 // The steps every MLP and density call starts with: resolve the engine, validate the network (head: with the colour
@@ -737,8 +752,12 @@ static int chunk_encode_xyz(const SparfMLP* mlp, const Call& c, long long Mc, in
   C2F c2f{mlp->use_c2f, mlp->c2f_start, mlp->c2f_range, mlp->progress};
   c2f_weights_kernel<<<1, 32, 0, st>>>(c2f, mlp->L_xyz, mlp->L_view, c.w.wts);
   SPARF_CHECK_LAUNCH("c2f_weights_kernel");
-  encode_xyz_kernel<<<ceil_div(Mc * d.E3p, 256), 256, 0, st>>>(Mc * d.E3p, S, mlp->L_xyz, d.E3p, origins, dirs, t, c.w.wts,
-                                                               enc);
+  if (c.rc.rows)
+    encode_xyz_kernel<true><<<ceil_div(Mc * d.E3p, 256), 256, 0, st>>>(Mc * d.E3p, S, mlp->L_xyz, d.E3p, origins, dirs, t,
+                                                                       c.w.wts, enc, c.rc);
+  else
+    encode_xyz_kernel<<<ceil_div(Mc * d.E3p, 256), 256, 0, st>>>(Mc * d.E3p, S, mlp->L_xyz, d.E3p, origins, dirs, t, c.w.wts,
+                                                                 enc, c.rc);
   SPARF_CHECK_LAUNCH("encode_xyz_kernel");
   if (c.tc) SPARF_TRY(tc_pack_rows(c.ep.fwd, (int)Mc, d.E3p, enc, d.E3p, 1, c.w.encimg, st));
   return SPARF_OK;
@@ -773,7 +792,12 @@ static int chunk_trunk(const SparfMLP* mlp, const Call& c, long long Mc, const f
                         sk ? enc : nullptr, d.E3p, d.E3p, d.E3, 1, Wl, ldw, d.W, bl, H[l], d.W, st));
     }
     if (last && (raw || sigma)) {
-      rowdot_kernel<0><<<ceil_div(Mc, 8), 256, 0, st>>>(Mc, d.W, in, d.W, mlp->trunk_w[l], ldw, mlp->trunk_b[l], noise, raw, sigma);
+      if (c.rc.rows)
+        rowdot_kernel<0, true><<<ceil_div(Mc, 8), 256, 0, st>>>(Mc, d.W, in, d.W, mlp->trunk_w[l], ldw, mlp->trunk_b[l], noise,
+                                                                raw, sigma, c.rc);
+      else
+        rowdot_kernel<0><<<ceil_div(Mc, 8), 256, 0, st>>>(Mc, d.W, in, d.W, mlp->trunk_w[l], ldw, mlp->trunk_b[l], noise, raw,
+                                                         sigma, c.rc);
       SPARF_CHECK_LAUNCH("rowdot_kernel<0>");
     }
     in = H[l];
@@ -788,8 +812,12 @@ static int chunk_forward(const SparfMLP* mlp, const Call& c, int nr, int S, cons
   const MlpDims& d = c.d;
   const long long Mc = (long long)nr * S;
   SPARF_TRY(chunk_encode_xyz(mlp, c, Mc, S, origins, dirs, t, v.enc, st));
-  encode_dir_kernel<<<ceil_div((long long)nr * d.Evp, 256), 256, 0, st>>>(nr * d.Evp, mlp->L_view, d.Evp, dirs, c.w.wts + 16,
-                                                                          v.denc);
+  if (c.rc.rows)
+    encode_dir_kernel<true><<<ceil_div((long long)nr * d.Evp, 256), 256, 0, st>>>(nr * d.Evp, mlp->L_view, d.Evp, dirs,
+                                                                                  c.w.wts + 16, v.denc, c.rc);
+  else
+    encode_dir_kernel<<<ceil_div((long long)nr * d.Evp, 256), 256, 0, st>>>(nr * d.Evp, mlp->L_view, d.Evp, dirs, c.w.wts + 16,
+                                                                            v.denc, c.rc);
   SPARF_CHECK_LAUNCH("encode_dir_kernel");
   if (c.tc) SPARF_TRY(tc_pack_rows(c.ep.fwd, (int)Mc, d.Evp, v.denc, d.Evp, S, c.w.dencimg, st));
   SPARF_TRY(chunk_trunk(mlp, c, Mc, v.enc, v.H, noise, v.raw, sigma, true, st));
@@ -799,24 +827,43 @@ static int chunk_forward(const SparfMLP* mlp, const Call& c, int nr, int S, cons
   else
     SPARF_TRY(gemm_nt((int)Mc, d.HW, v.H[d.nt - 1], d.W, d.W, d.W, v.denc, d.Evp, d.Evp, d.Ev, S, mlp->head_w[0], d.W + d.Ev,
                       d.W, mlp->head_b[0], v.hid, d.HW, st));
-  rowdot_kernel<1><<<ceil_div(Mc, 8), 256, 0, st>>>(Mc, d.HW, v.hid, d.HW, mlp->head_w[1], d.HW, mlp->head_b[1], nullptr, nullptr,
-                                                   rgb);
+  if (c.rc.rows)
+    rowdot_kernel<1, true><<<ceil_div(Mc, 8), 256, 0, st>>>(Mc, d.HW, v.hid, d.HW, mlp->head_w[1], d.HW, mlp->head_b[1], nullptr,
+                                                            nullptr, rgb, c.rc);
+  else
+    rowdot_kernel<1><<<ceil_div(Mc, 8), 256, 0, st>>>(Mc, d.HW, v.hid, d.HW, mlp->head_w[1], d.HW, mlp->head_b[1], nullptr,
+                                                     nullptr, rgb, c.rc);
   SPARF_CHECK_LAUNCH("rowdot_kernel<1>");
   return SPARF_OK;
 }
 
+// The taped calls with a device row count (sparf_mlp_*_tape_rows): tensor-core engines and one-sample rays only
+static int rows_call(const char* who, Call* c, int S, const int64_t* rows) {
+  if (!rows) return SPARF_OK;
+  if (!c->tc) {
+    set_error("%s: a device row count needs a tensor-core engine (tc_3x, tc_1x or tc_3x_w1)", who);
+    return SPARF_ERR_UNSUPPORTED;
+  }
+  SPARF_REQUIRE(S == 1, "%s: a device row count needs S = 1 (one-sample rays), got S = %d", who, S);
+  c->rc.rows = rows;
+  return SPARF_OK;
+}
+
 // The MLP forward, chunk by chunk.  tape == NULL: the activations stay in the workspace; else they go straight into the
-// tape.
+// tape.  rows != NULL (taped, S = 1): R is a capacity, *rows the rays evaluated.
 static int mlp_forward(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs, const float* t,
                        const float* noise, float* sigma, float* rgb, void* tape, size_t tape_bytes, void* workspace,
-                       size_t workspace_bytes, cudaStream_t st) {
+                       size_t workspace_bytes, cudaStream_t st, const int64_t* rows = nullptr) {
   Call c;
-  SPARF_TRY(begin_call(tape ? "mlp_forward_tape" : "mlp_forward", mlp, engine, R, S,
-                       tape ? Pass::kTapedForward : Pass::kForward, true, tape, tape_bytes, workspace, workspace_bytes, &c));
+  const char* who = rows ? "mlp_forward_tape_rows" : tape ? "mlp_forward_tape" : "mlp_forward";
+  SPARF_TRY(begin_call(who, mlp, engine, R, S, tape ? Pass::kTapedForward : Pass::kForward, true, tape, tape_bytes, workspace,
+                       workspace_bytes, &c));
+  SPARF_TRY(rows_call(who, &c, S, rows));
   Tape v = c.w.act;
   v.raw = nullptr;      // the plain forward does not keep the softplus argument
   for (int r0 = 0; r0 < R; r0 += c.nrc) {
     const int nr = std::min(c.nrc, R - r0);
+    c.at(r0);
     const size_t m0 = (size_t)r0 * S;
     SPARF_TRY(chunk_forward(mlp, c, nr, S, origins + (size_t)r0 * 3, dirs + (size_t)r0 * 3, t + m0, noise ? noise + m0 : nullptr,
                             tape ? tape_chunk(c.tape, c.d, r0, S) : v, sigma + m0, rgb + m0 * 3, st));
@@ -970,20 +1017,23 @@ static int trunk_backward_tc(const SparfMLP* mlp, const Call& c, long long Mc, c
 }
 
 // The MLP backward, chunk by chunk.  tape == NULL: recompute each chunk's forward in the workspace (noise as in the
-// forward call); else read the activations from the tape and the colour output from rgb_fwd, the forward's.
+// forward call); else read the activations from the tape and the colour output from rgb_fwd, the forward's.  rows: as
+// in mlp_forward.
 static int mlp_backward(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs, const float* t,
                         const float* noise, const float* rgb_fwd, void* tape, size_t tape_bytes, const float* d_sigma,
                         const float* d_rgb, const SparfMLPGrad* grad, float* d_origins, float* d_dirs, void* workspace,
-                        size_t workspace_bytes, cudaStream_t st) {
+                        size_t workspace_bytes, cudaStream_t st, const int64_t* rows = nullptr) {
   Call c;
-  SPARF_TRY(begin_call(tape ? "mlp_backward_tape" : "mlp_backward", mlp, engine, R, S,
-                       tape ? Pass::kTapedBackward : Pass::kRecomputeBackward, true, tape, tape_bytes, workspace,
-                       workspace_bytes, &c));
+  const char* who = rows ? "mlp_backward_tape_rows" : tape ? "mlp_backward_tape" : "mlp_backward";
+  SPARF_TRY(begin_call(who, mlp, engine, R, S, tape ? Pass::kTapedBackward : Pass::kRecomputeBackward, true, tape, tape_bytes,
+                       workspace, workspace_bytes, &c));
+  SPARF_TRY(rows_call(who, &c, S, rows));
   const MlpDims& d = c.d;
   const Ws& w = c.w;
   const bool need_rays = d_origins != nullptr || d_dirs != nullptr;
   for (int r0 = 0; r0 < R; r0 += c.nrc) {
     const int nr = std::min(c.nrc, R - r0);
+    c.at(r0);
     const long long Mc = (long long)nr * S;
     const size_t m0 = (size_t)r0 * S;
     const float* d_c = dirs + (size_t)r0 * 3;
@@ -995,17 +1045,28 @@ static int mlp_backward(const SparfMLP* mlp, int engine, int R, int S, const flo
     SPARF_TRY(c.tc ? head_backward_tc(mlp, c, Mc, S, d_rgb + m0 * 3, rgbv, d_sigma + m0, v, grad, d_dirs != nullptr, st)
                    : head_backward_simt(mlp, c, Mc, S, d_rgb + m0 * 3, rgbv, d_sigma + m0, v, grad, d_dirs != nullptr, st));
     if (d_dirs) {
-      ray_reduce_kernel<<<ceil_div((long long)nr * d.Evp, 256), 256, 0, st>>>(nr, S, d.Evp, w.Gdtmp, w.Gdenc);
-      SPARF_CHECK_LAUNCH("ray_reduce_kernel");
-      direnc_bwd_kernel<<<ceil_div(nr, 128), 128, 0, st>>>(nr, mlp->L_view, d.Evp, v.denc, w.Gdenc, d_c, d_dirs + (size_t)r0 * 3);
+      if (c.rc.rows) {
+        ray_reduce_kernel<true><<<ceil_div((long long)nr * d.Evp, 256), 256, 0, st>>>(nr, S, d.Evp, w.Gdtmp, w.Gdenc, c.rc);
+        SPARF_CHECK_LAUNCH("ray_reduce_kernel");
+        direnc_bwd_kernel<true><<<ceil_div(nr, 128), 128, 0, st>>>(nr, mlp->L_view, d.Evp, v.denc, w.Gdenc, d_c,
+                                                                   d_dirs + (size_t)r0 * 3, c.rc);
+      } else {
+        ray_reduce_kernel<<<ceil_div((long long)nr * d.Evp, 256), 256, 0, st>>>(nr, S, d.Evp, w.Gdtmp, w.Gdenc, c.rc);
+        SPARF_CHECK_LAUNCH("ray_reduce_kernel");
+        direnc_bwd_kernel<<<ceil_div(nr, 128), 128, 0, st>>>(nr, mlp->L_view, d.Evp, v.denc, w.Gdenc, d_c, d_dirs + (size_t)r0 * 3,
+                                                             c.rc);
+      }
       SPARF_CHECK_LAUNCH("direnc_bwd_kernel");
     }
     SPARF_TRY(c.tc ? trunk_backward_tc(mlp, c, Mc, v.enc, v.H, w.graw, grad, need_rays, st)
                    : trunk_backward_simt(mlp, c, Mc, v.enc, v.H, w.graw, grad, need_rays, st));
     if (need_rays) {
-      posenc_bwd_kernel<<<ceil_div(nr, 4), 128, 0, st>>>(nr, S, mlp->L_xyz, d.E3p, v.enc, w.Genc, t + m0,
-                                                        d_origins ? d_origins + (size_t)r0 * 3 : nullptr,
-                                                        d_dirs ? d_dirs + (size_t)r0 * 3 : nullptr);
+      float* d_o = d_origins ? d_origins + (size_t)r0 * 3 : nullptr;
+      float* d_d = d_dirs ? d_dirs + (size_t)r0 * 3 : nullptr;
+      if (c.rc.rows)
+        posenc_bwd_kernel<true><<<ceil_div(nr, 4), 128, 0, st>>>(nr, S, mlp->L_xyz, d.E3p, v.enc, w.Genc, t + m0, d_o, d_d, c.rc);
+      else
+        posenc_bwd_kernel<<<ceil_div(nr, 4), 128, 0, st>>>(nr, S, mlp->L_xyz, d.E3p, v.enc, w.Genc, t + m0, d_o, d_d, c.rc);
       SPARF_CHECK_LAUNCH("posenc_bwd_kernel");
     }
   }
@@ -1118,6 +1179,29 @@ extern "C" int sparf_mlp_backward_tape(const SparfMLP* mlp, int32_t engine, int3
                       d_dirs, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
+// the taped pair with a device row count: R = C is the capacity, *rows = K the rows evaluated
+extern "C" int sparf_mlp_forward_tape_rows(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S, const int64_t* rows,
+                                           const float* origins, const float* dirs, const float* t, const float* noise,
+                                           float* sigma, float* rgb, void* tape, size_t tape_bytes, void* workspace,
+                                           size_t workspace_bytes, sparf_stream_t stream) {
+  SPARF_REQUIRE(mlp && R > 0 && S > 0 && rows && origins && dirs && t && sigma && rgb && tape,
+                "mlp_forward_tape_rows: bad arguments");
+  return mlp_forward(mlp, engine, R, S, origins, dirs, t, noise, sigma, rgb, tape, tape_bytes, workspace, workspace_bytes,
+                     (cudaStream_t)stream, rows);
+}
+
+extern "C" int sparf_mlp_backward_tape_rows(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S, const int64_t* rows,
+                                            const float* origins, const float* dirs, const float* t, const float* sigma,
+                                            const float* rgb, const float* d_sigma, const float* d_rgb,
+                                            const SparfMLPGrad* grad, float* d_origins, float* d_dirs, void* tape,
+                                            size_t tape_bytes, void* workspace, size_t workspace_bytes,
+                                            sparf_stream_t stream) {
+  SPARF_REQUIRE(mlp && R > 0 && S > 0 && rows && origins && dirs && t && sigma && rgb && d_sigma && d_rgb && grad && tape,
+                "mlp_backward_tape_rows: bad arguments");
+  return mlp_backward(mlp, engine, R, S, origins, dirs, t, nullptr, rgb, tape, tape_bytes, d_sigma, d_rgb, grad, d_origins,
+                      d_dirs, workspace, workspace_bytes, (cudaStream_t)stream, rows);
+}
+
 extern "C" size_t sparf_density_workspace_bytes(const SparfMLP* mlp, int64_t M, int32_t backward, int32_t engine) {
   if (!mlp || M <= 0) return 0;
   const int e = resolve_engine(engine);
@@ -1179,7 +1263,7 @@ extern "C" int sparf_density_backward(const SparfMLP* mlp, int32_t engine, int64
                    : trunk_backward_simt(mlp, c, n, v.enc, v.H, dr, grad, d_points != nullptr, st));
     if (d_points) {
       posenc_bwd_kernel<<<ceil_div(n, 4), 128, 0, st>>>(n, 1, mlp->L_xyz, d.E3p, v.enc, c.w.Genc, nullptr,
-                                                       d_points + (size_t)p0 * 3, nullptr);
+                                                       d_points + (size_t)p0 * 3, nullptr, c.rc);
       SPARF_CHECK_LAUNCH("posenc_bwd_kernel");
     }
   }

@@ -101,14 +101,48 @@ def build_grid(opt, nerf, res=None, range=None, thres=0.01, engine=None, contrac
     engine: None = the current ops engine."""
     if contraction is None:
         res, rng, _ = mesh.trimesh_settings(opt, res, range)
-        sigma = mesh.density_grid(opt, nerf, res=res, range=rng, engine=engine)
-        return OccupancyGrid(ops.occupancy_build(sigma, thres), res, rng, thres)
+        return OccupancyGrid(ops.occupancy_build(_lattice_sigma(opt, nerf, res, rng, None, engine), thres), res, rng, thres)
     assert range is None, "a contracted grid covers the cube [-2, 2]^3 of the contracted space"
     res = mesh.trimesh_settings(opt, res)[0]
     contraction = _as_contraction(contraction)
-    sigma = mesh.lattice_density(nerf, mesh.lattice_axis(res, CONTRACTED_RANGE), engine=engine,
-                                 warp=contracted_warp(*contraction))
+    sigma = _lattice_sigma(opt, nerf, res, CONTRACTED_RANGE, contraction, engine)
     return OccupancyGrid(ops.occupancy_build(sigma, thres), res, CONTRACTED_RANGE, thres, contraction)
+
+
+def _lattice_sigma(opt, nerf, res, rng, contraction, engine):
+    """σ on the lattice a grid is built from: mesh.density_grid over the box rng, or the contracted lattice"""
+    if contraction is None:
+        return mesh.density_grid(opt, nerf, res=res, range=rng, engine=engine)
+    return mesh.lattice_density(nerf, mesh.lattice_axis(res, CONTRACTED_RANGE), engine=engine,
+                                warp=contracted_warp(*contraction))
+
+
+@torch.no_grad()
+def refresh_(grid: OccupancyGrid, opt, nerf, engine=None) -> OccupancyGrid:
+    """Rebuild `grid` in place from the network's current weights and nerf.progress: the lattice and threshold of
+    build_grid, written into the grid's existing `bits` tensor, so that a CUDA graph captured with the grid sees the new
+    cells on its next replay.  A grid is a snapshot of the network when it was built or last refreshed: in training
+    (Graph.set_training_occupancy) the samples it skips get no gradient until the next refresh, so refresh it every few
+    steps, between steps (outside any captured graph)."""
+    sigma = _lattice_sigma(opt, nerf, grid.res, grid.range, grid.contraction, engine)
+    grid.bits.copy_(ops.occupancy_build(sigma, grid.thres))
+    return grid
+
+
+def train_forward_samples(nerf, grid: OccupancyGrid, opt, center, ray, depth_samples, mode) -> dict:
+    """NeRF.forward_samples with gradients over the samples the grid keeps (ops.mlp_forward_grid): the skipped samples
+    get σ = 0, rgb = 0 and no gradient; the kept ones the values of the dense pass, with its density noise (the same
+    randn_like draw, taken at the kept samples).  Nothing in it synchronises, so a training step that calls it can be
+    captured into one CUDA graph.  center, ray [B,N,3]; depth_samples [B,N,S,1] -> dict(rgb_samples [B,N,S,3],
+    density_samples [B,N,S])."""
+    B, N, S = depth_samples.shape[:3]
+    t = depth_samples.reshape(B * N, S)
+    noise = None
+    if opt.nerf.density_noise_reg and mode == "train":
+        noise = (torch.randn_like(depth_samples[..., 0]).to(t.device) * opt.nerf.density_noise_reg).reshape(B * N, S)
+    sigma, rgb = ops.mlp_forward_grid(nerf._spec(), center.reshape(B * N, 3), ray.reshape(B * N, 3), t, grid,
+                                      nerf.kernel_params(), noise=noise, progress=nerf.progress)
+    return dict(rgb_samples=rgb.view(B, N, S, 3), density_samples=sigma.view(B, N, S))
 
 
 @torch.no_grad()

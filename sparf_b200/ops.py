@@ -267,6 +267,125 @@ def mlp_forward(spec: MLPSpec, origins, dirs, t, params: Sequence[torch.Tensor],
     return MLPFunction.apply(spec, eng, torch.is_grad_enabled(), origins, dirs, t, noise, progress, *params)
 
 
+def _grid_compact(grid, o, d, t, K, idx, o_k, d_k, t_k):
+    """The samples of o, d [R,3], t [R,S] that `grid` (occupancy.OccupancyGrid, box or contracted) keeps, into the
+    capacity-R*S buffers idx, o_k, d_k, t_k; their count into the device scalar K.  The host never reads K."""
+    L = _lib.lib()
+    R, S = t.shape
+    if grid.contraction is None:
+        ws = _workspace(L.sparf_occupancy_workspace_bytes(R, S), t.device)
+        args = (R, S, _ptr(o), _ptr(d), _ptr(t), _ptr(grid.bits), int(grid.res), float(grid.range[0]), float(grid.range[1]))
+        check(L.sparf_occupancy_count(*args, _ptr(K), _ptr(ws), ws.numel(), _stream()), "occupancy_count")
+        check(L.sparf_occupancy_emit(*args, _ptr(idx), _ptr(o_k), _ptr(d_k), _ptr(t_k), _ptr(ws), ws.numel(), _stream()),
+              "occupancy_emit")
+    else:
+        center, radius = grid.contraction
+        c = (ctypes.c_float * 3)(*center)
+        ws = _workspace(L.sparf_termination_workspace_bytes(R, S), t.device)
+        args = (R, S, 0, S, _ptr(o), _ptr(d), _ptr(t), None, _ptr(grid.bits), int(grid.res), c, float(radius))
+        check(L.sparf_contracted_count(*args, _ptr(K), _ptr(ws), ws.numel(), _stream()), "contracted_count")
+        check(L.sparf_contracted_emit(*args, _ptr(idx), _ptr(o_k), _ptr(d_k), _ptr(t_k), _ptr(ws), ws.numel(), _stream()),
+              "contracted_emit")
+
+
+class GridMLPFunction(torch.autograd.Function):
+    """mlp_forward over the samples an occupancy grid keeps, with gradients and without a host round trip: the
+    compaction writes the kept count K to device memory, the taped MLP pair with a device row count evaluates the K
+    kept samples out of a capacity of R*S, and scatter / gather / ray-sum kernels move rows between the dense and the
+    compacted layouts, all reading K on the device.  So the op is capturable into a CUDA graph."""
+
+    @staticmethod
+    @_on_tensor_device
+    def forward(ctx, spec: MLPSpec, engine: int, grid, origins, dirs, t, noise, progress, *params):
+        L = _lib.lib()
+        o, d, tt = _f32c(origins), _f32c(dirs), _f32c(t)
+        R, S = tt.shape
+        assert o.shape == (R, 3) and d.shape == (R, 3)
+        C, dev = R * S, tt.device
+        sigma = torch.zeros(R, S, device=dev)
+        rgb = torch.zeros(R, S, 3, device=dev)
+        ctx.C = C
+        if C == 0:
+            return sigma, rgb
+        K = torch.empty((), dtype=torch.int64, device=dev)
+        idx = torch.empty(C, dtype=torch.int64, device=dev)
+        o_k, d_k, t_k = torch.empty(C, 3, device=dev), torch.empty(C, 3, device=dev), torch.empty(C, 1, device=dev)
+        _grid_compact(grid, o, d, tt, K, idx, o_k, d_k, t_k)
+        noise_k = None
+        if noise is not None:         # drawn dense by the caller (the RNG stream of the dense pass), taken at the kept samples
+            noise_k = torch.empty(C, 1, device=dev)
+            check(L.sparf_compact_gather(C, _ptr(K), _ptr(idx), 1, _ptr(_f32c(noise)), _ptr(noise_k), _stream()),
+                  "compact_gather")
+        m, keep = spec.fill(params, progress)
+        tape_bytes = L.sparf_mlp_tape_bytes(ctypes.byref(m), engine, C, 1)
+        if not tape_bytes:
+            raise RuntimeError("mlp_forward_grid: no tape for %d samples (a tape above 16 GB); use smaller batches" % C)
+        tape = torch.empty(tape_bytes, dtype=torch.uint8, device=dev)
+        ws = _workspace(L.sparf_mlp_workspace_bytes(ctypes.byref(m), C, 1, 0, engine), dev)
+        sigma_k, rgb_k = torch.empty(C, 1, device=dev), torch.empty(C, 1, 3, device=dev)
+        with _timed("mlp_forward"):
+            check(L.sparf_mlp_forward_tape_rows(ctypes.byref(m), engine, C, 1, _ptr(K), _ptr(o_k), _ptr(d_k), _ptr(t_k),
+                                                _ptr(noise_k), _ptr(sigma_k), _ptr(rgb_k), _ptr(tape), tape_bytes, _ptr(ws),
+                                                ws.numel(), _stream()), "mlp_forward_tape_rows")
+        check(L.sparf_compact_scatter(C, _ptr(K), _ptr(idx), 1, _ptr(sigma_k), _ptr(sigma), _stream()), "compact_scatter")
+        check(L.sparf_compact_scatter(C, _ptr(K), _ptr(idx), 3, _ptr(rgb_k), _ptr(rgb), _stream()), "compact_scatter")
+        ctx.spec, ctx.engine, ctx.progress, ctx.tape = spec, engine, progress, tape
+        ctx.shape = (R, S)
+        ctx.param_refs = params if (ACCUMULATE_INTO_PARAM_GRAD[0] or
+                                    all(getattr(p, "_sparf_inplace_grad", False) for p in params)) else None
+        ctx.save_for_backward(K, idx, o_k, d_k, t_k, sigma_k, rgb_k, *params)
+        return sigma, rgb
+
+    @staticmethod
+    @_on_tensor_device
+    def backward(ctx, g_sigma, g_rgb):
+        R, S = ctx.shape if ctx.C else (0, 0)
+        if ctx.C == 0 or ctx.tape is None:
+            return (None,) * 8 + tuple(None for _ in ctx.needs_input_grad[8:])
+        L = _lib.lib()
+        K, idx, o_k, d_k, t_k, sigma_k, rgb_k, *params = ctx.saved_tensors
+        C, dev = ctx.C, t_k.device
+        g_sigma_k, g_rgb_k = torch.empty(C, 1, device=dev), torch.empty(C, 1, 3, device=dev)
+        check(L.sparf_compact_gather(C, _ptr(K), _ptr(idx), 1, _ptr(_f32c(g_sigma)), _ptr(g_sigma_k), _stream()),
+              "compact_gather")
+        check(L.sparf_compact_gather(C, _ptr(K), _ptr(idx), 3, _ptr(_f32c(g_rgb)), _ptr(g_rgb_k), _stream()), "compact_gather")
+        m, keep = ctx.spec.fill(params, ctx.progress)
+        grads, ret = _param_grads(ctx, params, dev)
+        gs = ctx.spec.grad_struct(grads)
+        need_o, need_d = ctx.needs_input_grad[3], ctx.needs_input_grad[4]
+        d_o_k = torch.zeros(C, 3, device=dev) if (need_o or need_d) else None
+        d_d_k = torch.zeros(C, 3, device=dev) if (need_o or need_d) else None
+        ws = _workspace(L.sparf_mlp_workspace_bytes(ctypes.byref(m), C, 1, 2, ctx.engine), dev)
+        with _timed("mlp_backward"):
+            check(L.sparf_mlp_backward_tape_rows(ctypes.byref(m), ctx.engine, C, 1, _ptr(K), _ptr(o_k), _ptr(d_k), _ptr(t_k),
+                                                 _ptr(sigma_k), _ptr(rgb_k), _ptr(g_sigma_k), _ptr(g_rgb_k), ctypes.byref(gs),
+                                                 _ptr(d_o_k), _ptr(d_d_k), _ptr(ctx.tape), ctx.tape.numel(), _ptr(ws),
+                                                 ws.numel(), _stream()), "mlp_backward_tape_rows")
+        ctx.tape = None
+        d_o = d_d = None
+        if need_o:
+            d_o = torch.empty(R, 3, device=dev)
+            check(L.sparf_compact_ray_sum(R, S, C, _ptr(K), _ptr(idx), 3, _ptr(d_o_k), _ptr(d_o), _stream()), "compact_ray_sum")
+        if need_d:
+            d_d = torch.empty(R, 3, device=dev)
+            check(L.sparf_compact_ray_sum(R, S, C, _ptr(K), _ptr(idx), 3, _ptr(d_d_k), _ptr(d_d), _stream()), "compact_ray_sum")
+        return (None, None, None, d_o, d_d, None, None, None, *ret)
+
+
+def mlp_forward_grid(spec: MLPSpec, origins, dirs, t, grid, params: Sequence[torch.Tensor], *, noise=None, progress=None,
+                     engine: Optional[int] = None):
+    """mlp_forward (origins/dirs [R,3], t [R,S] -> sigma [R,S], rgb [R,S,3]) with the samples that `grid`
+    (occupancy.OccupancyGrid, box or contracted) skips set to sigma = 0, rgb = 0 and given no gradient.  The kept
+    samples are evaluated exactly as mlp_forward evaluates them, and the call never synchronises with the host, so a
+    training step that uses it can be captured into a CUDA graph.  noise [R,S] (density noise) is drawn dense by the
+    caller and applied at the kept samples.  Differentiable w.r.t. origins, dirs, params; tensor-core engines only.
+    (K stays on the device: EVALS does not count these passes.)"""
+    eng = get_engine() if engine is None else engine
+    if eng == _lib.ENGINE_SIMT_FP32:
+        raise ValueError("mlp_forward_grid: the simt_fp32 engine has no device-side row count; use tc_3x, tc_1x or tc_3x_w1")
+    return GridMLPFunction.apply(spec, eng, grid, origins, dirs, t, noise, progress, *params)
+
+
 def _param_grads(ctx, params, device):
     """Gradient destinations of a backward: the parameters' own `.grad` when the forward opted in and every one exists
     (then autograd gets None), else fresh zeroed tensors in one flat buffer.  -> (grads for the C ABI, grads to return)."""

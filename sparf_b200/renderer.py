@@ -187,6 +187,14 @@ class Graph(torch.nn.Module):
         off: every other call renders densely.  Without a fine grid the fine pass stays dense."""
         self._occupancy = (grid, grid_fine)
 
+    def set_training_occupancy(self, grid, grid_fine=None):
+        """Attach occupancy grids for training: `render` in train and test-optim mode, with or without gradients, then
+        evaluates only the samples a network's grid keeps (occupancy.train_forward_samples); the others get σ = 0,
+        rgb = 0 and no gradient.  None detaches; without a fine grid the fine pass stays dense.  A grid is a snapshot:
+        refresh it between steps with occupancy.refresh_, which writes into the same tensor, so that a captured step
+        sees it.  Tensor-core engines only.  set_occupancy (inference) and render_to_max are unaffected."""
+        self._train_occupancy = (grid, grid_fine)
+
     def set_early_termination(self, eps=1e-4, window=16):
         """Stop evaluating a ray once its transmittance is below eps (sparf_b200.termination), checked every `window`
         samples, in the coarse and the fine pass and on top of any occupancy grid; None detaches.  Like the grids it
@@ -199,7 +207,12 @@ class Graph(torch.nn.Module):
 
     def _forward_samples(self, nerf, which, opt, center, ray, depth_samples, mode):
         """nerf.forward_samples, or in val / eval / test mode without gradients termination.forward_samples when early
-        termination is set, occupancy.forward_samples when only grid `which` (0 coarse, 1 fine) is attached"""
+        termination is set, occupancy.forward_samples when only grid `which` (0 coarse, 1 fine) is attached; in train and
+        test-optim mode occupancy.train_forward_samples when training grid `which` is attached"""
+        train_grid = getattr(self, "_train_occupancy", (None, None))[which]
+        if train_grid is not None and mode in ("train", "test-optim"):
+            from . import occupancy
+            return occupancy.train_forward_samples(nerf, train_grid, opt, center, ray, depth_samples, mode)
         grid = getattr(self, "_occupancy", (None, None))[which]
         term = getattr(self, "_termination", None)
         if (grid is not None or term is not None) and mode in ("val", "eval", "test") and not torch.is_grad_enabled():

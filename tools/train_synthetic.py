@@ -7,7 +7,11 @@ The scene is synthetic (no datasets in this image): a "teacher" NeRF with fixed 
 (full-image inference through `render_by_slices`); a freshly initialised "student" of the same architecture is trained on
 them.  Prints the photometric loss as it goes; `main()` returns (first_losses, last_losses) for the convergence test.
 
-    python tools/train_synthetic.py [--steps 400] [--views 3] [--size 48 64] [--rays 1024] [--fine 0]
+    python tools/train_synthetic.py [--steps 400] [--views 3] [--size 48 64] [--rays 1024] [--fine 0] [--grid RES]
+
+--grid RES trains with occupancy grids of RES^3 cells (Graph.set_training_occupancy), rebuilt from the student's weights
+every --grid-every steps between graph replays (occupancy.refresh_); `main()` then also returns the fraction of the
+training samples the grids keep at the end.
 """
 import argparse
 import os
@@ -34,6 +38,9 @@ def main(argv=None):
     ap.add_argument("--pose-noise", type=float, default=0.03)
     ap.add_argument("--lr-pose", type=float, default=2e-3)
     ap.add_argument("--engine", default="auto", help="MLP engine (auto | tc_3x | tc_3x_w1 | simt_fp32)")
+    ap.add_argument("--grid", type=int, default=0, help="occupancy grids of RES^3 cells in the training steps (0: dense)")
+    ap.add_argument("--grid-every", type=int, default=16, help="steps between grid refreshes")
+    ap.add_argument("--grid-thres", type=float, default=0.01, help="density threshold of the grids")
     ap.add_argument("--quiet", action="store_true")
     args = ap.parse_args(argv)
 
@@ -130,21 +137,37 @@ def main(argv=None):
 
     err0 = pose_error() if pose_net is not None else None
 
+    grids = []
+    if args.grid:     # built before the capture: the graph reads the grids' bits, which refresh_ rewrites in place
+        from sparf_b200 import occupancy
+        grids = [occupancy.build_grid(opt, m, res=args.grid, thres=args.grid_thres) for m in net.get_network_components()]
+        net.set_training_occupancy(*grids)
+
     step = GraphedStep(iteration, (), warmup=2)
     losses = []
     for it in range(args.steps):
+        if grids and it % args.grid_every == 0:
+            for g, m in zip(grids, net.get_network_components()):
+                occupancy.refresh_(g, opt, m)
         losses.append(step().clone())     # (the graph's output tensor is static: keep a copy of its value)
         if not args.quiet and (it % 50 == 0 or it == args.steps - 1):
             print("iter %4d  photometric loss %.5f" % (it, float(losses[-1])))
     torch.cuda.synchronize()
     vals = torch.stack(losses).float().cpu()
     k = max(1, args.steps // 10)
+    extra = ()
+    if grids:     # kept fraction of the last training batch's coarse samples (skipped samples have σ = 0 exactly)
+        with torch.no_grad():
+            out = net.render_image_at_specific_rays(opt, data, iter=0, ray_idx=sampler(opt.nerf.rand_rays), mode="train")
+        extra = ((out["density_samples"] != 0).float().mean().item(),)
+        if not args.quiet:
+            print("kept fraction of the coarse samples: %.3f" % extra[0])
     if pose_net is not None:
         err1 = pose_error()
         if not args.quiet:
             print("unaligned pose offset (rotation deg, camera centre): initial %.3f / %.4f -> final %.3f / %.4f" % (err0 + err1))
-        return vals[:k].mean().item(), vals[-k:].mean().item(), err0, err1
-    return vals[:k].mean().item(), vals[-k:].mean().item()
+        return (vals[:k].mean().item(), vals[-k:].mean().item(), err0, err1) + extra
+    return (vals[:k].mean().item(), vals[-k:].mean().item()) + extra
 
 
 if __name__ == "__main__":
