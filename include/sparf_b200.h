@@ -452,6 +452,17 @@ int sparf_tc_selftest_wgrad(const float* G, const float* X, int32_t M, int32_t N
  * caps the grids. */
 int sparf_tc_selftest_mask_bits(const float* G, const float* W, const float* X, int32_t M, int32_t N, int32_t K,
                                 int32_t max_ctas, uint16_t* img, sparf_stream_t stream);
+/* The trunk forward of width 256 as the tensor-core engines run it, in one fused kernel that keeps a row tile's
+ * activations in shared memory (chain != 0), or layer by layer through GEMMs chained by row images (chain == 0), on the
+ * same inputs: enc [M, E3p] (E3p = E3 rounded up to 32 <= 64, zero padded), W = the nt layers' [256, ldw_l] weights one
+ * after another (ldw_l = (l == 0 ? E3 : 256) + (l == skip ? E3 : 0)), bias [nt, 256]; passes 1 or 3, f16 != 0: fp16
+ * halves, else bf16.  H [nt, M, 256]: layer l is written iff bit l of outputs (bit nt-2 is required; without bit nt-1
+ * the last layer is not computed).  last (may be NULL): the last layer's row image, ceil(M/128) * 8 * 8192 elements.
+ * rows (may be NULL): M is a capacity and *rows (device) the rows computed.  max_ctas > 0 caps the grids.  Both runs must
+ * write the same bytes. */
+int sparf_tc_selftest_chain(const float* enc, int32_t M, int32_t E3, int32_t nt, int32_t skip, const float* W,
+                            const float* bias, int32_t passes, int32_t f16, int32_t max_ctas, int32_t chain,
+                            uint32_t outputs, const int64_t* rows, float* H, uint16_t* last, sparf_stream_t stream);
 
 #ifdef __cplusplus
 }

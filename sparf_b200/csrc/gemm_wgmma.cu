@@ -17,6 +17,11 @@
 //     gradients are never packed from fp32;
 //   staged weight-gradient gemm: the same walk, ring and MMAs, with B read as fp32 rows by bulk copies and split in
 //     shared memory by a fourth (converter) warpgroup, so the weight gradient's activation operand is never packed.
+//   trunk chain: the trunk forward at width 256 in one persistent kernel.  A tile of 64 rows goes through every layer
+//     with its activations in shared memory (each layer's epilogue splits its output over its input), the two consumer
+//     warpgroups splitting N; only the weights stream through the ring, and global memory gets the fp32 activations
+//     that are asked for and the last layer's row image.  Same MMA order and epilogue arithmetic per output element as
+//     the gemm, so the same bytes.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -1019,6 +1024,226 @@ __global__ void __launch_bounds__(STAGED_THREADS, 1) wg_gemm_staged_kernel(Opnd 
   }
 }
 
+// ---- The fused trunk forward: one tile of 64 rows goes through every trunk layer without leaving the SM.
+constexpr int CH_W = 256;                     // the trunk width it is built for: one 128-column N tile per warpgroup
+constexpr int CH_M = 64;                      // rows per tile
+constexpr int CH_KS = CH_W / TK;              // k-steps of a layer's activation input
+constexpr int CH_ENC_KS = 2;                  // k-steps of the encoding at most (64 columns)
+constexpr int CH_HALF = CH_M * TK * 2;        // one 16-bit half of a [64 x 32] k-step of A, 4 KB
+constexpr int CH_STAGES = 4;                  // weight ring: per stage the k-step's two [128 x 32] B tiles (hi, lo each)
+constexpr int CH_ENC = CH_KS * 2 * CH_HALF;               // byte offsets in shared memory: activations at 0 (64 KB),
+constexpr int CH_RING = CH_ENC + CH_ENC_KS * 2 * CH_HALF; // the encoding (16 KB), the ring (128 KB),
+constexpr int CH_BAR = CH_RING + CH_STAGES * STAGE_BYTES; // full[4], empty[4], enc_full, enc_empty
+constexpr int CH_SMEM = CH_BAR + (2 * CH_STAGES + 2) * 8;
+
+// Its own parameter struct (not Epi: see the note there).  Layer l < nl computes H[l] = relu(in_l W_l^T + bias[l]), in_0 =
+// enc, in_l = H[l-1] ( | enc at l == skip), from the weight image w[l] (256 rows, chain_ks(l) k-steps, as pack_kernel<NtB>
+// makes it).  H[l] == NULL: not written to global memory.  last (may be NULL): the row image of H[nl-1].
+struct Chain {
+  int M, nl, skip, enc_ks;
+  const uint16_t* enc;
+  const uint16_t* w[SPARF_MAX_TRUNK];
+  const float* bias[SPARF_MAX_TRUNK];
+  float* H[SPARF_MAX_TRUNK];
+  uint16_t* last;
+};
+
+__host__ __device__ __forceinline__ int chain_ks(int l, int skip, int enc_ks) {
+  return l == 0 ? enc_ks : CH_KS + (l == skip ? enc_ks : 0);
+}
+
+// The producer (one thread) walks (tile, layer, k-step): the tile's 64 rows of the encoding image once per tile (they
+// stay for layer 0 and the skip layer; the buffer is free once the previous tile's last reader has retired), and per
+// k-step both B tiles of the layer's weight image into a ring that runs on across layers and tiles.
+template <int PASSES>
+__device__ __forceinline__ void chain_produce(const Chain& c, int M, int tiles, uint64_t* full, uint64_t* empty, uint64_t* enc_full,
+                                              uint64_t* enc_empty) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  constexpr int HB = PASSES == 3 ? 2 : 1;     // halves copied
+  int it = 0, n = 0;
+  for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+    if (t * CH_M >= M) continue;
+    mbar_wait(enc_empty, (n & 1) ^ 1);
+    ++n;
+    mbar_expect_tx(enc_full, c.enc_ks * HB * CH_HALF);
+    for (int kt = 0; kt < c.enc_ks; ++kt)
+      for (int h = 0; h < HB; ++h)    // rows 64 (t & 1) ... + 63 of a half tile: its first or second 4 KB
+        bulk_g2s(smem + CH_ENC + (kt * 2 + h) * CH_HALF,
+                 c.enc + (((size_t)(t >> 1) * c.enc_ks + kt) * 2 + h) * TILE_ELEMS + (t & 1) * (CH_M * TK), CH_HALF, enc_full);
+    for (int l = 0; l < c.nl; ++l) {
+      const int nk = chain_ks(l, c.skip, c.enc_ks);
+      for (int kt = 0; kt < nk; ++kt, ++it) {
+        const int s = it % CH_STAGES;
+        mbar_wait(&empty[s], ((it / CH_STAGES) & 1) ^ 1);
+        uint8_t* st = smem + CH_RING + s * STAGE_BYTES;
+        mbar_expect_tx(&full[s], 2 * HB * TILE_BYTES);
+        for (int g = 0; g < 2; ++g)
+          bulk_g2s(st + g * 2 * TILE_BYTES, c.w[l] + ((size_t)g * nk + kt) * 2 * TILE_ELEMS, HB * TILE_BYTES, &full[s]);
+      }
+    }
+  }
+}
+
+// The MMAs of layer l for this warpgroup's 128 output columns of the tile's 64 rows: mma_unit's instruction sequence per
+// k-step (so every output element sums in the same order), A from the activation buffer (then the encoding's k-steps
+// at the skip layer; the encoding alone at layer 0), B this warpgroup's tile of the stage.
+template <bool F16, int PASSES>
+__device__ __forceinline__ void chain_mma(float (&acc)[64], const Chain& c, int l, int& it, uint64_t* full, uint64_t* empty) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
+  float acc_lo[PASSES == 3 ? 64 : 1];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < (PASSES == 3 ? 64 : 1); ++i) acc_lo[i] = 0.f;
+  const int nk = chain_ks(l, c.skip, c.enc_ks), na = l == 0 ? 0 : CH_KS;
+  for (int j = 0; j < nk; ++j, ++it) {
+    const int s = it % CH_STAGES;
+    mbar_wait(&full[s], (it / CH_STAGES) & 1);
+    const uint8_t* a = j < na ? smem + j * 2 * CH_HALF : smem + CH_ENC + (j - na) * 2 * CH_HALF;
+    const uint8_t* b = smem + CH_RING + s * STAGE_BYTES + wg * 2 * TILE_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < TK / 16; ++ks) {
+      const uint64_t ahi = smem_desc(a + ks * 256), bhi = smem_desc(b + ks * 256);
+      if constexpr (PASSES == 3) {
+        wgmma_m64n128k16<F16>(acc_lo, smem_desc(a + CH_HALF + ks * 256), bhi);
+        wgmma_m64n128k16<F16>(acc_lo, ahi, smem_desc(b + TILE_BYTES + ks * 256));
+      }
+      wgmma_m64n128k16<F16>(acc, ahi, bhi);
+    }
+    wgmma_commit();
+    wgmma_wait_1();
+    if (j > 0 && lane == 0) mbar_arrive(&empty[(it + CH_STAGES - 1) % CH_STAGES]);
+  }
+  wgmma_wait_all();
+  if (lane == 0) mbar_arrive(&empty[(it + CH_STAGES - 1) % CH_STAGES]);
+  if constexpr (PASSES == 3) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] += ldexpf(acc_lo[i], -LO_SHIFT);
+  }
+}
+
+// Layer l's epilogue of tile t, in place: bias and ReLU as epilogue_values kind 0 (acc becomes the layer's output, zero
+// past M), and its split (the same split2 as a row image's) over the layer's input in the activation buffer; the last
+// layer's split goes to its row image in global memory instead, where asked.
+template <bool F16, int PASSES>
+__device__ __forceinline__ void chain_epilogue(float (&acc)[64], const Chain& c, int M, int l, int t) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const float* bias = c.bias[l];
+#pragma unroll
+  for (int i = 0; i < 64; i += 2) {
+    const int m = t * CH_M + wq * 16 + (lane >> 2) + ((i >> 1) & 1) * 8, n = wg * TN + (i >> 2) * 8 + (lane & 3) * 2;
+    if (m >= M) {
+      acc[i] = acc[i + 1] = 0.f;
+      continue;
+    }
+    acc[i] = fmaxf(acc[i] + bias[n], 0.f);
+    acc[i + 1] = fmaxf(acc[i + 1] + bias[n + 1], 0.f);
+  }
+  const bool last = l == c.nl - 1;
+  if (last && !c.last) return;
+  // as the GEMM epilogue's row image: the fragment of (j, h) is one core matrix, this lane's pair its 32-bit word `lane`
+  uint16_t* img = last ? c.last + (size_t)(t >> 1) * CH_KS * 2 * TILE_ELEMS + (t & 1) * (CH_M * TK)
+                       : reinterpret_cast<uint16_t*>(smem);
+  const int kstride = last ? 2 * TILE_ELEMS : CH_HALF, lo_off = last ? TILE_ELEMS : CH_HALF / 2;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    uint16_t* kt = img + (size_t)(4 * wg + (j >> 2)) * kstride;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      uint32_t hi, lo;
+      split2<F16>(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], hi, lo);
+      const int core = (2 * wq + h) * (TK / 8) + (j & 3);
+      reinterpret_cast<uint32_t*>(kt + core * 64)[lane] = hi;
+      if (PASSES == 3) reinterpret_cast<uint32_t*>(kt + lo_off + core * 64)[lane] = lo;
+    }
+  }
+}
+
+// The fp32 output of layer l (acc after chain_epilogue) to H[l].  It runs after the proxy fence that follows the stores
+// into the activation buffer: a fence issued behind these global stores waits for them too, once per layer with no MMA
+// in flight; issued after it, they drain while the next layer's MMAs run.
+__device__ __forceinline__ void chain_store(const float (&acc)[64], float* H, int M, int t) {
+  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int i = 0; i < 64; i += 2) {
+    const int m = t * CH_M + wq * 16 + (lane >> 2) + ((i >> 1) & 1) * 8, n = wg * TN + (i >> 2) * 8 + (lane & 3) * 2;
+    if (m < M) *reinterpret_cast<float2*>(H + (size_t)m * CH_W + n) = make_float2(acc[i], acc[i + 1]);
+  }
+}
+
+// Persistent and warp-specialized like wg_gemm_kernel (thread 256 produces, warps 0-7 consume, the same register
+// hand-back), but the two consumer warpgroups split N: warpgroup g computes columns [128 g, 128 g + 128) of the tile's 64
+// rows from the same A.  A layer's input is overwritten by its output once both warpgroups' MMAs have retired (a
+// consumer barrier), and the next layer's MMAs start once those generic-proxy stores are fenced for the async proxy and
+// both warpgroups have passed a second barrier.  The epilogue is not overlapped with MMAs (the accumulators of one tile
+// fill both warpgroups); the ring keeps the next layer's weights coming meanwhile.
+// Tiles: 2 ceil(M / 128), so that the last image's 128-row tiles are written whole; a tile wholly past M only zeroes its
+// half of them.  DYN: c.M is a capacity, of which live_rows rows (M) are computed.
+template <bool F16, int PASSES, bool DYN = false>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) trunk_chain_kernel(const Chain c, RowCount rc) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int M = (int)live_rows<DYN>(c.M, rc);
+  if (DYN && M == 0) return;
+  const int tiles = (M + TM - 1) / TM * 2;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + CH_BAR);
+  uint64_t* empty = full + CH_STAGES;
+  uint64_t* enc_full = empty + CH_STAGES;
+  uint64_t* enc_empty = enc_full + 1;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < CH_STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], CONSUMERS / 32);
+    }
+    mbar_init(enc_full, 1);
+    mbar_init(enc_empty, CONSUMERS / 32);
+    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+  }
+  __syncthreads();
+  if (threadIdx.x >= CONSUMERS) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (threadIdx.x == CONSUMERS) chain_produce<PASSES>(c, M, tiles, full, empty, enc_full, enc_empty);
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  const int enc_last = c.skip > 0 && c.skip < c.nl ? c.skip : 0;   // the last layer that reads the encoding
+  int it = 0, n = 0;
+  for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+    if (t * CH_M >= M) {
+      if (c.last)
+        for (int i = 0; i < CH_KS * (PASSES == 3 ? 2 : 1); ++i)
+          reinterpret_cast<uint4*>(c.last + ((size_t)(t >> 1) * CH_KS * 2 + (PASSES == 3 ? i : 2 * i)) * TILE_ELEMS +
+                                   (t & 1) * (CH_M * TK))[threadIdx.x] = make_uint4(0, 0, 0, 0);
+      continue;
+    }
+    mbar_wait(enc_full, n & 1);
+    ++n;
+    for (int l = 0; l < c.nl; ++l) {
+      float acc[64];
+      chain_mma<F16, PASSES>(acc, c, l, it, full, empty);
+      if (l == enc_last && (threadIdx.x & 31) == 0) mbar_arrive(enc_empty);
+      consumer_sync();          // both warpgroups have read the layer's input
+      chain_epilogue<F16, PASSES>(acc, c, M, l, t);
+      if (l + 1 < c.nl) {
+        fence_proxy_async();    // the stores into the activation buffer, before the MMAs that read them
+        consumer_sync();
+      }
+      if (c.H[l]) chain_store(acc, c.H[l], M, t);
+    }
+  }
+}
+
+template <bool F16, int PASSES>
+static int launch_chain(const Chain& c, int ctas, RowCount rc, cudaStream_t st) {
+  auto kernel = rc.rows ? trunk_chain_kernel<F16, PASSES, true> : trunk_chain_kernel<F16, PASSES>;
+  SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM));
+  kernel<<<std::min(2 * ceil_div(c.M, TM), ctas), GEMM_THREADS, CH_SMEM, st>>>(c, rc);
+  SPARF_CHECK_LAUNCH("trunk_chain_kernel");
+  return SPARF_OK;
+}
+
 template <bool F16, int PASSES, bool KFAST, class F, bool DYN = false>
 static int launch_pack(F f, int rtiles, int ksteps, uint16_t* img, cudaStream_t st, RowCount rc = {nullptr, 0}) {
   pack_kernel<F16, PASSES, KFAST, F, DYN><<<dim3(ksteps, rtiles), 256, 0, st>>>(f, ksteps, img, rc);
@@ -1142,6 +1367,43 @@ int tc_gemm_nt(TcPrec p, int act, int M, int N, TcImage a1, int K1v, TcImage a2,
   SPARF_TRY(set_images(e, out, M, N));
   return SPARF_WG_RUN(true, p, opnd(a1, a2.p ? a2 : TcImage{}), M, NtB{W, ldw, wcol2, K1v, K2v, N, a1.ks}, N, ks, false, e,
                       out.row_passes, out.tr_passes, st);
+}
+
+bool tc_chain_supported(int W, int E3p, int nt, int skip) {
+  return W == CH_W && E3p <= CH_ENC_KS * TK && nt >= 3 && nt <= SPARF_MAX_TRUNK && skip != 0 && skip < nt;
+}
+
+int tc_chain_ksteps(int l, int skip, int E3p) { return chain_ks(l, skip, ceil_div(E3p, TK)); }
+
+int tc_pack_nt(TcPrec p, int N, int ks1, int K1v, int ks2, int K2v, const float* W, int ldw, int wcol2, TcImage img,
+               cudaStream_t st) {
+  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && img.p && img.ks == ks1 + ks2, "tc_pack_nt: passes=%d ks=%d, %d + %d k-steps",
+                p.passes, img.ks, ks1, ks2);
+  return SPARF_WG_PACK(true, NtB{W, ldw, wcol2, K1v, K2v, N, ks1}, ceil_div(N, TM), img.ks, img.p, st);
+}
+
+int tc_trunk_chain(TcPrec p, int M, int W, int nt, int skip, TcImage enc, const TcImage* wimg, const float* const* bias,
+                   float* const* H, const TcOut& last, cudaStream_t st) {
+  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && M >= 1 && enc.p && tc_chain_supported(W, enc.ks * TK, nt, skip),
+                "tc_trunk_chain: passes=%d M=%d W=%d nt=%d skip=%d encoding k-steps %d", p.passes, M, W, nt, skip, enc.ks);
+  Chain c{};
+  c.M = M; c.skip = skip; c.enc_ks = enc.ks; c.enc = enc.p;
+  c.nl = H[nt - 1] ? nt : nt - 1;       // without the last layer's output the chain ends at the density row's input
+  SPARF_REQUIRE(H[c.nl - 1], "tc_trunk_chain: no output asked for");
+  for (int l = 0; l < c.nl; ++l) {
+    SPARF_REQUIRE(wimg[l].p && wimg[l].ks == chain_ks(l, skip, enc.ks) && bias[l] && !(reinterpret_cast<uintptr_t>(H[l]) & 7),
+                  "tc_trunk_chain: layer %d: weight image of %d k-steps, bias, 8-byte aligned output", l,
+                  chain_ks(l, skip, enc.ks));
+    c.w[l] = wimg[l].p; c.bias[l] = bias[l]; c.H[l] = H[l];
+  }
+  if (last.row_passes) {
+    SPARF_REQUIRE(c.nl == nt && last.row_passes == p.passes && !last.tr_passes && last.row.p && last.row.ks == CH_KS,
+                  "tc_trunk_chain: the last layer's row image takes the chain's passes and %d k-steps", CH_KS);
+    c.last = last.row.p;
+  }
+  const int ctas = gemm_ctas(p);
+  return p.f16 ? (p.passes == 3 ? launch_chain<true, 3>(c, ctas, p.rows, st) : launch_chain<true, 1>(c, ctas, p.rows, st))
+               : (p.passes == 3 ? launch_chain<false, 3>(c, ctas, p.rows, st) : launch_chain<false, 1>(c, ctas, p.rows, st));
 }
 
 int tc_gemm_nn(TcPrec p, int M, int N, int Kout, int Kv, TcImage g, const float* W, int ldw, int wcol, const float* mask_src,
@@ -1373,4 +1635,71 @@ extern "C" int sparf_tc_selftest_mask_bits(const float* G, const float* W, const
 extern "C" int sparf_tc_selftest_persistent(const float* X, const float* W1, const float* E, const float* W2, int32_t M,
                                             float* Y, float* Z, float* db, int32_t max_ctas, sparf_stream_t stream) {
   return selftest_images(X, W1, E, W2, M, Y, Z, db, max_ctas, (cudaStream_t)stream);
+}
+
+// The fused trunk forward (chain != 0) or the same layers through tc_gemm_nt chained by row images (chain == 0), width
+// 256, on the same inputs: enc [M, E3p] (E3p = E3 rounded up to 32, zero padded), W = the layers' [256, ldw_l] weights one
+// after another (ldw_l = (l == 0 ? E3 : 256) + (l == skip ? E3 : 0)), bias [nt, 256].  H [nt, M, 256]: layer l is written
+// iff bit l of outputs; without bit nt-1 the last layer is not computed.  last (may be NULL): the last layer's row image.
+// rows (may be NULL): M is a capacity, *rows the rows computed.  The two runs must give the same bytes.
+extern "C" int sparf_tc_selftest_chain(const float* enc, int32_t M, int32_t E3, int32_t nt, int32_t skip, const float* W,
+                                       const float* bias, int32_t passes, int32_t f16, int32_t max_ctas, int32_t chain,
+                                       uint32_t outputs, const int64_t* rows, float* H, uint16_t* last,
+                                       sparf_stream_t stream) {
+  SPARF_REQUIRE(enc && W && bias && H && M >= 1 && M <= (1 << 20) && E3 >= 1 && (passes == 1 || passes == 3),
+                "tc_selftest_chain: M=%d E3=%d passes=%d", M, E3, passes);
+  const int E3p = ceil_div(E3, TK) * TK, eks = E3p / TK;
+  SPARF_REQUIRE(tc_chain_supported(CH_W, E3p, nt, skip) && (outputs >> (nt - 2) & 1), "tc_selftest_chain: nt=%d skip=%d", nt, skip);
+  cudaStream_t st = (cudaStream_t)stream;
+  TcPrec p{f16 != 0, passes};
+  p.max_ctas = max_ctas;
+  p.rows = RowCount{rows, 0};
+  const bool feat = outputs >> (nt - 1) & 1;
+  size_t wel = 0;
+  for (int l = 0; l < nt; ++l) wel += tc_image_elems(CH_W, chain_ks(l, skip, eks) * TK);
+  const size_t ne = tc_image_elems(M, E3p), nh = tc_image_elems(M, CH_W);
+  SPARF_TRY(alloc_images(std::max(ne + 2 * nh, wel), st, p));
+  float* scratch = nullptr;
+  SPARF_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch), (size_t)M * CH_W * sizeof(float), st));
+  const TcImage ei{p.pack_a, eks}, himg[2] = {{p.pack_a + ne, CH_KS}, {p.pack_a + ne + nh, CH_KS}};
+  TcOut lo;
+  if (feat && last) {
+    lo.row = TcImage{last, CH_KS};
+    lo.row_passes = passes;
+  }
+  int rc = tc_pack_rows(p, M, E3p, enc, E3p, 1, ei, st);
+  const float* Wl[SPARF_MAX_TRUNK];
+  const float* bl[SPARF_MAX_TRUNK];
+  float* Hl[SPARF_MAX_TRUNK];
+  TcImage wimg[SPARF_MAX_TRUNK];
+  size_t wo = 0, io = 0;
+  for (int l = 0; l < nt; ++l) {
+    Wl[l] = W + wo;
+    bl[l] = bias + (size_t)l * CH_W;
+    Hl[l] = outputs >> l & 1 ? H + (size_t)l * M * CH_W : nullptr;
+    wimg[l] = TcImage{p.pack_b + io, chain_ks(l, skip, eks)};
+    wo += (size_t)CH_W * ((l == 0 ? E3 : CH_W) + (l == skip ? E3 : 0));
+    io += tc_image_elems(CH_W, wimg[l].ks * TK);
+  }
+  if (chain) {
+    for (int l = 0; l < nt && !rc; ++l)
+      rc = tc_pack_nt(p, CH_W, l == 0 ? eks : CH_KS, l == 0 ? E3 : CH_W, l == skip ? eks : 0, E3, Wl[l],
+                      (l == 0 ? E3 : CH_W) + (l == skip ? E3 : 0), CH_W, wimg[l], st);
+    if (!rc) rc = tc_trunk_chain(p, M, CH_W, nt, skip, ei, wimg, bl, Hl, lo, st);
+  } else {
+    for (int l = 0; l < (feat ? nt : nt - 1) && !rc; ++l) {
+      TcOut o;
+      if (l < nt - 1) {
+        o.row = himg[l & 1];
+        o.row_passes = passes;
+      } else {
+        o = lo;
+      }
+      rc = tc_gemm_nt(p, 1, M, CH_W, l == 0 ? ei : himg[(l - 1) & 1], l == 0 ? E3 : CH_W, l == skip ? ei : TcImage{}, E3, Wl[l],
+                      (l == 0 ? E3 : CH_W) + (l == skip ? E3 : 0), CH_W, bl[l], Hl[l] ? Hl[l] : scratch, CH_W, o, st);
+    }
+  }
+  cudaFreeAsync(scratch, st);
+  free_images(p, st);
+  return rc;
 }

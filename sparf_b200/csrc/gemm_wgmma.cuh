@@ -55,6 +55,23 @@ int tc_pack_cols(TcPrec p, int M, int N, const float* X, int ldx, TcImage img, c
 // valid columns, A2 (a2.p may be NULL) K2v.  out: images of Y.
 int tc_gemm_nt(TcPrec p, int act, int M, int N, TcImage a1, int K1v, TcImage a2, int K2v, const float* W, int ldw, int wcol2,
                const float* bias, float* Y, int ldy, const TcOut& out, cudaStream_t st);
+// The fused trunk forward (trunk_chain_kernel): layers l = 0 ... nt-1 of width W, H[l] = relu(in_l W_l^T + bias[l]) with
+// in_0 = enc, in_l = H[l-1], [H[l-1] | enc] at l == skip, in one launch that keeps a 64-row tile's activations in shared
+// memory from layer to layer.  Every H[l], and the last layer's row image, is bit-identical to what the same layers give
+// through tc_gemm_nt chained by row images.
+// Whether the kernel is built for a trunk of this shape (width 256, an encoding of at most 64 padded columns, at least 3 layers):
+bool tc_chain_supported(int W, int E3p, int nt, int skip);
+// k-steps of layer l's weight image
+int tc_chain_ksteps(int l, int skip, int E3p);
+// img = the B operand image tc_gemm_nt packs of W (N rows): ks1 k-steps of W[n][k], k < K1v, then ks2 of W[n][wcol2 + k],
+// k < K2v
+int tc_pack_nt(TcPrec p, int N, int ks1, int K1v, int ks2, int K2v, const float* W, int ldw, int wcol2, TcImage img,
+               cudaStream_t st);
+// wimg[l]: layer l's weight image (tc_pack_nt, tc_chain_ksteps(l) k-steps), all alive at once.  H[l] == NULL: that
+// layer's fp32 output is not written; H[nt-1] == NULL ends the chain after layer nt-2.  last: the last layer's row image
+// (row_passes = p.passes, or 0: none).  p.rows as for the GEMMs.
+int tc_trunk_chain(TcPrec p, int M, int W, int nt, int skip, TcImage enc, const TcImage* wimg, const float* const* bias,
+                   float* const* H, const TcOut& last, cudaStream_t st);
 // D[m][k] = mask(m,k) * ( sum_n G[m][n] W[n][wcol+k] + r1_vec[m]*r1_row[k] )   (= or +=), G [M x N] as its row image.
 // mask(m,k) = mask_src[m][k] > 0, or bit k & 31 of mask_bits[m][k >> 5] (ceil(Kout / 32) words per row, as tc_gemm_tn
 // writes them; only with D NULL), or 1 when both are NULL.  D may be NULL when out writes images; db (may be NULL) +=

@@ -604,8 +604,8 @@ static Tape tape_chunk(const Tape& t, const MlpDims& d, int r0, int S) {
 }
 
 // Workspace of one call, per chunk of nrc rays.  Tensor-core engines keep their GEMM operands as images: the forward's
-// encodings and ping-pong trunk activations, the backward's ping-pong trunk gradients (a row image for the next input
-// gradient, a transposed one for the weight gradient; no fp32 copy), the colour-head gradient's two images (no fp32 copy
+// encodings and ping-pong trunk activations (fused trunk: the last layer's only, and every trunk weight), the backward's
+// ping-pong trunk gradients (a row image for the next input gradient, a transposed one for the weight gradient; no fp32 copy), the colour-head gradient's two images (no fp32 copy
 // either), the ReLU mask bits of one layer input (written by its weight-gradient GEMM, read by its input-gradient GEMM),
 // and a buffer for the weight operand packed per GEMM.  head = false (density calls, S = 1): no colour-head or
 // view-direction buffer.
@@ -613,15 +613,21 @@ struct Ws {
   float *wts, *rgbv, *G0, *G1, *Genc, *Ghid, *gpre, *graw, *Gdtmp, *Gdenc;
   Tape act;     // the forward's activations of one chunk (forward and recompute backward)
   TcImage encimg, dencimg, Himg[2], Grow[2], Gtr[2], ghid_row, ghid_tr;
+  TcImage wimg[SPARF_MAX_TRUNK];   // fused trunk forward: every trunk layer's weight image, alive at once
   uint32_t* mask_bits;   // [Mc x ceil(W / 32)]
   uint16_t* pack_b;
   size_t pack_elems;
 };
 
+// Whether the trunk forward runs as one fused kernel (tc_trunk_chain), from the shape alone: a tensor-core engine and a
+// trunk the kernel is built for.  Other shapes go layer by layer through tc_gemm_nt.
+static bool trunk_chained(const MlpDims& d, bool tc) { return tc && tc_chain_supported(d.W, d.E3p, d.nt, d.skip); }
+
 static size_t carve(const MlpDims& d, bool tc, int nrc, int S, Pass pass, bool head, char* base, Ws* out) {
   const size_t Mc = (size_t)nrc * S;
   const bool fwd_here = pass == Pass::kForward || pass == Pass::kRecomputeBackward;   // the activations are not taped
   const bool bwd = pass == Pass::kRecomputeBackward || pass == Pass::kTapedBackward;
+  const bool chain = trunk_chained(d, tc);
   Carver cv{base, 0};
   Ws w{};
   w.wts = cv.take(32);
@@ -633,9 +639,15 @@ static size_t carve(const MlpDims& d, bool tc, int nrc, int S, Pass pass, bool h
       w.act.raw = cv.take(Mc);
       w.rgbv = cv.take(Mc * 3);
     }
-    const int nH = pass == Pass::kForward ? 2 : d.nt;            // the forward ping-pongs, the backward keeps every layer
-    for (int l = 0; l < nH; ++l) w.act.H[l] = cv.take(Mc * d.W);
-    for (int l = nH; l < d.nt; ++l) w.act.H[l] = w.act.H[l & 1];
+    // the backward keeps every layer; the forward ping-pongs, or keeps the last two only (the density row's input and
+    // the colour head's) when the fused trunk leaves the others on the SM
+    const int nH = pass == Pass::kForward ? 2 : d.nt;
+    if (chain && nH == 2) {
+      for (int l = d.nt - 2; l < d.nt; ++l) w.act.H[l] = cv.take(Mc * d.W);
+    } else {
+      for (int l = 0; l < nH; ++l) w.act.H[l] = cv.take(Mc * d.W);
+      for (int l = nH; l < d.nt; ++l) w.act.H[l] = w.act.H[l & 1];
+    }
   }
   if (bwd && !tc) {
     w.G0 = cv.take(Mc * d.W);
@@ -656,7 +668,12 @@ static size_t carve(const MlpDims& d, bool tc, int nrc, int S, Pass pass, bool h
   if (tc && pass != Pass::kTapedBackward) {
     w.encimg = cv.image((int)Mc, d.E3p);
     if (head) w.dencimg = cv.image((int)Mc, d.Evp);
-    for (TcImage& h : w.Himg) h = cv.image((int)Mc, d.W);
+    if (chain) {    // only the last layer's image (the colour head reads it) and the weight images
+      if (head) w.Himg[(d.nt - 1) & 1] = cv.image((int)Mc, d.W);
+      for (int l = 0; l < d.nt; ++l) w.wimg[l] = cv.image(d.W, tc_chain_ksteps(l, d.skip, d.E3p) * 32);
+    } else {
+      for (TcImage& h : w.Himg) h = cv.image((int)Mc, d.W);
+    }
   }
   if (tc && bwd) {
     for (TcImage& g : w.Grow) g = cv.image((int)Mc, d.W);
@@ -765,21 +782,42 @@ static int chunk_encode_xyz(const SparfMLP* mlp, const Call& c, long long Mc, in
 
 // trunk layers 0 ... nt-1 of one chunk from its encoding.  H: array of nt activation buffers (may alias in pairs);
 // H[nt-1] == NULL skips the last layer's feature GEMM (the density row reads H[nt-2] only).  raw (the softplus argument,
-// noise added) and sigma may be NULL; both NULL skips the density row.  The tensor-core engines chain the layers through
-// the row images their epilogues write (the workspace's image buffers); last_image: the last layer's too (the colour
-// head reads it).
+// noise added) and sigma may be NULL; both NULL skips the density row.  The tensor-core engines run the layers in one
+// fused kernel where trunk_chained says so (H[l] == NULL then means layer l's activation is not kept), else chain them
+// through the row images their epilogues write (the workspace's image buffers); last_image: the last layer's row image is written too (the colour head reads it).
 static int chunk_trunk(const SparfMLP* mlp, const Call& c, long long Mc, const float* enc, float* const* H,
                        const float* noise, float* raw, float* sigma, bool last_image, cudaStream_t st) {
   const MlpDims& d = c.d;
   const Ws& w = c.w;
   const float* in = enc;
+  const bool chained = trunk_chained(d, c.tc);
+  if (chained) {
+    // the weights as the GEMMs would pack them one by one, then every layer in one launch; H[l] == NULL stays on the SM
+    const float* bias[SPARF_MAX_TRUNK];
+    for (int l = 0; l < d.nt; ++l) {
+      const bool last = l == d.nt - 1;
+      bias[l] = mlp->trunk_b[l] + (last ? 1 : 0);
+      if (last && !H[l]) break;
+      const int ldw = trunk_ldw(d, l);
+      SPARF_TRY(tc_pack_nt(c.ep.fwd, d.W, ceil_div(trunk_in_main(d, l), 32), trunk_in_main_valid(d, l),
+                           l == d.skip ? w.encimg.ks : 0, d.E3, mlp->trunk_w[l] + (last ? ldw : 0), ldw, d.W, w.wimg[l], st));
+    }
+    TcOut o;
+    if (last_image) {
+      o.row = w.Himg[(d.nt - 1) & 1];
+      o.row_passes = c.ep.fwd.passes;
+    }
+    SPARF_TRY(tc_trunk_chain(c.ep.fwd, (int)Mc, d.W, d.nt, d.skip, w.encimg, w.wimg, bias, H, o, st));
+  }
   for (int l = 0; l < d.nt; ++l) {
     const bool last = l == d.nt - 1;
     const int ldw = trunk_ldw(d, l);
     const float* Wl = mlp->trunk_w[l] + (last ? ldw : 0);  // last layer: row 0 is the density row
     const float* bl = mlp->trunk_b[l] + (last ? 1 : 0);
     const bool sk = l == d.skip;
-    if (c.tc && H[l]) {
+    if (chained) {
+      // done above
+    } else if (c.tc && H[l]) {
       TcOut o;
       if (!last || last_image) {
         o.row = w.Himg[l & 1];

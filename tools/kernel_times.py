@@ -16,7 +16,7 @@ import common
 from sparf_b200 import _lib, ops
 
 HBM_PEAK = 3.35e12      # H100 SXM data sheet, bytes/s
-GEMM_KERNELS = ("wg_gemm_kernel", "wg_gemm_staged_kernel")
+GEMM_KERNELS = ("wg_gemm_kernel", "wg_gemm_staged_kernel", "trunk_chain_kernel")
 # 16-bit passes of the images (forward, input gradient, weight gradient) per tensor-core engine
 PASSES = {"tc_3x": (3, 3, 3), "tc_1x": (1, 1, 1), "tc_3x_w1": (3, 3, 1), "auto": (3, 3, 3)}
 
@@ -34,9 +34,14 @@ def gemm_bytes_per_row(spec, passes, backward, pose):
     def img(cols, p):     # one row of an image: K padded to 32, 2 bytes per half, hi and lo halves when p == 3
         return -(-cols // 32) * 32 * 2 * (2 if p == 3 else 1)
 
-    # forward: trunk layer l reads its input image (+ enc at the skip layer), writes fp32 H and its row image; the colour
-    # head reads [H | denc] and writes fp32 hid
-    n = sum(img(W if l else E3p, pf) + (img(E3p, pf) if l == skip else 0) + 4 * W + img(W, pf) for l in range(nt))
+    # forward: the fused trunk (width 256, as MLPSpec's default) reads the encoding image once, keeps the activations on
+    # the SM, and writes fp32 H[l] where it is kept (every layer for the tape; the last two in an inference forward) and
+    # the last layer's row image; other widths go layer by layer, each reading its input image (+ enc at the skip layer)
+    # and writing fp32 H and its row image.  The colour head reads [H | denc] and writes fp32 hid
+    if W == 256 and E3p <= 64 and nt >= 3:
+        n = img(E3p, pf) + 4 * W * (nt if backward else 2) + img(W, pf)
+    else:
+        n = sum(img(W if l else E3p, pf) + (img(E3p, pf) if l == skip else 0) + 4 * W + img(W, pf) for l in range(nt))
     n += img(W, pf) + img(Evp, pf) + 4 * HW
     if not backward:
         return n
