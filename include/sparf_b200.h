@@ -463,6 +463,21 @@ int sparf_tc_selftest_mask_bits(const float* G, const float* W, const float* X, 
 int sparf_tc_selftest_chain(const float* enc, int32_t M, int32_t E3, int32_t nt, int32_t skip, const float* W,
                             const float* bias, int32_t passes, int32_t f16, int32_t max_ctas, int32_t chain,
                             uint32_t outputs, const int64_t* rows, float* H, uint16_t* last, sparf_stream_t stream);
+/* The fused forward (every output) with the ReLU masks it writes for the chained backward: bits [nt-2][M][8] uint32, bit
+ * n & 31 of word [l][m][n >> 5] = H[l][m][n] > 0, layers 0 ... nt-3. */
+int sparf_tc_selftest_chain_bits(const float* enc, int32_t M, int32_t E3, int32_t nt, int32_t skip, const float* W,
+                                 const float* bias, int32_t passes, int32_t f16, int32_t max_ctas, const int64_t* rows,
+                                 float* H, uint32_t* bits, sparf_stream_t stream);
+/* The trunk backward's input gradients of layers nt-2 ... 1 (width 256, bf16 halves), fused (chain != 0) or through the
+ * layer-by-layer input-gradient GEMMs with bit masks (chain == 0), on the same inputs: G [M, 256] the gradient of layer
+ * nt-2's output, W as sparf_tc_selftest_chain's, bits [nt-2][M][8] the masks of H[0] ... H[nt-3].  Writes tr [nt-2]
+ * transposed images of G[0] ... G[nt-3] (wg_passes; 2 * ceil(M/32) * 8192 elements each), db [nt-2][256] their column
+ * sums and, when row is not NULL (skip <= nt-3), row [2] the row images of G[0] and G[skip] (dg_passes; ceil(M/128) * 8 *
+ * 8192 elements each).  rows and max_ctas as sparf_tc_selftest_chain's.  Both runs must write the same image bytes. */
+int sparf_tc_selftest_dgrad_chain(const float* G, int32_t M, int32_t E3, int32_t nt, int32_t skip, const float* W,
+                                  const uint32_t* bits, int32_t dg_passes, int32_t wg_passes, int32_t max_ctas,
+                                  int32_t chain, const int64_t* rows, uint16_t* tr, uint16_t* row, float* db,
+                                  sparf_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -100,6 +100,10 @@ _SIGNATURES = {
     "sparf_tc_selftest_mask_bits": (c_int32, [_P, _P, _P, c_int32, c_int32, c_int32, c_int32, _P, _P]),
     "sparf_tc_selftest_chain": (c_int32, [_P, c_int32, c_int32, c_int32, c_int32, _P, _P, c_int32, c_int32, c_int32, c_int32,
                                           ctypes.c_uint32, _P, _P, _P, _P]),
+    "sparf_tc_selftest_chain_bits": (c_int32, [_P, c_int32, c_int32, c_int32, c_int32, _P, _P, c_int32, c_int32, c_int32,
+                                               _P, _P, _P, _P]),
+    "sparf_tc_selftest_dgrad_chain": (c_int32, [_P, c_int32, c_int32, c_int32, c_int32, _P, _P, c_int32, c_int32, c_int32,
+                                                c_int32, _P, _P, _P, _P, _P]),
 }
 
 _lib = None

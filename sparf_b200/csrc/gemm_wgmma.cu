@@ -1038,7 +1038,8 @@ constexpr int CH_SMEM = CH_BAR + (2 * CH_STAGES + 2) * 8;
 
 // Its own parameter struct (not Epi: see the note there).  Layer l < nl computes H[l] = relu(in_l W_l^T + bias[l]), in_0 =
 // enc, in_l = H[l-1] ( | enc at l == skip), from the weight image w[l] (256 rows, chain_ks(l) k-steps, as pack_kernel<NtB>
-// makes it).  H[l] == NULL: not written to global memory.  last (may be NULL): the row image of H[nl-1].
+// makes it).  H[l] == NULL: not written to global memory.  last (may be NULL): the row image of H[nl-1].  bits[l] (may
+// be NULL): the ReLU mask H[l] > 0, 8 words per row (trunk_chain_kernel's BITS instantiations only).
 struct Chain {
   int M, nl, skip, enc_ks;
   const uint16_t* enc;
@@ -1046,6 +1047,7 @@ struct Chain {
   const float* bias[SPARF_MAX_TRUNK];
   float* H[SPARF_MAX_TRUNK];
   uint16_t* last;
+  uint32_t* bits[SPARF_MAX_TRUNK];
 };
 
 __host__ __device__ __forceinline__ int chain_ks(int l, int skip, int enc_ks) {
@@ -1084,11 +1086,11 @@ __device__ __forceinline__ void chain_produce(const Chain& c, int M, int tiles, 
   }
 }
 
-// The MMAs of layer l for this warpgroup's 128 output columns of the tile's 64 rows: mma_unit's instruction sequence per
-// k-step (so every output element sums in the same order), A from the activation buffer (then the encoding's k-steps
-// at the skip layer; the encoding alone at layer 0), B this warpgroup's tile of the stage.
+// The MMAs of one layer for this warpgroup's 128 output columns of the tile's 64 rows: mma_unit's instruction sequence
+// per k-step (so every output element sums in the same order), nk k-steps of A, the first na from the activation buffer
+// and the rest from the encoding's (the skip layer; the encoding alone at layer 0), B this warpgroup's tile of the stage.
 template <bool F16, int PASSES>
-__device__ __forceinline__ void chain_mma(float (&acc)[64], const Chain& c, int l, int& it, uint64_t* full, uint64_t* empty) {
+__device__ __forceinline__ void chain_mma(float (&acc)[64], int nk, int na, int& it, uint64_t* full, uint64_t* empty) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   float acc_lo[PASSES == 3 ? 64 : 1];
@@ -1096,7 +1098,6 @@ __device__ __forceinline__ void chain_mma(float (&acc)[64], const Chain& c, int 
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
 #pragma unroll
   for (int i = 0; i < (PASSES == 3 ? 64 : 1); ++i) acc_lo[i] = 0.f;
-  const int nk = chain_ks(l, c.skip, c.enc_ks), na = l == 0 ? 0 : CH_KS;
   for (int j = 0; j < nk; ++j, ++it) {
     const int s = it % CH_STAGES;
     mbar_wait(&full[s], (it / CH_STAGES) & 1);
@@ -1174,6 +1175,32 @@ __device__ __forceinline__ void chain_store(const float (&acc)[64], float* H, in
   }
 }
 
+// The ReLU mask of layer l's output as tc_gemm_tn writes it, bit n & 31 of word [m][n >> 5] = H[m][n] > 0 (the predicate
+// the fp32 mask applies, so NaN and -0 give 0): a lane's 8 values of a 32-column word (4 j x 2 columns) go to its bits
+// 2 (lane % 4) + 8 (j % 4) + {0, 1}, the quad ORs them together, and lane % 4 stores word lane % 4 of its warpgroup's
+// four.  Like chain_store, it runs after the proxy fence.
+__device__ __forceinline__ void chain_store_bits(const float (&acc)[64], uint32_t* bits, int M, int t) {
+  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    uint32_t mine = 0;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      uint32_t w = 0;
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int i = 4 * (4 * q + jj) + 2 * h, b = 8 * jj + 2 * (lane & 3);
+        w |= (uint32_t)(acc[i] > 0.f) << b | (uint32_t)(acc[i + 1] > 0.f) << (b + 1);
+      }
+      w |= __shfl_xor_sync(0xffffffffu, w, 1);
+      w |= __shfl_xor_sync(0xffffffffu, w, 2);
+      if ((lane & 3) == q) mine = w;
+    }
+    const int m = t * CH_M + wq * 16 + (lane >> 2) + 8 * h;
+    if (m < M) bits[(size_t)m * (CH_W / 32) + wg * 4 + (lane & 3)] = mine;
+  }
+}
+
 // Persistent and warp-specialized like wg_gemm_kernel (thread 256 produces, warps 0-7 consume, the same register
 // hand-back), but the two consumer warpgroups split N: warpgroup g computes columns [128 g, 128 g + 128) of the tile's 64
 // rows from the same A.  A layer's input is overwritten by its output once both warpgroups' MMAs have retired (a
@@ -1181,8 +1208,9 @@ __device__ __forceinline__ void chain_store(const float (&acc)[64], float* H, in
 // both warpgroups have passed a second barrier.  The epilogue is not overlapped with MMAs (the accumulators of one tile
 // fill both warpgroups); the ring keeps the next layer's weights coming meanwhile.
 // Tiles: 2 ceil(M / 128), so that the last image's 128-row tiles are written whole; a tile wholly past M only zeroes its
-// half of them.  DYN: c.M is a capacity, of which live_rows rows (M) are computed.
-template <bool F16, int PASSES, bool DYN = false>
+// half of them.  DYN: c.M is a capacity, of which live_rows rows (M) are computed.  BITS: c.bits[l] are written where
+// not NULL (the other instantiations never read them).
+template <bool F16, int PASSES, bool DYN = false, bool BITS = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) trunk_chain_kernel(const Chain c, RowCount rc) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const int M = (int)live_rows<DYN>(c.M, rc);
@@ -1222,7 +1250,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) trunk_chain_kernel(const Chai
     ++n;
     for (int l = 0; l < c.nl; ++l) {
       float acc[64];
-      chain_mma<F16, PASSES>(acc, c, l, it, full, empty);
+      chain_mma<F16, PASSES>(acc, chain_ks(l, c.skip, c.enc_ks), l == 0 ? 0 : CH_KS, it, full, empty);
       if (l == enc_last && (threadIdx.x & 31) == 0) mbar_arrive(enc_empty);
       consumer_sync();          // both warpgroups have read the layer's input
       chain_epilogue<F16, PASSES>(acc, c, M, l, t);
@@ -1231,16 +1259,222 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) trunk_chain_kernel(const Chai
         consumer_sync();
       }
       if (c.H[l]) chain_store(acc, c.H[l], M, t);
+      if (BITS && c.bits[l]) chain_store_bits(acc, c.bits[l], M, t);
     }
   }
 }
 
 template <bool F16, int PASSES>
 static int launch_chain(const Chain& c, int ctas, RowCount rc, cudaStream_t st) {
-  auto kernel = rc.rows ? trunk_chain_kernel<F16, PASSES, true> : trunk_chain_kernel<F16, PASSES>;
+  bool bits = false;
+  for (int l = 0; l < c.nl; ++l) bits |= c.bits[l] != nullptr;
+  auto kernel = bits ? (rc.rows ? trunk_chain_kernel<F16, PASSES, true, true> : trunk_chain_kernel<F16, PASSES, false, true>)
+                     : (rc.rows ? trunk_chain_kernel<F16, PASSES, true> : trunk_chain_kernel<F16, PASSES>);
   SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM));
   kernel<<<std::min(2 * ceil_div(c.M, TM), ctas), GEMM_THREADS, CH_SMEM, st>>>(c, rc);
   SPARF_CHECK_LAUNCH("trunk_chain_kernel");
+  return SPARF_OK;
+}
+
+// ---- The trunk backward's input gradients in one persistent kernel, the same walk as trunk_chain_kernel.  Layer l
+// (top >= l >= 1) computes G[l-1] = mask_l * (G[l] W_l), W_l's [256 x 256] part over H[l-1], from its weight image w[l]
+// (256 rows, CH_KS k-steps, as tc_gemm_nn packs it: tc_pack_nn); mask_l = bits[l] (H[l-1] > 0, 8 words per row).  G[top]
+// comes in as its row image, and a tile's gradient stays in the activation buffer from layer to layer.  G[l-1] leaves as
+// its transposed image tr[l] (tr_ks k-steps per row tile), its column sums (db[l] +=) and, where row[l] is not NULL, its
+// row image.  Shared memory as trunk_chain_kernel's, with the column-sum reduction where the encoding would be.
+struct DgChain {
+  int M, top, tr_ks;
+  const uint16_t* in;
+  const uint16_t* w[SPARF_MAX_TRUNK];
+  const uint32_t* bits[SPARF_MAX_TRUNK];
+  float* db[SPARF_MAX_TRUNK];
+  uint16_t* tr[SPARF_MAX_TRUNK];
+  uint16_t* row[SPARF_MAX_TRUNK];
+};
+
+// The producer (one thread) walks (tile, layer, k-step): the tile's 64 rows of the input image once per tile, once the
+// previous tile's last MMAs have retired (act_empty), and the weights as chain_produce streams them.
+template <int DP>
+__device__ __forceinline__ void dg_produce(const DgChain& c, int M, int tiles, uint64_t* full, uint64_t* empty, uint64_t* act_full,
+                                           uint64_t* act_empty) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  constexpr int HB = DP == 3 ? 2 : 1;
+  int it = 0, n = 0;
+  for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+    if (t * CH_M >= M) continue;
+    mbar_wait(act_empty, (n & 1) ^ 1);
+    ++n;
+    mbar_expect_tx(act_full, CH_KS * HB * CH_HALF);
+    for (int kt = 0; kt < CH_KS; ++kt)
+      for (int h = 0; h < HB; ++h)
+        bulk_g2s(smem + (kt * 2 + h) * CH_HALF,
+                 c.in + (((size_t)(t >> 1) * CH_KS + kt) * 2 + h) * TILE_ELEMS + (t & 1) * (CH_M * TK), CH_HALF, act_full);
+    for (int l = c.top; l >= 1; --l)
+      for (int kt = 0; kt < CH_KS; ++kt, ++it) {
+        const int s = it % CH_STAGES;
+        mbar_wait(&empty[s], ((it / CH_STAGES) & 1) ^ 1);
+        uint8_t* st = smem + CH_RING + s * STAGE_BYTES;
+        mbar_expect_tx(&full[s], 2 * HB * TILE_BYTES);
+        for (int g = 0; g < 2; ++g)
+          bulk_g2s(st + g * 2 * TILE_BYTES, c.w[l] + ((size_t)g * CH_KS + kt) * 2 * TILE_ELEMS, HB * TILE_BYTES, &full[s]);
+      }
+  }
+}
+
+// this thread's two rows of its warpgroup's four mask words (one 16-byte load each); rows past M get none
+__device__ __forceinline__ void dg_mask_words(uint4 (&wd)[2], const uint32_t* bits, int M, int t) {
+  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = t * CH_M + wq * 16 + (lane >> 2) + 8 * h;
+    wd[h] = m < M ? *reinterpret_cast<const uint4*>(bits + (size_t)m * (CH_W / 32) + wg * 4) : make_uint4(0, 0, 0, 0);
+  }
+}
+
+// the tile's split (PASSES halves) as a row image at img: k-step stride kstride, lo half lo_off after the hi half (16-bit
+// elements); the fragment of (j, h) is one core matrix, this lane's pair its 32-bit word `lane`
+template <int PASSES>
+__device__ __forceinline__ void dg_split(const float (&acc)[64], uint16_t* img, int kstride, int lo_off) {
+  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    uint16_t* kt = img + (size_t)(4 * wg + (j >> 2)) * kstride;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      uint32_t hi, lo;
+      split2<false>(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], hi, lo);
+      const int core = (2 * wq + h) * (TK / 8) + (j & 3);
+      reinterpret_cast<uint32_t*>(kt + core * 64)[lane] = hi;
+      if (PASSES == 3) reinterpret_cast<uint32_t*>(kt + lo_off + core * 64)[lane] = lo;
+    }
+  }
+}
+
+// A tile wholly past M writes zeros where the layer-by-layer GEMMs' 128-row tiles would: its half of the row images, and
+// the transposed images' k-steps of its rows below tr_ks (a capacity's, with a device row count).
+template <int DP, int TP>
+__device__ __forceinline__ void dg_zero_tile(const DgChain& c, int t) {
+  const uint4 z = make_uint4(0, 0, 0, 0);
+  for (int l = c.top; l >= 1; --l) {
+    if (c.row[l])
+      for (int i = 0; i < CH_KS * (DP == 3 ? 2 : 1); ++i)
+        reinterpret_cast<uint4*>(c.row[l] + ((size_t)(t >> 1) * CH_KS * 2 + (DP == 3 ? i : 2 * i)) * TILE_ELEMS +
+                                 (t & 1) * (CH_M * TK))[threadIdx.x] = z;
+    for (int g = 0; g < 2; ++g)
+      for (int kt = 2 * t; kt < 2 * t + 2 && kt < c.tr_ks; ++kt)
+        for (int h = 0; h < (TP == 3 ? 2 : 1); ++h)
+          for (int i = threadIdx.x; i < TILE_ELEMS / 8; i += CONSUMERS)
+            reinterpret_cast<uint4*>(c.tr[l] + (((size_t)g * c.tr_ks + kt) * 2 + h) * TILE_ELEMS)[i] = z;
+  }
+}
+
+// Persistent and warp-specialized as trunk_chain_kernel (tiles, ring, register hand-back, the two warpgroups splitting
+// N), with the mask words of a layer loaded before its MMAs.  Per layer and tile: MMAs (tc_gemm_nn's per output element);
+// both warpgroups past them (consumer barrier); the mask (rows past M have no bits, so they are zero), the column sums'
+// per-warp partials, the split over the layer's input in the activation buffer (not after layer 1), proxy fence,
+// barrier; then the column sums' atomics and the global stores, which drain while the next layer's MMAs run.  The values
+// and the images' bytes are tc_gemm_nn's; the column sums add 64-row tiles instead of 128-row ones.
+// DP: the activation buffer's and row images' passes (the input gradients'), TP: the transposed images' (the weight
+// gradients').  DYN: c.M is a capacity, of which live_rows rows are computed.
+template <int DP, int TP, bool DYN = false>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) dgrad_chain_kernel(const DgChain c, RowCount rc) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int M = (int)live_rows<DYN>(c.M, rc);
+  if (DYN && M == 0) return;
+  const int tiles = (M + TM - 1) / TM * 2;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + CH_BAR);
+  uint64_t* empty = full + CH_STAGES;
+  uint64_t* act_full = empty + CH_STAGES;
+  uint64_t* act_empty = act_full + 1;
+  float* red = reinterpret_cast<float*>(smem + CH_ENC);     // [8 warps][128 columns]
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < CH_STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], CONSUMERS / 32);
+    }
+    mbar_init(act_full, 1);
+    mbar_init(act_empty, CONSUMERS / 32);
+    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+  }
+  __syncthreads();
+  if (threadIdx.x >= CONSUMERS) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (threadIdx.x == CONSUMERS) dg_produce<DP>(c, M, tiles, full, empty, act_full, act_empty);
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int it = 0, n = 0;
+  for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+    if (t * CH_M >= M) {
+      dg_zero_tile<DP, TP>(c, t);
+      continue;
+    }
+    mbar_wait(act_full, n & 1);
+    ++n;
+    for (int l = c.top; l >= 1; --l) {
+      uint4 wd[2];
+      dg_mask_words(wd, c.bits[l], M, t);
+      float acc[64];
+      chain_mma<false, DP>(acc, CH_KS, CH_KS, it, full, empty);
+      if (l == 1 && lane == 0) mbar_arrive(act_empty);
+      consumer_sync();          // both warpgroups have read G[l]
+      const uint32_t wds[2][4] = {{wd[0].x, wd[0].y, wd[0].z, wd[0].w}, {wd[1].x, wd[1].y, wd[1].z, wd[1].w}};
+#pragma unroll
+      for (int i = 0; i < 64; i += 2) {     // columns 8 j + 2 (lane % 4) + {0, 1} of word j / 4, j = i / 4
+        const int j = i >> 2;
+        const uint32_t k = wds[(i >> 1) & 1][j >> 2] >> (8 * (j & 3) + 2 * (lane & 3));
+        if (!(k & 1)) acc[i] = 0.f;
+        if (!(k & 2)) acc[i + 1] = 0.f;
+      }
+      // column sums as tile_colsum's: over the 16 rows of each warp (shuffles), then its warpgroup's 4 warps
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int cc = 0; cc < 2; ++cc) {
+          float s = acc[4 * j + cc] + acc[4 * j + 2 + cc];
+#pragma unroll
+          for (int o = 4; o < 32; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+          if (lane < 4) red[w * TN + 8 * j + 2 * lane + cc] = s;
+        }
+      if (l > 1) {
+        dg_split<DP>(acc, reinterpret_cast<uint16_t*>(smem), CH_HALF, CH_HALF / 2);
+        fence_proxy_async();    // the stores into the activation buffer, before the MMAs that read them
+      }
+      consumer_sync();
+      {
+        float s = 0.f;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) s += red[(4 * wg + i) * TN + (threadIdx.x & (TN - 1))];
+        atomicAdd(c.db[l] + threadIdx.x, s);
+      }
+      // the transposed image as epilogue<..., TRP>'s: rows n (row tile wg), k = m (k-step 2 t + wq / 2)
+      const int kt = 2 * t + (wq >> 1);
+      if (kt < c.tr_ks) {
+        uint16_t* tp = c.tr[l] + ((size_t)wg * c.tr_ks + kt) * 2 * TILE_ELEMS;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            uint32_t hi, lo;
+            split2<false>(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], hi, lo);
+            const int core = j * (TK / 8) + 2 * (wq & 1) + h;
+            reinterpret_cast<uint32_t*>(tp + core * 64)[lane] = movmatrix_trans(hi);
+            if (TP == 3) reinterpret_cast<uint32_t*>(tp + TILE_ELEMS + core * 64)[lane] = movmatrix_trans(lo);
+          }
+      }
+      if (c.row[l])
+        dg_split<DP>(acc, c.row[l] + (size_t)(t >> 1) * CH_KS * 2 * TILE_ELEMS + (t & 1) * (CH_M * TK), 2 * TILE_ELEMS, TILE_ELEMS);
+    }
+  }
+}
+
+template <int DP, int TP>
+static int launch_dgrad_chain(const DgChain& c, int ctas, RowCount rc, cudaStream_t st) {
+  auto kernel = rc.rows ? dgrad_chain_kernel<DP, TP, true> : dgrad_chain_kernel<DP, TP>;
+  SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM));
+  kernel<<<std::min(2 * ceil_div(c.M, TM), ctas), GEMM_THREADS, CH_SMEM, st>>>(c, rc);
+  SPARF_CHECK_LAUNCH("dgrad_chain_kernel");
   return SPARF_OK;
 }
 
@@ -1382,8 +1616,35 @@ int tc_pack_nt(TcPrec p, int N, int ks1, int K1v, int ks2, int K2v, const float*
   return SPARF_WG_PACK(true, NtB{W, ldw, wcol2, K1v, K2v, N, ks1}, ceil_div(N, TM), img.ks, img.p, st);
 }
 
+int tc_pack_nn(TcPrec p, int Kout, int N, int Kv, const float* W, int ldw, int wcol, TcImage img, cudaStream_t st) {
+  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && img.p && img.ks == ceil_div(N, TK), "tc_pack_nn: passes=%d ks=%d N=%d",
+                p.passes, img.ks, N);
+  return SPARF_WG_PACK(false, NnB{W, ldw, wcol, Kv, N}, ceil_div(Kout, TM), img.ks, img.p, st);
+}
+
+int tc_dgrad_chain(TcPrec dg, TcPrec wg, int M, int W, int top, TcImage in, const TcImage* wimg, const uint32_t* const* bits,
+                   float* const* db, const TcImage* tr, const TcImage* row, cudaStream_t st) {
+  SPARF_REQUIRE(!dg.f16 && !wg.f16 && M >= 1 && W == CH_W && top >= 1 && top < SPARF_MAX_TRUNK && in.p && in.ks == CH_KS,
+                "tc_dgrad_chain: bf16 images, M=%d W=%d top=%d, input row image of %d k-steps", M, W, top, CH_KS);
+  DgChain c{};
+  c.M = M; c.top = top; c.tr_ks = ceil_div(M, TK); c.in = in.p;
+  for (int l = 1; l <= top; ++l) {
+    SPARF_REQUIRE(wimg[l].p && wimg[l].ks == CH_KS && bits[l] && !(reinterpret_cast<uintptr_t>(bits[l]) & 15) && db[l] &&
+                      tr[l].p && tr[l].ks == c.tr_ks && (!row[l].p || row[l].ks == CH_KS),
+                  "tc_dgrad_chain: layer %d: weight image of %d k-steps, 16-byte aligned mask bits, column sums, transposed "
+                  "image of %d k-steps, row image of %d",
+                  l, CH_KS, c.tr_ks, CH_KS);
+    c.w[l] = wimg[l].p; c.bits[l] = bits[l]; c.db[l] = db[l]; c.tr[l] = tr[l].p; c.row[l] = row[l].p;
+  }
+  const int ctas = gemm_ctas(dg);
+  if (dg.passes == 3 && wg.passes == 3) return launch_dgrad_chain<3, 3>(c, ctas, dg.rows, st);
+  if (dg.passes == 3 && wg.passes == 1) return launch_dgrad_chain<3, 1>(c, ctas, dg.rows, st);
+  if (dg.passes == 1 && wg.passes == 1) return launch_dgrad_chain<1, 1>(c, ctas, dg.rows, st);
+  SPARF_REQUIRE(false, "tc_dgrad_chain: no kernel for %d-pass row and %d-pass transposed images", dg.passes, wg.passes);
+}
+
 int tc_trunk_chain(TcPrec p, int M, int W, int nt, int skip, TcImage enc, const TcImage* wimg, const float* const* bias,
-                   float* const* H, const TcOut& last, cudaStream_t st) {
+                   float* const* H, uint32_t* const* bits, const TcOut& last, cudaStream_t st) {
   SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && M >= 1 && enc.p && tc_chain_supported(W, enc.ks * TK, nt, skip),
                 "tc_trunk_chain: passes=%d M=%d W=%d nt=%d skip=%d encoding k-steps %d", p.passes, M, W, nt, skip, enc.ks);
   Chain c{};
@@ -1395,6 +1656,7 @@ int tc_trunk_chain(TcPrec p, int M, int W, int nt, int skip, TcImage enc, const 
                   "tc_trunk_chain: layer %d: weight image of %d k-steps, bias, 8-byte aligned output", l,
                   chain_ks(l, skip, enc.ks));
     c.w[l] = wimg[l].p; c.bias[l] = bias[l]; c.H[l] = H[l];
+    c.bits[l] = bits ? bits[l] : nullptr;
   }
   if (last.row_passes) {
     SPARF_REQUIRE(c.nl == nt && last.row_passes == p.passes && !last.tr_passes && last.row.p && last.row.ks == CH_KS,
@@ -1641,16 +1903,16 @@ extern "C" int sparf_tc_selftest_persistent(const float* X, const float* W1, con
 // 256, on the same inputs: enc [M, E3p] (E3p = E3 rounded up to 32, zero padded), W = the layers' [256, ldw_l] weights one
 // after another (ldw_l = (l == 0 ? E3 : 256) + (l == skip ? E3 : 0)), bias [nt, 256].  H [nt, M, 256]: layer l is written
 // iff bit l of outputs; without bit nt-1 the last layer is not computed.  last (may be NULL): the last layer's row image.
-// rows (may be NULL): M is a capacity, *rows the rows computed.  The two runs must give the same bytes.
-extern "C" int sparf_tc_selftest_chain(const float* enc, int32_t M, int32_t E3, int32_t nt, int32_t skip, const float* W,
-                                       const float* bias, int32_t passes, int32_t f16, int32_t max_ctas, int32_t chain,
-                                       uint32_t outputs, const int64_t* rows, float* H, uint16_t* last,
-                                       sparf_stream_t stream) {
+// rows (may be NULL): M is a capacity, *rows the rows computed.  The two runs must give the same bytes.  bits (may be
+// NULL; the chain only): [nt - 2][M][8] ReLU masks of layers 0 ... nt-3.
+static int selftest_chain(const float* enc, int M, int E3, int nt, int skip, const float* W, const float* bias, int passes,
+                          int f16, int max_ctas, int chain, uint32_t outputs, const int64_t* rows, float* H, uint16_t* last,
+                          uint32_t* bits, cudaStream_t st) {
   SPARF_REQUIRE(enc && W && bias && H && M >= 1 && M <= (1 << 20) && E3 >= 1 && (passes == 1 || passes == 3),
                 "tc_selftest_chain: M=%d E3=%d passes=%d", M, E3, passes);
   const int E3p = ceil_div(E3, TK) * TK, eks = E3p / TK;
   SPARF_REQUIRE(tc_chain_supported(CH_W, E3p, nt, skip) && (outputs >> (nt - 2) & 1), "tc_selftest_chain: nt=%d skip=%d", nt, skip);
-  cudaStream_t st = (cudaStream_t)stream;
+  SPARF_REQUIRE(!bits || chain, "tc_selftest_chain: mask bits come from the chain only");
   TcPrec p{f16 != 0, passes};
   p.max_ctas = max_ctas;
   p.rows = RowCount{rows, 0};
@@ -1671,12 +1933,14 @@ extern "C" int sparf_tc_selftest_chain(const float* enc, int32_t M, int32_t E3, 
   const float* Wl[SPARF_MAX_TRUNK];
   const float* bl[SPARF_MAX_TRUNK];
   float* Hl[SPARF_MAX_TRUNK];
+  uint32_t* bl_bits[SPARF_MAX_TRUNK] = {};
   TcImage wimg[SPARF_MAX_TRUNK];
   size_t wo = 0, io = 0;
   for (int l = 0; l < nt; ++l) {
     Wl[l] = W + wo;
     bl[l] = bias + (size_t)l * CH_W;
     Hl[l] = outputs >> l & 1 ? H + (size_t)l * M * CH_W : nullptr;
+    if (bits && l < nt - 2) bl_bits[l] = bits + (size_t)l * M * (CH_W / 32);
     wimg[l] = TcImage{p.pack_b + io, chain_ks(l, skip, eks)};
     wo += (size_t)CH_W * ((l == 0 ? E3 : CH_W) + (l == skip ? E3 : 0));
     io += tc_image_elems(CH_W, wimg[l].ks * TK);
@@ -1685,7 +1949,7 @@ extern "C" int sparf_tc_selftest_chain(const float* enc, int32_t M, int32_t E3, 
     for (int l = 0; l < nt && !rc; ++l)
       rc = tc_pack_nt(p, CH_W, l == 0 ? eks : CH_KS, l == 0 ? E3 : CH_W, l == skip ? eks : 0, E3, Wl[l],
                       (l == 0 ? E3 : CH_W) + (l == skip ? E3 : 0), CH_W, wimg[l], st);
-    if (!rc) rc = tc_trunk_chain(p, M, CH_W, nt, skip, ei, wimg, bl, Hl, lo, st);
+    if (!rc) rc = tc_trunk_chain(p, M, CH_W, nt, skip, ei, wimg, bl, Hl, bl_bits, lo, st);
   } else {
     for (int l = 0; l < (feat ? nt : nt - 1) && !rc; ++l) {
       TcOut o;
@@ -1701,5 +1965,83 @@ extern "C" int sparf_tc_selftest_chain(const float* enc, int32_t M, int32_t E3, 
   }
   cudaFreeAsync(scratch, st);
   free_images(p, st);
+  return rc;
+}
+
+extern "C" int sparf_tc_selftest_chain(const float* enc, int32_t M, int32_t E3, int32_t nt, int32_t skip, const float* W,
+                                       const float* bias, int32_t passes, int32_t f16, int32_t max_ctas, int32_t chain,
+                                       uint32_t outputs, const int64_t* rows, float* H, uint16_t* last,
+                                       sparf_stream_t stream) {
+  return selftest_chain(enc, M, E3, nt, skip, W, bias, passes, f16, max_ctas, chain, outputs, rows, H, last, nullptr,
+                        (cudaStream_t)stream);
+}
+
+// The fused trunk forward with every output and the ReLU masks of layers 0 ... nt-3, bits [nt - 2][M][8]
+extern "C" int sparf_tc_selftest_chain_bits(const float* enc, int32_t M, int32_t E3, int32_t nt, int32_t skip, const float* W,
+                                            const float* bias, int32_t passes, int32_t f16, int32_t max_ctas,
+                                            const int64_t* rows, float* H, uint32_t* bits, sparf_stream_t stream) {
+  SPARF_REQUIRE(bits && nt >= 3 && nt <= SPARF_MAX_TRUNK, "tc_selftest_chain_bits: nt=%d, bits", nt);
+  return selftest_chain(enc, M, E3, nt, skip, W, bias, passes, f16, max_ctas, 1, (1u << nt) - 1, rows, H, nullptr, bits,
+                        (cudaStream_t)stream);
+}
+
+// The trunk backward's input gradients of layers nt-2 ... 1 through dgrad_chain_kernel (chain != 0) or layer by layer
+// through tc_gemm_nn with bit masks (chain == 0), width 256, on the same inputs: G [M, 256] = G[nt-2] in fp32 (packed
+// into its row image first), W as sparf_tc_selftest_chain's, bits [nt-2][M][8] the masks of H[0] ... H[nt-3].  Outputs:
+// tr [nt-2] the transposed images of G[0] ... G[nt-3] (wg_passes), db [nt-2][256] their column sums, row (may be NULL)
+// [2] the row images of G[0] and G[skip] (skip <= nt-3).  rows as sparf_tc_selftest_chain's.  The images must be the
+// same bytes.
+extern "C" int sparf_tc_selftest_dgrad_chain(const float* G, int32_t M, int32_t E3, int32_t nt, int32_t skip, const float* W,
+                                             const uint32_t* bits, int32_t dg_passes, int32_t wg_passes, int32_t max_ctas,
+                                             int32_t chain, const int64_t* rows, uint16_t* tr, uint16_t* row, float* db,
+                                             sparf_stream_t stream) {
+  SPARF_REQUIRE(G && W && bits && tr && db && M >= 1 && M <= (1 << 20) && E3 >= 1 && nt >= 3 && nt <= SPARF_MAX_TRUNK &&
+                    skip > 0 && skip < nt && (!row || skip <= nt - 3),
+                "tc_selftest_dgrad_chain: M=%d E3=%d nt=%d skip=%d", M, E3, nt, skip);
+  cudaStream_t st = (cudaStream_t)stream;
+  TcPrec dg{false, dg_passes}, wg{false, wg_passes};
+  dg.max_ctas = wg.max_ctas = max_ctas;
+  dg.rows = wg.rows = RowCount{rows, 0};
+  const int top = nt - 2;
+  const size_t nh = tc_image_elems(M, CH_W), ntr = tc_image_elems(CH_W, M), nw = tc_image_elems(CH_W, CH_W);
+  SPARF_TRY(alloc_images(std::max(3 * nh, (top + 1) * nw), st, dg));
+  SPARF_CHECK_CUDA(cudaMemsetAsync(db, 0, (size_t)top * CH_W * sizeof(float), st));
+  const TcImage gin{dg.pack_a, CH_KS}, scratch[2] = {{dg.pack_a + nh, CH_KS}, {dg.pack_a + 2 * nh, CH_KS}};
+  const float* Wl[SPARF_MAX_TRUNK];
+  int ldw[SPARF_MAX_TRUNK];
+  size_t wo = 0;
+  for (int l = 0; l < nt; ++l) {
+    Wl[l] = W + wo;
+    ldw[l] = (l == 0 ? E3 : CH_W) + (l == skip ? E3 : 0);
+    wo += (size_t)CH_W * ldw[l];
+  }
+  TcImage trl[SPARF_MAX_TRUNK], rowl[SPARF_MAX_TRUNK], wimg[SPARF_MAX_TRUNK];
+  const uint32_t* bl[SPARF_MAX_TRUNK] = {};
+  float* dbl[SPARF_MAX_TRUNK] = {};
+  for (int l = 1; l <= top; ++l) {
+    trl[l] = TcImage{tr + (size_t)(l - 1) * ntr, ceil_div(M, TK)};
+    if (row && (l == 1 || l - 1 == skip)) rowl[l] = TcImage{row + (l == 1 ? 0 : nh), CH_KS};
+    bl[l] = bits + (size_t)(l - 1) * M * (CH_W / 32);
+    dbl[l] = db + (size_t)(l - 1) * CH_W;
+    wimg[l] = TcImage{dg.pack_b + (size_t)l * nw, CH_KS};
+  }
+  int rc = tc_pack_rows(dg, M, CH_W, G, CH_W, 1, gin, st);
+  if (chain) {
+    for (int l = 1; l <= top && !rc; ++l) rc = tc_pack_nn(dg, CH_W, CH_W, CH_W, Wl[l], ldw[l], 0, wimg[l], st);
+    if (!rc) rc = tc_dgrad_chain(dg, wg, M, CH_W, top, gin, wimg, bl, dbl, trl, rowl, st);
+  } else {
+    TcImage g = gin;
+    for (int l = top; l >= 1 && !rc; --l) {
+      TcOut o;
+      o.row = rowl[l].p ? rowl[l] : scratch[l & 1];
+      o.tr = trl[l];
+      o.row_passes = dg_passes;
+      o.tr_passes = wg_passes;
+      rc = tc_gemm_nn(dg, M, CH_W, CH_W, CH_W, g, Wl[l], ldw[l], 0, nullptr, 0, bl[l], nullptr, nullptr, nullptr, 0, 0, o,
+                      dbl[l], nullptr, st);
+      g = o.row;
+    }
+  }
+  free_images(dg, st);
   return rc;
 }

@@ -68,10 +68,21 @@ int tc_chain_ksteps(int l, int skip, int E3p);
 int tc_pack_nt(TcPrec p, int N, int ks1, int K1v, int ks2, int K2v, const float* W, int ldw, int wcol2, TcImage img,
                cudaStream_t st);
 // wimg[l]: layer l's weight image (tc_pack_nt, tc_chain_ksteps(l) k-steps), all alive at once.  H[l] == NULL: that
-// layer's fp32 output is not written; H[nt-1] == NULL ends the chain after layer nt-2.  last: the last layer's row image
-// (row_passes = p.passes, or 0: none).  p.rows as for the GEMMs.
+// layer's fp32 output is not written; H[nt-1] == NULL ends the chain after layer nt-2.  bits (may be NULL; else bits[l]
+// may be NULL): the ReLU mask H[l] > 0 of layer l as tc_gemm_tn writes it ([M x 8] words), for tc_dgrad_chain.  last: the
+// last layer's row image (row_passes = p.passes, or 0: none).  p.rows as for the GEMMs.
 int tc_trunk_chain(TcPrec p, int M, int W, int nt, int skip, TcImage enc, const TcImage* wimg, const float* const* bias,
-                   float* const* H, const TcOut& last, cudaStream_t st);
+                   float* const* H, uint32_t* const* bits, const TcOut& last, cudaStream_t st);
+// img = the B operand image tc_gemm_nn packs of W (Kout rows k, contraction over N): W[n][wcol + k], k < Kv
+int tc_pack_nn(TcPrec p, int Kout, int N, int Kv, const float* W, int ldw, int wcol, TcImage img, cudaStream_t st);
+// The trunk backward's input gradients in one launch (dgrad_chain_kernel), width W = 256, for layers l = top ... 1:
+//   G[l-1] = (bit k of bits[l][m]) * sum_n G[l][m][n] W_l[n][k],  db[l][k] += sum_m G[l-1][m][k]
+// from G[top] as its row image `in` (dg passes) and wimg[l] (tc_pack_nn of W_l's first 256 columns, dg passes), keeping a
+// 64-row tile's gradient in shared memory from layer to layer.  G[l-1] leaves as its transposed image tr[l] (wg passes)
+// and, where row[l].p is not NULL, its row image (dg passes).  Values and images are bit-identical to tc_gemm_nn's with
+// the same bit masks (bf16 halves); the column sums add 64-row tiles.  dg.rows as for the GEMMs.
+int tc_dgrad_chain(TcPrec dg, TcPrec wg, int M, int W, int top, TcImage in, const TcImage* wimg, const uint32_t* const* bits,
+                   float* const* db, const TcImage* tr, const TcImage* row, cudaStream_t st);
 // D[m][k] = mask(m,k) * ( sum_n G[m][n] W[n][wcol+k] + r1_vec[m]*r1_row[k] )   (= or +=), G [M x N] as its row image.
 // mask(m,k) = mask_src[m][k] > 0, or bit k & 31 of mask_bits[m][k >> 5] (ceil(Kout / 32) words per row, as tc_gemm_tn
 // writes them; only with D NULL), or 1 when both are NULL.  D may be NULL when out writes images; db (may be NULL) +=

@@ -570,21 +570,31 @@ struct Carver {
 
 // The forward's activations that the backward reads: the encodings, the nt trunk activations, the colour-head
 // activations and the softplus argument of the density (noise added).  A taped forward keeps them for the whole batch in
-// the tape; the workspace holds one chunk's (its trunk activations ping-pong in a plain forward).
+// the tape; the workspace holds one chunk's (its trunk activations ping-pong in a plain forward).  With the fused trunk
+// (trunk_chained) the taped and recompute forwards also keep the ReLU masks of H[0] ... H[nt-3] as bits (8 words per row
+// of width 256; in the tape after everything else): the chained input gradients read them, since they all run before
+// the weight gradients that would otherwise write them.
 struct Tape {
   float *enc, *denc, *hid, *raw;
   float* H[SPARF_MAX_TRUNK];
+  uint32_t* bits[SPARF_MAX_TRUNK];
 };
 
-static size_t tape_layout(const MlpDims& d, int R, int S, char* base, Tape* tp) {
+// Whether the trunk forward runs as one fused kernel (tc_trunk_chain), and the input gradients of layers nt-2 ... 1 as
+// another (tc_dgrad_chain), from the shape alone: a tensor-core engine and a trunk the kernels are built for.  Other
+// shapes go layer by layer through tc_gemm_nt and tc_gemm_nn.
+static bool trunk_chained(const MlpDims& d, bool tc) { return tc && tc_chain_supported(d.W, d.E3p, d.nt, d.skip); }
+
+static size_t tape_layout(const MlpDims& d, bool tc, int R, int S, char* base, Tape* tp) {
   const size_t M = (size_t)R * S;
   Carver cv{base, 0};
-  Tape t;
+  Tape t{};
   t.enc = cv.take(M * d.E3p);
   t.denc = cv.take((size_t)R * d.Evp);
   t.hid = cv.take(M * d.HW);
   t.raw = cv.take(M);
   for (int l = 0; l < d.nt; ++l) t.H[l] = cv.take(M * d.W);
+  for (int l = 0; trunk_chained(d, tc) && l < d.nt - 2; ++l) t.bits[l] = reinterpret_cast<uint32_t*>(cv.take(M * (d.W / 32)));
   if (tp) *tp = t;
   return cv.used + 256;
 }
@@ -599,29 +609,29 @@ static Tape tape_chunk(const Tape& t, const MlpDims& d, int r0, int S) {
   c.denc = t.denc + (size_t)r0 * d.Evp;
   c.hid = t.hid + m0 * d.HW;
   c.raw = t.raw + m0;
-  for (int l = 0; l < d.nt; ++l) c.H[l] = t.H[l] + m0 * d.W;
+  for (int l = 0; l < d.nt; ++l) {
+    c.H[l] = t.H[l] + m0 * d.W;
+    c.bits[l] = t.bits[l] ? t.bits[l] + m0 * (d.W / 32) : nullptr;
+  }
   return c;
 }
 
 // Workspace of one call, per chunk of nrc rays.  Tensor-core engines keep their GEMM operands as images: the forward's
 // encodings and ping-pong trunk activations (fused trunk: the last layer's only, and every trunk weight), the backward's
-// ping-pong trunk gradients (a row image for the next input gradient, a transposed one for the weight gradient; no fp32 copy), the colour-head gradient's two images (no fp32 copy
-// either), the ReLU mask bits of one layer input (written by its weight-gradient GEMM, read by its input-gradient GEMM),
-// and a buffer for the weight operand packed per GEMM.  head = false (density calls, S = 1): no colour-head or
-// view-direction buffer.
+// trunk gradients (a row image for the next input gradient, a transposed one for the weight gradient; no fp32 copy; see
+// grad_row), the colour-head gradient's two images (no fp32 copy either), the ReLU mask bits of one layer input (written
+// by its weight-gradient GEMM, read by its input-gradient GEMM), and a buffer for the weight operand packed per GEMM.
+// head = false (density calls, S = 1): no colour-head or view-direction buffer.
 struct Ws {
   float *wts, *rgbv, *G0, *G1, *Genc, *Ghid, *gpre, *graw, *Gdtmp, *Gdenc;
   Tape act;     // the forward's activations of one chunk (forward and recompute backward)
-  TcImage encimg, dencimg, Himg[2], Grow[2], Gtr[2], ghid_row, ghid_tr;
+  TcImage encimg, dencimg, Himg[2], Grow[2], Gtr[SPARF_MAX_TRUNK - 1], ghid_row, ghid_tr;
   TcImage wimg[SPARF_MAX_TRUNK];   // fused trunk forward: every trunk layer's weight image, alive at once
+  TcImage nnimg[SPARF_MAX_TRUNK];  // chained input gradients: the weight images of layers 1 ... nt-2, alive at once
   uint32_t* mask_bits;   // [Mc x ceil(W / 32)]
   uint16_t* pack_b;
   size_t pack_elems;
 };
-
-// Whether the trunk forward runs as one fused kernel (tc_trunk_chain), from the shape alone: a tensor-core engine and a
-// trunk the kernel is built for.  Other shapes go layer by layer through tc_gemm_nt.
-static bool trunk_chained(const MlpDims& d, bool tc) { return tc && tc_chain_supported(d.W, d.E3p, d.nt, d.skip); }
 
 static size_t carve(const MlpDims& d, bool tc, int nrc, int S, Pass pass, bool head, char* base, Ws* out) {
   const size_t Mc = (size_t)nrc * S;
@@ -648,6 +658,7 @@ static size_t carve(const MlpDims& d, bool tc, int nrc, int S, Pass pass, bool h
       for (int l = 0; l < nH; ++l) w.act.H[l] = cv.take(Mc * d.W);
       for (int l = nH; l < d.nt; ++l) w.act.H[l] = w.act.H[l & 1];
     }
+    for (int l = 0; chain && bwd && l < d.nt - 2; ++l) w.act.bits[l] = reinterpret_cast<uint32_t*>(cv.take(Mc * (d.W / 32)));
   }
   if (bwd && !tc) {
     w.G0 = cv.take(Mc * d.W);
@@ -677,7 +688,8 @@ static size_t carve(const MlpDims& d, bool tc, int nrc, int S, Pass pass, bool h
   }
   if (tc && bwd) {
     for (TcImage& g : w.Grow) g = cv.image((int)Mc, d.W);
-    for (TcImage& g : w.Gtr) g = cv.image(d.W, (int)Mc);
+    for (int i = 0; i < (chain ? d.nt - 1 : 2); ++i) w.Gtr[i] = cv.image(d.W, (int)Mc);
+    for (int l = 1; chain && l <= d.nt - 2; ++l) w.nnimg[l] = cv.image(d.W, d.W);
     if (head) {
       w.ghid_row = cv.image((int)Mc, d.HW);
       w.ghid_tr = cv.image(d.HW, (int)Mc);
@@ -736,9 +748,9 @@ static int begin_call(const char* who, const SparfMLP* mlp, int engine, long lon
   c->d = mlp_dims(mlp);
   c->tc = is_tc(e);
   if (tape) {
-    SPARF_REQUIRE(tape_bytes >= tape_layout(c->d, (int)R, S, nullptr, nullptr), "%s: tape %zu bytes too small", who,
+    SPARF_REQUIRE(tape_bytes >= tape_layout(c->d, c->tc, (int)R, S, nullptr, nullptr), "%s: tape %zu bytes too small", who,
                   tape_bytes);
-    tape_layout(c->d, (int)R, S, reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(tape), 256)), &c->tape);
+    tape_layout(c->d, c->tc, (int)R, S, reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(tape), 256)), &c->tape);
   }
   const size_t need = workspace_need(c->d, c->tc, R, S, pass, head);
   if (workspace_bytes < need) {
@@ -783,10 +795,11 @@ static int chunk_encode_xyz(const SparfMLP* mlp, const Call& c, long long Mc, in
 // trunk layers 0 ... nt-1 of one chunk from its encoding.  H: array of nt activation buffers (may alias in pairs);
 // H[nt-1] == NULL skips the last layer's feature GEMM (the density row reads H[nt-2] only).  raw (the softplus argument,
 // noise added) and sigma may be NULL; both NULL skips the density row.  The tensor-core engines run the layers in one
-// fused kernel where trunk_chained says so (H[l] == NULL then means layer l's activation is not kept), else chain them
-// through the row images their epilogues write (the workspace's image buffers); last_image: the last layer's row image is written too (the colour head reads it).
+// fused kernel where trunk_chained says so (H[l] == NULL then means layer l's activation is not kept; bits[l] != NULL
+// keeps its ReLU mask), else chain them through the row images their epilogues write (the workspace's image buffers);
+// last_image: the last layer's row image is written too (the colour head reads it).
 static int chunk_trunk(const SparfMLP* mlp, const Call& c, long long Mc, const float* enc, float* const* H,
-                       const float* noise, float* raw, float* sigma, bool last_image, cudaStream_t st) {
+                       uint32_t* const* bits, const float* noise, float* raw, float* sigma, bool last_image, cudaStream_t st) {
   const MlpDims& d = c.d;
   const Ws& w = c.w;
   const float* in = enc;
@@ -807,7 +820,7 @@ static int chunk_trunk(const SparfMLP* mlp, const Call& c, long long Mc, const f
       o.row = w.Himg[(d.nt - 1) & 1];
       o.row_passes = c.ep.fwd.passes;
     }
-    SPARF_TRY(tc_trunk_chain(c.ep.fwd, (int)Mc, d.W, d.nt, d.skip, w.encimg, w.wimg, bias, H, o, st));
+    SPARF_TRY(tc_trunk_chain(c.ep.fwd, (int)Mc, d.W, d.nt, d.skip, w.encimg, w.wimg, bias, H, bits, o, st));
   }
   for (int l = 0; l < d.nt; ++l) {
     const bool last = l == d.nt - 1;
@@ -858,7 +871,7 @@ static int chunk_forward(const SparfMLP* mlp, const Call& c, int nr, int S, cons
                                                                             v.denc, c.rc);
   SPARF_CHECK_LAUNCH("encode_dir_kernel");
   if (c.tc) SPARF_TRY(tc_pack_rows(c.ep.fwd, (int)Mc, d.Evp, v.denc, d.Evp, S, c.w.dencimg, st));
-  SPARF_TRY(chunk_trunk(mlp, c, Mc, v.enc, v.H, noise, v.raw, sigma, true, st));
+  SPARF_TRY(chunk_trunk(mlp, c, Mc, v.enc, v.H, v.bits, noise, v.raw, sigma, true, st));
   if (c.tc)
     SPARF_TRY(tc_gemm_nt(c.ep.fwd, 1, (int)Mc, d.HW, c.w.Himg[(d.nt - 1) & 1], d.W, c.w.dencimg, d.Ev, mlp->head_w[0],
                          d.W + d.Ev, d.W, mlp->head_b[0], v.hid, d.HW, TcOut{}, st));
@@ -1015,14 +1028,48 @@ static int trunk_backward_simt(const SparfMLP* mlp, const Call& c, long long Mc,
   return SPARF_OK;
 }
 
+// The image buffers of G_l, the gradient of trunk layer l's output (G_{nt-1} is buffer 0, the head's or the caller's).
+// Layer by layer they ping-pong.  With the chained input gradients every transposed image of G_{nt-2} ... G_0 is alive
+// until the weight gradients that follow the chain, G_0's in G_{nt-1}'s buffer (whose weight gradient ran before the
+// chain); the chain's input is G_{nt-2}'s row image, and the row images it writes for the encoding's gradient go to the
+// two row buffers: G_0's over G_{nt-1}'s, G_skip's over G_{nt-2}'s, each 64-row tile of which is read only by the CTA
+// that writes it there afterwards.
+static int grad_tr_buf(const MlpDims& d, bool chained, int l) { return chained ? (l ? d.nt - 1 - l : 0) : (d.nt - 1 - l) & 1; }
+static int grad_row(const MlpDims& d, bool chained, int l) {
+  return chained ? (l == 0 || l == d.nt - 1 ? 0 : 1) : (d.nt - 1 - l) & 1;
+}
+
+// The input gradients of layers nt-2 ... 1 in one launch (tc_dgrad_chain), from G_{nt-2}'s row image and the masks the
+// fused forward kept (bits[l - 1] = H_{l-1} > 0), into the transposed images of G_{nt-3} ... G_0, the bias gradients of
+// layers nt-3 ... 0 and, with enc_grad, the row images of G_skip and G_0.
+static int chunk_dgrad_chain(const SparfMLP* mlp, const Call& c, long long Mc, uint32_t* const* bits, const SparfMLPGrad* grad,
+                             bool enc_grad, cudaStream_t st) {
+  const MlpDims& d = c.d;
+  const int top = d.nt - 2;
+  const uint32_t* mask[SPARF_MAX_TRUNK] = {};
+  float* db[SPARF_MAX_TRUNK] = {};
+  TcImage tr[SPARF_MAX_TRUNK], row[SPARF_MAX_TRUNK];
+  for (int l = top; l >= 1; --l) {
+    SPARF_TRY(tc_pack_nn(c.ep.dgrad, d.W, d.W, d.W, mlp->trunk_w[l], trunk_ldw(d, l), 0, c.w.nnimg[l], st));
+    mask[l] = bits[l - 1];
+    db[l] = grad->trunk_b[l - 1];
+    tr[l] = grad_tr(c.w, grad_tr_buf(d, true, l - 1), Mc);
+    if (enc_grad && (l - 1 == 0 || l - 1 == d.skip)) row[l] = c.w.Grow[grad_row(d, true, l - 1)];
+  }
+  return tc_dgrad_chain(c.ep.dgrad, c.ep.wgrad, (int)Mc, d.W, top, c.w.Grow[grad_row(d, true, top)], c.w.nnimg, mask, db, tr,
+                        row, st);
+}
+
 // The same on the tensor cores, from the last layer's feature gradient as image pair 0.  The last layer's bias gradient
 // is the caller's: the kernel that made image pair 0 adds it (the SIMT path adds the column sums of G0).  The last layer's
 // input-gradient epilogue also sums the density row's weight gradient.
+// bits: the fused forward's ReLU masks of H_0 ... H_{nt-3} (trunk_chained: the input gradients of layers nt-2 ... 1 run
+// as one chain once layer nt-1 is done, and the weight gradients of the layers below it after that).
 static int trunk_backward_tc(const SparfMLP* mlp, const Call& c, long long Mc, const float* enc, float* const* H,
-                             const float* graw, const SparfMLPGrad* grad, bool enc_grad, cudaStream_t st) {
+                             uint32_t* const* bits, const float* graw, const SparfMLPGrad* grad, bool enc_grad, cudaStream_t st) {
   const MlpDims& d = c.d;
   const EnginePrec& ep = c.ep;
-  int gi = 0;       // the layer's output gradient is image pair gi
+  const bool chained = trunk_chained(d, true);
   bool genc_written = false;
   for (int l = d.nt - 1; l >= 0; --l) {
     const bool last = l == d.nt - 1;
@@ -1033,23 +1080,26 @@ static int trunk_backward_tc(const SparfMLP* mlp, const Call& c, long long Mc, c
     const int rowoff = last ? 1 : 0;
     float* dWl = grad->trunk_w[l] + (size_t)rowoff * ldw;
     const float* Wl = mlp->trunk_w[l] + (size_t)rowoff * ldw;
+    const int gi = (d.nt - 1 - l) & 1;   // layer by layer: the layer's output gradient is image pair gi
+    const TcImage gt = grad_tr(c.w, grad_tr_buf(d, chained, l), Mc);
+    const bool nn = l > 0 && (!chained || last);   // the input gradient is a GEMM of its own
     // The input gradient's ReLU mask is H_{l-1} > 0: as bits that the weight gradient writes while it reads H_{l-1} anyway,
     // except with the density row's rank-1 term, whose weight gradient (r1_wgrad) the epilogue sums from the fp32 values
     // of H_{l-1}: that layer reads them as its mask.
-    uint32_t* bits = l > 0 && !r1 ? c.w.mask_bits : nullptr;
-    SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, Kin, Kinv, grad_tr(c.w, gi, Mc), in, Kin, 1, dWl, ldw, 0, bits, st));
-    if (l == d.skip)
-      SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, d.E3p, d.E3, grad_tr(c.w, gi, Mc), enc, d.E3p, 1, dWl, ldw, d.W, nullptr, st));
-    if (l > 0)
-      SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.W, d.W, c.w.Grow[gi], Wl, ldw, 0, bits ? nullptr : in, d.W, bits,
+    uint32_t* wbits = nn && !r1 ? c.w.mask_bits : nullptr;
+    SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, Kin, Kinv, gt, in, Kin, 1, dWl, ldw, 0, wbits, st));
+    if (l == d.skip) SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, d.E3p, d.E3, gt, enc, d.E3p, 1, dWl, ldw, d.W, nullptr, st));
+    if (nn)
+      SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.W, d.W, c.w.Grow[gi], Wl, ldw, 0, wbits ? nullptr : in, d.W, wbits,
                            r1 ? graw : nullptr, r1 ? mlp->trunk_w[l] : nullptr, nullptr, 0, 0, grad_images(c, gi ^ 1, Mc),
                            grad->trunk_b[l - 1], r1 ? grad->trunk_w[l] : nullptr, st));
     if (enc_grad && (l == d.skip || l == 0)) {
-      SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.E3p, d.E3, c.w.Grow[gi], Wl, ldw, l == 0 ? 0 : d.W, nullptr, 0, nullptr,
-                           nullptr, nullptr, c.w.Genc, d.E3p, genc_written ? 1 : 0, TcOut{}, nullptr, nullptr, st));
+      SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.E3p, d.E3, c.w.Grow[grad_row(d, chained, l)], Wl, ldw, l == 0 ? 0 : d.W,
+                           nullptr, 0, nullptr, nullptr, nullptr, c.w.Genc, d.E3p, genc_written ? 1 : 0, TcOut{}, nullptr,
+                           nullptr, st));
       genc_written = true;
     }
-    gi ^= 1;
+    if (chained && last) SPARF_TRY(chunk_dgrad_chain(mlp, c, Mc, bits, grad, enc_grad, st));
   }
   return SPARF_OK;
 }
@@ -1096,7 +1146,7 @@ static int mlp_backward(const SparfMLP* mlp, int engine, int R, int S, const flo
       }
       SPARF_CHECK_LAUNCH("direnc_bwd_kernel");
     }
-    SPARF_TRY(c.tc ? trunk_backward_tc(mlp, c, Mc, v.enc, v.H, w.graw, grad, need_rays, st)
+    SPARF_TRY(c.tc ? trunk_backward_tc(mlp, c, Mc, v.enc, v.H, v.bits, w.graw, grad, need_rays, st)
                    : trunk_backward_simt(mlp, c, Mc, v.enc, v.H, w.graw, grad, need_rays, st));
     if (need_rays) {
       float* d_o = d_origins ? d_origins + (size_t)r0 * 3 : nullptr;
@@ -1193,7 +1243,7 @@ extern "C" int sparf_mlp_backward(const SparfMLP* mlp, int32_t engine, int32_t R
 // tape variants: the training forward keeps what the backward needs, so that the backward does not recompute the forward
 extern "C" size_t sparf_mlp_tape_bytes(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S) {
   if (!mlp || R <= 0 || S <= 0 || resolve_engine(engine) < 0 || validate_mlp(mlp)) return 0;
-  const size_t n = tape_layout(mlp_dims(mlp), R, S, nullptr, nullptr);
+  const size_t n = tape_layout(mlp_dims(mlp), is_tc(resolve_engine(engine)), R, S, nullptr, nullptr);
   return n <= kMaxTapeBytes ? n : 0;
 }
 
@@ -1261,7 +1311,7 @@ extern "C" int sparf_density_forward(const SparfMLP* mlp, int32_t engine, int64_
     const int n = (int)std::min<long long>(c.nrc, M - p0);
     v.H[d.nt - 1] = feat ? feat + (size_t)p0 * d.W : nullptr;     // the features go straight to the caller, or nowhere
     SPARF_TRY(chunk_encode_xyz(mlp, c, n, 1, points + (size_t)p0 * 3, nullptr, nullptr, v.enc, st));
-    SPARF_TRY(chunk_trunk(mlp, c, n, v.enc, v.H, nullptr, raw + p0, nullptr, false, st));
+    SPARF_TRY(chunk_trunk(mlp, c, n, v.enc, v.H, nullptr, nullptr, raw + p0, nullptr, false, st));
   }
   return SPARF_OK;
 }
@@ -1287,7 +1337,7 @@ extern "C" int sparf_density_backward(const SparfMLP* mlp, int32_t engine, int64
     const float* dr = d_raw ? d_raw + p0 : nullptr;
     const float* df = d_feat ? d_feat + (size_t)p0 * d.W : nullptr;
     SPARF_TRY(chunk_encode_xyz(mlp, c, n, 1, points + (size_t)p0 * 3, nullptr, nullptr, v.enc, st));
-    SPARF_TRY(chunk_trunk(mlp, c, n, v.enc, v.H, nullptr, nullptr, nullptr, false, st));
+    SPARF_TRY(chunk_trunk(mlp, c, n, v.enc, v.H, v.bits, nullptr, nullptr, nullptr, false, st));
     if (c.tc) {
       SPARF_TRY(tc_feat_backward(c.ep.dgrad, c.ep.wgrad, n, d.W, dr, df, v.H[d.nt - 1], c.w.Grow[0], grad_tr(c.w, 0, n), db,
                                  db + 1, st));
@@ -1297,7 +1347,7 @@ extern "C" int sparf_density_backward(const SparfMLP* mlp, int32_t engine, int64
     } else {
       SPARF_CHECK_CUDA(cudaMemsetAsync(c.w.G0, 0, (size_t)n * d.W * sizeof(float), st));
     }
-    SPARF_TRY(c.tc ? trunk_backward_tc(mlp, c, n, v.enc, v.H, dr, grad, d_points != nullptr, st)
+    SPARF_TRY(c.tc ? trunk_backward_tc(mlp, c, n, v.enc, v.H, v.bits, dr, grad, d_points != nullptr, st)
                    : trunk_backward_simt(mlp, c, n, v.enc, v.H, dr, grad, d_points != nullptr, st));
     if (d_points) {
       posenc_bwd_kernel<<<ceil_div(n, 4), 128, 0, st>>>(n, 1, mlp->L_xyz, d.E3p, v.enc, c.w.Genc, nullptr,

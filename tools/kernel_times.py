@@ -16,7 +16,7 @@ import common
 from sparf_b200 import _lib, ops
 
 HBM_PEAK = 3.35e12      # H100 SXM data sheet, bytes/s
-GEMM_KERNELS = ("wg_gemm_kernel", "wg_gemm_staged_kernel", "trunk_chain_kernel")
+GEMM_KERNELS = ("wg_gemm_kernel", "wg_gemm_staged_kernel", "trunk_chain_kernel", "dgrad_chain_kernel")
 # 16-bit passes of the images (forward, input gradient, weight gradient) per tensor-core engine
 PASSES = {"tc_3x": (3, 3, 3), "tc_1x": (1, 1, 1), "tc_3x_w1": (3, 3, 1), "auto": (3, 3, 3)}
 
@@ -25,7 +25,8 @@ def gemm_bytes_per_row(spec, passes, backward, pose):
     """HBM bytes per sample row that the wgmma GEMMs must read and write, counted from the shapes: the A operand images,
     the weight-gradient GEMMs' B operands (the activations, read as fp32 and split inside the GEMM), the fp32 outputs,
     the epilogue images and the ReLU masks (bits, 1/8 byte per value, written by the weight-gradient GEMM; fp32 at the
-    last trunk layer, whose epilogue sums the density row's weight gradient from the values).  The weights' images are
+    last trunk layer, whose epilogue sums the density row's weight gradient from the values; with the fused trunk, the
+    masks of H[0] ... H[nt-3] are written by the forward and read by the fused input gradients).  The weights' images are
     small and stay in L2; they are not counted."""
     pf, pd, pw = passes
     W, HW, skip, nt = spec.width, spec.head_width, spec.skip_layer, spec.n_trunk
@@ -37,9 +38,11 @@ def gemm_bytes_per_row(spec, passes, backward, pose):
     # forward: the fused trunk (width 256, as MLPSpec's default) reads the encoding image once, keeps the activations on
     # the SM, and writes fp32 H[l] where it is kept (every layer for the tape; the last two in an inference forward) and
     # the last layer's row image; other widths go layer by layer, each reading its input image (+ enc at the skip layer)
-    # and writing fp32 H and its row image.  The colour head reads [H | denc] and writes fp32 hid
-    if W == 256 and E3p <= 64 and nt >= 3:
-        n = img(E3p, pf) + 4 * W * (nt if backward else 2) + img(W, pf)
+    # and writing fp32 H and its row image; a training forward through the fused trunk also writes the masks of H[0] ...
+    # H[nt-3].  The colour head reads [H | denc] and writes fp32 hid
+    chained = W == 256 and E3p <= 64 and nt >= 3
+    if chained:
+        n = img(E3p, pf) + 4 * W * (nt if backward else 2) + img(W, pf) + (W / 8 * (nt - 2) if backward else 0)
     else:
         n = sum(img(W if l else E3p, pf) + (img(E3p, pf) if l == skip else 0) + 4 * W + img(W, pf) for l in range(nt))
     n += img(W, pf) + img(Evp, pf) + 4 * HW
@@ -55,7 +58,11 @@ def gemm_bytes_per_row(spec, passes, backward, pose):
         n += img(W, pw) + 4 * (W if l else E3p)                         # weight gradient
         if l == skip:
             n += img(W, pw) + 4 * E3p
-        if l > 0:                                                       # input gradient: G image, mask, two images out
+        if l > 0 and chained and l < nt - 1:
+            # the fused input gradients of layers nt-2 ... 1: G[nt-2]'s row image once, per layer the mask and the
+            # transposed image out, and the row images of G[skip] and G[0] for the encoding's gradient
+            n += (img(W, pd) if l == nt - 2 else 0) + W / 8 + img(W, pw) + (img(W, pd) if pose and (l - 1 in (skip, 0)) else 0)
+        elif l > 0:                                                     # input gradient: G image, mask, two images out
             n += img(W, pd) + (4 * W if l == nt - 1 else W / 8) + img(W, pd) + img(W, pw)
         if pose and (l == skip or l == 0):                              # encoding gradient, fp32 (+= at layer 0)
             n += img(W, pd) + 4 * E3p + (4 * E3p if l == 0 and skip > 0 else 0)
