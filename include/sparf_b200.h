@@ -205,6 +205,50 @@ int sparf_compact_gather(int64_t C, const int64_t* K, const int64_t* sample_idx,
 int sparf_compact_ray_sum(int64_t R, int32_t S, int64_t C, const int64_t* K, const int64_t* sample_idx, int32_t width,
                           const float* src, float* dst, sparf_stream_t stream);
 
+/* ---------------------------------------------------------------- early ray termination in training
+ * A training pass (train / test-optim, with or without gradients; sparf_b200/termination.py train_forward_samples) over
+ * the windows of the inference termination below, without a host round trip, with one tape and one backward per pass.
+ *   kept set:  exactly the inference rule (same windows [k0, min(k0 + window, S)), the same tau update, op order and
+ *              tau_max = fp32(-ln eps), a NaN tau stays alive, the box or contracted grid lookup when a grid is given),
+ *              except that sigma is the training pass's own output: with density noise (drawn dense by the caller, as
+ *              on the grid path) sigma = softplus(raw + noise).
+ *   layout:    ends [W + 1] (device int64, W = ceil(S / window), ends[0] = 0 set by the caller).  Window w compacts its
+ *              kept samples, in increasing r*S + k, to rows [ends[w], ends[w + 1]) of capacity-R*S buffers (sample_idx,
+ *              origins_k, dirs_k, t_k): sparf_termination_append (box grid, or bits = NULL: none) and
+ *              sparf_contracted_append take the arguments of the count / emit pair plus (ends, w), run count, scan and
+ *              emit on one workspace (sparf_termination_workspace_bytes(R, k1 - k0)) and write ends[w + 1] = ends[w] + K_w.
+ *              64-bit offsets, no atomics; rows outside [ends[w], ends[w + 1]) are not written.
+ *   outputs:   sigma and rgb equal the dense training pass's with sigma = rgb = 0 at the skipped samples, bit for bit:
+ *              every kept sample is evaluated as a one-sample ray by sparf_mlp_forward_tape_span.  Gradients are those of
+ *              that masked pass; skipped samples get none.  One sparf_mlp_backward_tape_rows with rows = &ends[W] over
+ *              capacity C = R*S runs the pass's backward.  d_origins / d_dirs (sparf_compact_ray_sum_segments) have the
+ *              bits of sparf_compact_ray_sum over the same kept set; parameter gradients agree up to float atomic order.
+ *   bounds:    against the non-terminated pass with the same t and noise, those of the inference termination below.
+ *   host:      only W is known on the host; no count is read back, so a step that uses it can be one CUDA graph.
+ * Tensor-core engines only (TC_3X, TC_1X, TC_3X_W1).
+ *
+ * sparf_mlp_forward_tape_span: sparf_mlp_forward_tape_rows over the device-side row span [*begin, min(*end, *begin +
+ * cap)) of capacity-C buffers: it reads origins, dirs, t, noise and writes sigma, rgb and the tape's rows (the tape of C
+ * rows, sparf_mlp_tape_bytes(C, 1)) at those global rows; cap sizes the chunk loop and the workspace
+ * (sparf_mlp_workspace_bytes(cap, 1, 0)), whose images stay call-local.  The caller keeps *end <= C.  Rows outside the
+ * span are neither read nor written.  sigma, rgb and the tape rows have the bits sparf_mlp_forward_tape_rows gives on
+ * the same rows moved to row 0, so a tape written by several spans is read by one sparf_mlp_backward_tape_rows with
+ * R = C and rows = the last span's end.
+ * sparf_compact_scatter_span / _gather_span: sparf_compact_scatter / _gather over rows [ends[w], ends[w + 1]) only, at
+ * most C (the window's capacity, R * window) of them.
+ * sparf_compact_ray_sum_segments: sparf_compact_ray_sum over the W segments [ends[w], ends[w + 1]): per ray, the rows of
+ * each segment in window order, each in increasing k, from 0. */
+int sparf_mlp_forward_tape_span(const SparfMLP* mlp, int32_t engine, int32_t C, int32_t cap, const int64_t* begin,
+                                const int64_t* end, const float* origins, const float* dirs, const float* t,
+                                const float* noise, float* sigma, float* rgb, void* tape, size_t tape_bytes,
+                                void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+int sparf_compact_scatter_span(int64_t C, const int64_t* ends, int32_t w, const int64_t* sample_idx, int32_t width,
+                               const float* src, float* dst, sparf_stream_t stream);
+int sparf_compact_gather_span(int64_t C, const int64_t* ends, int32_t w, const int64_t* sample_idx, int32_t width,
+                              const float* src, float* dst, sparf_stream_t stream);
+int sparf_compact_ray_sum_segments(int64_t R, int32_t S, int32_t W, const int64_t* ends, const int64_t* sample_idx,
+                                   int32_t width, const float* src, float* dst, sparf_stream_t stream);
+
 /* ---------------------------------------------------------------- density queries
  * NeRF.compute_raw_density (frequency_nerf.py:149-170): the trunk alone at M arbitrary points [M,3] (x = p; no view
  * direction, no colour head).  Outputs raw [M], the density row before the softplus, without noise, and, when feat is
@@ -319,6 +363,11 @@ int sparf_termination_emit(int64_t R, int32_t S, int32_t k0, int32_t k1, const f
                            size_t workspace_bytes, sparf_stream_t stream);
 int sparf_termination_update(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* sigma, const float* t,
                              const float* dirs, float tau_max, float* tau, uint8_t* alive, sparf_stream_t stream);
+/* the appending compaction of window w for training termination (section above sparf_mlp_forward_tape_span) */
+int sparf_termination_append(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins, const float* dirs,
+                             const float* t, const uint8_t* alive, const uint32_t* bits, int32_t res, float r0, float r1,
+                             int64_t* ends, int32_t w, int64_t* sample_idx, float* origins_k, float* dirs_k, float* t_k,
+                             void* workspace, size_t workspace_bytes, sparf_stream_t stream);
 
 /* ---------------------------------------------------------------- contracted occupancy grid
  * An occupancy grid over all of space for inverse-depth and unbounded scenes (sparf_b200/occupancy.py with
@@ -353,6 +402,10 @@ int sparf_contracted_emit(int64_t R, int32_t S, int32_t k0, int32_t k1, const fl
                           const float* t, const uint8_t* alive, const uint32_t* bits, int32_t res, const float* center,
                           float radius, int64_t* sample_idx, float* origins_k, float* dirs_k, float* t_k,
                           void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+int sparf_contracted_append(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins, const float* dirs,
+                            const float* t, const uint8_t* alive, const uint32_t* bits, int32_t res, const float* center,
+                            float radius, int64_t* ends, int32_t w, int64_t* sample_idx, float* origins_k, float* dirs_k,
+                            float* t_k, void* workspace, size_t workspace_bytes, sparf_stream_t stream);
 
 /* ---------------------------------------------------------------- compositing
  * NeRF.composite (frequency_nerf.py:283-343).  Outputs: rgb_map [R,3], depth/opacity/depth_var/rgb_var

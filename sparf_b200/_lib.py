@@ -59,6 +59,11 @@ _SIGNATURES = {
     "sparf_compact_scatter": (c_int32, [c_int64, _P, _P, c_int32, _P, _P, _P]),
     "sparf_compact_gather": (c_int32, [c_int64, _P, _P, c_int32, _P, _P, _P]),
     "sparf_compact_ray_sum": (c_int32, [c_int64, c_int32, c_int64, _P, _P, c_int32, _P, _P, _P]),
+    "sparf_mlp_forward_tape_span": (c_int32, [POINTER(SparfMLP), c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, _P, _P, _P,
+                                              _P, c_size_t, _P, c_size_t, _P]),
+    "sparf_compact_scatter_span": (c_int32, [c_int64, _P, c_int32, _P, c_int32, _P, _P, _P]),
+    "sparf_compact_gather_span": (c_int32, [c_int64, _P, c_int32, _P, c_int32, _P, _P, _P]),
+    "sparf_compact_ray_sum_segments": (c_int32, [c_int64, c_int32, c_int32, _P, _P, c_int32, _P, _P, _P]),
     "sparf_density_workspace_bytes": (c_size_t, [POINTER(SparfMLP), c_int64, c_int32, c_int32]),
     "sparf_density_forward": (c_int32, [POINTER(SparfMLP), c_int32, c_int64, _P, _P, _P, _P, c_size_t, _P]),
     "sparf_density_backward": (c_int32, [POINTER(SparfMLP), c_int32, c_int64, _P, _P, _P, POINTER(SparfMLPGrad), _P, _P,
@@ -78,6 +83,10 @@ _SIGNATURES = {
     "sparf_termination_emit": (c_int32, [c_int64, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, c_int32, c_float, c_float,
                                          _P, _P, _P, _P, _P, c_size_t, _P]),
     "sparf_termination_update": (c_int32, [c_int64, c_int32, c_int32, c_int32, _P, _P, _P, c_float, _P, _P, _P]),
+    "sparf_termination_append": (c_int32, [c_int64, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, c_int32, c_float, c_float,
+                                           _P, c_int32, _P, _P, _P, _P, _P, c_size_t, _P]),
+    "sparf_contracted_append": (c_int32, [c_int64, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, c_int32, POINTER(c_float),
+                                          c_float, _P, c_int32, _P, _P, _P, _P, _P, c_size_t, _P]),
     "sparf_contracted_count": (c_int32, [c_int64, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, c_int32, POINTER(c_float),
                                          c_float, _P, _P, c_size_t, _P]),
     "sparf_contracted_emit": (c_int32, [c_int64, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, c_int32, POINTER(c_float),

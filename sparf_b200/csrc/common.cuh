@@ -51,17 +51,27 @@ extern unsigned long long g_launch_count;
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// A row count read on the device (the *_rows MLP entry points): of the cap rows a kernel is sized for, starting at row
-// m0 of the call, it processes min(cap, max(0, *rows - m0)).  Kernels take it behind a template flag DYN; without it
-// they process cap rows and never touch `rows`.
+// A row count read on the device (the *_rows and *_span MLP entry points): of the cap rows a kernel is sized for,
+// starting at row m0 of the call, it processes min(cap, max(0, *rows - s - m0)), s = *start (start NULL: s = 0).  The
+// span forward (start != NULL) adds s to the row of every global input, output and tape buffer it touches; workspace
+// buffers stay call-local.  Kernels take it behind a template flag DYN; without it they process cap rows and never touch
+// `rows` or `start`.
 struct RowCount {
   const int64_t* rows;
   long long m0;
+  const int64_t* start;
 };
 template <bool DYN>
+__device__ __forceinline__ long long row_start(const RowCount& rc) {
+  if constexpr (DYN) return rc.start ? *rc.start : 0;
+  else return 0;
+}
+// START = false: the kernel is never given a start (the backward's kernels; the large GEMM and trunk-chain kernels take
+// the span forward's rows through instantiations of their own), so its code stays that of the *_rows calls
+template <bool DYN, bool START = true>
 __device__ __forceinline__ long long live_rows(long long cap, const RowCount& rc) {
   if constexpr (DYN) {
-    const long long k = *rc.rows - rc.m0;
+    const long long k = *rc.rows - (START ? row_start<true>(rc) : 0) - rc.m0;
     return k < 0 ? 0 : (k < cap ? k : cap);
   } else {
     return cap;

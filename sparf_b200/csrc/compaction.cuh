@@ -104,9 +104,13 @@ __device__ __forceinline__ void block_scan(T& x, T& total) {
   __syncthreads();  // the next call reuses sx
 }
 
-// the body of a one-CTA (kScanThreads) scan kernel: tile totals -> exclusive 64-bit tile bases (in place); *K = the sum
-__device__ __forceinline__ void scan_tiles(long long* __restrict__ tiles, long long ntiles, int64_t* __restrict__ K) {
-  long long carry = 0;
+// the body of a one-CTA (kScanThreads) scan kernel: tile totals -> exclusive 64-bit tile bases (in place); *K = the sum.
+// APPEND: the bases start at *start instead of 0 (the emit then writes after the rows already there), and *K = *start
+// + the sum
+template <bool APPEND = false>
+__device__ __forceinline__ void scan_tiles(long long* __restrict__ tiles, long long ntiles, int64_t* __restrict__ K,
+                                           const int64_t* __restrict__ start = nullptr) {
+  long long carry = APPEND ? *start : 0;
   for (long long base = 0; base < ntiles; base += (long long)kScanThreads * kOcItems) {
     const long long t0 = base + (long long)threadIdx.x * kOcItems;
     long long e[kOcItems], s = 0;

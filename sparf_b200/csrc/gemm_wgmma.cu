@@ -170,7 +170,8 @@ struct TnB {
 
 // image tile (row tile rt, k-step kt) at ((rt * ksteps + kt) * 2 + half) * TILE_ELEMS.  Loads follow the operand's
 // contiguous dimension (KFAST); the split tile is assembled in shared memory and leaves in 16-byte vectors.
-// DYN (Rows only): f.M is a capacity, of which live_rows rows are packed; row tiles past them are not written.
+// DYN (Rows only): f.M is a capacity, of which live_rows rows are packed; row tiles past them are not written.  f.X's
+// rows start at row_start (the span forward's global rows); the image's at 0.
 template <bool F16, int PASSES, bool KFAST, class F, bool DYN = false>
 __global__ void __launch_bounds__(256) pack_kernel(F f, int ksteps, uint16_t* __restrict__ img, RowCount rc) {
   __shared__ __align__(16) uint16_t t[2 * TILE_ELEMS];
@@ -178,6 +179,7 @@ __global__ void __launch_bounds__(256) pack_kernel(F f, int ksteps, uint16_t* __
   if constexpr (DYN) {
     f.M = (int)live_rows<true>(f.M, rc);
     if (rt * TM >= f.M) return;
+    f.X += row_start<true>(rc) * f.ldx;
   }
   float v[16];
 #pragma unroll
@@ -301,7 +303,7 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(const HeadBwd p, RowCount
   float* rsum = w9 + 3 * TN;                // [4 warps][4]: sums of gpre 0..2 and graw
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int m0 = blockIdx.x * TM;
-  const int M = (int)live_rows<DYN>(p.M, rc);
+  const int M = (int)live_rows<DYN, false>(p.M, rc);
   if (DYN && m0 >= M) return;
   if (tid < TM) {
     const int m = m0 + tid;
@@ -825,14 +827,16 @@ __device__ __forceinline__ void epilogue(float (&acc)[64], int bx, int by, const
 // its share back (setmaxnreg), so that the consumers get 232 each (128 x 40 + 256 x 232 <= 64 K) and the epilogue,
 // with its loads issued together, does not spill.
 // DYN (output tiles only, nsplit = 1): e.M is a capacity, of which live_rows rows are computed; the units of A row
-// tiles past them are skipped.
-template <bool F16, int PASSES, bool F32, int ROWP, int TRP, bool DYN = false>
+// tiles past them are skipped.  SPAN (with DYN and F32; the span forward): the fp32 output's rows start at row_start, the
+// images' at 0; without it rc.start is never read.
+template <bool F16, int PASSES, bool F32, int ROWP, int TRP, bool DYN = false, bool SPAN = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) wg_gemm_kernel(Opnd a, Opnd b, Units w, Epi e, RowCount rc) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if constexpr (DYN) {
-    e.M = (int)live_rows<true>(e.M, rc);
+    e.M = (int)live_rows<true, SPAN>(e.M, rc);
     if (e.M == 0) return;
     w.tiles = (e.M + TM - 1) / TM * w.rtb;
+    if constexpr (SPAN) e.out += row_start<true>(rc) * e.ldo;
   }
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + RED_BYTES);
   uint64_t* empty = full + STAGES;
@@ -986,7 +990,7 @@ __global__ void __launch_bounds__(STAGED_THREADS, 1) wg_gemm_staged_kernel(Opnd 
                                                                            int ctas) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if constexpr (DYN) {
-    x.M = (int)live_rows<true>(x.M, rc);
+    x.M = (int)live_rows<true, false>(x.M, rc);
     if (x.M == 0) return;
     w.nk = (x.M + TK - 1) / TK;
     w.nsplit = max(1, min(w.nk, (ctas + w.tiles - 1) / w.tiles * ((w.nk + 1023) / 1024)));
@@ -1208,12 +1212,14 @@ __device__ __forceinline__ void chain_store_bits(const float (&acc)[64], uint32_
 // both warpgroups have passed a second barrier.  The epilogue is not overlapped with MMAs (the accumulators of one tile
 // fill both warpgroups); the ring keeps the next layer's weights coming meanwhile.
 // Tiles: 2 ceil(M / 128), so that the last image's 128-row tiles are written whole; a tile wholly past M only zeroes its
-// half of them.  DYN: c.M is a capacity, of which live_rows rows (M) are computed.  BITS: c.bits[l] are written where
+// half of them.  DYN: c.M is a capacity, of which live_rows rows (M) are computed.  SPAN (with DYN; the span forward): H
+// and bits take their rows from row_start on (the last image's rows start at 0); without it rc.start is never read.
+// BITS: c.bits[l] are written where
 // not NULL (the other instantiations never read them).
-template <bool F16, int PASSES, bool DYN = false, bool BITS = false>
+template <bool F16, int PASSES, bool DYN = false, bool BITS = false, bool SPAN = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) trunk_chain_kernel(const Chain c, RowCount rc) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int M = (int)live_rows<DYN>(c.M, rc);
+  const int M = (int)live_rows<DYN, SPAN>(c.M, rc);
   if (DYN && M == 0) return;
   const int tiles = (M + TM - 1) / TM * 2;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + CH_BAR);
@@ -1237,6 +1243,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) trunk_chain_kernel(const Chai
   }
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
   const int enc_last = c.skip > 0 && c.skip < c.nl ? c.skip : 0;   // the last layer that reads the encoding
+  const long long s0 = row_start<SPAN>(rc);   // the span forward: H and bits at global rows s0 + m; 0 otherwise
   int it = 0, n = 0;
   for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
     if (t * CH_M >= M) {
@@ -1258,8 +1265,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) trunk_chain_kernel(const Chai
         fence_proxy_async();    // the stores into the activation buffer, before the MMAs that read them
         consumer_sync();
       }
-      if (c.H[l]) chain_store(acc, c.H[l], M, t);
-      if (BITS && c.bits[l]) chain_store_bits(acc, c.bits[l], M, t);
+      if (c.H[l]) chain_store(acc, c.H[l] + s0 * CH_W, M, t);
+      if (BITS && c.bits[l]) chain_store_bits(acc, c.bits[l] + s0 * (CH_W / 32), M, t);
     }
   }
 }
@@ -1270,6 +1277,13 @@ static int launch_chain(const Chain& c, int ctas, RowCount rc, cudaStream_t st) 
   for (int l = 0; l < c.nl; ++l) bits |= c.bits[l] != nullptr;
   auto kernel = bits ? (rc.rows ? trunk_chain_kernel<F16, PASSES, true, true> : trunk_chain_kernel<F16, PASSES, false, true>)
                      : (rc.rows ? trunk_chain_kernel<F16, PASSES, true> : trunk_chain_kernel<F16, PASSES>);
+  if (rc.start) {       // the span forward: a taped forward, which keeps the mask bits
+    if (!bits) {
+      set_error("trunk_chain: a row start needs the mask bits (taped forward)");
+      return SPARF_ERR_UNSUPPORTED;
+    }
+    kernel = trunk_chain_kernel<F16, PASSES, true, true, true>;
+  }
   SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM));
   kernel<<<std::min(2 * ceil_div(c.M, TM), ctas), GEMM_THREADS, CH_SMEM, st>>>(c, rc);
   SPARF_CHECK_LAUNCH("trunk_chain_kernel");
@@ -1379,7 +1393,7 @@ __device__ __forceinline__ void dg_zero_tile(const DgChain& c, int t) {
 template <int DP, int TP, bool DYN = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) dgrad_chain_kernel(const DgChain c, RowCount rc) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int M = (int)live_rows<DYN>(c.M, rc);
+  const int M = (int)live_rows<DYN, false>(c.M, rc);
   if (DYN && M == 0) return;
   const int tiles = (M + TM - 1) / TM * 2;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + CH_BAR);
@@ -1488,6 +1502,14 @@ static int launch_pack(F f, int rtiles, int ksteps, uint16_t* img, cudaStream_t 
 template <bool F16, int PASSES, bool F32, int ROWP, int TRP>
 static int launch_gemm(const Opnd& a, const Opnd& b, const Units& w, int ctas, const Epi& e, RowCount rc, cudaStream_t st) {
   auto kernel = rc.rows ? wg_gemm_kernel<F16, PASSES, F32, ROWP, TRP, true> : wg_gemm_kernel<F16, PASSES, F32, ROWP, TRP>;
+  if (rc.start) {       // the span forward: only GEMMs with an fp32 output (into the tape) take global rows
+    if constexpr (F32) {
+      kernel = wg_gemm_kernel<F16, PASSES, F32, ROWP, TRP, true, true>;
+    } else {
+      set_error("a GEMM without an fp32 output takes no row start");
+      return SPARF_ERR_UNSUPPORTED;
+    }
+  }
   SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
   kernel<<<std::min(w.tiles * w.nsplit, ctas), GEMM_THREADS, GEMM_SMEM, st>>>(a, b, w, e, rc);
   SPARF_CHECK_LAUNCH("wg_gemm_kernel");

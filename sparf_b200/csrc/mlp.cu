@@ -27,13 +27,21 @@ __global__ void c2f_weights_kernel(C2F c, int L_xyz, int L_view, float* __restri
 
 // enc[m][0:3] = x = o + t*d ; enc[m][3 + c*2L + {0,L} + j] = w_j * {sin,cos}(x_c * 2^j pi) ; zero pad to E3p
 // dirs == NULL: the origins are the points themselves, x = o (S = 1; the value o + 0*d takes)
-// DYN (S = 1): total / E3p rows is a capacity, of which live_rows are encoded (the same for every kernel below with DYN)
+// DYN (S = 1): total / E3p rows is a capacity, of which live_rows are encoded (the same for every kernel below with DYN);
+// the rows of the global buffers start at row_start (RowCount)
 template <bool DYN = false>
 __global__ void encode_xyz_kernel(long long total, int S, int L, int E3p, const float* __restrict__ origins,
                                   const float* __restrict__ dirs, const float* __restrict__ t,
                                   const float* __restrict__ wts, float* __restrict__ enc, RowCount rc) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (DYN ? live_rows<DYN>(total / E3p, rc) * E3p : total)) return;
+  if constexpr (DYN) {
+    const long long s0 = row_start<true>(rc);
+    origins += s0 * 3;
+    if (dirs) dirs += s0 * 3;
+    t += s0;
+    enc += s0 * E3p;
+  }
   int col = (int)(idx % E3p);
   long long m = idx / E3p;
   long long r = m / S;
@@ -60,6 +68,11 @@ __global__ void encode_dir_kernel(int total, int L, int Evp, const float* __rest
                                   const float* __restrict__ wts_view, float* __restrict__ denc, RowCount rc) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (DYN ? (int)live_rows<DYN>(total / Evp, rc) * Evp : total)) return;
+  if constexpr (DYN) {
+    const long long s0 = row_start<true>(rc);
+    dirs += s0 * 3;
+    denc += s0 * Evp;
+  }
   int col = idx % Evp, r = idx / Evp;
   float val = 0.f;
   if (col < 3 + 6 * L) {
@@ -299,6 +312,13 @@ __global__ void rowdot_kernel(long long M, int K, const float* __restrict__ X, i
   const int lane = threadIdx.x & 31;
   long long m = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (m >= live_rows<DYN>(M, rc)) return;
+  if constexpr (DYN) {
+    const long long s0 = row_start<true>(rc);
+    X += s0 * ldx;
+    if (noise) noise += s0;
+    if (raw_out) raw_out += s0;
+    if (out) out += s0 * (MODE == 0 ? 1 : 3);
+  }
   constexpr int NS = MODE == 0 ? 1 : 3;
   float acc[NS];
 #pragma unroll
@@ -412,7 +432,7 @@ template <bool DYN = false>
 __global__ void ray_reduce_kernel(int nrays, int S, int C, const float* __restrict__ in, float* __restrict__ out,
                                   RowCount rc) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (int)live_rows<DYN>(nrays, rc) * C) return;
+  if (idx >= (int)live_rows<DYN, false>(nrays, rc) * C) return;
   int c = idx % C, r = idx / C;
   float acc = 0.f;
   for (int k = 0; k < S; ++k) acc += in[((size_t)r * S + k) * C + c];
@@ -428,7 +448,7 @@ __global__ void posenc_bwd_kernel(int nrays, int S, int L, int E3p, const float*
                                   float* __restrict__ d_o, float* __restrict__ d_d, RowCount rc) {
   const int lane = threadIdx.x & 31;
   int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (r >= (int)live_rows<DYN>(nrays, rc)) return;
+  if (r >= (int)live_rows<DYN, false>(nrays, rc)) return;
   float so[3] = {0.f, 0.f, 0.f}, sd[3] = {0.f, 0.f, 0.f};
   for (int k = lane; k < S; k += 32) {
     size_t m = (size_t)r * S + k;
@@ -470,7 +490,7 @@ __global__ void direnc_bwd_kernel(int nrays, int L, int Evp, const float* __rest
                                   const float* __restrict__ Gdenc, const float* __restrict__ dirs,
                                   float* __restrict__ d_d, RowCount rc) {
   int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= (int)live_rows<DYN>(nrays, rc)) return;
+  if (r >= (int)live_rows<DYN, false>(nrays, rc)) return;
   const float* e = denc + (size_t)r * Evp;
   const float* g = Gdenc + (size_t)r * Evp;
   float gu[3];
@@ -738,7 +758,7 @@ struct Call {
 // head), check the tape (taped passes: tape != NULL) and the workspace against the pass's sizes, carve the workspace for
 // one chunk, and give the GEMMs its pack buffer.  who: the entry point, for the error text.
 static int begin_call(const char* who, const SparfMLP* mlp, int engine, long long R, int S, Pass pass, bool head, void* tape,
-                      size_t tape_bytes, void* workspace, size_t workspace_bytes, Call* c) {
+                      size_t tape_bytes, void* workspace, size_t workspace_bytes, Call* c, long long tape_R = -1) {
   const int e = resolve_engine(engine);
   if (e < 0) {
     set_error("%s: engine %d not available in this build", who, engine);
@@ -747,10 +767,12 @@ static int begin_call(const char* who, const SparfMLP* mlp, int engine, long lon
   SPARF_TRY(head ? validate_mlp(mlp) : validate_trunk(mlp));
   c->d = mlp_dims(mlp);
   c->tc = is_tc(e);
+  if (tape_R < 0) tape_R = R;     // the span forward's tape holds more rows (its capacity) than one call processes
   if (tape) {
-    SPARF_REQUIRE(tape_bytes >= tape_layout(c->d, c->tc, (int)R, S, nullptr, nullptr), "%s: tape %zu bytes too small", who,
-                  tape_bytes);
-    tape_layout(c->d, c->tc, (int)R, S, reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(tape), 256)), &c->tape);
+    SPARF_REQUIRE(tape_bytes >= tape_layout(c->d, c->tc, (int)tape_R, S, nullptr, nullptr), "%s: tape %zu bytes too small",
+                  who, tape_bytes);
+    tape_layout(c->d, c->tc, (int)tape_R, S, reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(tape), 256)),
+                &c->tape);
   }
   const size_t need = workspace_need(c->d, c->tc, R, S, pass, head);
   if (workspace_bytes < need) {
@@ -888,8 +910,9 @@ static int chunk_forward(const SparfMLP* mlp, const Call& c, int nr, int S, cons
   return SPARF_OK;
 }
 
-// The taped calls with a device row count (sparf_mlp_*_tape_rows): tensor-core engines and one-sample rays only
-static int rows_call(const char* who, Call* c, int S, const int64_t* rows) {
+// The taped calls with a device row count (sparf_mlp_*_tape_rows, sparf_mlp_forward_tape_span): tensor-core engines and
+// one-sample rays only.  start (span forward only; may be NULL): the device row the call's rows start at.
+static int rows_call(const char* who, Call* c, int S, const int64_t* rows, const int64_t* start = nullptr) {
   if (!rows) return SPARF_OK;
   if (!c->tc) {
     set_error("%s: a device row count needs a tensor-core engine (tc_3x, tc_1x or tc_3x_w1)", who);
@@ -897,19 +920,22 @@ static int rows_call(const char* who, Call* c, int S, const int64_t* rows) {
   }
   SPARF_REQUIRE(S == 1, "%s: a device row count needs S = 1 (one-sample rays), got S = %d", who, S);
   c->rc.rows = rows;
+  c->rc.start = start;
   return SPARF_OK;
 }
 
 // The MLP forward, chunk by chunk.  tape == NULL: the activations stay in the workspace; else they go straight into the
-// tape.  rows != NULL (taped, S = 1): R is a capacity, *rows the rays evaluated.
+// tape.  rows != NULL (taped, S = 1): R is a capacity, *rows the rays evaluated.  start != NULL as well (the span
+// forward): the rows [*start, *rows) of the global buffers, at most R of them, and the tape holds tape_R rows.
 static int mlp_forward(const SparfMLP* mlp, int engine, int R, int S, const float* origins, const float* dirs, const float* t,
                        const float* noise, float* sigma, float* rgb, void* tape, size_t tape_bytes, void* workspace,
-                       size_t workspace_bytes, cudaStream_t st, const int64_t* rows = nullptr) {
+                       size_t workspace_bytes, cudaStream_t st, const int64_t* rows = nullptr,
+                       const int64_t* start = nullptr, long long tape_R = -1) {
   Call c;
-  const char* who = rows ? "mlp_forward_tape_rows" : tape ? "mlp_forward_tape" : "mlp_forward";
+  const char* who = start ? "mlp_forward_tape_span" : rows ? "mlp_forward_tape_rows" : tape ? "mlp_forward_tape" : "mlp_forward";
   SPARF_TRY(begin_call(who, mlp, engine, R, S, tape ? Pass::kTapedForward : Pass::kForward, true, tape, tape_bytes, workspace,
-                       workspace_bytes, &c));
-  SPARF_TRY(rows_call(who, &c, S, rows));
+                       workspace_bytes, &c, tape_R));
+  SPARF_TRY(rows_call(who, &c, S, rows, start));
   Tape v = c.w.act;
   v.raw = nullptr;      // the plain forward does not keep the softplus argument
   for (int r0 = 0; r0 < R; r0 += c.nrc) {
@@ -1276,6 +1302,17 @@ extern "C" int sparf_mlp_forward_tape_rows(const SparfMLP* mlp, int32_t engine, 
                 "mlp_forward_tape_rows: bad arguments");
   return mlp_forward(mlp, engine, R, S, origins, dirs, t, noise, sigma, rgb, tape, tape_bytes, workspace, workspace_bytes,
                      (cudaStream_t)stream, rows);
+}
+
+// the taped forward over the device-side row span [*begin, min(*end, *begin + cap)) of capacity-C buffers and tape
+extern "C" int sparf_mlp_forward_tape_span(const SparfMLP* mlp, int32_t engine, int32_t C, int32_t cap, const int64_t* begin,
+                                           const int64_t* end, const float* origins, const float* dirs, const float* t,
+                                           const float* noise, float* sigma, float* rgb, void* tape, size_t tape_bytes,
+                                           void* workspace, size_t workspace_bytes, sparf_stream_t stream) {
+  SPARF_REQUIRE(mlp && C > 0 && cap > 0 && cap <= C && begin && end && origins && dirs && t && sigma && rgb && tape,
+                "mlp_forward_tape_span: bad arguments");
+  return mlp_forward(mlp, engine, cap, 1, origins, dirs, t, noise, sigma, rgb, tape, tape_bytes, workspace, workspace_bytes,
+                     (cudaStream_t)stream, end, begin, C);
 }
 
 extern "C" int sparf_mlp_backward_tape_rows(const SparfMLP* mlp, int32_t engine, int32_t R, int32_t S, const int64_t* rows,

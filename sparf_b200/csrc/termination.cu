@@ -6,6 +6,8 @@
 //          compaction).  The kernels are templated on the lookup.  Output in increasing order of r * S + k;
 //   update: one thread per alive ray adds the window's sd_k = sigma_k * (gap_k * len) to tau in sample order, with
 //          explicit rounding (include/sparf_b200.h states the op order), and clears alive[r] when tau > tau_max.
+//   append: (training, sparf_*_append) count / scan / emit with the scan's bases starting at ends[w] instead of 0, so
+//          that window w's samples land after the earlier windows' in one compacted set, and ends[w + 1] written.
 // Deterministic (no atomics).  Workspace: that of a compaction over R * (k1 - k0) samples.
 #include <cmath>
 
@@ -44,9 +46,12 @@ __global__ void __launch_bounds__(kOcThreads) termination_count_kernel(Window<Lk
   if (threadIdx.x == 0) tiles[blockIdx.x] = total;
 }
 
+// APPEND (training termination, sparf_*_append): the window's rows go after those of the windows before it, from
+// K[-1] = ends[w] on, and K = ends[w + 1] = ends[w] + the window's count
+template <bool APPEND = false>
 __global__ void __launch_bounds__(kScanThreads) termination_scan_kernel(long long* __restrict__ tiles, long long ntiles,
                                                                         int64_t* __restrict__ K) {
-  scan_tiles(tiles, ntiles, K);
+  scan_tiles<APPEND>(tiles, ntiles, K, APPEND ? K - 1 : nullptr);
 }
 
 template <class Lk>
@@ -133,16 +138,17 @@ static int window_setup(const char* name, int64_t R, int32_t S, int32_t k0, int3
   return SPARF_OK;
 }
 
-// count: K = 0 for R == 0, else the count and scan kernels
-template <class Lk>
+// count: K = 0 for R == 0, else the count and scan kernels.  APPEND: K = ends + w + 1, and the count starts at K[-1]
+template <bool APPEND = false, class Lk>
 static int launch_count(int64_t R, const Window<Lk>& wn, const Carve& c, int64_t* K, cudaStream_t s) {
   if (R == 0) {
-    SPARF_CHECK_CUDA(cudaMemsetAsync(K, 0, sizeof(int64_t), s));
+    if (APPEND) SPARF_CHECK_CUDA(cudaMemcpyAsync(K, K - 1, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
+    else SPARF_CHECK_CUDA(cudaMemsetAsync(K, 0, sizeof(int64_t), s));
     return SPARF_OK;
   }
   termination_count_kernel<<<(unsigned)c.ntiles, kOcThreads, 0, s>>>(wn, c.local, c.tiles);
   SPARF_CHECK_LAUNCH("termination_count_kernel");
-  termination_scan_kernel<<<1, kScanThreads, 0, s>>>(c.tiles, c.ntiles, K);
+  termination_scan_kernel<APPEND><<<1, kScanThreads, 0, s>>>(c.tiles, c.ntiles, K);
   SPARF_CHECK_LAUNCH("termination_scan_kernel");
   return SPARF_OK;
 }
@@ -240,6 +246,40 @@ extern "C" int sparf_contracted_emit(int64_t R, int32_t S, int32_t k0, int32_t k
   SPARF_TRY(contracted_setup("contracted_emit", R, S, k0, k1, origins, dirs, t, alive, bits, res, center, radius,
                              workspace, workspace_bytes, &wn, &c));
   return launch_emit(R, wn, c, sample_idx, origins_k, dirs_k, t_k, (cudaStream_t)stream);
+}
+
+// the appending compaction of window w: count, scan from ends[w] (writing ends[w + 1]) and emit, on one workspace
+template <class Lk>
+static int launch_append(int64_t R, const Window<Lk>& wn, const Carve& c, int64_t* ends, int32_t w, int64_t* sample_idx,
+                         float* origins_k, float* dirs_k, float* t_k, cudaStream_t s) {
+  SPARF_TRY(launch_count<true>(R, wn, c, ends + w + 1, s));
+  return launch_emit(R, wn, c, sample_idx, origins_k, dirs_k, t_k, s);
+}
+
+extern "C" int sparf_termination_append(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins,
+                                        const float* dirs, const float* t, const uint8_t* alive, const uint32_t* bits,
+                                        int32_t res, float r0, float r1, int64_t* ends, int32_t w, int64_t* sample_idx,
+                                        float* origins_k, float* dirs_k, float* t_k, void* workspace,
+                                        size_t workspace_bytes, sparf_stream_t stream) {
+  SPARF_REQUIRE(ends && w >= 0, "termination_append: NULL ends or w %d < 0", (int)w);
+  Window<Lookup> wn;
+  Carve c;
+  SPARF_TRY(termination_setup("termination_append", R, S, k0, k1, origins, dirs, t, alive, bits, res, r0, r1, workspace,
+                              workspace_bytes, &wn, &c));
+  return launch_append(R, wn, c, ends, w, sample_idx, origins_k, dirs_k, t_k, (cudaStream_t)stream);
+}
+
+extern "C" int sparf_contracted_append(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* origins,
+                                       const float* dirs, const float* t, const uint8_t* alive, const uint32_t* bits,
+                                       int32_t res, const float* center, float radius, int64_t* ends, int32_t w,
+                                       int64_t* sample_idx, float* origins_k, float* dirs_k, float* t_k, void* workspace,
+                                       size_t workspace_bytes, sparf_stream_t stream) {
+  SPARF_REQUIRE(ends && w >= 0, "contracted_append: NULL ends or w %d < 0", (int)w);
+  Window<ContractedLookup> wn;
+  Carve c;
+  SPARF_TRY(contracted_setup("contracted_append", R, S, k0, k1, origins, dirs, t, alive, bits, res, center, radius,
+                             workspace, workspace_bytes, &wn, &c));
+  return launch_append(R, wn, c, ends, w, sample_idx, origins_k, dirs_k, t_k, (cudaStream_t)stream);
 }
 
 extern "C" int sparf_termination_update(int64_t R, int32_t S, int32_t k0, int32_t k1, const float* sigma,

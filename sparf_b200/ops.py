@@ -386,6 +386,150 @@ def mlp_forward_grid(spec: MLPSpec, origins, dirs, t, grid, params: Sequence[tor
     return GridMLPFunction.apply(spec, eng, grid, origins, dirs, t, noise, progress, *params)
 
 
+def _row_ptr(t: torch.Tensor, i: int) -> ctypes.c_void_p:
+    """a pointer to element i of a contiguous tensor (a device address; nothing is read)"""
+    return ctypes.c_void_p(t.data_ptr() + i * t.element_size())
+
+
+def _window_append(grid, o, d, t, k0, k1, alive, ends, w, idx, o_k, d_k, t_k):
+    """Window w = samples [k0, k1) of the alive rays of o, d [R,3], t [R,S] that `grid` (box, contracted or None) keeps,
+    appended to rows [ends[w], ends[w+1]) of the capacity-R*S buffers idx, o_k, d_k, t_k; ends[w+1] is written on the
+    device.  The host never reads it."""
+    L = _lib.lib()
+    R, S = t.shape
+    ws = _workspace(L.sparf_termination_workspace_bytes(R, k1 - k0), t.device)
+    head = (R, S, int(k0), int(k1), _ptr(o), _ptr(d), _ptr(t), _ptr(alive))
+    tail = (_ptr(ends), int(w), _ptr(idx), _ptr(o_k), _ptr(d_k), _ptr(t_k), _ptr(ws), ws.numel(), _stream())
+    if grid is not None and grid.contraction is not None:
+        center, radius = grid.contraction
+        c = (ctypes.c_float * 3)(*center)
+        check(L.sparf_contracted_append(*head, _ptr(grid.bits), int(grid.res), c, float(radius), *tail), "contracted_append")
+    elif grid is not None:
+        check(L.sparf_termination_append(*head, _ptr(grid.bits), int(grid.res), float(grid.range[0]), float(grid.range[1]),
+                                         *tail), "termination_append")
+    else:
+        check(L.sparf_termination_append(*head, None, 0, 0.0, 1.0, *tail), "termination_append")
+
+
+class TerminatedMLPFunction(torch.autograd.Function):
+    """mlp_forward with early ray termination in windows, on top of an optional occupancy grid, with gradients and
+    without a host round trip.  Each window appends its kept samples (alive rays, grid-kept samples) to one compacted
+    set per pass, rows [ends[w], ends[w+1]), and runs the taped forward over that device-side span into one tape; the
+    backward is one taped backward over rows [0, ends[W]).  Only W = ceil(S / window) is known on the host, so the op
+    is capturable into a CUDA graph."""
+
+    @staticmethod
+    @_on_tensor_device
+    def forward(ctx, spec: MLPSpec, engine: int, grid, tau_max: float, window: int, origins, dirs, t, noise, progress,
+                *params):
+        L = _lib.lib()
+        o, d, tt = _f32c(origins), _f32c(dirs), _f32c(t)
+        R, S = tt.shape
+        assert o.shape == (R, 3) and d.shape == (R, 3)
+        C, dev = R * S, tt.device
+        ctx.C = C
+        m, keep = spec.fill(params, progress)
+        tape_bytes = L.sparf_mlp_tape_bytes(ctypes.byref(m), engine, C, 1) if C else 0
+        if C and not tape_bytes:
+            raise RuntimeError("mlp_forward_terminated: no tape for %d samples (a tape above 16 GB); use smaller batches" % C)
+        sigma = torch.zeros(R, S, device=dev)
+        rgb = torch.zeros(R, S, 3, device=dev)
+        if C == 0:
+            return sigma, rgb
+        W = -(-S // window)
+        cap = R * min(window, S)
+        ends = torch.zeros(W + 1, dtype=torch.int64, device=dev)
+        alive = torch.ones(R, dtype=torch.uint8, device=dev)
+        tau = torch.zeros(R, device=dev)
+        idx = torch.empty(C, dtype=torch.int64, device=dev)
+        o_k, d_k, t_k = torch.empty(C, 3, device=dev), torch.empty(C, 3, device=dev), torch.empty(C, 1, device=dev)
+        noise_c = _f32c(noise) if noise is not None else None     # drawn dense by the caller, taken at the kept samples
+        noise_k = torch.empty(C, 1, device=dev) if noise is not None else None
+        sigma_k, rgb_k = torch.empty(C, 1, device=dev), torch.empty(C, 1, 3, device=dev)
+        tape = torch.empty(tape_bytes, dtype=torch.uint8, device=dev)
+        for w in range(W):
+            k0, k1 = w * window, min((w + 1) * window, S)
+            cw = R * (k1 - k0)
+            _window_append(grid, o, d, tt, k0, k1, alive, ends, w, idx, o_k, d_k, t_k)
+            if noise is not None:
+                check(L.sparf_compact_gather_span(cw, _ptr(ends), w, _ptr(idx), 1, _ptr(noise_c), _ptr(noise_k), _stream()),
+                      "compact_gather_span")
+            ws = _workspace(L.sparf_mlp_workspace_bytes(ctypes.byref(m), cap, 1, 0, engine), dev)
+            with _timed("mlp_forward"):
+                check(L.sparf_mlp_forward_tape_span(ctypes.byref(m), engine, C, cw, _row_ptr(ends, w), _row_ptr(ends, w + 1),
+                                                    _ptr(o_k), _ptr(d_k), _ptr(t_k), _ptr(noise_k), _ptr(sigma_k), _ptr(rgb_k),
+                                                    _ptr(tape), tape_bytes, _ptr(ws), ws.numel(), _stream()),
+                      "mlp_forward_tape_span")
+            check(L.sparf_compact_scatter_span(cw, _ptr(ends), w, _ptr(idx), 1, _ptr(sigma_k), _ptr(sigma), _stream()),
+                  "compact_scatter_span")
+            check(L.sparf_compact_scatter_span(cw, _ptr(ends), w, _ptr(idx), 3, _ptr(rgb_k), _ptr(rgb), _stream()),
+                  "compact_scatter_span")
+            if k1 < S:
+                check(L.sparf_termination_update(R, S, k0, k1, _ptr(sigma), _ptr(tt), _ptr(d), float(tau_max), _ptr(tau),
+                                                 _ptr(alive), _stream()), "termination_update")
+        ctx.spec, ctx.engine, ctx.progress, ctx.tape = spec, engine, progress, tape
+        ctx.shape, ctx.W = (R, S), W
+        ctx.param_refs = params if (ACCUMULATE_INTO_PARAM_GRAD[0] or
+                                    all(getattr(p, "_sparf_inplace_grad", False) for p in params)) else None
+        ctx.save_for_backward(ends, idx, o_k, d_k, t_k, sigma_k, rgb_k, *params)
+        return sigma, rgb
+
+    @staticmethod
+    @_on_tensor_device
+    def backward(ctx, g_sigma, g_rgb):
+        if ctx.C == 0 or ctx.tape is None:
+            return (None,) * 10 + tuple(None for _ in ctx.needs_input_grad[10:])
+        L = _lib.lib()
+        ends, idx, o_k, d_k, t_k, sigma_k, rgb_k, *params = ctx.saved_tensors
+        (R, S), W, C, dev = ctx.shape, ctx.W, ctx.C, t_k.device
+        K = _row_ptr(ends, W)       # every window's rows: [0, ends[W])
+        g_sigma_k, g_rgb_k = torch.empty(C, 1, device=dev), torch.empty(C, 1, 3, device=dev)
+        check(L.sparf_compact_gather(C, K, _ptr(idx), 1, _ptr(_f32c(g_sigma)), _ptr(g_sigma_k), _stream()), "compact_gather")
+        check(L.sparf_compact_gather(C, K, _ptr(idx), 3, _ptr(_f32c(g_rgb)), _ptr(g_rgb_k), _stream()), "compact_gather")
+        m, keep = ctx.spec.fill(params, ctx.progress)
+        grads, ret = _param_grads(ctx, params, dev)
+        gs = ctx.spec.grad_struct(grads)
+        need_o, need_d = ctx.needs_input_grad[5], ctx.needs_input_grad[6]
+        d_o_k = torch.zeros(C, 3, device=dev) if (need_o or need_d) else None
+        d_d_k = torch.zeros(C, 3, device=dev) if (need_o or need_d) else None
+        ws = _workspace(L.sparf_mlp_workspace_bytes(ctypes.byref(m), C, 1, 2, ctx.engine), dev)
+        with _timed("mlp_backward"):
+            check(L.sparf_mlp_backward_tape_rows(ctypes.byref(m), ctx.engine, C, 1, K, _ptr(o_k), _ptr(d_k), _ptr(t_k),
+                                                 _ptr(sigma_k), _ptr(rgb_k), _ptr(g_sigma_k), _ptr(g_rgb_k), ctypes.byref(gs),
+                                                 _ptr(d_o_k), _ptr(d_d_k), _ptr(ctx.tape), ctx.tape.numel(), _ptr(ws),
+                                                 ws.numel(), _stream()), "mlp_backward_tape_rows")
+        ctx.tape = None
+        d_o = d_d = None
+        if need_o:
+            d_o = torch.empty(R, 3, device=dev)
+            check(L.sparf_compact_ray_sum_segments(R, S, W, _ptr(ends), _ptr(idx), 3, _ptr(d_o_k), _ptr(d_o), _stream()),
+                  "compact_ray_sum_segments")
+        if need_d:
+            d_d = torch.empty(R, 3, device=dev)
+            check(L.sparf_compact_ray_sum_segments(R, S, W, _ptr(ends), _ptr(idx), 3, _ptr(d_d_k), _ptr(d_d), _stream()),
+                  "compact_ray_sum_segments")
+        return (None,) * 5 + (d_o, d_d) + (None,) * 3 + tuple(ret)
+
+
+def mlp_forward_terminated(spec: MLPSpec, origins, dirs, t, grid, eps: float, window: int, params: Sequence[torch.Tensor], *,
+                           noise=None, progress=None, engine: Optional[int] = None):
+    """mlp_forward (origins/dirs [R,3], t [R,S] -> sigma [R,S], rgb [R,S,3]) with early ray termination: the samples of
+    [k0, k0 + window) are evaluated for the rays still alive, and a ray dies once its optical depth exceeds fp32(-ln eps)
+    (the rule of the inference termination, termination.forward_samples, on this pass's own sigma, density noise
+    included); with `grid` (occupancy.OccupancyGrid, box or contracted; or None) only the samples it keeps are evaluated.
+    Every other sample gets sigma = 0, rgb = 0 and no gradient; the kept ones the bits of mlp_forward.  noise [R,S] is
+    drawn dense by the caller.  The call never synchronises with the host, so a training step that uses it can be
+    captured into a CUDA graph.  Differentiable w.r.t. origins, dirs, params; tensor-core engines only."""
+    eng = get_engine() if engine is None else engine
+    if eng == _lib.ENGINE_SIMT_FP32:
+        raise ValueError("mlp_forward_terminated: the simt_fp32 engine has no device-side row count; use tc_3x, tc_1x or "
+                         "tc_3x_w1")
+    if not (0 <= eps < 1) or int(window) != window or window < 1:
+        raise ValueError("mlp_forward_terminated: eps %r (0 <= eps < 1), window %r (an integer >= 1)" % (eps, window))
+    from .termination import tau_max
+    return TerminatedMLPFunction.apply(spec, eng, grid, tau_max(eps), int(window), origins, dirs, t, noise, progress, *params)
+
+
 def _param_grads(ctx, params, device):
     """Gradient destinations of a backward: the parameters' own `.grad` when the forward opted in and every one exists
     (then autograd gets None), else fresh zeroed tensors in one flat buffer.  -> (grads for the C ABI, grads to return)."""

@@ -205,11 +205,31 @@ class Graph(torch.nn.Module):
         assert 0 <= eps < 1 and int(window) == window >= 1, (eps, window)
         self._termination = (float(eps), int(window))
 
+    def set_training_termination(self, eps=1e-4, window=16):
+        """Stop evaluating a ray in training once its transmittance is below eps, checked every `window` samples
+        (termination.train_forward_samples): `render` in train and test-optim mode, with or without gradients, in the
+        coarse and the fine pass, on top of the training grid a pass has (set_training_occupancy) or alone.  The samples
+        skipped get σ = 0, rgb = 0 and no gradient; a step stays one CUDA graph.  None detaches.  Tensor-core engines
+        only.  set_early_termination (inference) and render_to_max are unaffected."""
+        if eps is None:
+            self._train_termination = None
+            return
+        if isinstance(eps, bool) or not isinstance(eps, (int, float)) or not 0 <= eps < 1:
+            raise ValueError("set_training_termination: eps %r (a number, 0 <= eps < 1)" % (eps,))
+        if isinstance(window, bool) or not isinstance(window, (int, np.integer)) or window < 1:
+            raise ValueError("set_training_termination: window %r (an integer >= 1)" % (window,))
+        self._train_termination = (float(eps), int(window))
+
     def _forward_samples(self, nerf, which, opt, center, ray, depth_samples, mode):
         """nerf.forward_samples, or in val / eval / test mode without gradients termination.forward_samples when early
         termination is set, occupancy.forward_samples when only grid `which` (0 coarse, 1 fine) is attached; in train and
-        test-optim mode occupancy.train_forward_samples when training grid `which` is attached"""
+        test-optim mode termination.train_forward_samples (with training grid `which`, if any) when training termination
+        is set, else occupancy.train_forward_samples when training grid `which` is attached"""
         train_grid = getattr(self, "_train_occupancy", (None, None))[which]
+        train_term = getattr(self, "_train_termination", None)
+        if train_term is not None and mode in ("train", "test-optim"):
+            from . import termination
+            return termination.train_forward_samples(nerf, train_grid, *train_term, opt, center, ray, depth_samples, mode)
         if train_grid is not None and mode in ("train", "test-optim"):
             from . import occupancy
             return occupancy.train_forward_samples(nerf, train_grid, opt, center, ray, depth_samples, mode)

@@ -14,6 +14,10 @@ move with the coarse weights, so its error is not bounded.  Each window reads it
 on this path cannot be captured into a CUDA graph.  Scenes whose rays mostly turn opaque gain; soft or small objects
 gain little, and so does inverse-depth sampling alone, which crowds the samples in front of the surface.  A contracted
 occupancy grid (sparf_b200.occupancy) skips those front samples, and termination on top of it skips the ones behind.
+
+Training steps can terminate too (train_forward_samples, Graph.set_training_termination): the same kept set on the
+pass's own σ (density noise included), with gradients, one tape and one backward per pass, and nothing read back on the
+host, so that a step stays one CUDA graph.
 """
 from __future__ import annotations
 
@@ -58,4 +62,21 @@ def forward_samples(nerf, grid, eps: float, window: int, center, ray, depth_samp
             rgb.index_copy_(0, idx, rgb_k.view(-1, 3))
         if k1 < S:
             ops.termination_update(sigma, t, d, k0, k1, limit, tau, alive)
+    return dict(rgb_samples=rgb.view(B, N, S, 3), density_samples=sigma.view(B, N, S))
+
+
+def train_forward_samples(nerf, grid, eps: float, window: int, opt, center, ray, depth_samples, mode) -> dict:
+    """NeRF.forward_samples with gradients and early ray termination (ops.mlp_forward_terminated), on top of the
+    training occupancy grid `grid` (box or contracted; or None): the samples behind an opaque point of the ray, and those
+    the grid skips, get σ = 0, rgb = 0 and no gradient; the others the values of the dense pass, with its density noise
+    (the same randn_like draw, taken at the kept samples).  A ray dies on this pass's own σ, noise included.  Nothing in
+    it synchronises, so a training step that calls it can be captured into one CUDA graph.  center, ray [B,N,3];
+    depth_samples [B,N,S,1] -> dict(rgb_samples [B,N,S,3], density_samples [B,N,S])."""
+    B, N, S = depth_samples.shape[:3]
+    t = depth_samples.reshape(B * N, S)
+    noise = None
+    if opt.nerf.density_noise_reg and mode == "train":
+        noise = (torch.randn_like(depth_samples[..., 0]).to(t.device) * opt.nerf.density_noise_reg).reshape(B * N, S)
+    sigma, rgb = ops.mlp_forward_terminated(nerf._spec(), center.reshape(B * N, 3), ray.reshape(B * N, 3), t, grid, eps,
+                                            window, nerf.kernel_params(), noise=noise, progress=nerf.progress)
     return dict(rgb_samples=rgb.view(B, N, S, 3), density_samples=sigma.view(B, N, S))

@@ -11,7 +11,9 @@ them.  Prints the photometric loss as it goes; `main()` returns (first_losses, l
 
 --grid RES trains with occupancy grids of RES^3 cells (Graph.set_training_occupancy), rebuilt from the student's weights
 every --grid-every steps between graph replays (occupancy.refresh_); `main()` then also returns the fraction of the
-training samples the grids keep at the end.
+training samples the grids keep at the end.  --term EPS adds early ray termination to the training steps
+(Graph.set_training_termination(EPS, --term-window)), alone or on top of the grids; the kept fraction is then returned
+as well.
 """
 import argparse
 import os
@@ -41,6 +43,9 @@ def main(argv=None):
     ap.add_argument("--grid", type=int, default=0, help="occupancy grids of RES^3 cells in the training steps (0: dense)")
     ap.add_argument("--grid-every", type=int, default=16, help="steps between grid refreshes")
     ap.add_argument("--grid-thres", type=float, default=0.01, help="density threshold of the grids")
+    ap.add_argument("--term", type=float, default=None, help="early ray termination at transmittance EPS in the training "
+                    "steps (default: off)")
+    ap.add_argument("--term-window", type=int, default=16, help="samples per termination window")
     ap.add_argument("--quiet", action="store_true")
     args = ap.parse_args(argv)
 
@@ -142,6 +147,8 @@ def main(argv=None):
         from sparf_b200 import occupancy
         grids = [occupancy.build_grid(opt, m, res=args.grid, thres=args.grid_thres) for m in net.get_network_components()]
         net.set_training_occupancy(*grids)
+    if args.term is not None:
+        net.set_training_termination(args.term, args.term_window)
 
     step = GraphedStep(iteration, (), warmup=2)
     losses = []
@@ -156,7 +163,7 @@ def main(argv=None):
     vals = torch.stack(losses).float().cpu()
     k = max(1, args.steps // 10)
     extra = ()
-    if grids:     # kept fraction of the last training batch's coarse samples (skipped samples have σ = 0 exactly)
+    if grids or args.term is not None:     # kept fraction of the coarse samples of a training batch (skipped: σ = 0 exactly)
         with torch.no_grad():
             out = net.render_image_at_specific_rays(opt, data, iter=0, ray_idx=sampler(opt.nerf.rand_rays), mode="train")
         extra = ((out["density_samples"] != 0).float().mean().item(),)
