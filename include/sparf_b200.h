@@ -407,6 +407,45 @@ int sparf_contracted_append(int64_t R, int32_t S, int32_t k0, int32_t k1, const 
                             float radius, int64_t* ends, int32_t w, int64_t* sample_idx, float* origins_k, float* dirs_k,
                             float* t_k, void* workspace, size_t workspace_bytes, sparf_stream_t stream);
 
+/* ---------------------------------------------------------------- occupancy grid update
+ * Keeping a box or contracted grid current inside a training step (sparf_b200/occupancy.py update_): each cell keeps a
+ * decaying density, a fixed budget of random cells is re-sampled and the bits are re-thresholded (Instant-NGP's
+ * update).  Its cost is set by the budget, not by res^3, and every size is fixed, so it can be captured in a CUDA graph.
+ *   density: fp32 [res^3], indexed by the cell's linear index like the bits.  occupancy.build_grid(ema=True) starts it
+ *            at the max over the cell's 8 corner lattice points of the build's sigma, NaN and +inf mapped to FLT_MAX;
+ *            the bits it builds are the dilated ones of sparf_occupancy_build.
+ *   interior: a box grid's every cell; a contracted grid's cells with every index in [2, res-3] (res >= 8).  The
+ *            contracted grid's outer two-cell shell is never sampled or changed and stays occupied.
+ *   sample:  N = n_uniform + n_occupied samples from u_cell [N] and u_jit [N,3] (fp32, in [0, 1)); I = the interior
+ *            cell count, K = the number of occupied interior cells in the bits before the update (kept on the device).
+ *            Sample i < n_uniform takes interior cell number min(floor((double)u_cell[i] * I), I-1) in increasing
+ *            linear index; sample i >= n_uniform the min(floor((double)u_cell[i] * K), K-1)-th occupied interior cell
+ *            in increasing linear index, or the uniform rule when K = 0.  Its cell (c_x, c_y, c_z) goes to cells[i]
+ *            (int64 linear index) and its point to points[i] (fp32 [N,3]), computed in fp64 with every op rounded to
+ *            nearest (no FMA) and rounded once to fp32:
+ *              box:        x_a = r0 + (c_a + u_jit[i,a]) * (r1 - r0) / res
+ *              contracted: v_a = -2 + (c_a + u_jit[i,a]) * 4 / res, n = ||v||_inf, x = center + radius * y with
+ *                          y = v (n <= 1) or v / (n (2 - n)): the world point of occupancy.contracted_warp.
+ *   ema:     with s_i = sigma[i] (NaN and +inf mapped to FLT_MAX), for every interior cell c
+ *              density[c] = max(__fmul_rn(decay, density[c]), max over {i: cells[i] = c} of s_i)
+ *            (cells with no sample just decay), then for every cell bits = !(density < thres), the contracted shell
+ *            always set.  sigma must be >= 0 or NaN (the softplus of the density query).  max is exact and order-
+ *            independent, so the result is deterministic bit for bit although duplicates combine through atomics.
+ * sparf_occupancy_sample: center = NULL for a box grid over [r0, r1]^3 (finite, r1 > r0), else a host float[3] of finite
+ * values read during the call (r0, r1 ignored; radius finite and > 0).  0 <= n_uniform, n_occupied <= 2^30; 1 <= res <=
+ * 4096.  Samples outside [0, 1) are clamped into the rules' ranges.  sparf_occupancy_ema: contracted != 0 for a
+ * contracted grid; 0 <= N <= 2^31; 0 < decay <= 1; cells outside [0, res^3) are ignored.  Both calls take one workspace
+ * of sparf_occupancy_sample_workspace_bytes(res) bytes (0 for an invalid res; the ema uses 4 B per cell of it, the
+ * sample about 4 B per 32 cells); the ema does not read what the sample left there.  No call synchronises; all are
+ * capturable. */
+size_t sparf_occupancy_sample_workspace_bytes(int32_t res);
+int sparf_occupancy_sample(int32_t res, const uint32_t* bits, float r0, float r1, const float* center, float radius,
+                           int64_t n_uniform, int64_t n_occupied, const float* u_cell, const float* u_jit, int64_t* cells,
+                           float* points, void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+int sparf_occupancy_ema(int32_t res, int32_t contracted, int64_t n, const int64_t* cells, const float* sigma, float decay,
+                        float thres, float* density, uint32_t* bits, void* workspace, size_t workspace_bytes,
+                        sparf_stream_t stream);
+
 /* ---------------------------------------------------------------- compositing
  * NeRF.composite (frequency_nerf.py:283-343).  Outputs: rgb_map [R,3], depth/opacity/depth_var/rgb_var
  * [R], weights [R,S], all_cumulated [R] (= T at sample S-2).  white_bg: rgb += 1 - opacity.

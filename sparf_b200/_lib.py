@@ -91,6 +91,10 @@ _SIGNATURES = {
                                          c_float, _P, _P, c_size_t, _P]),
     "sparf_contracted_emit": (c_int32, [c_int64, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, c_int32, POINTER(c_float),
                                         c_float, _P, _P, _P, _P, _P, c_size_t, _P]),
+    "sparf_occupancy_sample_workspace_bytes": (c_size_t, [c_int32]),
+    "sparf_occupancy_sample": (c_int32, [c_int32, _P, c_float, c_float, POINTER(c_float), c_float, c_int64, c_int64, _P, _P,
+                                         _P, _P, _P, c_size_t, _P]),
+    "sparf_occupancy_ema": (c_int32, [c_int32, c_int32, c_int64, _P, _P, c_float, c_float, _P, _P, _P, c_size_t, _P]),
     "sparf_composite_forward":(c_int32, [c_int32, c_int32, _P, _P, _P, _P, c_int32, _P, _P, _P, _P, _P, _P, _P, _P]),
     "sparf_composite_backward": (c_int32, [c_int32, c_int32, _P, _P, _P, _P, c_int32, _P, _P, _P, _P, _P, _P, _P, _P]),
     "sparf_huber2_fwd_bwd": (c_int32, [c_int64, _P, _P, c_float, _P, _P, _P]),

@@ -678,6 +678,51 @@ def occupancy_compact(bits, res: int, range, origins, dirs, t):
     return sample_idx, o_k, d_k, t_k
 
 
+@torch.no_grad()
+@_on_tensor_device
+def occupancy_sample(bits, res: int, range, contraction, n_uniform: int, n_occupied: int, u_cell, u_jit):
+    """The cells an occupancy-grid update re-samples and a jittered point in each -> (cells [N] int64 linear indices,
+    points [N,3] fp32), N = n_uniform + n_occupied: the first n_uniform drawn uniformly from the interior cells, the rest
+    from the occupied interior cells of `bits` (uniformly when none is), by u_cell [N] and u_jit [N,3] in [0, 1)
+    (semantics in include/sparf_b200.h).  contraction None: a box grid over range^3; (center, radius): a contracted
+    grid.  The occupied count stays on the device: nothing synchronises."""
+    L = _lib.lib()
+    n = int(n_uniform) + int(n_occupied)
+    uc, uj = _f32c(u_cell), _f32c(u_jit)
+    assert uc.shape == (n,) and uj.shape == (n, 3), "occupancy_sample: u_cell [N], u_jit [N,3]"
+    assert bits.dtype == torch.int32 and bits.is_contiguous() and bits.numel() == (res ** 3 + 31) // 32
+    dev = uc.device
+    cells = torch.empty(n, dtype=torch.int64, device=dev)
+    points = torch.empty(n, 3, device=dev)
+    if contraction is None:
+        r0, r1, c, radius = float(range[0]), float(range[1]), None, 0.0
+    else:
+        r0, r1, c, radius = 0.0, 0.0, (ctypes.c_float * 3)(*[float(v) for v in contraction[0]]), float(contraction[1])
+    ws = _workspace(L.sparf_occupancy_sample_workspace_bytes(int(res)), dev)
+    check(L.sparf_occupancy_sample(int(res), _ptr(bits), r0, r1, c, radius, int(n_uniform), int(n_occupied), _ptr(uc),
+                                   _ptr(uj), _ptr(cells), _ptr(points), _ptr(ws), ws.numel(), _stream()), "occupancy_sample")
+    return cells, points
+
+
+@torch.no_grad()
+@_on_tensor_device
+def occupancy_ema_(density, bits, res: int, contracted: bool, cells, sigma, decay: float, thres: float):
+    """In place on density (fp32 [res^3]) and bits: every interior cell's density becomes max(decay * density, the
+    largest sigma sampled in it), then bits = !(density < thres), a contracted grid's outer two-cell shell untouched and
+    occupied (semantics in include/sparf_b200.h).  cells [N] int64 and sigma [N] as occupancy_sample and the density
+    query give them.  Deterministic; nothing synchronises."""
+    L = _lib.lib()
+    s = _f32c(sigma).reshape(-1)
+    n = s.numel()
+    assert cells.dtype == torch.int64 and cells.is_contiguous() and cells.shape == (n,)
+    assert density.dtype == torch.float32 and density.is_contiguous() and density.numel() == res ** 3
+    assert bits.dtype == torch.int32 and bits.is_contiguous() and bits.numel() == (res ** 3 + 31) // 32
+    ws = _workspace(L.sparf_occupancy_sample_workspace_bytes(int(res)), density.device)
+    check(L.sparf_occupancy_ema(int(res), int(bool(contracted)), n, _ptr(cells), _ptr(s), float(decay), float(thres),
+                                _ptr(density), _ptr(bits), _ptr(ws), ws.numel(), _stream()), "occupancy_ema")
+    return density, bits
+
+
 # ------------------------------------------------------------------------------------------------
 # early ray termination (no gradient)
 # ------------------------------------------------------------------------------------------------

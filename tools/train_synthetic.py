@@ -11,7 +11,9 @@ them.  Prints the photometric loss as it goes; `main()` returns (first_losses, l
 
 --grid RES trains with occupancy grids of RES^3 cells (Graph.set_training_occupancy), rebuilt from the student's weights
 every --grid-every steps between graph replays (occupancy.refresh_); `main()` then also returns the fraction of the
-training samples the grids keep at the end.  --term EPS adds early ray termination to the training steps
+training samples the grids keep at the end.  --grid-update N keeps the grids current on the device instead: every
+--grid-every steps a CUDA graph of its own, captured once, replays occupancy.update_(grid, net, N, N) on each network
+(N cells drawn uniformly and N from the occupied ones, per-cell density decay 0.95), with no host-side rebuild.  --term EPS adds early ray termination to the training steps
 (Graph.set_training_termination(EPS, --term-window)), alone or on top of the grids; the kept fraction is then returned
 as well.
 """
@@ -41,7 +43,9 @@ def main(argv=None):
     ap.add_argument("--lr-pose", type=float, default=2e-3)
     ap.add_argument("--engine", default="auto", help="MLP engine (auto | tc_3x | tc_3x_w1 | simt_fp32)")
     ap.add_argument("--grid", type=int, default=0, help="occupancy grids of RES^3 cells in the training steps (0: dense)")
-    ap.add_argument("--grid-every", type=int, default=16, help="steps between grid refreshes")
+    ap.add_argument("--grid-every", type=int, default=16, help="steps between grid refreshes or updates")
+    ap.add_argument("--grid-update", type=int, default=0, help="N: update the grids on the device (occupancy.update_ "
+                    "with N uniform and N occupied cells, in a graph of its own) instead of rebuilding them (0: refresh_)")
     ap.add_argument("--grid-thres", type=float, default=0.01, help="density threshold of the grids")
     ap.add_argument("--term", type=float, default=None, help="early ray termination at transmittance EPS in the training "
                     "steps (default: off)")
@@ -145,15 +149,25 @@ def main(argv=None):
     grids = []
     if args.grid:     # built before the capture: the graph reads the grids' bits, which refresh_ rewrites in place
         from sparf_b200 import occupancy
-        grids = [occupancy.build_grid(opt, m, res=args.grid, thres=args.grid_thres) for m in net.get_network_components()]
+        grids = [occupancy.build_grid(opt, m, res=args.grid, thres=args.grid_thres, ema=bool(args.grid_update))
+                 for m in net.get_network_components()]
         net.set_training_occupancy(*grids)
+    grid_step = None
+    if grids and args.grid_update:
+
+        def grid_update():
+            for g, m in zip(grids, net.get_network_components()):
+                occupancy.update_(g, m, args.grid_update, args.grid_update)
+        grid_step = GraphedStep(grid_update, (), warmup=1)
     if args.term is not None:
         net.set_training_termination(args.term, args.term_window)
 
     step = GraphedStep(iteration, (), warmup=2)
     losses = []
     for it in range(args.steps):
-        if grids and it % args.grid_every == 0:
+        if grid_step is not None and it % args.grid_every == 0 and it > 0:
+            grid_step()
+        elif grids and grid_step is None and it % args.grid_every == 0:
             for g, m in zip(grids, net.get_network_components()):
                 occupancy.refresh_(g, opt, m)
         losses.append(step().clone())     # (the graph's output tensor is static: keep a copy of its value)
