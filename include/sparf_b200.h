@@ -130,7 +130,8 @@ int sparf_sample_depth(int32_t R, int32_t S, float near, float range, int32_t in
 
 /* Graph.sample_depth_from_pdf + cat + sort (renderer.py:421-456, :334-336).
  *   weights [R,S], t_coarse [R,S], u [S_fine] = mid-points of the shared grid, bins = linspace(near,far,S+1)
- *   outputs t_fine [R,S_fine] (may be NULL) and t_all [R,S+S_fine] ascending. */
+ *   outputs t_fine [R,S_fine] (may be NULL) and t_all [R,S+S_fine] ascending.
+ *   Limit: S + S_fine <= 4096 (one block per ray sorts S+S_fine values in shared memory); larger -> SPARF_ERR_INVALID. */
 int sparf_sample_pdf_merge(int32_t R, int32_t S, int32_t S_fine, float near, float far, const float* weights,
                            const float* t_coarse, const float* u, float* t_fine, float* t_all,
                            sparf_stream_t stream);
@@ -448,14 +449,16 @@ int sparf_occupancy_ema(int32_t res, int32_t contracted, int64_t n, const int64_
 
 /* ---------------------------------------------------------------- compositing
  * NeRF.composite (frequency_nerf.py:283-343).  Outputs: rgb_map [R,3], depth/opacity/depth_var/rgb_var
- * [R], weights [R,S], all_cumulated [R] (= T at sample S-2).  white_bg: rgb += 1 - opacity.
+ * [R], weights [R,S], all_cumulated [R] (= T at sample S-2).  white_bg: rgb += 1 - opacity.  S >= 2, no upper limit.
  */
 int sparf_composite_forward(int32_t R, int32_t S, const float* sigma, const float* rgb, const float* t,
                             const float* dirs, int32_t white_bg, float* rgb_map, float* depth,
                             float* opacity, float* depth_var, float* rgb_var, float* weights,
                             float* all_cumulated, sparf_stream_t stream);
 /* Grads of (rgb_map, depth, opacity[, weights]) -> d_sigma [R,S], d_rgb [R,S,3] (written, not
- * accumulated) and d_dirs [R,3] (+=, through the ray length; may be NULL).  g_weights may be NULL. */
+ * accumulated) and d_dirs [R,3] (+=, through the ray length; may be NULL).  Any of g_rgb_map / g_depth / g_opacity /
+ * g_weights may be NULL (that output has no gradient).  Limit: S <= 4096 (each ray keeps 2*S floats in shared memory;
+ * above S = 1536 the kernel opts into more than 48 KB); larger -> SPARF_ERR_INVALID. */
 int sparf_composite_backward(int32_t R, int32_t S, const float* sigma, const float* rgb, const float* t,
                              const float* dirs, int32_t white_bg, const float* g_rgb_map,
                              const float* g_depth, const float* g_opacity, const float* g_weights,

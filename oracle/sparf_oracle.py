@@ -173,18 +173,21 @@ def sample_depth_to_max(depth_max: Tensor, S: int, near: float) -> Tensor:
 
 
 def sample_pdf(weights: Tensor, S: int, S_fine: int, depth_range: Sequence[float],
-               grid: Optional[Tensor] = None) -> Tensor:
+               grid: Optional[Tensor] = None, u: Optional[Tensor] = None) -> Tensor:
     """Inverse-transform sampling of the coarse weights.   renderer.py:421-456.
     weights [B,R,S]; grid = the ONE shared (S_fine+1,) grid (linspace when deterministic, or the
-    recorded torch.rand(S_fine+1) draw).  Returns [B,R,S_fine]."""
+    recorded torch.rand(S_fine+1) draw); u = the (S_fine,) sample positions themselves, in place of the
+    grid's mid-points.  Returns [B,R,S_fine]."""
     near, far = depth_range[0], depth_range[1]   # torch.linspace takes the 0-dim tensors as they are
     dt = weights.dtype
     pdf = weights / (weights.sum(-1, keepdim=True) + 1e-6)
     cdf = torch.cat([torch.zeros_like(pdf[..., :1]), pdf.cumsum(-1)], dim=-1)      # [B,R,S+1]
-    if grid is None:
-        grid = torch.linspace(0, 1, S_fine + 1, device=weights.device, dtype=dt)
-    grid = grid.to(dt)
-    u = (0.5 * (grid[:-1] + grid[1:])).expand(*cdf.shape[:-1], S_fine).contiguous()
+    if u is None:
+        if grid is None:
+            grid = torch.linspace(0, 1, S_fine + 1, device=weights.device, dtype=dt)
+        grid = grid.to(dt)
+        u = 0.5 * (grid[:-1] + grid[1:])
+    u = u.to(dt).expand(*cdf.shape[:-1], S_fine).contiguous()
     idx = torch.searchsorted(cdf, u, right=True)
     lo = (idx - 1).clamp(min=0)
     hi = idx.clamp(max=S)
@@ -211,14 +214,14 @@ def c2f_weights(L: int, progress: float, barf_c2f, device=None, dtype=torch.floa
 
 
 def posenc(x: Tensor, L: int, mask: Optional[Tensor]) -> Tensor:
-    """[...,3] -> [...,6L]: per coordinate, L sines then L cosines, f_j = 2^j*pi (fp32 product of the
+    """[...,C] -> [...,2CL]: per coordinate, L sines then L cosines, f_j = 2^j*pi (fp32 product of the
     fp32 power of two and float(pi)); optional c2f mask per frequency.   frequency_nerf.py:47-69, :256."""
     freq = (2.0 ** torch.arange(L, dtype=torch.float32, device=x.device) * math.pi).to(x.dtype)
     spec = x[..., None] * freq                                           # [...,3,L]
     s, c = spec.sin(), spec.cos()
     if mask is not None:
         s, c = s * mask, c * mask
-    return torch.stack([s, c], dim=-2).reshape(*x.shape[:-1], 6 * L)
+    return torch.stack([s, c], dim=-2).reshape(*x.shape[:-1], 2 * x.shape[-1] * L)
 
 
 def mlp_forward(params: Dict[str, Tensor], pts: Tensor, ray: Tensor, *, L_3D: int = 10, L_view: int = 4,

@@ -134,7 +134,7 @@ __global__ void sample_depth_kernel(long long total, int S, float near, float ra
 
 // ------------------------------------------------------------------------------------------------
 // hierarchical resampling: Graph.sample_depth_from_pdf + cat + sort (renderer.py:421-456, 334-336)
-// one 128-thread block per ray; S, S_fine <= 1024
+// one 128-thread block per ray; S + S_fine <= 4096 (the sort buffer and the cdf live in shared memory)
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float linspace_at(float a, float b, float step, int steps, int i) {
   // torch.linspace: symmetric evaluation from both ends
@@ -390,7 +390,8 @@ __global__ void huber2_kernel(long long n, const float* __restrict__ pred, const
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     float z = pred[i] - target[i], az = fabsf(z);
     acc += az < delta ? 0.5f * z * z : delta * (az - 0.5f * delta);
-    if (d_pred) d_pred[i] = norm * (az < delta ? z : copysignf(delta, z));
+    // torch's clamp form: a NaN residual keeps a NaN gradient (a copysign of delta would hide it), +-inf gives +-delta
+    if (d_pred) d_pred[i] = norm * (z < -delta ? -delta : (z > delta ? delta : z));
   }
   acc = warp_sum(acc);
   __shared__ float red[32];
@@ -509,7 +510,9 @@ extern "C" int sparf_sample_depth(int32_t R, int32_t S, float near, float range,
 extern "C" int sparf_sample_pdf_merge(int32_t R, int32_t S, int32_t S_fine, float near, float far,
                                       const float* weights, const float* t_coarse, const float* u, float* t_fine,
                                       float* t_all, sparf_stream_t stream) {
-  SPARF_REQUIRE(R >= 0 && S > 0 && S_fine > 0 && S + S_fine <= 4096, "sample_pdf: bad sizes R=%d S=%d Sf=%d", R, S, S_fine);
+  SPARF_REQUIRE(R >= 0 && S > 0 && S_fine > 0, "sample_pdf: bad sizes R=%d S=%d Sf=%d", R, S, S_fine);
+  SPARF_REQUIRE(S <= 4096 - S_fine, "sample_pdf: S + S_fine = %lld exceeds the limit S + S_fine <= 4096",
+                (long long)S + S_fine);
   if (R == 0) return SPARF_OK;
   int npow2 = 1;
   while (npow2 < S + S_fine) npow2 <<= 1;
@@ -537,7 +540,8 @@ extern "C" int sparf_composite_backward(int32_t R, int32_t S, const float* sigma
                                         const float* dirs, int32_t white_bg, const float* g_rgb_map,
                                         const float* g_depth, const float* g_opacity, const float* g_weights,
                                         float* d_sigma, float* d_rgb, float* d_dirs, sparf_stream_t stream) {
-  SPARF_REQUIRE(R >= 0 && S >= 2 && S <= 4096, "composite: bad sizes R=%d S=%d", R, S);
+  SPARF_REQUIRE(R >= 0 && S >= 2, "composite: bad sizes R=%d S=%d", R, S);
+  SPARF_REQUIRE(S <= 4096, "composite_backward: S = %d exceeds the limit S <= 4096 (2*S floats of shared memory per ray)", S);
   if (R == 0) return SPARF_OK;
   size_t smem = (size_t)4 * 2 * S * sizeof(float);
   if (smem > 48 * 1024) {

@@ -917,11 +917,31 @@ def cached(tag: str, tensor: torch.Tensor, fn):
 
 
 def raygen(pose_w2c, intr, W: int, *, ray_idx=None, pixels=None):
-    """pose_w2c [B,3,4], intr [B,3,3] -> (center, ray) [B,n,3] at ray_idx ((n,)/(B,n) int) or float pixels."""
-    assert (ray_idx is None) != (pixels is None)
+    """pose_w2c [B,3,4], intr [B,3,3] (or [1,3,3] / [3,3], shared by the B poses) -> (center, ray) [B,n,3] at
+    ray_idx (int [n] / [1,n] shared, or [B,n] per image) or at float pixels ([n,2] / [1,n,2] shared, or [B,n,2]).
+    Any other shape raises ValueError before anything is launched."""
+    if (ray_idx is None) == (pixels is None):
+        raise ValueError("raygen: give exactly one of ray_idx / pixels")
+    if pose_w2c.dim() != 3 or tuple(pose_w2c.shape[1:]) != (3, 4):
+        raise ValueError("raygen: pose_w2c must be [B,3,4], got %s" % (tuple(pose_w2c.shape),))
+    B = pose_w2c.shape[0]
+    if not (tuple(intr.shape) == (3, 3) or (intr.dim() == 3 and intr.shape[0] in (1, B) and tuple(intr.shape[1:]) == (3, 3))):
+        raise ValueError("raygen: intr must be [B,3,3], [1,3,3] or [3,3] for B=%d poses, got %s" % (B, tuple(intr.shape)))
+    if pixels is not None:
+        if not (pixels.shape[-1:] == (2,) and (pixels.dim() == 2 or (pixels.dim() == 3 and pixels.shape[0] in (1, B)))):
+            raise ValueError("raygen: pixels must be [n,2], [1,n,2] or [B,n,2] for B=%d poses, got %s"
+                             % (B, tuple(pixels.shape)))
+        if pixels.dim() == 3 and pixels.shape[0] != B:
+            pixels = pixels[0]               # [1,n,2]: one list shared by the B images
+    else:
+        if not (ray_idx.dim() == 1 or (ray_idx.dim() == 2 and ray_idx.shape[0] in (1, B))):
+            raise ValueError("raygen: ray_idx must be [n], [1,n] or [B,n] for B=%d poses, got %s"
+                             % (B, tuple(ray_idx.shape)))
     # camera.py:318-319; intrinsics carry no gradient and are constant over training: invert once
     # (inv_ex: no host-side singularity check, i.e. no synchronisation)
     intr_inv = cached("Kinv", intr, lambda k: torch.linalg.inv_ex(k.detach().float()).inverse)
+    if intr_inv.dim() == 2 or intr_inv.shape[0] != B:
+        intr_inv = intr_inv.reshape(1, 3, 3).expand(B, 3, 3)   # the kernel reads one K^-1 per image
     return RayGenFunction.apply(pose_w2c, intr_inv, W, ray_idx, pixels)
 
 

@@ -295,29 +295,44 @@ def test_gradcheck_composite_fp32_vs_autograd():
         assert rel_err(gk, rk) < 2e-5
 
 
-@pytest.mark.parametrize("c2f", [None, (0.1, 0.5)])
-def test_standalone_posenc_matches_oracle(c2f):
+@pytest.mark.parametrize("C", [1, 3])
+@pytest.mark.parametrize("L", [1, 4, 10, 16])
+@pytest.mark.parametrize("c2f,progress", [(None, 0.3), ((0.1, 0.5), 0.3), ((0.0, 0.5), 0.25)])
+def test_standalone_posenc_matches_oracle(c2f, progress, L, C):
     """FrequencyEmbedder.__call__ / NeRF.positional_encoding as tensor ops (sparf_posenc_forward / _backward) vs the
-    oracle's restatement of frequency_nerf.py:47-69, 248-257: values to fp32 rounding of sin / cos at arguments up to
-    2^9 pi x, gradient w.r.t. the input vs autograd through the oracle formula in fp64."""
+    oracle's restatement of frequency_nerf.py:47-69, 248-257, for L bands of C channels (n * 2CL = 370CL values: never a
+    multiple of the 256-thread block).  c2f (0, 0.5) at progress 0.25 puts alpha = L/2, so for L >= 4 one band sits
+    exactly at alpha - j = 1 (weight 1) and the next at alpha - j = 0 (weight 0).
+    Yardstick (as in _error_vs_fp64): distance from the fp64 oracle within 4x the fp32 oracle's own distance.  Both
+    round the argument x * 2^j pi to fp32 alike, which dominates at the top band (~2^L pi |x| rad); floors: 8 unit
+    round-offs (2^-24) for the values, 64 of the largest entry for the input gradient (a sum over 2L terms)."""
     from oracle import sparf_oracle as O
     from sparf_b200.frequency_nerf import FrequencyEmbedder, NeRF
+    ulp = 2.0 ** -24
     opt = common.make_opt(barf_c2f=c2f)
     nerf = NeRF(opt).cuda()
-    nerf.progress.data.fill_(0.3)
+    nerf.progress.data.fill_(progress)
     g = torch.Generator(device="cuda").manual_seed(4)
-    x = ((torch.rand(5, 37, 3, device="cuda", generator=g) - 0.5) * 4).requires_grad_(True)
-    L = 10
+    x = ((torch.rand(5, 37, C, device="cuda", generator=g) - 0.5) * 4).requires_grad_(True)
     enc = nerf.positional_encoding(opt, x, FrequencyEmbedder(opt), L)
-    mask = O.c2f_weights(L, 0.3, c2f, device="cuda", dtype=torch.float64)
-    x64 = x.detach().double().requires_grad_(True)
-    ref = O.posenc(x64, L, mask)
-    assert enc.shape == ref.shape == (5, 37, 6 * L)
-    # the argument of the top band is ~3e3 rad: one fp32 ulp of the product is 2.4e-4 rad
-    assert (enc.double() - ref).abs().max().item() < 5e-4
     w = torch.randn(enc.shape, device="cuda", generator=g)
     (enc * w).sum().backward()
-    (ref * w.double()).sum().backward()
-    assert rel_err(x.grad, x64.grad) < 2e-3
+    refs = []
+    for dt in (torch.float64, torch.float32):
+        mask = O.c2f_weights(L, progress, c2f, device="cuda", dtype=dt)
+        xr = x.detach().to(dt).requires_grad_(True)
+        ref = O.posenc(xr, L, mask)
+        (ref * w.to(dt)).sum().backward()
+        refs.append((ref, xr.grad))
+    (ref64, gx64), (ref32, gx32) = refs
+    assert enc.shape == ref64.shape == (5, 37, 2 * C * L)
+    e_k, e_o = (enc.double() - ref64).abs().max().item(), (ref32.double() - ref64).abs().max().item()
+    assert e_k <= 4 * e_o + 8 * ulp, (e_k, e_o)
+    if c2f is not None and progress == 0.25 and L >= 4:
+        j = L // 2
+        assert (mask[j - 1] == 1).item() and (mask[j] == 0).item()
+        assert (enc[..., j] == 0).all() and (enc[..., L + j] == 0).all()
+    g_k, g_o = rel_err(x.grad, gx64), rel_err(gx32, gx64)
+    assert g_k <= 4 * g_o + 64 * ulp, (g_k, g_o)
     plain = FrequencyEmbedder(opt)(opt, x.detach(), 4)
     assert (plain.double() - O.posenc(x.detach().double(), 4, None)).abs().max().item() < 1e-5
