@@ -539,6 +539,10 @@ int sparf_tc_selftest_featgrad(const float* d_raw, const float* d_feat, const fl
  * caps the grid (else one CTA per SM). */
 int sparf_tc_selftest_wgrad(const float* G, const float* X, int32_t M, int32_t N, int32_t K, int32_t Kv, int32_t ldx,
                             int32_t div, int32_t passes, int32_t max_ctas, float* dW, uint32_t* bits, sparf_stream_t stream);
+/* The same GEMM with a device row count: M is a capacity, of which the GEMM sums the rows m < *rows (device, int64). */
+int sparf_tc_selftest_wgrad_rows(const float* G, const float* X, int32_t M, int32_t N, int32_t K, int32_t Kv, int32_t ldx,
+                                 int32_t div, int32_t passes, int32_t max_ctas, const int64_t* rows, float* dW,
+                                 uint32_t* bits, sparf_stream_t stream);
 /* The input-gradient GEMM's two ReLU masks against each other, 3-pass bf16: D = (X > 0) * (G W), G [M,N], W [N,K],
  * X [M,K] fp32 row-major, written only as its row and transposed images, once with the fp32 mask X and once with the
  * bits of X > 0 that the weight-gradient GEMM G^T X writes.  img gets, after a fill with 0xFFFF, the fp32-mask run's

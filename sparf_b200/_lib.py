@@ -110,6 +110,8 @@ _SIGNATURES = {
     "sparf_tc_selftest_featgrad": (c_int32, [_P, _P, _P, c_int32, c_int32, c_int32, c_int32, _P, _P, _P]),
     "sparf_tc_selftest_wgrad": (c_int32, [_P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
                                           _P, _P, _P]),
+    "sparf_tc_selftest_wgrad_rows": (c_int32, [_P, _P, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                               c_int32, _P, _P, _P, _P]),
     "sparf_tc_selftest_mask_bits": (c_int32, [_P, _P, _P, c_int32, c_int32, c_int32, c_int32, _P, _P]),
     "sparf_tc_selftest_chain": (c_int32, [_P, c_int32, c_int32, c_int32, c_int32, _P, _P, c_int32, c_int32, c_int32, c_int32,
                                           ctypes.c_uint32, _P, _P, _P, _P]),

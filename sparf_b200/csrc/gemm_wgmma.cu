@@ -550,8 +550,8 @@ __device__ __forceinline__ void produce(const Opnd& a, const Opnd& b, const Unit
 // fragment of the warpgroup's [64 x 128] block: acc[4 j + 2 h + c] is row 16 warp + lane/4 + 8 h, column
 // 8 j + 2 (lane % 4) + c.  One MMA group stays in flight: each warp releases a stage once the group that read it has
 // retired.  CONV (the staged weight-gradient GEMM): a stage is ready once its copies are complete (full) and its B
-// operand has been split in place (conv).
-template <bool F16, int PASSES, bool CONV = false>
+// operand has been split in place (conv).  NST: the ring's depth in stages.
+template <bool F16, int PASSES, bool CONV = false, int NST = STAGES>
 __device__ __forceinline__ void mma_unit(float (&acc)[64], int nk, int& it, uint64_t* full, uint64_t* empty,
                                          uint64_t* conv = nullptr) {
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -563,9 +563,9 @@ __device__ __forceinline__ void mma_unit(float (&acc)[64], int nk, int& it, uint
   for (int i = 0; i < (PASSES == 3 ? 64 : 1); ++i) acc_lo[i] = 0.f;
   if (nk <= 0) return;
   for (int j = 0; j < nk; ++j, ++it) {
-    const int s = it % STAGES;
-    mbar_wait(&full[s], (it / STAGES) & 1);
-    if constexpr (CONV) mbar_wait(&conv[s], (it / STAGES) & 1);
+    const int s = it % NST;
+    mbar_wait(&full[s], (it / NST) & 1);
+    if constexpr (CONV) mbar_wait(&conv[s], (it / NST) & 1);
     const uint8_t* st = smem + s * STAGE_BYTES;
     wgmma_fence();
 #pragma unroll
@@ -581,10 +581,10 @@ __device__ __forceinline__ void mma_unit(float (&acc)[64], int nk, int& it, uint
     }
     wgmma_commit();
     wgmma_wait_1();               // the MMAs of the previous k-step are done: its stage is free
-    if (j > 0 && lane == 0) mbar_arrive(&empty[(it + STAGES - 1) % STAGES]);
+    if (j > 0 && lane == 0) mbar_arrive(&empty[(it + NST - 1) % NST]);
   }
   wgmma_wait_all();
-  if (lane == 0) mbar_arrive(&empty[(it + STAGES - 1) % STAGES]);
+  if (lane == 0) mbar_arrive(&empty[(it + NST - 1) % NST]);
   if constexpr (PASSES == 3) {
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] += ldexpf(acc_lo[i], -LO_SHIFT);
@@ -874,7 +874,9 @@ struct Staged {
 };
 
 constexpr int STAGED_THREADS = CONSUMERS + 256;   // + the converter warpgroup (8-11) + the producer warpgroup (12-15)
-constexpr int STAGED_SMEM = STAGES * STAGE_BYTES + 3 * STAGES * 8;
+constexpr int STAGED_STAGES = 5;                  // one stage fewer than the other GEMMs: room for the partial tile
+constexpr int PART_BYTES = TM * TN * 4;           // the partial tile, [128 x 128] fp32
+constexpr int STAGED_SMEM = STAGED_STAGES * STAGE_BYTES + PART_BYTES + 3 * STAGED_STAGES * 8;
 
 // split8 with the lo half's scaling by 2^LO_SHIFT as a multiply: the same bytes (the scaling of the residual is exact,
 // it overflows to the same infinity, and NaN stays NaN), without the special-case code of ldexpf, which made up most of
@@ -897,7 +899,7 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 // The producer warp: per k-step, the A tile with one copy and the 32 rows m of B (X[m / div][128 bx, 128 bx + 128) in
 // fp32, 512 bytes per row at most) with one copy per lane, into the stage's 16 KB of B halves.  Rows at or past M are not
 // copied and the bytes past K of a row not written; the converter never reads either.
-template <int PASSES>
+template <int PASSES, int NST = STAGES>
 __device__ __forceinline__ void produce_staged(const Opnd& a, const Staged& x, const Units& w, uint64_t* full,
                                                uint64_t* empty) {
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -910,8 +912,8 @@ __device__ __forceinline__ void produce_staged(const Opnd& a, const Staged& x, c
     const int k0 = bx * TM;
     const uint32_t rbytes = 4 * min(TM, x.K - k0);
     for (int j = 0; j < nk; ++j, ++it) {
-      const int s = it % STAGES, m0 = (kt0 + j) * TK;
-      mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+      const int s = it % NST, m0 = (kt0 + j) * TK;
+      mbar_wait(&empty[s], ((it / NST) & 1) ^ 1);
       uint8_t* st = smem + s * STAGE_BYTES;
       if (lane == 0) {
         mbar_expect_tx(&full[s], abytes + min(TK, x.M - m0) * rbytes);
@@ -928,7 +930,7 @@ __device__ __forceinline__ void produce_staged(const Opnd& a, const Staged& x, c
 // bank conflicts), zero at or past M and K, and once the warpgroup has read the whole tile writes them in place as the
 // K-major image pack_kernel<TnB> makes (four 16-byte core-matrix rows per half), then hands the stage to the consumers
 // on conv[s].  Its warps also write the ReLU bits of units with by == 0 (one per (bx, k-step)): a ballot per row m.
-template <int PASSES>
+template <int PASSES, int NST = STAGES>
 __device__ __forceinline__ void convert_staged(const Staged& x, const Units& w, uint64_t* full, uint64_t* conv) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const int t = threadIdx.x - CONSUMERS, lane = t & 31;
@@ -939,8 +941,8 @@ __device__ __forceinline__ void convert_staged(const Staged& x, const Units& w, 
     const bool kin = bx * TM + t < x.K, bits = x.bits && by == 0;
     const int bword = bx * (TM / 32) + (t >> 5);
     for (int j = 0; j < nk; ++j, ++it) {
-      const int s = it % STAGES, m0 = (kt0 + j) * TK;
-      mbar_wait(&full[s], (it / STAGES) & 1);
+      const int s = it % NST, m0 = (kt0 + j) * TK;
+      mbar_wait(&full[s], (it / NST) & 1);
       uint8_t* st = smem + s * STAGE_BYTES + 2 * TILE_BYTES;
       const float* src = reinterpret_cast<const float*>(st);
       float v[TK];
@@ -980,9 +982,49 @@ __device__ __forceinline__ void convert_staged(const Staged& x, const Units& w, 
   }
 }
 
-// The weight-gradient GEMM dW += G^T X with B read as fp32 (Staged): wg_gemm_kernel's units, ring, MMAs and atomic
-// epilogue, with a fourth warpgroup that splits each stage's B in place between its copies and its MMAs, so no pack
-// kernel writes and no GEMM reads an image of X.  Registers: producer 40, converter 64, consumers 200 (<= 64 K).
+// Element (r, c) of the staged GEMM's partial tile, [128 rows x 128 columns] fp32 after the ring: the 8-column groups of
+// row r are permuted by r % 8, so that a warp's fragment stores (8 rows x one column group) and the flush's reads (32
+// columns of one row) are free of bank conflicts.
+__device__ __forceinline__ int part_off(int r, int c) { return r * TN + (((c >> 3) ^ (r & 7)) << 3) + (c & 7); }
+
+// The staged GEMM's epilogue of unit (bx, by).  A CTA's consecutive units of one output tile (with a grid that is a
+// multiple of the tile count, all of its units) sum their partial tiles in shared memory, in unit order, and the last
+// of them adds the sum to dW with one atomic per element: a warp's atomics cover 128 contiguous bytes of a row.  The
+// first unit stores its partial instead of adding it to zeros, which would turn -0 into +0.  Each warp stores, adds and
+// flushes the 16 rows of its own fragments, so only its own lanes share them.
+__device__ __forceinline__ void presum_epilogue(const float (&acc)[64], float* part, bool first, bool flush, int bx, int by,
+                                                const Epi& e) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int i = 0; i < 64; i += 2) {
+    float2* p = reinterpret_cast<float2*>(part + part_off(frag_row(i), frag_col(i)));
+    if (first) {
+      *p = make_float2(acc[i], acc[i + 1]);
+    } else {
+      const float2 o = *p;
+      *p = make_float2(o.x + acc[i], o.y + acc[i + 1]);
+    }
+  }
+  if (!flush) return;
+  __syncwarp();
+  const int m0 = by * TM, n0 = bx * TN;
+  float* out = e.out + e.col_off + n0;
+  for (int i = 0; i < 16; ++i) {
+    const int r = 16 * w + i, m = m0 + r;
+    if (m >= e.M) continue;
+#pragma unroll
+    for (int q = 0; q < TN / 32; ++q) {
+      const int c = 32 * q + lane, n = n0 + c;
+      if (n < e.N && n < e.Kv) atomicAdd(out + (size_t)m * e.ldo + c, part[part_off(r, c)]);
+    }
+  }
+  __syncwarp();                 // the tile has been read before the next unit's partial overwrites it
+}
+
+// The weight-gradient GEMM dW += G^T X with B read as fp32 (Staged): wg_gemm_kernel's units and MMAs on a ring of
+// STAGED_STAGES, with a fourth warpgroup that splits each stage's B in place between its copies and its MMAs, so no pack
+// kernel writes and no GEMM reads an image of X, and an epilogue that adds each CTA's partials of one tile once
+// (presum_epilogue).  Registers: producer 40, converter 64, consumers 200 (<= 64 K).
 // DYN: x.M is a capacity, of which live_rows rows are summed; the k-range split is gemm_units' for that count, computed
 // here from ctas (the CTAs gemm_units was given).
 template <int PASSES, bool DYN = false>
@@ -995,11 +1037,12 @@ __global__ void __launch_bounds__(STAGED_THREADS, 1) wg_gemm_staged_kernel(Opnd 
     w.nk = (x.M + TK - 1) / TK;
     w.nsplit = max(1, min(w.nk, (ctas + w.tiles - 1) / w.tiles * ((w.nk + 1023) / 1024)));
   }
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* empty = full + STAGES;
-  uint64_t* conv = empty + STAGES;
+  float* part = reinterpret_cast<float*>(smem + STAGED_STAGES * STAGE_BYTES);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGED_STAGES * STAGE_BYTES + PART_BYTES);
+  uint64_t* empty = full + STAGED_STAGES;
+  uint64_t* conv = empty + STAGED_STAGES;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) {
+    for (int i = 0; i < STAGED_STAGES; ++i) {
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], CONSUMERS / 32);
       mbar_init(&conv[i], 4);
@@ -1009,22 +1052,26 @@ __global__ void __launch_bounds__(STAGED_THREADS, 1) wg_gemm_staged_kernel(Opnd 
   __syncthreads();
   if (threadIdx.x >= CONSUMERS + 128) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
-    if (threadIdx.x < CONSUMERS + 128 + 32) produce_staged<PASSES>(a, x, w, full, empty);
+    if (threadIdx.x < CONSUMERS + 128 + 32) produce_staged<PASSES, STAGED_STAGES>(a, x, w, full, empty);
     return;
   }
   if (threadIdx.x >= CONSUMERS) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 64;\n" ::: "memory");
-    convert_staged<PASSES>(x, w, full, conv);
+    convert_staged<PASSES, STAGED_STAGES>(x, w, full, conv);
     return;
   }
   asm volatile("setmaxnreg.inc.sync.aligned.u32 200;\n" ::: "memory");
+  const int units = w.tiles * w.nsplit, grid = gridDim.x;
   int it = 0;
-  for (int u = blockIdx.x; u < w.tiles * w.nsplit; u += gridDim.x) {
+  for (int u = blockIdx.x; u < units; u += grid) {
     int bx, by, kt0, nk;
     w.get(u, bx, by, kt0, nk);
     float acc[64];
-    mma_unit<false, PASSES, true>(acc, nk, it, full, empty, conv);
-    epilogue<false, true, 0, 0>(acc, bx, by, e);
+    mma_unit<false, PASSES, true, STAGED_STAGES>(acc, nk, it, full, empty, conv);
+    const int t = u % w.tiles;
+    const bool first = u < grid || (u - grid) % w.tiles != t;
+    const bool flush = u + grid >= units || (u + grid) % w.tiles != t;
+    presum_epilogue(acc, part, first, flush, bx, by, e);
   }
 }
 
@@ -1860,23 +1907,35 @@ extern "C" int sparf_tc_selftest_images(const float* X, const float* W1, const f
   return selftest_images(X, W1, E, W2, M, Y, Z, db, 0, (cudaStream_t)stream);
 }
 
-extern "C" int sparf_tc_selftest_wgrad(const float* G, const float* X, int32_t M, int32_t N, int32_t K, int32_t Kv, int32_t ldx,
-                                       int32_t div, int32_t passes, int32_t max_ctas, float* dW, uint32_t* bits,
-                                       sparf_stream_t stream) {
+static int selftest_wgrad(const float* G, const float* X, int M, int N, int K, int Kv, int ldx, int div, int passes,
+                          int max_ctas, const int64_t* rows, float* dW, uint32_t* bits, cudaStream_t st) {
   SPARF_REQUIRE(M >= 1 && M <= (1 << 20) && N >= 1 && N <= 512 && K >= 1 && K <= 512 && Kv >= 0 && Kv <= K && ldx >= K &&
                     div >= 1 && (passes == 1 || passes == 3),
                 "tc_selftest_wgrad: M=%d N=%d K=%d Kv=%d ldx=%d div=%d passes=%d", M, N, K, Kv, ldx, div, passes);
   SPARF_REQUIRE(G && X && dW, "tc_selftest_wgrad: NULL tensor");
-  cudaStream_t st = (cudaStream_t)stream;
   SPARF_CHECK_CUDA(cudaMemsetAsync(dW, 0, (size_t)N * K * sizeof(float), st));
   TcPrec p{false, passes};
   p.max_ctas = max_ctas;
   SPARF_TRY(alloc_images(std::max(tc_image_elems(N, M), tc_pack_elems(K, ceil_div(M, TK), 0)), st, p));
   const TcImage gt{p.pack_a, ceil_div(M, TK)};
   int rc = tc_pack_cols(p, M, N, G, N, gt, st);
+  p.rows = RowCount{rows, 0};
   if (!rc) rc = tc_gemm_tn(p, M, N, K, Kv, gt, X, ldx, div, dW, K, 0, bits, st);
   free_images(p, st);
   return rc;
+}
+
+extern "C" int sparf_tc_selftest_wgrad(const float* G, const float* X, int32_t M, int32_t N, int32_t K, int32_t Kv, int32_t ldx,
+                                       int32_t div, int32_t passes, int32_t max_ctas, float* dW, uint32_t* bits,
+                                       sparf_stream_t stream) {
+  return selftest_wgrad(G, X, M, N, K, Kv, ldx, div, passes, max_ctas, nullptr, dW, bits, (cudaStream_t)stream);
+}
+
+extern "C" int sparf_tc_selftest_wgrad_rows(const float* G, const float* X, int32_t M, int32_t N, int32_t K, int32_t Kv,
+                                            int32_t ldx, int32_t div, int32_t passes, int32_t max_ctas, const int64_t* rows,
+                                            float* dW, uint32_t* bits, sparf_stream_t stream) {
+  SPARF_REQUIRE(rows, "tc_selftest_wgrad_rows: NULL row count");
+  return selftest_wgrad(G, X, M, N, K, Kv, ldx, div, passes, max_ctas, rows, dW, bits, (cudaStream_t)stream);
 }
 
 extern "C" int sparf_tc_selftest_mask_bits(const float* G, const float* W, const float* X, int32_t M, int32_t N, int32_t K,

@@ -5,7 +5,10 @@ network: K = 256 (trunk layers, the colour head's features), 64 (the position en
   staged: X with 16-byte aligned rows, split inside the GEMM (wg_gemm_staged_kernel);
   packed: X copied to rows of K + 1 floats, which the bulk copies cannot read: pack_kernel<TnB> + wg_gemm_kernel.
 Device time per call from torch.profiler over repeated calls after a warm-up (sparf_tc_selftest_wgrad; its transposed
-image of G and its memsets are not counted).
+image of G and its memsets are not counted).  Beside the times, each shape's bounds from the data sheet of the H100 SXM:
+  HBM: the transposed image of G (2 bytes per value and pass, N padded to 128-row tiles) and X in fp32, at 3.35 TB/s;
+  MMA: the products of the passes at 989 dense bf16 TFLOP/s, N x K per row with K padded to the 128-wide B tile (the
+  products the GEMM issues; K = 64 and 32 half- or quarter-fill it).
 Usage: [SPARF_TW_PASSES=3|1] python tools/time_wgrad.py [calls]"""
 import ctypes
 import os
@@ -21,6 +24,8 @@ from torch.profiler import ProfilerActivity, profile
 from sparf_b200 import _lib
 
 M = 131072
+HBM_PEAK = 3.35e12      # H100 SXM data sheet, bytes/s
+MMA_PEAK = 989e12       # dense bf16 FLOP/s, same source
 SHAPES = [(256, 256, 1), (256, 128, 1), (64, 256, 1), (64, 128, 1), (32, 256, 128), (32, 128, 128)]   # K, N, div
 
 
@@ -37,10 +42,12 @@ def main():
                                                                            passes, calls))
     stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     g = torch.Generator(device="cuda").manual_seed(0)
-    print("%5s %5s %5s | %10s %10s %10s | %10s | %6s" % ("K", "N", "div", "pack us", "gemm us", "sum us", "staged us",
-                                                         "ratio"))
+    print("%5s %5s %5s | %8s %8s | %10s %10s %10s | %10s | %6s" % ("K", "N", "div", "HBM us", "MMA us", "pack us",
+                                                                     "gemm us", "sum us", "staged us", "ratio"))
     for K, N, div in SHAPES:
         rows = -(-M // div)
+        hbm = (M * -(-N // 128) * 128 * 2 * (2 if passes == 3 else 1) + rows * K * 4) / HBM_PEAK * 1e6
+        mma = passes * 2.0 * M * N * -(-K // 128) * 128 / MMA_PEAK * 1e6
         G = torch.randn(M, N, device="cuda", generator=g)
         X = torch.randn(rows, K, device="cuda", generator=g)
         Xodd = torch.empty(rows, K + 1, device="cuda")
@@ -72,8 +79,8 @@ def main():
                 elif "pack_kernel" in ev.name and "TnB" in ev.name:
                     t["pack"] += ev.device_time / calls
         packed = t["pack"] + t["gemm"]
-        print("%5d %5d %5d | %10.1f %10.1f %10.1f | %10.1f | %6.3f" % (K, N, div, t["pack"], t["gemm"], packed,
-                                                                      t["staged"], t["staged"] / packed))
+        print("%5d %5d %5d | %8.1f %8.1f | %10.1f %10.1f %10.1f | %10.1f | %6.3f" % (
+            K, N, div, hbm, mma, t["pack"], t["gemm"], packed, t["staged"], t["staged"] / packed))
 
 
 if __name__ == "__main__":
