@@ -300,6 +300,54 @@ int sparf_mcubes_emit(const float* vol, int64_t nx, int64_t ny, int64_t nz, floa
  * so two cells sharing a face cut it the same way. */
 int sparf_mcubes_table(int8_t* table);
 
+/* ---------------------------------------------------------------- sparse marching cubes
+ * The mesh of the same lattice as above for res large enough that the dense volume does not fit, with the density
+ * evaluated only in blocks near the surface (sparf_b200/mesh.py, extract_mesh_sparse).
+ *   lattice:   BARF's, [res+1]^3 points over axis [res+1] (fp32, host-computed linspace(r0, r1, res+1); axis 0 = x).
+ *              res is a multiple of B = SPARF_MCUBES_BLOCK = 8 in [8, 8192].  Block b = (bi, bj, bk), nb = res / 8 per
+ *              axis, linear index (bi*nb + bj)*nb + bk, owns the lattice points [8b, 8b+8] on each axis ((B+1)^3 = 729,
+ *              faces shared with its neighbours) and the 8^3 cells between them.
+ *   coarse:    sigma [nb+1]^3 at the lattice points whose indices are all multiples of 8 (axis[::8]).
+ *   active:    block b is active iff the coarse points with indices [b-1, b+2] per axis, clipped to [0, nb], contain a
+ *              NaN, or both a value >= iso and a value < iso (the occupancy build's dilation-1 window, over blocks).
+ *              A feature smaller than a block that no coarse point of a window sees is missed: this is the trade-off
+ *              against the dense extractor.
+ *   output:    the dense mesh (sparf_mcubes_count / _emit) of the full lattice without the triangles of cells in
+ *              inactive blocks and without the vertices no remaining triangle uses; the remaining vertices keep their
+ *              order (linear index of the owner point p, then axis) and are renumbered 0, 1, ...; positions, triangle
+ *              order and orientation are the dense ones.  So when every cell with a crossing lies in an active block,
+ *              the output is byte-identical to the dense one.  Deterministic; 64-bit ids.
+ * Classification: sparf_mcubes_sparse_classify reads coarse and writes slots [nb^3] (int32: -1 for an inactive block,
+ * else the block's rank among the active blocks in linear order) and n_active (device int64).  The caller reads
+ * n_active; sparf_mcubes_sparse_blocks then writes block_ids [n_active] (int64, increasing).  Workspace:
+ * sparf_mcubes_sparse_workspace_bytes(res, 0, 0).
+ * Points: sparf_mcubes_sparse_points writes points [n_blocks * 729][3] for the active blocks [b0, b0 + n_blocks): per
+ * block its 729 points, k fastest, point (i, j, k) = (axis[i], axis[j], axis[k]).  axis is a device copy.
+ * Marching cubes: sigma_blocks [n_active][9][9][9] (fp32; the density at those points), slots and block_ids as above.
+ * sparf_mcubes_sparse_count writes totals [2] = {V, F} (device int64) with a workspace of
+ * sparf_mcubes_sparse_workspace_bytes(res, n_active, 0) bytes.  sparf_mcubes_sparse_emit writes verts [V][3] (fp32,
+ * index space) and faces [F][3] (int64) into buffers of max_verts and max_faces rows, with a workspace of
+ * sparf_mcubes_sparse_workspace_bytes(res, n_active, max_verts) bytes; it recomputes what it needs and takes nothing
+ * from count but the caller's capacities, so max_verts >= V and F <= max_faces <= 2560 n_active (5 triangles per
+ * cell) are required; rows past the capacities are never written.  Both are capturable and neither synchronises.
+ * Workspace: the larger of 4 B per block (the classification's flags) and 8 B x (2 + 128) per active block + 44 B per
+ * vertex of capacity, plus scan / sort scratch; 0 for invalid sizes (res, n_active > nb^3, 64 n_active or max_verts
+ * >= 2^31) and where no CUDA device is current (the scratch is sized for the device).  Invalid arguments give
+ * SPARF_ERR_INVALID.  sparf_mcubes_sparse_blocks needs no call when n_active is 0. */
+#define SPARF_MCUBES_BLOCK 8
+size_t sparf_mcubes_sparse_workspace_bytes(int32_t res, int64_t n_active, int64_t max_verts);
+int sparf_mcubes_sparse_classify(const float* coarse, int32_t res, float iso, int32_t* slots, int64_t* n_active,
+                                 void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+int sparf_mcubes_sparse_blocks(const int32_t* slots, int32_t res, int64_t* block_ids, sparf_stream_t stream);
+int sparf_mcubes_sparse_points(const float* axis, int32_t res, const int64_t* block_ids, int64_t b0, int64_t n_blocks,
+                               float* points, sparf_stream_t stream);
+int sparf_mcubes_sparse_count(const float* sigma_blocks, int32_t res, const int32_t* slots, const int64_t* block_ids,
+                              int64_t n_active, float iso, int64_t* totals, void* workspace, size_t workspace_bytes,
+                              sparf_stream_t stream);
+int sparf_mcubes_sparse_emit(const float* sigma_blocks, int32_t res, const int32_t* slots, const int64_t* block_ids,
+                             int64_t n_active, float iso, int64_t max_verts, int64_t max_faces, float* verts,
+                             int64_t* faces, void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+
 /* ---------------------------------------------------------------- occupancy grid
  * Empty-space skipping for inference renders (sparf_b200/occupancy.py): a bitfield over the box [r0, r1]^3 split into
  * res^3 cells, built from the density lattice sigma [res+1]^3 of mesh.density_grid (lattice point (a,b,c) at

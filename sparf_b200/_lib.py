@@ -10,6 +10,7 @@ from . import build as _build
 
 MAX_TRUNK = 12
 MCUBES_MAX_TRIS = 5     # SPARF_MCUBES_MAX_TRIS: a row of the marching-cubes case table holds 3 * 5 edge ids
+MCUBES_BLOCK = 8        # SPARF_MCUBES_BLOCK: cells per block edge of sparse marching cubes
 
 ENGINE_AUTO, ENGINE_SIMT_FP32, ENGINE_TC_3X, ENGINE_TC_1X, ENGINE_TC_3X_W1 = 0, 1, 2, 3, 4
 ENGINES = {"auto": 0, "simt_fp32": 1, "tc_3x": 2, "tc_1x": 3, "tc_3x_w1": 4}
@@ -72,6 +73,13 @@ _SIGNATURES = {
     "sparf_mcubes_count": (c_int32, [_P, c_int64, c_int64, c_int64, c_float, _P, _P, c_size_t, _P]),
     "sparf_mcubes_emit": (c_int32, [_P, c_int64, c_int64, c_int64, c_float, _P, _P, _P, c_size_t, _P]),
     "sparf_mcubes_table": (c_int32, [_P]),
+    "sparf_mcubes_sparse_workspace_bytes": (c_size_t, [c_int32, c_int64, c_int64]),
+    "sparf_mcubes_sparse_classify": (c_int32, [_P, c_int32, c_float, _P, _P, _P, c_size_t, _P]),
+    "sparf_mcubes_sparse_blocks": (c_int32, [_P, c_int32, _P, _P]),
+    "sparf_mcubes_sparse_points": (c_int32, [_P, c_int32, _P, c_int64, c_int64, _P, _P]),
+    "sparf_mcubes_sparse_count": (c_int32, [_P, c_int32, _P, _P, c_int64, c_float, _P, _P, c_size_t, _P]),
+    "sparf_mcubes_sparse_emit": (c_int32, [_P, c_int32, _P, _P, c_int64, c_float, c_int64, c_int64, _P, _P, _P, c_size_t,
+                                           _P]),
     "sparf_occupancy_build": (c_int32, [_P, c_int32, c_float, _P, _P]),
     "sparf_occupancy_workspace_bytes": (c_size_t, [c_int64, c_int32]),
     "sparf_occupancy_count": (c_int32, [c_int64, c_int32, _P, _P, _P, _P, c_int32, c_float, c_float, _P, _P, c_size_t, _P]),

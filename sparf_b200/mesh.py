@@ -127,6 +127,66 @@ def extract_mesh(opt, nerf, normals: bool = False, engine=None) -> dict:
     return out
 
 
+BLOCK = _lib.MCUBES_BLOCK       # cells per block edge of extract_mesh_sparse
+
+
+def check_sparse_res(res: int) -> None:
+    if res < BLOCK or res % BLOCK:
+        raise ValueError("sparse mesh extraction needs res to be a positive multiple of %d (got %d)" % (BLOCK, res))
+
+
+@torch.no_grad()
+def coarse_density(nerf, axis: torch.Tensor, engine=None) -> torch.Tensor:
+    """sigma [nb+1]^3 at the lattice points whose indices are all multiples of BLOCK: lattice_density over axis[::BLOCK],
+    so the values are density_grid's at those points bit for bit"""
+    return lattice_density(nerf, axis[::BLOCK], engine=engine)
+
+
+@torch.no_grad()
+def block_density(nerf, axis: torch.Tensor, block_ids: torch.Tensor, engine=None) -> torch.Tensor:
+    """sigma [n_active, 9, 9, 9] at the points of the given blocks (ops.mcubes_sparse_points), in slabs of about
+    SLAB_POINTS points; each point is evaluated as density_grid evaluates it (same fp32 input, rows independent)"""
+    dev = nerf.progress.device
+    t = axis.to(dev)
+    P = BLOCK + 1
+    n = block_ids.numel()
+    sigma = torch.empty(n, P, P, P, device=dev, dtype=torch.float32)
+    spec, trunk = nerf._spec(), _trunk(nerf)
+    per = max(1, SLAB_POINTS // P ** 3)
+    for b0 in range(0, n, per):
+        nblk = min(per, n - b0)
+        pts = ops.mcubes_sparse_points(t, block_ids, b0, nblk)
+        raw, _ = ops.density_forward(spec, pts, trunk, progress=nerf.progress.detach(), engine=_engine(engine),
+                                     features=False)
+        sigma[b0:b0 + nblk] = torch.nn.functional.softplus(raw).view(nblk, P, P, P)
+    return sigma
+
+
+def extract_mesh_sparse(opt, nerf, normals: bool = False, engine=None, stats=None) -> dict:
+    """extract_mesh for high lattice resolutions: the density only in the 8^3-cell blocks near the surface.  A coarse pass
+    over every 8th lattice point marks the active blocks (include/sparf_b200.h: a NaN or both sides of the iso value in
+    the block's dilated window), the fine pass evaluates the 729 points of each active block, and marching cubes runs
+    over those blocks.  The result is extract_mesh's mesh without the triangles of inactive blocks (and the vertices
+    only they used); it equals extract_mesh's whenever every cell the surface crosses is in an active block.  A feature
+    smaller than a block that no coarse point sees can be missed.  opt.trimesh.res must be a multiple of 8 (ValueError
+    otherwise).  stats: an optional dict that receives n_blocks, n_active and points_evaluated."""
+    res, rng, thres = trimesh_settings(opt)
+    check_sparse_res(res)
+    axis = lattice_axis(res, rng)
+    slots, block_ids = ops.mcubes_sparse_classify(coarse_density(nerf, axis, engine=engine), thres)
+    sigma = block_density(nerf, axis, block_ids, engine=engine)
+    verts, faces = ops.marching_cubes_sparse(sigma, res, slots, block_ids, thres)
+    if stats is not None:
+        nb = res // BLOCK
+        stats.update(n_blocks=nb ** 3, n_active=block_ids.numel(),
+                     points_evaluated=(nb + 1) ** 3 + block_ids.numel() * (BLOCK + 1) ** 3)
+    del sigma
+    out = dict(vertices=to_world(verts, res, rng), faces=faces)
+    if normals:
+        out["normals"] = density_normals(nerf, out["vertices"], engine=engine)
+    return out
+
+
 def write_ply(path, vertices, faces, normals=None) -> None:
     """Binary little-endian PLY: float x, y, z (and nx, ny, nz) per vertex, a uchar-counted int list per face"""
     as_np = lambda x: x.detach().cpu().numpy() if torch.is_tensor(x) else np.asarray(x)

@@ -634,6 +634,75 @@ def marching_cubes(vol, iso: float):
     return verts, faces
 
 
+@torch.no_grad()
+@_on_tensor_device
+def mcubes_sparse_classify(coarse, iso: float):
+    """Coarse density [nb+1]^3 (the lattice points at multiples of SPARF_MCUBES_BLOCK) -> (slots [nb^3] int32, -1 or
+    the block's rank; block_ids [n_active] int64, the active blocks in linear order).  A block is active iff its
+    coarse window (indices [b-1, b+2] per axis, clipped) holds a NaN or values on both sides of iso (include/sparf_b200.h).
+    One device-to-host copy: the active count."""
+    L = _lib.lib()
+    c = _f32c(coarse)
+    assert c.dim() == 3 and c.shape[0] == c.shape[1] == c.shape[2] >= 2, "mcubes_sparse_classify takes an [nb+1]^3 lattice"
+    res = (c.shape[0] - 1) * _lib.MCUBES_BLOCK
+    ws = torch.empty(max(L.sparf_mcubes_sparse_workspace_bytes(res, 0, 0), 1), dtype=torch.uint8, device=c.device)
+    slots = torch.empty((res // _lib.MCUBES_BLOCK) ** 3, dtype=torch.int32, device=c.device)
+    n_active = torch.empty(1, dtype=torch.int64, device=c.device)
+    check(L.sparf_mcubes_sparse_classify(_ptr(c), res, float(iso), _ptr(slots), _ptr(n_active), _ptr(ws), ws.numel(),
+                                         _stream()), "mcubes_sparse_classify")
+    block_ids = torch.empty(int(n_active.item()), dtype=torch.int64, device=c.device)
+    if block_ids.numel():       # no active block: nothing to list (and an empty tensor has no storage to pass)
+        check(L.sparf_mcubes_sparse_blocks(_ptr(slots), res, _ptr(block_ids), _stream()), "mcubes_sparse_blocks")
+    return slots, block_ids
+
+
+@torch.no_grad()
+@_on_tensor_device
+def mcubes_sparse_points(axis, block_ids, b0: int, n_blocks: int):
+    """The lattice points [n_blocks * 729, 3] of the active blocks block_ids[b0 : b0 + n_blocks] over the lattice axis
+    [res+1] (on the device): per block its (B+1)^3 points, k fastest."""
+    L = _lib.lib()
+    t = _f32c(axis)
+    res = t.numel() - 1
+    ids = block_ids.contiguous()
+    assert ids.dtype == torch.int64 and 0 <= b0 and b0 + n_blocks <= ids.numel()
+    pts = torch.empty(n_blocks * (_lib.MCUBES_BLOCK + 1) ** 3, 3, device=t.device, dtype=torch.float32)
+    check(L.sparf_mcubes_sparse_points(_ptr(t), res, _ptr(ids), int(b0), int(n_blocks), _ptr(pts), _stream()),
+          "mcubes_sparse_points")
+    return pts
+
+
+@torch.no_grad()
+@_on_tensor_device
+def marching_cubes_sparse(sigma_blocks, res: int, slots, block_ids, iso: float):
+    """Marching cubes over the active blocks only: sigma_blocks [n_active, 9, 9, 9] (the density at the points of
+    block_ids, as mcubes_sparse_points lays them out), slots / block_ids of mcubes_sparse_classify -> (verts [V, 3] fp32 in
+    index space, faces [F, 3] int64): the dense mesh of the [res+1]^3 lattice restricted to the cells of active blocks
+    (include/sparf_b200.h).  One device-to-host copy: the two totals that size the outputs.  Not differentiable."""
+    L = _lib.lib()
+    s = _f32c(sigma_blocks)
+    P = _lib.MCUBES_BLOCK + 1
+    n = block_ids.numel()
+    assert s.shape == (n, P, P, P), "marching_cubes_sparse takes sigma_blocks [n_active, 9, 9, 9]"
+    assert slots.dtype == torch.int32 and block_ids.dtype == torch.int64
+    assert res % _lib.MCUBES_BLOCK == 0 and slots.numel() == (res // _lib.MCUBES_BLOCK) ** 3, \
+        "marching_cubes_sparse: slots [%d] is not the block table of res %d" % (slots.numel(), res)
+    sl, ids = slots.contiguous(), block_ids.contiguous()
+    dev = s.device
+    ws = torch.empty(max(L.sparf_mcubes_sparse_workspace_bytes(res, n, 0), 1), dtype=torch.uint8, device=dev)
+    totals = torch.empty(2, dtype=torch.int64, device=dev)
+    check(L.sparf_mcubes_sparse_count(_ptr(s), res, _ptr(sl), _ptr(ids), n, float(iso), _ptr(totals), _ptr(ws),
+                                      ws.numel(), _stream()), "mcubes_sparse_count")
+    n_verts, n_faces = totals.tolist()
+    verts = torch.empty(n_verts, 3, device=dev, dtype=torch.float32)
+    faces = torch.empty(n_faces, 3, device=dev, dtype=torch.int64)
+    del ws
+    ws = torch.empty(max(L.sparf_mcubes_sparse_workspace_bytes(res, n, n_verts), 1), dtype=torch.uint8, device=dev)
+    check(L.sparf_mcubes_sparse_emit(_ptr(s), res, _ptr(sl), _ptr(ids), n, float(iso), n_verts, n_faces, _ptr(verts),
+                                     _ptr(faces), _ptr(ws), ws.numel(), _stream()), "mcubes_sparse_emit")
+    return verts, faces
+
+
 # ------------------------------------------------------------------------------------------------
 # occupancy grid (no gradient)
 # ------------------------------------------------------------------------------------------------

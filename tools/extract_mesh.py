@@ -3,12 +3,14 @@
 opt.trimesh, on the GPU).
 
     python tools/extract_mesh.py model.pth.tar --out mesh.ply [--network nerf|nerf_fine] [--res 128]
-                                 [--range -1.2 1.2] [--thres 25] [--normals] [--barf-c2f START END]
+                                 [--range -1.2 1.2] [--thres 25] [--normals] [--barf-c2f START END] [--sparse]
 
 The snapshot is what the reference's trainer saves (base_trainer.py:196-216): the model dict is ckpt["state_dict"],
 with the Graph's keys nerf.* / nerf_fine.* (or, from a joint pose trainer, those under "nerf_net").  The architecture
 is read from the tensor shapes.  The BARF mask applies at the snapshot's progress when --barf-c2f gives the schedule
-the model was trained with.  Prints V, F and the time of each phase.
+the model was trained with.  --sparse extracts with mesh.extract_mesh_sparse's phases (the density only in the 8^3-cell
+blocks near the surface; for high resolutions) and also prints the active-block count and the points evaluated.
+Prints V, F and the time of each phase.
 """
 import argparse
 import os
@@ -49,6 +51,7 @@ def main(argv=None):
     ap.add_argument("--thres", type=float, default=25.0)
     ap.add_argument("--normals", action="store_true")
     ap.add_argument("--barf-c2f", type=float, nargs=2, default=None)
+    ap.add_argument("--sparse", action="store_true", help="evaluate only the blocks near the surface (res: multiple of 8)")
     args = ap.parse_args(argv)
     assert torch.cuda.is_available(), "extract_mesh.py runs on a GPU"
     from sparf_b200 import mesh
@@ -77,8 +80,20 @@ def main(argv=None):
         return out
 
     phases["load"] = time.perf_counter() - t0
-    sigma = phase("density_grid", lambda: mesh.density_grid(opt, nerf))
-    verts, faces = phase("marching_cubes", lambda: mesh.marching_cubes(sigma, thres))
+    if args.sparse:
+        from sparf_b200 import ops
+        mesh.check_sparse_res(res)
+        axis = mesh.lattice_axis(res, rng)
+        coarse = phase("coarse", lambda: mesh.coarse_density(nerf, axis))
+        slots, ids = phase("classify", lambda: ops.mcubes_sparse_classify(coarse, thres))
+        sigma = phase("fine", lambda: mesh.block_density(nerf, axis, ids))
+        verts, faces = phase("marching_cubes", lambda: ops.marching_cubes_sparse(sigma, res, slots, ids, thres))
+        nb = res // mesh.BLOCK
+        print("active blocks %d of %d, points evaluated %d (dense lattice %d)"
+              % (ids.numel(), nb ** 3, coarse.numel() + sigma.numel(), (res + 1) ** 3))
+    else:
+        sigma = phase("density_grid", lambda: mesh.density_grid(opt, nerf))
+        verts, faces = phase("marching_cubes", lambda: mesh.marching_cubes(sigma, thres))
     del sigma
     verts = mesh.to_world(verts, res, rng)
     normals = phase("normals", lambda: mesh.density_normals(nerf, verts)) if args.normals else None
