@@ -256,8 +256,9 @@ int sparf_compact_ray_sum_segments(int64_t R, int32_t S, int32_t W, const int64_
  * not NULL, feat [M,width] = relu of the last trunk layer's feature rows.  The BARF mask applies as in the MLP entry
  * points.  These calls read no head tensor: SparfMLP.head_* and SparfMLPGrad.head_* may be NULL.  M may exceed 2^31;
  * M = 0 is a no-op.  Engines as for the MLP (AUTO: TC_3X on sm_90, else SIMT_FP32).
- * sparf_density_workspace_bytes: `backward` = 0 sparf_density_forward, 1 sparf_density_backward.  A forward without
- * feat skips the last layer's feature GEMM (the density row reads the layer below). */
+ * sparf_density_workspace_bytes: `backward` = 0 sparf_density_forward, 1 sparf_density_backward, 2
+ * sparf_density_gradient (never more than 1).  A forward without feat skips the last layer's feature GEMM (the density
+ * row reads the layer below). */
 size_t sparf_density_workspace_bytes(const SparfMLP* mlp, int64_t M, int32_t backward, int32_t engine);
 int sparf_density_forward(const SparfMLP* mlp, int32_t engine, int64_t M, const float* points, float* raw, float* feat,
                           void* workspace, size_t workspace_bytes, sparf_stream_t stream);
@@ -266,6 +267,15 @@ int sparf_density_forward(const SparfMLP* mlp, int32_t engine, int64_t M, const 
 int sparf_density_backward(const SparfMLP* mlp, int32_t engine, int64_t M, const float* points, const float* d_raw,
                            const float* d_feat, const SparfMLPGrad* grad, float* d_points, void* workspace,
                            size_t workspace_bytes, sparf_stream_t stream);
+/* The point gradient of the density: grad_points [M,3] (written, not added) = d raw / d x at each point, raw as
+ * sparf_density_forward computes it (no noise, the BARF mask at progress); normals are -grad_points / |grad_points|.
+ * It equals, bit for bit, the d_points sparf_density_backward adds to zeros for d_raw = 1 and d_feat = NULL, on every
+ * engine: the same input-gradient kernels on the same operand images, each ReLU mask H > 0 read from the recomputed fp32
+ * activations instead of the bits the weight-gradient GEMMs write.  It computes no weight or bias gradient (no
+ * SparfMLPGrad) and reads no head tensor.  M = 0 is a no-op; M may exceed 2^31.  Workspace:
+ * sparf_density_workspace_bytes(mlp, M, 2, engine). */
+int sparf_density_gradient(const SparfMLP* mlp, int32_t engine, int64_t M, const float* points, float* grad_points,
+                           void* workspace, size_t workspace_bytes, sparf_stream_t stream);
 
 /* ---------------------------------------------------------------- marching cubes
  * A triangle mesh of the iso-surface of a dense fp32 volume vol [nx][ny][nz] (row-major, k fastest), in index space,

@@ -69,6 +69,7 @@ _SIGNATURES = {
     "sparf_density_forward": (c_int32, [POINTER(SparfMLP), c_int32, c_int64, _P, _P, _P, _P, c_size_t, _P]),
     "sparf_density_backward": (c_int32, [POINTER(SparfMLP), c_int32, c_int64, _P, _P, _P, POINTER(SparfMLPGrad), _P, _P,
                                          c_size_t, _P]),
+    "sparf_density_gradient": (c_int32, [POINTER(SparfMLP), c_int32, c_int64, _P, _P, _P, c_size_t, _P]),
     "sparf_mcubes_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64]),
     "sparf_mcubes_count": (c_int32, [_P, c_int64, c_int64, c_int64, c_float, _P, _P, c_size_t, _P]),
     "sparf_mcubes_emit": (c_int32, [_P, c_int64, c_int64, c_int64, c_float, _P, _P, _P, c_size_t, _P]),

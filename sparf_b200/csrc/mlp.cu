@@ -419,6 +419,12 @@ __global__ void colsum_kernel(long long M, int N, int rows_per_block, const floa
   }
 }
 
+// out[i] = v: the density row's upstream gradient of the point-gradient query (d raw / d raw = 1)
+__global__ void fill_kernel(long long n, float v, float* __restrict__ out) {
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = v;
+}
+
 // G[i] = (feat[i] > 0) * d_feat[i]: the last trunk layer's gradient when the caller gives it (density backward)
 __global__ void relu_mask_kernel(long long total, const float* __restrict__ feat, const float* __restrict__ d_feat,
                                  float* __restrict__ G) {
@@ -557,8 +563,9 @@ static int validate_mlp(const SparfMLP* mlp) {
 }
 
 // The passes of the MLP calls.  The taped forward writes the activations to a caller-held tape that the taped backward
-// reads; the recompute backward recomputes them chunk by chunk.  The density calls run kForward and kRecomputeBackward.
-enum class Pass { kForward, kTapedForward, kRecomputeBackward, kTapedBackward };
+// reads; the recompute backward recomputes them chunk by chunk.  The density calls run kForward and kRecomputeBackward,
+// and kGradient: the recompute backward of the points' gradient alone, without weight gradients.
+enum class Pass { kForward, kTapedForward, kRecomputeBackward, kTapedBackward, kGradient };
 
 // Rows per chunk: the recompute backward keeps every trunk activation of its chunk, so it takes the smallest chunks; the
 // taped passes keep only a chunk's images and gradients (about 1 GB at 131072 rows of the default net) and take the
@@ -566,7 +573,8 @@ enum class Pass { kForward, kTapedForward, kRecomputeBackward, kTapedBackward };
 static int chunk_rows(Pass pass) {
   switch (pass) {
     case Pass::kForward: return 65536;
-    case Pass::kRecomputeBackward: return 32768;
+    case Pass::kRecomputeBackward:
+    case Pass::kGradient: return 32768;
     default: return 131072;
   }
 }
@@ -641,9 +649,12 @@ static Tape tape_chunk(const Tape& t, const MlpDims& d, int r0, int S) {
 // trunk gradients (a row image for the next input gradient, a transposed one for the weight gradient; no fp32 copy; see
 // grad_row), the colour-head gradient's two images (no fp32 copy either), the ReLU mask bits of one layer input (written
 // by its weight-gradient GEMM, read by its input-gradient GEMM), and a buffer for the weight operand packed per GEMM.
-// head = false (density calls, S = 1): no colour-head or view-direction buffer.
+// head = false (density calls, S = 1): no colour-head or view-direction buffer.  kGradient takes no more than
+// kRecomputeBackward: it keeps no last-layer features and no mask bits, and its transposed gradient images, which no
+// weight gradient reads, share one buffer; it adds a row of ones and, on the tensor cores, one row of bias sums.
 struct Ws {
   float *wts, *rgbv, *G0, *G1, *Genc, *Ghid, *gpre, *graw, *Gdtmp, *Gdenc;
+  float *ones, *colsum_sink;    // kGradient: the density row's upstream gradient (1 per row); bias sums nobody reads
   Tape act;     // the forward's activations of one chunk (forward and recompute backward)
   TcImage encimg, dencimg, Himg[2], Grow[2], Gtr[SPARF_MAX_TRUNK - 1], ghid_row, ghid_tr;
   TcImage wimg[SPARF_MAX_TRUNK];   // fused trunk forward: every trunk layer's weight image, alive at once
@@ -655,8 +666,9 @@ struct Ws {
 
 static size_t carve(const MlpDims& d, bool tc, int nrc, int S, Pass pass, bool head, char* base, Ws* out) {
   const size_t Mc = (size_t)nrc * S;
-  const bool fwd_here = pass == Pass::kForward || pass == Pass::kRecomputeBackward;   // the activations are not taped
-  const bool bwd = pass == Pass::kRecomputeBackward || pass == Pass::kTapedBackward;
+  const bool grad_only = pass == Pass::kGradient;
+  const bool fwd_here = pass == Pass::kForward || pass == Pass::kRecomputeBackward || grad_only;   // not taped
+  const bool bwd = pass == Pass::kRecomputeBackward || pass == Pass::kTapedBackward || grad_only;
   const bool chain = trunk_chained(d, tc);
   Carver cv{base, 0};
   Ws w{};
@@ -671,13 +683,14 @@ static size_t carve(const MlpDims& d, bool tc, int nrc, int S, Pass pass, bool h
     }
     // the backward keeps every layer; the forward ping-pongs, or keeps the last two only (the density row's input and
     // the colour head's) when the fused trunk leaves the others on the SM
-    const int nH = pass == Pass::kForward ? 2 : d.nt;
-    if (chain && nH == 2) {
+    const int nH = pass == Pass::kForward ? 2 : grad_only ? d.nt - 1 : d.nt;
+    if (chain && pass == Pass::kForward) {
       for (int l = d.nt - 2; l < d.nt; ++l) w.act.H[l] = cv.take(Mc * d.W);
     } else {
       for (int l = 0; l < nH; ++l) w.act.H[l] = cv.take(Mc * d.W);
       for (int l = nH; l < d.nt; ++l) w.act.H[l] = w.act.H[l & 1];
     }
+    if (grad_only) w.act.H[d.nt - 1] = nullptr;     // the point gradient needs no last-layer features
     for (int l = 0; chain && bwd && l < d.nt - 2; ++l) w.act.bits[l] = reinterpret_cast<uint32_t*>(cv.take(Mc * (d.W / 32)));
   }
   if (bwd && !tc) {
@@ -686,6 +699,7 @@ static size_t carve(const MlpDims& d, bool tc, int nrc, int S, Pass pass, bool h
   }
   if (bwd) {
     w.Genc = cv.take(Mc * d.E3p);
+    if (grad_only) w.ones = cv.take(Mc);
     if (!tc && head) {
       w.Ghid = cv.take(Mc * d.HW);
       w.gpre = cv.take(Mc * 4);
@@ -708,13 +722,16 @@ static size_t carve(const MlpDims& d, bool tc, int nrc, int S, Pass pass, bool h
   }
   if (tc && bwd) {
     for (TcImage& g : w.Grow) g = cv.image((int)Mc, d.W);
-    for (int i = 0; i < (chain ? d.nt - 1 : 2); ++i) w.Gtr[i] = cv.image(d.W, (int)Mc);
+    const int ntr = chain ? d.nt - 1 : 2;
+    for (int i = 0; i < (grad_only ? 1 : ntr); ++i) w.Gtr[i] = cv.image(d.W, (int)Mc);
+    for (int i = 1; grad_only && i < ntr; ++i) w.Gtr[i] = w.Gtr[0];
     for (int l = 1; chain && l <= d.nt - 2; ++l) w.nnimg[l] = cv.image(d.W, d.W);
     if (head) {
       w.ghid_row = cv.image((int)Mc, d.HW);
       w.ghid_tr = cv.image(d.HW, (int)Mc);
     }
-    w.mask_bits = reinterpret_cast<uint32_t*>(cv.take(Mc * ceil_div(d.W, 32)));
+    if (grad_only) w.colsum_sink = cv.take(d.W);
+    else w.mask_bits = reinterpret_cast<uint32_t*>(cv.take(Mc * ceil_div(d.W, 32)));
   }
   if (tc) {     // largest B operand image: a weight [width x (W + encoding)] (the weight gradients read theirs as fp32)
     const int HW = head ? d.HW : 0, Evp = head ? d.Evp : 0;
@@ -1018,6 +1035,7 @@ static int head_backward_tc(const SparfMLP* mlp, const Call& c, long long Mc, in
 // Backward through trunk layers nt-1 ... 0 of one chunk of Mc rows on the CUDA cores, from the gradient of the last
 // layer's features in w.G0 and of its density row, graw (may be NULL: zero).  H: the chunk's nt-1 first trunk
 // activations, enc its encoding.  Parameter gradients +=, the encoding's gradient into w.Genc when enc_grad.
+// grad == NULL: no weight or bias gradient, only the input gradients (the point gradient of sparf_density_gradient).
 static int trunk_backward_simt(const SparfMLP* mlp, const Call& c, long long Mc, const float* enc, float* const* H,
                                const float* graw, const SparfMLPGrad* grad, bool enc_grad, cudaStream_t st) {
   const MlpDims& d = c.d;
@@ -1031,15 +1049,18 @@ static int trunk_backward_simt(const SparfMLP* mlp, const Call& c, long long Mc,
     const float* in = l == 0 ? enc : H[l - 1];
     const int Kin = trunk_in_main(d, l), Kinv = trunk_in_main_valid(d, l);
     const int rowoff = last ? 1 : 0;
-    float* dWl = grad->trunk_w[l] + (size_t)rowoff * ldw;
     const float* Wl = mlp->trunk_w[l] + (size_t)rowoff * ldw;
-    SPARF_TRY(gemm_tn((int)Mc, d.W, Kin, Kinv, kSimtSlab, G, d.W, in, Kin, 1, dWl, ldw, 0, st));
-    if (l == d.skip) SPARF_TRY(gemm_tn((int)Mc, d.W, d.E3p, d.E3, kSimtSlab, G, d.W, enc, d.E3p, 1, dWl, ldw, d.W, st));
-    colsum_kernel<<<dim3(ceil_div(d.W, 32), ceil_div(Mc, 1024)), 256, 0, st>>>(Mc, d.W, 1024, G, d.W, grad->trunk_b[l] + rowoff);
-    SPARF_CHECK_LAUNCH("colsum_kernel(trunk)");
-    if (r1) {
-      narrow_wgrad_kernel<1><<<ceil_div(Mc, 512), 128, 0, st>>>(Mc, d.W, 512, graw, 1, in, d.W, grad->trunk_w[l], ldw, grad->trunk_b[l]);
-      SPARF_CHECK_LAUNCH("narrow_wgrad_kernel<1>");
+    if (grad) {
+      float* dWl = grad->trunk_w[l] + (size_t)rowoff * ldw;
+      SPARF_TRY(gemm_tn((int)Mc, d.W, Kin, Kinv, kSimtSlab, G, d.W, in, Kin, 1, dWl, ldw, 0, st));
+      if (l == d.skip) SPARF_TRY(gemm_tn((int)Mc, d.W, d.E3p, d.E3, kSimtSlab, G, d.W, enc, d.E3p, 1, dWl, ldw, d.W, st));
+      colsum_kernel<<<dim3(ceil_div(d.W, 32), ceil_div(Mc, 1024)), 256, 0, st>>>(Mc, d.W, 1024, G, d.W, grad->trunk_b[l] + rowoff);
+      SPARF_CHECK_LAUNCH("colsum_kernel(trunk)");
+      if (r1) {
+        narrow_wgrad_kernel<1><<<ceil_div(Mc, 512), 128, 0, st>>>(Mc, d.W, 512, graw, 1, in, d.W, grad->trunk_w[l], ldw,
+                                                                   grad->trunk_b[l]);
+        SPARF_CHECK_LAUNCH("narrow_wgrad_kernel<1>");
+      }
     }
     if (l > 0)
       SPARF_TRY(gemm_nn((int)Mc, d.W, d.W, d.W, G, d.W, Wl, ldw, 0, in, d.W, r1 ? graw : nullptr, r1 ? mlp->trunk_w[l] : nullptr,
@@ -1078,7 +1099,7 @@ static int chunk_dgrad_chain(const SparfMLP* mlp, const Call& c, long long Mc, u
   for (int l = top; l >= 1; --l) {
     SPARF_TRY(tc_pack_nn(c.ep.dgrad, d.W, d.W, d.W, mlp->trunk_w[l], trunk_ldw(d, l), 0, c.w.nnimg[l], st));
     mask[l] = bits[l - 1];
-    db[l] = grad->trunk_b[l - 1];
+    db[l] = grad ? grad->trunk_b[l - 1] : c.w.colsum_sink;    // the chain always sums its columns
     tr[l] = grad_tr(c.w, grad_tr_buf(d, true, l - 1), Mc);
     if (enc_grad && (l - 1 == 0 || l - 1 == d.skip)) row[l] = c.w.Grow[grad_row(d, true, l - 1)];
   }
@@ -1091,6 +1112,8 @@ static int chunk_dgrad_chain(const SparfMLP* mlp, const Call& c, long long Mc, u
 // input-gradient epilogue also sums the density row's weight gradient.
 // bits: the fused forward's ReLU masks of H_0 ... H_{nt-3} (trunk_chained: the input gradients of layers nt-2 ... 1 run
 // as one chain once layer nt-1 is done, and the weight gradients of the layers below it after that).
+// grad == NULL: no weight gradient GEMM; every input gradient reads its mask from the fp32 H_{l-1}, the chain's bias sums
+// go to w.colsum_sink and the transposed images, which only weight gradients read, to one shared buffer.
 static int trunk_backward_tc(const SparfMLP* mlp, const Call& c, long long Mc, const float* enc, float* const* H,
                              uint32_t* const* bits, const float* graw, const SparfMLPGrad* grad, bool enc_grad, cudaStream_t st) {
   const MlpDims& d = c.d;
@@ -1104,21 +1127,23 @@ static int trunk_backward_tc(const SparfMLP* mlp, const Call& c, long long Mc, c
     const float* in = l == 0 ? enc : H[l - 1];
     const int Kin = trunk_in_main(d, l), Kinv = trunk_in_main_valid(d, l);
     const int rowoff = last ? 1 : 0;
-    float* dWl = grad->trunk_w[l] + (size_t)rowoff * ldw;
     const float* Wl = mlp->trunk_w[l] + (size_t)rowoff * ldw;
     const int gi = (d.nt - 1 - l) & 1;   // layer by layer: the layer's output gradient is image pair gi
-    const TcImage gt = grad_tr(c.w, grad_tr_buf(d, chained, l), Mc);
     const bool nn = l > 0 && (!chained || last);   // the input gradient is a GEMM of its own
     // The input gradient's ReLU mask is H_{l-1} > 0: as bits that the weight gradient writes while it reads H_{l-1} anyway,
     // except with the density row's rank-1 term, whose weight gradient (r1_wgrad) the epilogue sums from the fp32 values
     // of H_{l-1}: that layer reads them as its mask.
-    uint32_t* wbits = nn && !r1 ? c.w.mask_bits : nullptr;
-    SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, Kin, Kinv, gt, in, Kin, 1, dWl, ldw, 0, wbits, st));
-    if (l == d.skip) SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, d.E3p, d.E3, gt, enc, d.E3p, 1, dWl, ldw, d.W, nullptr, st));
+    uint32_t* wbits = grad && nn && !r1 ? c.w.mask_bits : nullptr;
+    if (grad) {
+      float* dWl = grad->trunk_w[l] + (size_t)rowoff * ldw;
+      const TcImage gt = grad_tr(c.w, grad_tr_buf(d, chained, l), Mc);
+      SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, Kin, Kinv, gt, in, Kin, 1, dWl, ldw, 0, wbits, st));
+      if (l == d.skip) SPARF_TRY(tc_gemm_tn(ep.wgrad, (int)Mc, d.W, d.E3p, d.E3, gt, enc, d.E3p, 1, dWl, ldw, d.W, nullptr, st));
+    }
     if (nn)
       SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.W, d.W, c.w.Grow[gi], Wl, ldw, 0, wbits ? nullptr : in, d.W, wbits,
                            r1 ? graw : nullptr, r1 ? mlp->trunk_w[l] : nullptr, nullptr, 0, 0, grad_images(c, gi ^ 1, Mc),
-                           grad->trunk_b[l - 1], r1 ? grad->trunk_w[l] : nullptr, st));
+                           grad ? grad->trunk_b[l - 1] : nullptr, grad && r1 ? grad->trunk_w[l] : nullptr, st));
     if (enc_grad && (l == d.skip || l == 0)) {
       SPARF_TRY(tc_gemm_nn(ep.dgrad, (int)Mc, d.W, d.E3p, d.E3, c.w.Grow[grad_row(d, chained, l)], Wl, ldw, l == 0 ? 0 : d.W,
                            nullptr, 0, nullptr, nullptr, nullptr, c.w.Genc, d.E3p, genc_written ? 1 : 0, TcOut{}, nullptr,
@@ -1330,8 +1355,9 @@ extern "C" int sparf_mlp_backward_tape_rows(const SparfMLP* mlp, int32_t engine,
 extern "C" size_t sparf_density_workspace_bytes(const SparfMLP* mlp, int64_t M, int32_t backward, int32_t engine) {
   if (!mlp || M <= 0) return 0;
   const int e = resolve_engine(engine);
-  if (e < 0 || backward < 0 || backward > 1) return 0;
-  return workspace_need(mlp_dims(mlp), is_tc(e), M, 1, backward ? Pass::kRecomputeBackward : Pass::kForward, false);
+  if (e < 0 || backward < 0 || backward > 2) return 0;
+  const Pass pass = backward == 0 ? Pass::kForward : backward == 1 ? Pass::kRecomputeBackward : Pass::kGradient;
+  return workspace_need(mlp_dims(mlp), is_tc(e), M, 1, pass, false);
 }
 
 extern "C" int sparf_density_forward(const SparfMLP* mlp, int32_t engine, int64_t M, const float* points, float* raw,
@@ -1391,6 +1417,40 @@ extern "C" int sparf_density_backward(const SparfMLP* mlp, int32_t engine, int64
                                                        d_points + (size_t)p0 * 3, nullptr, c.rc);
       SPARF_CHECK_LAUNCH("posenc_bwd_kernel");
     }
+  }
+  return SPARF_OK;
+}
+
+// sparf_density_backward's input-gradient path with d_raw = 1 and d_feat = NULL (G_{nt-1} = 0), without the weight
+// gradients; grad_points is written
+extern "C" int sparf_density_gradient(const SparfMLP* mlp, int32_t engine, int64_t M, const float* points, float* grad_points,
+                                      void* workspace, size_t workspace_bytes, sparf_stream_t stream) {
+  SPARF_REQUIRE(mlp && M >= 0, "density_gradient: bad arguments");
+  if (M == 0) return SPARF_OK;
+  SPARF_REQUIRE(points && grad_points, "density_gradient: NULL tensor");
+  Call c;
+  SPARF_TRY(begin_call("density_gradient", mlp, engine, M, 1, Pass::kGradient, false, nullptr, 0, workspace, workspace_bytes,
+                       &c));
+  const cudaStream_t st = (cudaStream_t)stream;
+  const MlpDims& d = c.d;
+  const Tape& v = c.w.act;
+  fill_kernel<<<ceil_div(c.nrc, 256), 256, 0, st>>>(c.nrc, 1.f, c.w.ones);
+  SPARF_CHECK_LAUNCH("fill_kernel");
+  for (long long p0 = 0; p0 < M; p0 += c.nrc) {
+    const int n = (int)std::min<long long>(c.nrc, M - p0);
+    float* gp = grad_points + (size_t)p0 * 3;
+    SPARF_CHECK_CUDA(cudaMemsetAsync(gp, 0, (size_t)n * 3 * sizeof(float), st));   // posenc_bwd_kernel adds
+    SPARF_TRY(chunk_encode_xyz(mlp, c, n, 1, points + (size_t)p0 * 3, nullptr, nullptr, v.enc, st));
+    SPARF_TRY(chunk_trunk(mlp, c, n, v.enc, v.H, v.bits, nullptr, nullptr, nullptr, false, st));
+    // the last layer's feature gradient is 0: the images tc_feat_backward writes for d_feat = NULL, or G0
+    if (c.tc)
+      SPARF_CHECK_CUDA(cudaMemsetAsync(c.w.Grow[0].p, 0, tc_image_elems(n, d.W) * sizeof(uint16_t), st));
+    else
+      SPARF_CHECK_CUDA(cudaMemsetAsync(c.w.G0, 0, (size_t)n * d.W * sizeof(float), st));
+    SPARF_TRY(c.tc ? trunk_backward_tc(mlp, c, n, v.enc, v.H, v.bits, c.w.ones, nullptr, true, st)
+                   : trunk_backward_simt(mlp, c, n, v.enc, v.H, c.w.ones, nullptr, true, st));
+    posenc_bwd_kernel<<<ceil_div(n, 4), 128, 0, st>>>(n, 1, mlp->L_xyz, d.E3p, v.enc, c.w.Genc, nullptr, gp, nullptr, c.rc);
+    SPARF_CHECK_LAUNCH("posenc_bwd_kernel");
   }
   return SPARF_OK;
 }

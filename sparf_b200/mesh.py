@@ -101,18 +101,20 @@ def to_world(verts: torch.Tensor, res: int, range) -> torch.Tensor:
 @torch.no_grad()
 def density_normals(nerf, points: torch.Tensor, engine=None) -> torch.Tensor:
     """-grad(raw) / |grad(raw)| at points [M, 3] (the direction of falling density), 0 where the gradient is 0; the
-    density backward in chunks of NORMAL_CHUNK points"""
+    point gradient (ops.density_gradient, no weight gradients) in chunks of NORMAL_CHUNK points"""
     spec, trunk = nerf._spec(), _trunk(nerf)
     out = torch.empty_like(points)
     for c0 in range(0, points.shape[0], NORMAL_CHUNK):
-        x = points[c0:c0 + NORMAL_CHUNK].detach().clone().requires_grad_(True)
-        with torch.enable_grad():
-            raw, _ = ops.density_forward(spec, x, trunk, progress=nerf.progress.detach(), engine=_engine(engine),
-                                         features=False)
-            (g,) = torch.autograd.grad(raw.sum(), x)
-        norm = g.norm(dim=-1, keepdim=True)
-        out[c0:c0 + NORMAL_CHUNK] = torch.where(norm > 0, -g / norm, torch.zeros_like(g))
+        g = ops.density_gradient(spec, points[c0:c0 + NORMAL_CHUNK], trunk, progress=nerf.progress.detach(),
+                                 engine=_engine(engine))
+        out[c0:c0 + NORMAL_CHUNK] = unit_normals(g)
     return out
+
+
+def unit_normals(g: torch.Tensor) -> torch.Tensor:
+    """-g / |g| over the last axis, 0 where |g| = 0: the normal of a density gradient g [..., 3]"""
+    norm = g.norm(dim=-1, keepdim=True)
+    return torch.where(norm > 0, -g / norm, torch.zeros_like(g))
 
 
 def extract_mesh(opt, nerf, normals: bool = False, engine=None) -> dict:

@@ -609,6 +609,44 @@ def density_forward(spec: MLPSpec, points, trunk_params: Sequence[torch.Tensor],
     return DensityFunction.apply(spec, eng, torch.is_grad_enabled(), bool(features), points, progress, *trunk_params)
 
 
+@torch.no_grad()
+def density_gradient(spec: MLPSpec, points, trunk_params: Sequence[torch.Tensor], progress=None, engine: Optional[int] = None):
+    """d raw / d x at points [..., 3] -> [..., 3], raw as density_forward computes it (no noise, the BARF mask at
+    progress): sparf_density_gradient, the density backward's input gradients without its weight gradients.  Bit for bit
+    the points' gradient of density_forward(...)[0].sum() on every engine.  No autograd; counted in EVALS["bwd"]."""
+    eng = get_engine() if engine is None else int(engine)
+    if not torch.is_tensor(points) or points.dim() < 1 or points.shape[-1] != 3:
+        raise ValueError("density_gradient: points must be a tensor [..., 3], got %s"
+                         % ((tuple(points.shape),) if torch.is_tensor(points) else type(points).__name__))
+    if not points.is_cuda:
+        raise ValueError("density_gradient: points must be a CUDA tensor")
+    if len(trunk_params) != 2 * spec.n_trunk:
+        raise ValueError("density_gradient takes the trunk's 2 * n_trunk = %d tensors, got %d"
+                         % (2 * spec.n_trunk, len(trunk_params)))
+    if eng not in _lib.ENGINES.values():
+        raise ValueError("density_gradient: unknown engine %r" % (engine,))
+    if spec.barf_c2f is not None and progress is None:
+        raise ValueError("density_gradient: a BARF coarse-to-fine spec needs progress")
+    return _density_gradient(spec, eng, points, progress, trunk_params)
+
+
+@_on_tensor_device
+def _density_gradient(spec, eng, points, progress, trunk_params):
+    L = _lib.lib()
+    pts = _f32c(points).reshape(-1, 3)
+    M = pts.shape[0]
+    out = torch.empty_like(pts)
+    if M == 0:
+        return out.view(points.shape)
+    m, keep = spec.fill(trunk_params, progress)
+    ws = _workspace(L.sparf_density_workspace_bytes(ctypes.byref(m), M, 2, eng), pts.device)
+    EVALS["bwd"] += M
+    with _timed("density_gradient"):
+        check(L.sparf_density_gradient(ctypes.byref(m), eng, M, _ptr(pts), _ptr(out), _ptr(ws), ws.numel(), _stream()),
+              "density_gradient")
+    return out.view(points.shape)
+
+
 # ------------------------------------------------------------------------------------------------
 # marching cubes (no gradient)
 # ------------------------------------------------------------------------------------------------

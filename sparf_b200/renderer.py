@@ -220,6 +220,22 @@ class Graph(torch.nn.Module):
             raise ValueError("set_training_termination: window %r (an integer >= 1)" % (window,))
         self._train_termination = (float(eps), int(window))
 
+    def set_normals(self, enabled=True):
+        """Add normal maps to renders (sparf_b200.normals): `render` in val / eval / test mode with gradients off then also
+        returns `normal` [B,N,3] (and `normal_fine` from the fine pass), the composite weight-sum of the density normals
+        -grad(raw) / |grad(raw)| over the samples with w != 0: world-space and unnormalised (|normal| <= opacity).  Every
+        other output is unchanged; train and test-optim renders, render_to_max and renders with gradients return no normal.
+        False detaches."""
+        if not isinstance(enabled, bool):
+            raise ValueError("set_normals: enabled %r (True or False)" % (enabled,))
+        self._normals = enabled
+
+    def _add_normals(self, nerf, pred, center, ray, depth_samples, mode):
+        if getattr(self, "_normals", False) and mode in ("val", "eval", "test") and not torch.is_grad_enabled():
+            from . import normals
+            pred["normal"] = normals.composite_normals(nerf, center, ray, depth_samples, pred["weights"])
+        return pred
+
     def _forward_samples(self, nerf, which, opt, center, ray, depth_samples, mode):
         """nerf.forward_samples, or in val / eval / test mode without gradients termination.forward_samples when early
         termination is set, occupancy.forward_samples when only grid `which` (0 coarse, 1 fine) is attached; in train and
@@ -256,7 +272,8 @@ class Graph(torch.nn.Module):
                                           H=H, W=W, depth_range=depth_range, mode=mode)   # [B,N,S,1]
         pred_coarse = self._forward_samples(self.nerf, 0, opt, center, ray, depth_samples, mode)
         pred_coarse["t"] = depth_samples
-        pred_coarse = self.nerf.composite(opt, ray, pred_coarse, depth_samples)
+        pred_coarse = self._add_normals(self.nerf, self.nerf.composite(opt, ray, pred_coarse, depth_samples), center, ray,
+                                        depth_samples, mode)
         pred.update(pred_coarse)
         if opt.nerf.fine_sampling and not self._fine_disabled(opt, iter):
             with torch.no_grad():
@@ -265,7 +282,8 @@ class Graph(torch.nn.Module):
                                                      depth_range, det)           # [B,N,S+Sf,1]
             pred_fine = self._forward_samples(self.nerf_fine, 1, opt, center, ray, depth_all, mode)
             pred_fine["t"] = depth_all
-            pred_fine = self.nerf_fine.composite(opt, ray, pred_fine, depth_all)
+            pred_fine = self._add_normals(self.nerf_fine, self.nerf_fine.composite(opt, ray, pred_fine, depth_all), center,
+                                          ray, depth_all, mode)
             pred.update({k + "_fine": v for k, v in pred_fine.items()})
         return pred
 
