@@ -23,6 +23,7 @@
 //     that are asked for and the last layer's row image.  Same MMA order and epilogue arithmetic per output element as
 //     the gemm, so the same bytes.
 #include <cuda_bf16.h>
+#include <cudaTypedefs.h>
 #include <cuda_fp16.h>
 
 #include <algorithm>
@@ -476,6 +477,11 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
                ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
+// a box of a 2D tensor map at column c0, row r0 (elements), zeros where it leaves the tensor
+__device__ __forceinline__ void tensor_g2s(void* dst, const CUtensorMap* map, int c0, int r0, uint64_t* bar) {
+  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n"
+               ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(r0), "r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;\n" ::: "memory"); }
 
 // A GEMM operand as images: k-steps [0, ks0) of each row tile from image p0 (ks0 k-steps per row tile), the rest from
@@ -897,11 +903,13 @@ __device__ __forceinline__ void converter_sync() { asm volatile("bar.sync 2, 128
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
 // The producer warp: per k-step, the A tile with one copy and the 32 rows m of B (X[m / div][128 bx, 128 bx + 128) in
-// fp32, 512 bytes per row at most) with one copy per lane, into the stage's 16 KB of B halves.  Rows at or past M are not
-// copied and the bytes past K of a row not written; the converter never reads either.
+// fp32, 512 bytes per row at most) into the stage's 16 KB of B halves, row m at 512 (m - m0) bytes.  With div = 1 the
+// rows are one box of the tensor map xmap (zeros past M and K), so a k-step is two copies; the time of a k-step's
+// copies followed their count more than their bytes.  Per-ray rows (div > 1) take one copy per lane; rows at or past M
+// are not copied and the bytes past K of a row not written.  The converter reads neither.
 template <int PASSES, int NST = STAGES>
-__device__ __forceinline__ void produce_staged(const Opnd& a, const Staged& x, const Units& w, uint64_t* full,
-                                               uint64_t* empty) {
+__device__ __forceinline__ void produce_staged(const Opnd& a, const Staged& x, const CUtensorMap* xmap, const Units& w,
+                                               uint64_t* full, uint64_t* empty) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const int lane = threadIdx.x & 31;
   const uint32_t abytes = PASSES == 3 ? 2 * TILE_BYTES : TILE_BYTES;
@@ -915,6 +923,14 @@ __device__ __forceinline__ void produce_staged(const Opnd& a, const Staged& x, c
       const int s = it % NST, m0 = (kt0 + j) * TK;
       mbar_wait(&empty[s], ((it / NST) & 1) ^ 1);
       uint8_t* st = smem + s * STAGE_BYTES;
+      if (x.div == 1) {
+        if (lane == 0) {
+          mbar_expect_tx(&full[s], abytes + TK * TM * 4);
+          bulk_g2s(st, a.tile(by, kt0 + j), abytes, &full[s]);
+          tensor_g2s(st + 2 * TILE_BYTES, xmap, k0, m0, &full[s]);
+        }
+        continue;
+      }
       if (lane == 0) {
         mbar_expect_tx(&full[s], abytes + min(TK, x.M - m0) * rbytes);
         bulk_g2s(st, a.tile(by, kt0 + j), abytes, &full[s]);
@@ -1024,12 +1040,13 @@ __device__ __forceinline__ void presum_epilogue(const float (&acc)[64], float* p
 // The weight-gradient GEMM dW += G^T X with B read as fp32 (Staged): wg_gemm_kernel's units and MMAs on a ring of
 // STAGED_STAGES, with a fourth warpgroup that splits each stage's B in place between its copies and its MMAs, so no pack
 // kernel writes and no GEMM reads an image of X, and an epilogue that adds each CTA's partials of one tile once
-// (presum_epilogue).  Registers: producer 40, converter 64, consumers 200 (<= 64 K).
+// (presum_epilogue).  Registers: producer 40, converter 64, consumers 200 (<= 64 K).  xmap: X as a tensor of x.M rows
+// (the capacity with DYN) by x.K columns, read where div = 1 (produce_staged).
 // DYN: x.M is a capacity, of which live_rows rows are summed; the k-range split is gemm_units' for that count, computed
 // here from ctas (the CTAs gemm_units was given).
 template <int PASSES, bool DYN = false>
 __global__ void __launch_bounds__(STAGED_THREADS, 1) wg_gemm_staged_kernel(Opnd a, Staged x, Units w, Epi e, RowCount rc,
-                                                                           int ctas) {
+                                                                           int ctas, const __grid_constant__ CUtensorMap xmap) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if constexpr (DYN) {
     x.M = (int)live_rows<true, false>(x.M, rc);
@@ -1052,7 +1069,7 @@ __global__ void __launch_bounds__(STAGED_THREADS, 1) wg_gemm_staged_kernel(Opnd 
   __syncthreads();
   if (threadIdx.x >= CONSUMERS + 128) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
-    if (threadIdx.x < CONSUMERS + 128 + 32) produce_staged<PASSES, STAGED_STAGES>(a, x, w, full, empty);
+    if (threadIdx.x < CONSUMERS + 128 + 32) produce_staged<PASSES, STAGED_STAGES>(a, x, &xmap, w, full, empty);
     return;
   }
   if (threadIdx.x >= CONSUMERS) {
@@ -1599,14 +1616,36 @@ static int run(const TcPrec& p, const Opnd& a, int a_rows, FB fb, int b_rows, in
                 row_passes, tr_passes);
 }
 
+// X (div = 1) as a 2D tensor of x.M rows by x.K fp32 columns, row pitch ldx, read in boxes of one k-step's 32 rows by
+// 128 columns; zeros outside the tensor
+static int staged_tensor_map(const Staged& x, CUtensorMap* map) {
+  static PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
+  if (!encode) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    SPARF_CHECK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
+    SPARF_REQUIRE(fn && q == cudaDriverEntryPointSuccess, "tc_gemm_tn: the driver has no cuTensorMapEncodeTiled");
+    encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
+  }
+  const cuuint64_t dims[2] = {(cuuint64_t)x.K, (cuuint64_t)x.M}, pitch[1] = {(cuuint64_t)x.ldx * 4};
+  const cuuint32_t box[2] = {TM, TK}, step[2] = {1, 1};
+  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(x.X), dims, pitch, box, step,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  SPARF_REQUIRE(r == CUDA_SUCCESS, "tc_gemm_tn: cuTensorMapEncodeTiled failed (%d)", (int)r);
+  return SPARF_OK;
+}
+
 // the weight-gradient GEMM with B = x read as fp32 (no pack), N output rows, over the k-steps of gt
 template <int PASSES>
 static int run_staged(const TcPrec& p, const Opnd& gt, int N, const Staged& x, int ksteps, const Epi& e, cudaStream_t st) {
+  CUtensorMap xmap{};
+  if (x.div == 1 && x.M > 0) SPARF_TRY(staged_tensor_map(x, &xmap));
   const int ctas = gemm_ctas(p);
   const Units w = gemm_units(ceil_div(N, TM), ceil_div(x.K, TM), ksteps, true, ctas);
   auto kernel = p.rows.rows ? wg_gemm_staged_kernel<PASSES, true> : wg_gemm_staged_kernel<PASSES>;
   SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, STAGED_SMEM));
-  kernel<<<std::min(w.tiles * w.nsplit, ctas), STAGED_THREADS, STAGED_SMEM, st>>>(gt, x, w, e, p.rows, ctas);
+  kernel<<<std::min(w.tiles * w.nsplit, ctas), STAGED_THREADS, STAGED_SMEM, st>>>(gt, x, w, e, p.rows, ctas, xmap);
   SPARF_CHECK_LAUNCH("wg_gemm_staged_kernel");
   return SPARF_OK;
 }
