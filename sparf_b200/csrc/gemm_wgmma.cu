@@ -89,6 +89,10 @@ __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_grou
 // that carry one lo factor accumulate separately and are scaled back once at the end
 constexpr int LO_SHIFT = 11;
 
+// x 2^-LO_SHIFT, rounded once as ldexpf(x, -LO_SHIFT) is (exact unless the result is subnormal); __fmul_rn keeps the
+// multiply out of an FMA with the add that follows it, which would skip that rounding
+__device__ __forceinline__ float lo_unscale(float x) { return __fmul_rn(x, 1.f / (1 << LO_SHIFT)); }
+
 template <bool F16>
 __device__ __forceinline__ void split16(float x, uint16_t& hi, uint16_t& lo) {
   if constexpr (F16) {
@@ -593,7 +597,7 @@ __device__ __forceinline__ void mma_unit(float (&acc)[64], int nk, int& it, uint
   if (lane == 0) mbar_arrive(&empty[(it + NST - 1) % NST]);
   if constexpr (PASSES == 3) {
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] += ldexpf(acc_lo[i], -LO_SHIFT);
+    for (int i = 0; i < 64; ++i) acc[i] += lo_unscale(acc_lo[i]);
   }
 }
 
@@ -643,6 +647,8 @@ __device__ __forceinline__ void st2(float* p, float x, float y, bool two) {
 
 // the consumer warpgroups only (the producer warpgroup never joins)
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;\n" ::"n"(CONSUMERS) : "memory"); }
+// the 4 warps of this consumer warpgroup (barriers 3 and 4)
+__device__ __forceinline__ void warpgroup_sync() { asm volatile("bar.sync %0, 128;\n" ::"r"(3 + (threadIdx.x >> 7)) : "memory"); }
 
 // dst[n0 + c] += column c of the tile summed over its rows, from part[2 j + c'] = this thread's share of column
 // 8 j + 2 (lane % 4) + c' (its two rows): over the 16 rows of each warp (shuffles), the 8 warps (the 4 KB of shared
@@ -1101,8 +1107,8 @@ constexpr int CH_HALF = CH_M * TK * 2;        // one 16-bit half of a [64 x 32] 
 constexpr int CH_STAGES = 4;                  // weight ring: per stage the k-step's two [128 x 32] B tiles (hi, lo each)
 constexpr int CH_ENC = CH_KS * 2 * CH_HALF;               // byte offsets in shared memory: activations at 0 (64 KB),
 constexpr int CH_RING = CH_ENC + CH_ENC_KS * 2 * CH_HALF; // the encoding (16 KB), the ring (128 KB),
-constexpr int CH_BAR = CH_RING + CH_STAGES * STAGE_BYTES; // full[4], empty[4], enc_full, enc_empty
-constexpr int CH_SMEM = CH_BAR + (2 * CH_STAGES + 2) * 8;
+constexpr int CH_BAR = CH_RING + CH_STAGES * STAGE_BYTES; // full[4], empty[4], enc_full, enc_empty, rd[2], wr[2]
+constexpr int CH_SMEM = CH_BAR + (2 * CH_STAGES + 6) * 8;
 
 // Its own parameter struct (not Epi: see the note there).  Layer l < nl computes H[l] = relu(in_l W_l^T + bias[l]), in_0 =
 // enc, in_l = H[l-1] ( | enc at l == skip), from the weight image w[l] (256 rows, chain_ks(l) k-steps, as pack_kernel<NtB>
@@ -1154,11 +1160,26 @@ __device__ __forceinline__ void chain_produce(const Chain& c, int M, int tiles, 
   }
 }
 
+// The hand-offs of the activation buffer between the two warpgroups.  Half h of the buffer (k-steps [4 h, 4 h + 4), the
+// layer's output columns [128 h, 128 h + 128)) is written by warpgroup h and read by both.  rd[h] completes once all 8
+// consumer warps have retired their MMAs on half h (warpgroup h may then overwrite it), wr[h] once warpgroup h's 4 warps
+// have stored and proxy-fenced its split there (the MMAs on it may then start).  Each warpgroup waits only for the half
+// it is about to touch, so the two drift apart by up to the weight ring's depth instead of meeting twice per layer.
+// Both complete once per generation of the buffer, in the same order on every thread; a wait takes the parity of the
+// generation's index, which is never more than one phase from where the barrier stands.
+struct Halves {
+  uint64_t* rd;
+  uint64_t* wr;
+};
+
 // The MMAs of one layer for this warpgroup's 128 output columns of the tile's 64 rows: mma_unit's instruction sequence
-// per k-step (so every output element sums in the same order), nk k-steps of A, the first na from the activation buffer
-// and the rest from the encoding's (the skip layer; the encoding alone at layer 0), B this warpgroup's tile of the stage.
+// per k-step (so every output element sums in the same order), nk k-steps of A, the first na (0 or CH_KS) from the
+// activation buffer and the rest from the encoding's (the skip layer; the encoding alone at layer 0), B this warpgroup's
+// tile of the stage.  wr_parity >= 0: the buffer holds a generation the epilogues wrote, waited for half by half in front
+// of the half's first k-step.  rd_arrive: arrive on rd[h] as soon as half h's MMAs have retired.
 template <bool F16, int PASSES>
-__device__ __forceinline__ void chain_mma(float (&acc)[64], int nk, int na, int& it, uint64_t* full, uint64_t* empty) {
+__device__ __forceinline__ void chain_mma(float (&acc)[64], int nk, int na, int& it, uint64_t* full, uint64_t* empty,
+                                          Halves hv, int wr_parity, bool rd_arrive) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   float acc_lo[PASSES == 3 ? 64 : 1];
@@ -1168,6 +1189,7 @@ __device__ __forceinline__ void chain_mma(float (&acc)[64], int nk, int na, int&
   for (int i = 0; i < (PASSES == 3 ? 64 : 1); ++i) acc_lo[i] = 0.f;
   for (int j = 0; j < nk; ++j, ++it) {
     const int s = it % CH_STAGES;
+    if (wr_parity >= 0 && j < na && j % (CH_KS / 2) == 0) mbar_wait(&hv.wr[j / (CH_KS / 2)], wr_parity);
     mbar_wait(&full[s], (it / CH_STAGES) & 1);
     const uint8_t* a = j < na ? smem + j * 2 * CH_HALF : smem + CH_ENC + (j - na) * 2 * CH_HALF;
     const uint8_t* b = smem + CH_RING + s * STAGE_BYTES + wg * 2 * TILE_BYTES;
@@ -1182,41 +1204,32 @@ __device__ __forceinline__ void chain_mma(float (&acc)[64], int nk, int na, int&
       wgmma_m64n128k16<F16>(acc, ahi, bhi);
     }
     wgmma_commit();
-    wgmma_wait_1();
+    wgmma_wait_1();             // k-steps 0 ... j - 1 have retired
     if (j > 0 && lane == 0) mbar_arrive(&empty[(it + CH_STAGES - 1) % CH_STAGES]);
+    if (rd_arrive && lane == 0 && j > 0 && j <= na && j % (CH_KS / 2) == 0) mbar_arrive(&hv.rd[j / (CH_KS / 2) - 1]);
   }
   wgmma_wait_all();
   if (lane == 0) mbar_arrive(&empty[(it + CH_STAGES - 1) % CH_STAGES]);
+  if (rd_arrive && lane == 0 && nk == na) mbar_arrive(&hv.rd[1]);
   if constexpr (PASSES == 3) {
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] += ldexpf(acc_lo[i], -LO_SHIFT);
+    for (int i = 0; i < 64; ++i) acc[i] += lo_unscale(acc_lo[i]);
   }
 }
 
-// Layer l's epilogue of tile t, in place: bias and ReLU as epilogue_values kind 0 (acc becomes the layer's output, zero
-// past M), and its split (the same split2 as a row image's) over the layer's input in the activation buffer; the last
-// layer's split goes to its row image in global memory instead, where asked.
+// this warpgroup's 4 warps have stored and proxy-fenced their part of half wg of the buffer
+__device__ __forceinline__ void chain_written(Halves hv) {
+  fence_proxy_async();          // the stores into the activation buffer, before the MMAs that read them
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(&hv.wr[threadIdx.x >> 7]);
+}
+
+// the tile's split (PASSES halves) of this warpgroup's columns as a row image at img: k-step stride kstride, lo half
+// lo_off after the hi half (16-bit elements); the fragment of (j, h) is one core matrix, this lane's pair its 32-bit
+// word `lane`
 template <bool F16, int PASSES>
-__device__ __forceinline__ void chain_epilogue(float (&acc)[64], const Chain& c, int M, int l, int t) {
-  extern __shared__ __align__(1024) uint8_t smem[];
+__device__ __forceinline__ void chain_split(const float (&acc)[64], uint16_t* img, int kstride, int lo_off) {
   const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-  const float* bias = c.bias[l];
-#pragma unroll
-  for (int i = 0; i < 64; i += 2) {
-    const int m = t * CH_M + wq * 16 + (lane >> 2) + ((i >> 1) & 1) * 8, n = wg * TN + (i >> 2) * 8 + (lane & 3) * 2;
-    if (m >= M) {
-      acc[i] = acc[i + 1] = 0.f;
-      continue;
-    }
-    acc[i] = fmaxf(acc[i] + bias[n], 0.f);
-    acc[i + 1] = fmaxf(acc[i + 1] + bias[n + 1], 0.f);
-  }
-  const bool last = l == c.nl - 1;
-  if (last && !c.last) return;
-  // as the GEMM epilogue's row image: the fragment of (j, h) is one core matrix, this lane's pair its 32-bit word `lane`
-  uint16_t* img = last ? c.last + (size_t)(t >> 1) * CH_KS * 2 * TILE_ELEMS + (t & 1) * (CH_M * TK)
-                       : reinterpret_cast<uint16_t*>(smem);
-  const int kstride = last ? 2 * TILE_ELEMS : CH_HALF, lo_off = last ? TILE_ELEMS : CH_HALF / 2;
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     uint16_t* kt = img + (size_t)(4 * wg + (j >> 2)) * kstride;
@@ -1231,7 +1244,33 @@ __device__ __forceinline__ void chain_epilogue(float (&acc)[64], const Chain& c,
   }
 }
 
-// The fp32 output of layer l (acc after chain_epilogue) to H[l].  It runs after the proxy fence that follows the stores
+// this thread's bias pairs of layer l, columns wg 128 + 8 j + 2 (lane % 4) + {0, 1}; loaded before the layer's MMAs.
+// Two scalar loads per pair: a bias in a flat parameter bank may start at an odd float.
+__device__ __forceinline__ void chain_bias(float2 (&bv)[16], const float* bias) {
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const float* b = bias + wg * TN + j * 8 + (lane & 3) * 2;
+    bv[j] = make_float2(b[0], b[1]);
+  }
+}
+
+// Layer l's bias and ReLU of tile t as epilogue_values kind 0: acc becomes the layer's output, zero past M.
+__device__ __forceinline__ void chain_bias_relu(float (&acc)[64], const float2 (&bv)[16], int M, int t) {
+  const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int i = 0; i < 64; i += 2) {
+    const int m = t * CH_M + wq * 16 + (lane >> 2) + ((i >> 1) & 1) * 8;
+    if (m >= M) {
+      acc[i] = acc[i + 1] = 0.f;
+      continue;
+    }
+    acc[i] = fmaxf(acc[i] + bv[i >> 2].x, 0.f);
+    acc[i + 1] = fmaxf(acc[i + 1] + bv[i >> 2].y, 0.f);
+  }
+}
+
+// The fp32 output of layer l (acc after chain_bias_relu) to H[l].  It runs after the proxy fence that follows the stores
 // into the activation buffer: a fence issued behind these global stores waits for them too, once per layer with no MMA
 // in flight; issued after it, they drain while the next layer's MMAs run.
 __device__ __forceinline__ void chain_store(const float (&acc)[64], float* H, int M, int t) {
@@ -1271,10 +1310,10 @@ __device__ __forceinline__ void chain_store_bits(const float (&acc)[64], uint32_
 
 // Persistent and warp-specialized like wg_gemm_kernel (thread 256 produces, warps 0-7 consume, the same register
 // hand-back), but the two consumer warpgroups split N: warpgroup g computes columns [128 g, 128 g + 128) of the tile's 64
-// rows from the same A.  A layer's input is overwritten by its output once both warpgroups' MMAs have retired (a
-// consumer barrier), and the next layer's MMAs start once those generic-proxy stores are fenced for the async proxy and
-// both warpgroups have passed a second barrier.  The epilogue is not overlapped with MMAs (the accumulators of one tile
-// fill both warpgroups); the ring keeps the next layer's weights coming meanwhile.
+// rows from the same A.  Each warpgroup overwrites its half of the layer's input with its half of the output (the same
+// split2 as a row image's) once every warp's MMAs on that half have retired, and the next layer's MMAs on a half start
+// once its stores are fenced for the async proxy (Halves).  So one warpgroup's epilogue runs while the other's MMAs do;
+// the last layer's split goes to its row image in global memory instead, where asked.
 // Tiles: 2 ceil(M / 128), so that the last image's 128-row tiles are written whole; a tile wholly past M only zeroes its
 // half of them.  DYN: c.M is a capacity, of which live_rows rows (M) are computed.  SPAN (with DYN; the span forward): H
 // and bits take their rows from row_start on (the last image's rows start at 0); without it rc.start is never read.
@@ -1290,6 +1329,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) trunk_chain_kernel(const Chai
   uint64_t* empty = full + CH_STAGES;
   uint64_t* enc_full = empty + CH_STAGES;
   uint64_t* enc_empty = enc_full + 1;
+  const Halves hv{enc_empty + 1, enc_empty + 3};
   if (threadIdx.x == 0) {
     for (int i = 0; i < CH_STAGES; ++i) {
       mbar_init(&full[i], 1);
@@ -1297,6 +1337,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) trunk_chain_kernel(const Chai
     }
     mbar_init(enc_full, 1);
     mbar_init(enc_empty, CONSUMERS / 32);
+    for (int h = 0; h < 2; ++h) {
+      mbar_init(&hv.rd[h], CONSUMERS / 32);
+      mbar_init(&hv.wr[h], 4);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   __syncthreads();
@@ -1308,7 +1352,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) trunk_chain_kernel(const Chai
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
   const int enc_last = c.skip > 0 && c.skip < c.nl ? c.skip : 0;   // the last layer that reads the encoding
   const long long s0 = row_start<SPAN>(rc);   // the span forward: H and bits at global rows s0 + m; 0 otherwise
-  int it = 0, n = 0;
+  const int wg = threadIdx.x >> 7;
+  // p: generations of the activation buffer written so far.  Every layer l > 0 reads generation p - 1 (layer l - 1's
+  // output) and every layer but the last writes generation p over it, after the reads of generation p - 1: the same
+  // tile's at l > 0, the previous tile's last layer at l == 0.
+  int it = 0, n = 0, p = 0;
   for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
     if (t * CH_M >= M) {
       if (c.last)
@@ -1320,14 +1368,21 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) trunk_chain_kernel(const Chai
     mbar_wait(enc_full, n & 1);
     ++n;
     for (int l = 0; l < c.nl; ++l) {
+      float2 bv[16];
+      chain_bias(bv, c.bias[l]);
       float acc[64];
-      chain_mma<F16, PASSES>(acc, chain_ks(l, c.skip, c.enc_ks), l == 0 ? 0 : CH_KS, it, full, empty);
+      chain_mma<F16, PASSES>(acc, chain_ks(l, c.skip, c.enc_ks), l == 0 ? 0 : CH_KS, it, full, empty, hv,
+                             l == 0 ? -1 : (p - 1) & 1, l > 0);
       if (l == enc_last && (threadIdx.x & 31) == 0) mbar_arrive(enc_empty);
-      consumer_sync();          // both warpgroups have read the layer's input
-      chain_epilogue<F16, PASSES>(acc, c, M, l, t);
+      chain_bias_relu(acc, bv, M, t);
       if (l + 1 < c.nl) {
-        fence_proxy_async();    // the stores into the activation buffer, before the MMAs that read them
-        consumer_sync();
+        if (p > 0) mbar_wait(&hv.rd[wg], (p - 1) & 1);    // every warp has read generation p - 1 of this half
+        chain_split<F16, PASSES>(acc, reinterpret_cast<uint16_t*>(smem), CH_HALF, CH_HALF / 2);
+        chain_written(hv);
+        ++p;
+      } else if (c.last) {
+        chain_split<F16, PASSES>(acc, c.last + (size_t)(t >> 1) * CH_KS * 2 * TILE_ELEMS + (t & 1) * (CH_M * TK),
+                                 2 * TILE_ELEMS, TILE_ELEMS);
       }
       if (c.H[l]) chain_store(acc, c.H[l] + s0 * CH_W, M, t);
       if (BITS && c.bits[l]) chain_store_bits(acc, c.bits[l] + s0 * (CH_W / 32), M, t);
@@ -1409,25 +1464,6 @@ __device__ __forceinline__ void dg_mask_words(uint4 (&wd)[2], const uint32_t* bi
   }
 }
 
-// the tile's split (PASSES halves) as a row image at img: k-step stride kstride, lo half lo_off after the hi half (16-bit
-// elements); the fragment of (j, h) is one core matrix, this lane's pair its 32-bit word `lane`
-template <int PASSES>
-__device__ __forceinline__ void dg_split(const float (&acc)[64], uint16_t* img, int kstride, int lo_off) {
-  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    uint16_t* kt = img + (size_t)(4 * wg + (j >> 2)) * kstride;
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      uint32_t hi, lo;
-      split2<false>(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], hi, lo);
-      const int core = (2 * wq + h) * (TK / 8) + (j & 3);
-      reinterpret_cast<uint32_t*>(kt + core * 64)[lane] = hi;
-      if (PASSES == 3) reinterpret_cast<uint32_t*>(kt + lo_off + core * 64)[lane] = lo;
-    }
-  }
-}
-
 // A tile wholly past M writes zeros where the layer-by-layer GEMMs' 128-row tiles would: its half of the row images, and
 // the transposed images' k-steps of its rows below tr_ks (a capacity's, with a device row count).
 template <int DP, int TP>
@@ -1447,11 +1483,12 @@ __device__ __forceinline__ void dg_zero_tile(const DgChain& c, int t) {
 }
 
 // Persistent and warp-specialized as trunk_chain_kernel (tiles, ring, register hand-back, the two warpgroups splitting
-// N), with the mask words of a layer loaded before its MMAs.  Per layer and tile: MMAs (tc_gemm_nn's per output element);
-// both warpgroups past them (consumer barrier); the mask (rows past M have no bits, so they are zero), the column sums'
-// per-warp partials, the split over the layer's input in the activation buffer (not after layer 1), proxy fence,
-// barrier; then the column sums' atomics and the global stores, which drain while the next layer's MMAs run.  The values
-// and the images' bytes are tc_gemm_nn's; the column sums add 64-row tiles instead of 128-row ones.
+// N, each on its half of the activation buffer through Halves), with the mask words of a layer loaded before its MMAs.
+// Per layer and tile: MMAs (tc_gemm_nn's per output element); the mask (rows past M have no bits, so they are zero),
+// the column sums' per-warp partials, the split over this warpgroup's half of the layer's input in the activation
+// buffer (not after layer 1) once every warp has read that half; then, past a barrier of the warpgroup's own 4 warps,
+// the column sums' atomics and the global stores, which drain while the next layer's MMAs run.  The values and the
+// images' bytes are tc_gemm_nn's; the column sums add 64-row tiles instead of 128-row ones.
 // DP: the activation buffer's and row images' passes (the input gradients'), TP: the transposed images' (the weight
 // gradients').  DYN: c.M is a capacity, of which live_rows rows are computed.
 template <int DP, int TP, bool DYN = false>
@@ -1464,7 +1501,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) dgrad_chain_kernel(const DgCh
   uint64_t* empty = full + CH_STAGES;
   uint64_t* act_full = empty + CH_STAGES;
   uint64_t* act_empty = act_full + 1;
-  float* red = reinterpret_cast<float*>(smem + CH_ENC);     // [8 warps][128 columns]
+  const Halves hv{act_empty + 1, act_empty + 3};
+  // [2][8 warps][128 columns]: a layer's partials go to the other buffer than the previous layer's, so a warp that is
+  // ahead never overwrites partials that the rest of its warpgroup has still to read
+  float* red = reinterpret_cast<float*>(smem + CH_ENC);
   if (threadIdx.x == 0) {
     for (int i = 0; i < CH_STAGES; ++i) {
       mbar_init(&full[i], 1);
@@ -1472,6 +1512,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) dgrad_chain_kernel(const DgCh
     }
     mbar_init(act_full, 1);
     mbar_init(act_empty, CONSUMERS / 32);
+    for (int h = 0; h < 2; ++h) {
+      mbar_init(&hv.rd[h], CONSUMERS / 32);
+      mbar_init(&hv.wr[h], 4);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   __syncthreads();
@@ -1482,7 +1526,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) dgrad_chain_kernel(const DgCh
   }
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
   const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int it = 0, n = 0;
+  // p: generations of the activation buffer the epilogues have written (G[l-1] at layers l > 1).  Layer top reads the
+  // producer's copy (act_full), a layer l < top generation p - 1; a layer l > 1 writes generation p once every warp has
+  // read what it overwrites, the same layer's input.  r: layers run, for the column sums' buffer.
+  int it = 0, n = 0, p = 0, r = 0;
   for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
     if (t * CH_M >= M) {
       dg_zero_tile<DP, TP>(c, t);
@@ -1490,13 +1537,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) dgrad_chain_kernel(const DgCh
     }
     mbar_wait(act_full, n & 1);
     ++n;
-    for (int l = c.top; l >= 1; --l) {
+    for (int l = c.top; l >= 1; --l, ++r) {
       uint4 wd[2];
       dg_mask_words(wd, c.bits[l], M, t);
       float acc[64];
-      chain_mma<false, DP>(acc, CH_KS, CH_KS, it, full, empty);
+      chain_mma<false, DP>(acc, CH_KS, CH_KS, it, full, empty, hv, l == c.top ? -1 : (p - 1) & 1, l > 1);
       if (l == 1 && lane == 0) mbar_arrive(act_empty);
-      consumer_sync();          // both warpgroups have read G[l]
+      float* rb = red + (r & 1) * (CONSUMERS / 32) * TN;
       const uint32_t wds[2][4] = {{wd[0].x, wd[0].y, wd[0].z, wd[0].w}, {wd[1].x, wd[1].y, wd[1].z, wd[1].w}};
 #pragma unroll
       for (int i = 0; i < 64; i += 2) {     // columns 8 j + 2 (lane % 4) + {0, 1} of word j / 4, j = i / 4
@@ -1513,17 +1560,19 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) dgrad_chain_kernel(const DgCh
           float s = acc[4 * j + cc] + acc[4 * j + 2 + cc];
 #pragma unroll
           for (int o = 4; o < 32; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-          if (lane < 4) red[w * TN + 8 * j + 2 * lane + cc] = s;
+          if (lane < 4) rb[w * TN + 8 * j + 2 * lane + cc] = s;
         }
       if (l > 1) {
-        dg_split<DP>(acc, reinterpret_cast<uint16_t*>(smem), CH_HALF, CH_HALF / 2);
-        fence_proxy_async();    // the stores into the activation buffer, before the MMAs that read them
+        mbar_wait(&hv.rd[wg], p & 1);     // every warp has read this half of G[l]
+        chain_split<false, DP>(acc, reinterpret_cast<uint16_t*>(smem), CH_HALF, CH_HALF / 2);
+        chain_written(hv);
+        ++p;
       }
-      consumer_sync();
+      warpgroup_sync();         // the warpgroup's partials are in rb
       {
         float s = 0.f;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) s += red[(4 * wg + i) * TN + (threadIdx.x & (TN - 1))];
+        for (int i = 0; i < 4; ++i) s += rb[(4 * wg + i) * TN + (threadIdx.x & (TN - 1))];
         atomicAdd(c.db[l] + threadIdx.x, s);
       }
       // the transposed image as epilogue<..., TRP>'s: rows n (row tile wg), k = m (k-step 2 t + wq / 2)
@@ -1542,7 +1591,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) dgrad_chain_kernel(const DgCh
           }
       }
       if (c.row[l])
-        dg_split<DP>(acc, c.row[l] + (size_t)(t >> 1) * CH_KS * 2 * TILE_ELEMS + (t & 1) * (CH_M * TK), 2 * TILE_ELEMS, TILE_ELEMS);
+        chain_split<false, DP>(acc, c.row[l] + (size_t)(t >> 1) * CH_KS * 2 * TILE_ELEMS + (t & 1) * (CH_M * TK), 2 * TILE_ELEMS, TILE_ELEMS);
     }
   }
 }
