@@ -303,6 +303,16 @@ int sparf_mcubes_count(const float* vol, int64_t nx, int64_t ny, int64_t nz, flo
                        size_t workspace_bytes, sparf_stream_t stream);
 int sparf_mcubes_emit(const float* vol, int64_t nx, int64_t ny, int64_t nz, float iso, float* verts, int64_t* faces,
                       void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+/* Masked marching cubes: the same two-call contract, workspace and arguments, for volumes whose unobserved points are
+ * NaN (the TSDF volumes of sparf_tsdf_integrate).  A cell with a non-finite corner emits no triangle, and a vertex is
+ * emitted only if an emitted triangle uses it; the remaining vertices keep the dense order (linear index of the owner
+ * point p, then axis) and are renumbered 0, 1, ...; positions, triangle order and orientation are the dense ones.  So on
+ * a volume without NaN or infinity the output is byte-identical to sparf_mcubes_count / _emit's, and where observed
+ * inside space meets unobserved space no false surface appears. */
+int sparf_mcubes_count_masked(const float* vol, int64_t nx, int64_t ny, int64_t nz, float iso, int64_t* totals,
+                              void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+int sparf_mcubes_emit_masked(const float* vol, int64_t nx, int64_t ny, int64_t nz, float iso, float* verts,
+                             int64_t* faces, void* workspace, size_t workspace_bytes, sparf_stream_t stream);
 /* Host only: the case table, table [256][3 * SPARF_MCUBES_MAX_TRIS] (host int8).  Row c lists the triangles of case c
  * as cell-edge ids, three per triangle, padded with -1.  Edge e = 4a + m runs along axis a from the corner whose
  * offsets along the two other axes b < b' are (m & 1, m >> 1); its vertex is owned by that corner.  The table is
@@ -357,6 +367,36 @@ int sparf_mcubes_sparse_count(const float* sigma_blocks, int32_t res, const int3
 int sparf_mcubes_sparse_emit(const float* sigma_blocks, int32_t res, const int32_t* slots, const int64_t* block_ids,
                              int64_t n_active, float iso, int64_t max_verts, int64_t max_faces, float* verts,
                              int64_t* faces, void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+
+/* ---------------------------------------------------------------- TSDF fusion
+ * Coloured meshes from rendered depth and colour maps (sparf_b200/tsdf.py): the maps of B views are integrated into a
+ * truncated signed distance volume, whose zero level the masked marching cubes above extracts.
+ *   volume:    BARF's lattice, n points per axis at axis [n] (fp32, device; mesh.lattice_axis(res, range), n = res + 1),
+ *              point (i, j, k) = (axis[i], axis[j], axis[k]), linear index (i*n + j)*n + k (axis 0 = x, k fastest).  The
+ *              caller owns the state: tsdf [n^3] (initially 1), weight [n^3] (initially 0), color [n^3][3] (initially 0).
+ *   views:     pose_w2c [B,3,4] = (R | t), intr [B,3,3] = K (its last row is taken to be (0, 0, 1)), depth [B,H,W] =
+ *              camera z-depth (the renderer's t: a camera-space ray has z = 1), rgb [B,H,W,3] or NULL, valid [B,H,W]
+ *              (uint8, nonzero = valid) or NULL = all valid.
+ *   rule:      every lattice point p takes the views b = 0 .. B-1 in order, each op rounded to nearest (no FMA):
+ *                x_r = __fadd_rn(__fadd_rn(__fadd_rn(R_r0 p_x, R_r1 p_y), R_r2 p_z), t_r)   (products __fmul_rn)
+ *                skip the view unless x_z > 0;
+ *                u = __fdiv_rn(K_00 x_x + K_01 x_y + K_02 x_z, x_z), v = __fdiv_rn(K_10 x_x + K_11 x_y + K_12 x_z, x_z)
+ *                    (the sums left to right, as x_r's); skip unless 0 <= u < W and 0 <= v < H;
+ *                pixel (floor u, floor v): this inverts the ray generation above, whose pixel centres sit at +0.5, so
+ *                    a point on the ray of pixel (i, j) lands in pixel (i, j);
+ *                skip if valid is 0 there, or unless d = depth[b, floor v, floor u] is finite and > 0;
+ *                s = __fsub_rn(d, x_z); skip if s < -trunc (the point is occluded);
+ *                f = min(1, __fdiv_rn(s, trunc)); W' = W + 1; tsdf += (f - tsdf) / W'; color += (rgb - color) / W' per
+ *                    channel, only when rgb is given; W = W'.
+ *              The updates equal (W tsdf + f) / (W + 1) and (W color + rgb) / (W + 1); written as increments they leave
+ *              a value that every view observes alike exactly unchanged.  Observation weight 1.
+ *   writes:    each point's state once, after all views: no atomics, deterministic, no synchronisation, capturable.
+ *              color is neither read nor written when rgb is NULL (it may then be NULL).
+ * SPARF_ERR_INVALID for n < 2 or n^3 > 2^38, trunc not finite or <= 0, B, H or W < 1, H or W > 2^24, B*H*W > 2^60, and
+ * NULL for a required pointer. */
+int sparf_tsdf_integrate(const float* axis, int32_t n, float trunc, int32_t B, int32_t H, int32_t W,
+                         const float* pose_w2c, const float* intr, const float* depth, const float* rgb,
+                         const uint8_t* valid, float* tsdf, float* weight, float* color, sparf_stream_t stream);
 
 /* ---------------------------------------------------------------- occupancy grid
  * Empty-space skipping for inference renders (sparf_b200/occupancy.py): a bitfield over the box [r0, r1]^3 split into

@@ -73,6 +73,8 @@ _SIGNATURES = {
     "sparf_mcubes_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64]),
     "sparf_mcubes_count": (c_int32, [_P, c_int64, c_int64, c_int64, c_float, _P, _P, c_size_t, _P]),
     "sparf_mcubes_emit": (c_int32, [_P, c_int64, c_int64, c_int64, c_float, _P, _P, _P, c_size_t, _P]),
+    "sparf_mcubes_count_masked": (c_int32, [_P, c_int64, c_int64, c_int64, c_float, _P, _P, c_size_t, _P]),
+    "sparf_mcubes_emit_masked": (c_int32, [_P, c_int64, c_int64, c_int64, c_float, _P, _P, _P, c_size_t, _P]),
     "sparf_mcubes_table": (c_int32, [_P]),
     "sparf_mcubes_sparse_workspace_bytes": (c_size_t, [c_int32, c_int64, c_int64]),
     "sparf_mcubes_sparse_classify": (c_int32, [_P, c_int32, c_float, _P, _P, _P, c_size_t, _P]),
@@ -81,6 +83,8 @@ _SIGNATURES = {
     "sparf_mcubes_sparse_count": (c_int32, [_P, c_int32, _P, _P, c_int64, c_float, _P, _P, c_size_t, _P]),
     "sparf_mcubes_sparse_emit": (c_int32, [_P, c_int32, _P, _P, c_int64, c_float, c_int64, c_int64, _P, _P, _P, c_size_t,
                                            _P]),
+    "sparf_tsdf_integrate": (c_int32, [_P, c_int32, c_float, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, _P, _P, _P,
+                                       _P]),
     "sparf_occupancy_build": (c_int32, [_P, c_int32, c_float, _P, _P]),
     "sparf_occupancy_workspace_bytes": (c_size_t, [c_int64, c_int32]),
     "sparf_occupancy_count": (c_int32, [c_int64, c_int32, _P, _P, _P, _P, c_int32, c_float, c_float, _P, _P, c_size_t, _P]),

@@ -7,6 +7,8 @@
 //          the rank of the edge's axis among that point's crossing axes.
 // Workspace: per point one uint32 (local vertex offset << 3 | crossing mask) and one uint32 (local triangle offset),
 // per tile two int64: 8 B per point + 16 B per 2048 points.
+// The masked mode (kMasked) of both passes drops the cells with a non-finite corner, and with them every crossing edge
+// that no remaining cell has; the same passes then renumber what is left.
 #include <cstring>
 
 #include "common.cuh"
@@ -60,6 +62,36 @@ __device__ __forceinline__ int edge_mask(const Vol& V, long long p, long long i,
   return m;
 }
 
+// every corner of the cell with origin p is finite
+__device__ __forceinline__ bool cell_finite(const Vol& V, long long p) {
+  bool ok = true;
+#pragma unroll
+  for (int q = 0; q < 8; ++q) ok &= isfinite(__ldg(V.v + p + (q & 1) * V.nyz + ((q >> 1) & 1) * V.nz + ((q >> 2) & 1)));
+  return ok;
+}
+
+// bits of mask m (edge_mask at (i,j,k)) whose lattice edge lies in a cell with finite corners.  The cells of the edge
+// along a have origin p - d e_b - d' e_b' (d, d' in {0, 1}) for the two other axes b < b'.  A cell of the table uses
+// every crossing edge it has, so these are the edges of the triangles kept.
+__device__ __forceinline__ int finite_cell_edges(const Vol& V, long long p, long long i, long long j, long long k, int m) {
+  const long long c[3] = {i, j, k}, n[3] = {V.nx, V.ny, V.nz}, stride[3] = {V.nyz, V.nz, 1};
+  int out = 0;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    if (!(m >> a & 1)) continue;
+    const int b = a == 0 ? 1 : 0, b2 = a == 2 ? 1 : 2;
+    bool used = false;
+#pragma unroll
+    for (int q = 0; q < 4 && !used; ++q) {
+      const long long ob = c[b] - (q & 1), ob2 = c[b2] - (q >> 1);
+      if (ob >= 0 && ob + 1 < n[b] && ob2 >= 0 && ob2 + 1 < n[b2])
+        used = cell_finite(V, p - (q & 1) * stride[b] - (q >> 1) * stride[b2]);
+    }
+    out |= (int)used << a;
+  }
+  return out;
+}
+
 __device__ __forceinline__ void advance(const Vol& V, long long& i, long long& j, long long& k) {
   if (++k == V.nz) {
     k = 0;
@@ -70,8 +102,9 @@ __device__ __forceinline__ void advance(const Vol& V, long long& i, long long& j
   }
 }
 
-// exclusive block scan of two values per thread; tx, ty = the block's totals
-template <typename T, int THREADS>
+// exclusive block scan of two values per thread; tx, ty = the block's totals.  Each TAG has its own shared arrays, so
+// that no two kernels share them and each kernel's shared layout is its own.
+template <typename T, int THREADS, int TAG = 0>
 __device__ __forceinline__ void block_scan2(T& x, T& y, T& tx, T& ty) {
   constexpr int NW = THREADS / 32;
   __shared__ T sx[NW], sy[NW];
@@ -113,16 +146,11 @@ __device__ __forceinline__ void block_scan2(T& x, T& y, T& tx, T& ty) {
   __syncthreads();  // the next call reuses sx, sy
 }
 
-__global__ void __launch_bounds__(kMcThreads) mcubes_count_kernel(Vol V, uint32_t* __restrict__ vpack,
-                                                                  uint32_t* __restrict__ tloc,
-                                                                  longlong2* __restrict__ tiles) {
-  __shared__ unsigned char ntri[256];
-  if (threadIdx.x < 256) {
-    int n = 0;
-    while (n < SPARF_MCUBES_MAX_TRIS && kTableDev[threadIdx.x][3 * n] >= 0) ++n;
-    ntri[threadIdx.x] = (unsigned char)n;
-  }
-  __syncthreads();
+// the count pass of one tile; ntri [256] = the triangle count of each case.  The kernels below own the shared table
+// (a template kernel would place it after block_scan2's arrays).
+template <bool kMasked>
+__device__ __forceinline__ void count_tile(Vol V, const unsigned char* ntri, uint32_t* __restrict__ vpack,
+                                           uint32_t* __restrict__ tloc, longlong2* __restrict__ tiles) {
   const long long p0 = (long long)blockIdx.x * kMcTile + (long long)threadIdx.x * kMcItems;
   int mask[kMcItems], nt[kMcItems];
   int sv = 0, st = 0;
@@ -135,7 +163,8 @@ __global__ void __launch_bounds__(kMcThreads) mcubes_count_kernel(Vol V, uint32_
       mask[u] = nt[u] = 0;
       if (p < V.n) {
         mask[u] = edge_mask(V, p, i, j, k, V.in(p));
-        if (i + 1 < V.nx && j + 1 < V.ny && k + 1 < V.nz) nt[u] = ntri[cell_case(V, p)];
+        if constexpr (kMasked) mask[u] = finite_cell_edges(V, p, i, j, k, mask[u]);
+        if (i + 1 < V.nx && j + 1 < V.ny && k + 1 < V.nz && (!kMasked || cell_finite(V, p))) nt[u] = ntri[cell_case(V, p)];
         advance(V, i, j, k);
       }
       sv += __popc(mask[u]);
@@ -143,7 +172,7 @@ __global__ void __launch_bounds__(kMcThreads) mcubes_count_kernel(Vol V, uint32_
     }
   }
   int tv, tt;
-  block_scan2<int, kMcThreads>(sv, st, tv, tt);
+  block_scan2<int, kMcThreads, kMasked>(sv, st, tv, tt);
   if (p0 < V.n) {
 #pragma unroll
     for (int u = 0; u < kMcItems; ++u) {
@@ -157,6 +186,31 @@ __global__ void __launch_bounds__(kMcThreads) mcubes_count_kernel(Vol V, uint32_
     }
   }
   if (threadIdx.x == 0) tiles[blockIdx.x] = make_longlong2(tv, tt);
+}
+
+__device__ __forceinline__ void fill_ntri(unsigned char* ntri) {
+  if (threadIdx.x < 256) {
+    int n = 0;
+    while (n < SPARF_MCUBES_MAX_TRIS && kTableDev[threadIdx.x][3 * n] >= 0) ++n;
+    ntri[threadIdx.x] = (unsigned char)n;
+  }
+  __syncthreads();
+}
+
+__global__ void __launch_bounds__(kMcThreads) mcubes_count_kernel(Vol V, uint32_t* __restrict__ vpack,
+                                                                  uint32_t* __restrict__ tloc,
+                                                                  longlong2* __restrict__ tiles) {
+  __shared__ unsigned char ntri[256];
+  fill_ntri(ntri);
+  count_tile<false>(V, ntri, vpack, tloc, tiles);
+}
+
+__global__ void __launch_bounds__(kMcThreads) mcubes_count_masked_kernel(Vol V, uint32_t* __restrict__ vpack,
+                                                                         uint32_t* __restrict__ tloc,
+                                                                         longlong2* __restrict__ tiles) {
+  __shared__ unsigned char ntri[256];
+  fill_ntri(ntri);
+  count_tile<true>(V, ntri, vpack, tloc, tiles);
 }
 
 // tile totals -> exclusive 64-bit tile bases (in place); totals = {V, F}
@@ -192,6 +246,7 @@ __global__ void __launch_bounds__(kScanThreads) mcubes_scan_kernel(longlong2* __
   }
 }
 
+template <bool kMasked>
 __global__ void __launch_bounds__(kMcThreads) mcubes_emit_kernel(Vol V, const uint32_t* __restrict__ vpack,
                                                                  const uint32_t* __restrict__ tloc,
                                                                  const longlong2* __restrict__ tiles,
@@ -224,7 +279,7 @@ __global__ void __launch_bounds__(kMcThreads) mcubes_emit_kernel(Vol V, const ui
         o[2] = a == 2 ? __fadd_rn(c[2], s) : c[2];
       }
     }
-    if (i + 1 < V.nx && j + 1 < V.ny && k + 1 < V.nz) {
+    if (i + 1 < V.nx && j + 1 < V.ny && k + 1 < V.nz && (!kMasked || cell_finite(V, p))) {
       const signed char* row = tab + cell_case(V, p) * kMcRow;
       int64_t* f = faces + 3 * (base.y + tloc[p]);
       for (int q = 0; q < kMcRow && row[q] >= 0; ++q) {
@@ -266,6 +321,48 @@ Vol make_vol(const float* vol, int64_t nx, int64_t ny, int64_t nz, float iso) {
   return Vol{vol, nx, ny, nz, (long long)ny * nz, (long long)nx * ny * nz, iso};
 }
 
+template <bool kMasked>
+int mcubes_count(const char* what, const float* vol, int64_t nx, int64_t ny, int64_t nz, float iso, int64_t* totals,
+                 void* workspace, size_t workspace_bytes, sparf_stream_t stream) {
+  SPARF_REQUIRE(extents_ok(nx, ny, nz), "%s: extents %lld x %lld x %lld (each >= 2, at most 2^58 points)", what,
+                (long long)nx, (long long)ny, (long long)nz);
+  SPARF_REQUIRE(vol && totals && workspace, "%s: NULL pointer", what);
+  Carve c;
+  const size_t need = carve(nx, ny, nz, workspace, &c);
+  if (workspace_bytes < need) {
+    set_error("%s: workspace %zu B < %zu B", what, workspace_bytes, need);
+    return SPARF_ERR_WORKSPACE;
+  }
+  SPARF_REQUIRE(c.ntiles < (1ll << 31), "%s: volume too large", what);
+  cudaStream_t s = (cudaStream_t)stream;
+  const Vol V = make_vol(vol, nx, ny, nz, iso);
+  (kMasked ? mcubes_count_masked_kernel : mcubes_count_kernel)<<<(unsigned)c.ntiles, kMcThreads, 0, s>>>(
+      V, c.vpack, c.tloc, c.tiles);
+  SPARF_CHECK_LAUNCH(kMasked ? "mcubes_count_masked_kernel" : "mcubes_count_kernel");
+  mcubes_scan_kernel<<<1, kScanThreads, 0, s>>>(c.tiles, c.ntiles, totals);
+  SPARF_CHECK_LAUNCH("mcubes_scan_kernel");
+  return SPARF_OK;
+}
+
+template <bool kMasked>
+int mcubes_emit(const char* what, const float* vol, int64_t nx, int64_t ny, int64_t nz, float iso, float* verts,
+                int64_t* faces, void* workspace, size_t workspace_bytes, sparf_stream_t stream) {
+  SPARF_REQUIRE(extents_ok(nx, ny, nz), "%s: extents %lld x %lld x %lld (each >= 2, at most 2^58 points)", what,
+                (long long)nx, (long long)ny, (long long)nz);
+  SPARF_REQUIRE(vol && workspace, "%s: NULL pointer", what);
+  Carve c;
+  const size_t need = carve(nx, ny, nz, workspace, &c);
+  if (workspace_bytes < need) {
+    set_error("%s: workspace %zu B < %zu B", what, workspace_bytes, need);
+    return SPARF_ERR_WORKSPACE;
+  }
+  SPARF_REQUIRE(c.ntiles < (1ll << 31), "%s: volume too large", what);
+  mcubes_emit_kernel<kMasked><<<(unsigned)c.ntiles, kMcThreads, 0, (cudaStream_t)stream>>>(
+      make_vol(vol, nx, ny, nz, iso), c.vpack, c.tloc, c.tiles, verts, faces);
+  SPARF_CHECK_LAUNCH(kMasked ? "mcubes_emit_kernel<true>" : "mcubes_emit_kernel<false>");
+  return SPARF_OK;
+}
+
 }  // namespace
 }  // namespace sparf
 
@@ -277,41 +374,23 @@ extern "C" size_t sparf_mcubes_workspace_bytes(int64_t nx, int64_t ny, int64_t n
 
 extern "C" int sparf_mcubes_count(const float* vol, int64_t nx, int64_t ny, int64_t nz, float iso, int64_t* totals,
                                   void* workspace, size_t workspace_bytes, sparf_stream_t stream) {
-  SPARF_REQUIRE(extents_ok(nx, ny, nz), "mcubes_count: extents %lld x %lld x %lld (each >= 2, at most 2^58 points)",
-                (long long)nx, (long long)ny, (long long)nz);
-  SPARF_REQUIRE(vol && totals && workspace, "mcubes_count: NULL pointer");
-  Carve c;
-  const size_t need = carve(nx, ny, nz, workspace, &c);
-  if (workspace_bytes < need) {
-    set_error("mcubes_count: workspace %zu B < %zu B", workspace_bytes, need);
-    return SPARF_ERR_WORKSPACE;
-  }
-  SPARF_REQUIRE(c.ntiles < (1ll << 31), "mcubes_count: volume too large");
-  cudaStream_t s = (cudaStream_t)stream;
-  const Vol V = make_vol(vol, nx, ny, nz, iso);
-  mcubes_count_kernel<<<(unsigned)c.ntiles, kMcThreads, 0, s>>>(V, c.vpack, c.tloc, c.tiles);
-  SPARF_CHECK_LAUNCH("mcubes_count_kernel");
-  mcubes_scan_kernel<<<1, kScanThreads, 0, s>>>(c.tiles, c.ntiles, totals);
-  SPARF_CHECK_LAUNCH("mcubes_scan_kernel");
-  return SPARF_OK;
+  return mcubes_count<false>("mcubes_count", vol, nx, ny, nz, iso, totals, workspace, workspace_bytes, stream);
 }
 
 extern "C" int sparf_mcubes_emit(const float* vol, int64_t nx, int64_t ny, int64_t nz, float iso, float* verts,
                                  int64_t* faces, void* workspace, size_t workspace_bytes, sparf_stream_t stream) {
-  SPARF_REQUIRE(extents_ok(nx, ny, nz), "mcubes_emit: extents %lld x %lld x %lld (each >= 2, at most 2^58 points)",
-                (long long)nx, (long long)ny, (long long)nz);
-  SPARF_REQUIRE(vol && workspace, "mcubes_emit: NULL pointer");
-  Carve c;
-  const size_t need = carve(nx, ny, nz, workspace, &c);
-  if (workspace_bytes < need) {
-    set_error("mcubes_emit: workspace %zu B < %zu B", workspace_bytes, need);
-    return SPARF_ERR_WORKSPACE;
-  }
-  SPARF_REQUIRE(c.ntiles < (1ll << 31), "mcubes_emit: volume too large");
-  mcubes_emit_kernel<<<(unsigned)c.ntiles, kMcThreads, 0, (cudaStream_t)stream>>>(make_vol(vol, nx, ny, nz, iso), c.vpack,
-                                                                                  c.tloc, c.tiles, verts, faces);
-  SPARF_CHECK_LAUNCH("mcubes_emit_kernel");
-  return SPARF_OK;
+  return mcubes_emit<false>("mcubes_emit", vol, nx, ny, nz, iso, verts, faces, workspace, workspace_bytes, stream);
+}
+
+extern "C" int sparf_mcubes_count_masked(const float* vol, int64_t nx, int64_t ny, int64_t nz, float iso,
+                                         int64_t* totals, void* workspace, size_t workspace_bytes,
+                                         sparf_stream_t stream) {
+  return mcubes_count<true>("mcubes_count_masked", vol, nx, ny, nz, iso, totals, workspace, workspace_bytes, stream);
+}
+
+extern "C" int sparf_mcubes_emit_masked(const float* vol, int64_t nx, int64_t ny, int64_t nz, float iso, float* verts,
+                                        int64_t* faces, void* workspace, size_t workspace_bytes, sparf_stream_t stream) {
+  return mcubes_emit<true>("mcubes_emit_masked", vol, nx, ny, nz, iso, verts, faces, workspace, workspace_bytes, stream);
 }
 
 extern "C" int sparf_mcubes_table(int8_t* table) {

@@ -189,14 +189,16 @@ def extract_mesh_sparse(opt, nerf, normals: bool = False, engine=None, stats=Non
     return out
 
 
-def write_ply(path, vertices, faces, normals=None) -> None:
-    """Binary little-endian PLY: float x, y, z (and nx, ny, nz) per vertex, a uchar-counted int list per face"""
+def write_ply(path, vertices, faces, normals=None, colors=None) -> None:
+    """Binary little-endian PLY: float x, y, z (and nx, ny, nz) per vertex, then, when colors [V, 3] is given, uchar
+    red, green, blue = round(clamp(c, 0, 1) * 255) (to nearest, ties to even); a uchar-counted int list per face"""
     as_np = lambda x: x.detach().cpu().numpy() if torch.is_tensor(x) else np.asarray(x)
     v = as_np(vertices).astype(np.float32).reshape(-1, 3)
     f = as_np(faces).astype(np.int64).reshape(-1, 3)
     assert f.size == 0 or (f.min() >= 0 and f.max() < min(len(v), 2 ** 31)), "face ids out of range"
     names = ["x", "y", "z"] + (["nx", "ny", "nz"] if normals is not None else [])
-    vert = np.empty(len(v), np.dtype([(k, "<f4") for k in names]))
+    rgb = ["red", "green", "blue"] if colors is not None else []
+    vert = np.empty(len(v), np.dtype([(k, "<f4") for k in names] + [(k, "u1") for k in rgb]))
     for c, k in enumerate("xyz"):
         vert[k] = v[:, c]
     if normals is not None:
@@ -204,11 +206,17 @@ def write_ply(path, vertices, faces, normals=None) -> None:
         assert len(nrm) == len(v)
         for c, k in enumerate(["nx", "ny", "nz"]):
             vert[k] = nrm[:, c]
+    if colors is not None:
+        col = as_np(colors).astype(np.float32).reshape(-1, 3)
+        assert len(col) == len(v)
+        col = np.round(np.clip(col, 0.0, 1.0) * np.float32(255)).astype(np.uint8)
+        for c, k in enumerate(rgb):
+            vert[k] = col[:, c]
     face = np.empty(len(f), np.dtype([("n", "u1"), ("v", "<i4", (3,))]))
     face["n"] = 3
     face["v"] = f
     header = ["ply", "format binary_little_endian 1.0", "element vertex %d" % len(v)]
-    header += ["property float %s" % k for k in names]
+    header += ["property float %s" % k for k in names] + ["property uchar %s" % k for k in rgb]
     header += ["element face %d" % len(f), "property list uchar int vertex_indices", "end_header"]
     with open(path, "wb") as fh:
         fh.write(("\n".join(header) + "\n").encode("ascii"))

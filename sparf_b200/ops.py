@@ -657,18 +657,30 @@ def marching_cubes(vol, iso: float):
     [F, 3] int64), on vol's device; the semantics of mcubes.marching_cubes, specified in include/sparf_b200.h.  One
     device-to-host copy: the two totals that size the outputs.  Not differentiable."""
     L = _lib.lib()
+    return _marching_cubes(vol, iso, L.sparf_mcubes_count, L.sparf_mcubes_emit, "mcubes")
+
+
+@torch.no_grad()
+@_on_tensor_device
+def marching_cubes_masked(vol, iso: float):
+    """marching_cubes for a volume whose unobserved points are NaN: a cell with a non-finite corner emits no triangle,
+    and only the vertices the remaining triangles use are kept, renumbered in the dense order (sparf_mcubes_count_masked
+    / _emit_masked).  On a volume without NaN or infinity the output is marching_cubes's, byte for byte."""
+    L = _lib.lib()
+    return _marching_cubes(vol, iso, L.sparf_mcubes_count_masked, L.sparf_mcubes_emit_masked, "mcubes_masked")
+
+
+def _marching_cubes(vol, iso, count, emit, what):
     v = _f32c(vol)
     assert v.dim() == 3, "marching_cubes takes a 3-D volume"
     nx, ny, nz = v.shape
-    ws = torch.empty(max(L.sparf_mcubes_workspace_bytes(nx, ny, nz), 1), dtype=torch.uint8, device=v.device)
+    ws = torch.empty(max(_lib.lib().sparf_mcubes_workspace_bytes(nx, ny, nz), 1), dtype=torch.uint8, device=v.device)
     totals = torch.empty(2, dtype=torch.int64, device=v.device)
-    check(L.sparf_mcubes_count(_ptr(v), nx, ny, nz, float(iso), _ptr(totals), _ptr(ws), ws.numel(), _stream()),
-          "mcubes_count")
+    check(count(_ptr(v), nx, ny, nz, float(iso), _ptr(totals), _ptr(ws), ws.numel(), _stream()), what + "_count")
     n_verts, n_faces = totals.tolist()
     verts = torch.empty(n_verts, 3, device=v.device, dtype=torch.float32)
     faces = torch.empty(n_faces, 3, device=v.device, dtype=torch.int64)
-    check(L.sparf_mcubes_emit(_ptr(v), nx, ny, nz, float(iso), _ptr(verts), _ptr(faces), _ptr(ws), ws.numel(), _stream()),
-          "mcubes_emit")
+    check(emit(_ptr(v), nx, ny, nz, float(iso), _ptr(verts), _ptr(faces), _ptr(ws), ws.numel(), _stream()), what + "_emit")
     return verts, faces
 
 

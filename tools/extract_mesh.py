@@ -4,12 +4,19 @@ opt.trimesh, on the GPU).
 
     python tools/extract_mesh.py model.pth.tar --out mesh.ply [--network nerf|nerf_fine] [--res 128]
                                  [--range -1.2 1.2] [--thres 25] [--normals] [--barf-c2f START END] [--sparse]
+    python tools/extract_mesh.py model.pth.tar --out mesh.ply --tsdf cameras.npz [--res 128] [--range -1.2 1.2]
+                                 [--trunc T] [--samples 128] [--samples-fine 128] [--barf-c2f START END]
 
 The snapshot is what the reference's trainer saves (base_trainer.py:196-216): the model dict is ckpt["state_dict"],
 with the Graph's keys nerf.* / nerf_fine.* (or, from a joint pose trainer, those under "nerf_net").  The architecture
 is read from the tensor shapes.  The BARF mask applies at the snapshot's progress when --barf-c2f gives the schedule
 the model was trained with.  --sparse extracts with mesh.extract_mesh_sparse's phases (the density only in the 8^3-cell
 blocks near the surface; for high resolutions) and also prints the active-block count and the points evaluated.
+--tsdf CAMERAS fuses renders instead (sparf_b200.tsdf): a Graph with both networks of the snapshot (the fine one when
+present) renders the views of CAMERAS, a .npz or .pt file with pose_w2c [B,3,4], intr [B,3,3], H, W and depth_range [2]
+(metric near, far), with --samples / --samples-fine samples per ray; the depth and colour maps are integrated into a TSDF
+volume over --res / --range with truncation --trunc (default tsdf.TRUNC_VOXELS voxels), and the coloured mesh of its
+zero level is written.
 Prints V, F and the time of each phase.
 """
 import argparse
@@ -41,6 +48,70 @@ def opt_from_state_dict(sd, barf_c2f=None):
     return opt
 
 
+def graph_opt_from_state_dict(sd, barf_c2f, depth_range, samples, samples_fine):
+    """The options of a Graph with the networks of a snapshot's state dict (keys nerf.* and, if present, nerf_fine.*) that
+    renders metric-depth views deterministically (val mode) with the given samples per ray"""
+    from sparf_b200.utils.edict import edict
+    opt = opt_from_state_dict({k[len("nerf."):]: v for k, v in sd.items() if k.startswith("nerf.")}, barf_c2f)
+    fine = any(k.startswith("nerf_fine.") for k in sd)
+    opt.nerf = edict(view_dep=True, depth=edict(param="metric", range=[float(x) for x in depth_range]),
+                     sample_intvs=samples, sample_stratified=False, fine_sampling=fine, sample_intvs_fine=samples_fine,
+                     rand_rays=1024, density_noise_reg=False, setbg_opaque=False)
+    opt.camera = edict(model="perspective", ndc=False)
+    opt.mask_img, opt.max_iter = False, 1
+    return opt
+
+
+def load_cameras(path):
+    """pose_w2c [B,3,4], intr [B,3,3] (fp32 tensors), H, W, depth_range (near, far) of a .npz or .pt camera file"""
+    import numpy as np
+    if path.endswith(".npz"):
+        with np.load(path) as z:
+            cams = {k: z[k] for k in z.files}
+    else:
+        cams = torch.load(path, map_location="cpu", weights_only=False)
+    t = lambda x: torch.as_tensor(np.asarray(x), dtype=torch.float32)
+    return (t(cams["pose_w2c"]), t(cams["intr"]), int(cams["H"]), int(cams["W"]),
+            tuple(float(x) for x in np.asarray(cams["depth_range"]).reshape(2)))
+
+
+def main_tsdf(args):
+    from sparf_b200 import mesh, tsdf
+    from sparf_b200.renderer import Graph
+    t0 = time.perf_counter()
+    sd = torch.load(args.snapshot, map_location="cpu", weights_only=False)["state_dict"]
+    sd = sd.get("nerf_net", sd)
+    assert any(k.startswith("nerf.") for k in sd), "the snapshot has no nerf.* tensors"
+    pose, intr, H, W, depth_range = load_cameras(args.tsdf)
+    opt = graph_opt_from_state_dict(sd, args.barf_c2f, depth_range, args.samples, args.samples_fine)
+    graph = Graph(opt, torch.device("cuda"))
+    graph.load_state_dict({k: v for k, v in sd.items() if k.startswith(("nerf.", "nerf_fine."))})
+    vol = tsdf.TSDFVolume(res=args.res, range=args.range, trunc=args.trunc)
+    phases = {"load": time.perf_counter() - t0}
+
+    def phase(name, fn):
+        torch.cuda.synchronize()
+        t = time.perf_counter()
+        out = fn()
+        torch.cuda.synchronize()
+        phases[name] = phases.get(name, 0.0) + time.perf_counter() - t
+        return out
+
+    # tsdf.fuse_renders, with the renders and the integrations timed apart
+    batches = tsdf.render_batches(opt, graph, pose, intr, H, W, depth_range, device=vol.tsdf.device)
+    while True:
+        batch = phase("render", lambda: next(batches, None))
+        if batch is None:
+            break
+        phase("integrate", lambda: tsdf.integrate_(vol, batch[0], batch[1], batch[2], rgb=batch[3], valid=batch[4]))
+    m = phase("marching_cubes", lambda: tsdf.extract_mesh(vol))
+    phase("write_ply", lambda: mesh.write_ply(args.out, m["vertices"], m["faces"], colors=m["colors"]))
+    print("%s: V %d, F %d (TSDF of %d views %dx%d, res %d, range %s, trunc %g)"
+          % (args.out, m["vertices"].shape[0], m["faces"].shape[0], pose.shape[0], H, W, vol.res, list(vol.range),
+             vol.trunc))
+    print("  " + ", ".join("%s %.3f s" % kv for kv in phases.items()))
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("snapshot")
@@ -52,8 +123,14 @@ def main(argv=None):
     ap.add_argument("--normals", action="store_true")
     ap.add_argument("--barf-c2f", type=float, nargs=2, default=None)
     ap.add_argument("--sparse", action="store_true", help="evaluate only the blocks near the surface (res: multiple of 8)")
+    ap.add_argument("--tsdf", metavar="CAMERAS", default=None, help="fuse renders of these cameras (.npz / .pt) instead")
+    ap.add_argument("--trunc", type=float, default=None, help="TSDF truncation in world units (--tsdf)")
+    ap.add_argument("--samples", type=int, default=128, help="coarse samples per ray of the renders (--tsdf)")
+    ap.add_argument("--samples-fine", type=int, default=128, help="fine samples per ray of the renders (--tsdf)")
     args = ap.parse_args(argv)
     assert torch.cuda.is_available(), "extract_mesh.py runs on a GPU"
+    if args.tsdf:
+        return main_tsdf(args)
     from sparf_b200 import mesh
     from sparf_b200.frequency_nerf import NeRF
     from sparf_b200.utils.edict import edict
