@@ -398,6 +398,44 @@ int sparf_tsdf_integrate(const float* axis, int32_t n, float trunc, int32_t B, i
                          const float* pose_w2c, const float* intr, const float* depth, const float* rgb,
                          const uint8_t* valid, float* tsdf, float* weight, float* color, sparf_stream_t stream);
 
+/* ---------------------------------------------------------------- mesh components
+ * Floater removal for the meshes above (sparf_b200/mesh.py, keep_components): the connected components of a triangle
+ * mesh, and the mesh of a chosen subset of them.  The extractors' meshes are vertex-welded (one vertex per crossing
+ * lattice edge), so connectivity is read from the face ids alone.
+ *   input:       faces [F][3] (int64) over V vertices, every id in [0, V); 0 <= V, F <= INT32_MAX, F = 0 when V = 0.
+ *                Ids outside [0, V) cause no out-of-bounds access; the results are then unspecified.
+ *   connected:   two vertices are connected when some face holds both; the components are the connected classes of
+ *                vertices, so two triangles that share one vertex are in one component.  A vertex that no face uses is
+ *                a component of its own (with 0 faces); degenerate faces (repeated ids) are allowed.
+ *   labels:      labels [V] (int32): a component's label is the rank of its smallest vertex id among all components'
+ *                smallest vertex ids, so labels run 0 .. C-1 in order of first vertex.  The definition depends neither
+ *                on the schedule nor on the order of the faces: identical bytes on every run.
+ *   face counts: face_counts [C] (int64): the faces of each component, counted by the label of each face's first
+ *                vertex (integer atomics: deterministic).
+ *   selection:   keep [C] (uint8, nonzero = kept).  The kept vertices (those of kept components) in their original
+ *                order are renumbered 0 .. V'-1, vert_ids [V'] (int64, increasing) gets each one's old id, and the kept
+ *                faces (those whose first vertex is kept) are written in their original order with renumbered ids,
+ *                faces_out [F'][3] (int64).  labels must be sparf_mesh_components' labels of the same faces.
+ * sparf_mesh_components writes labels and n_components (device int64, C); the caller reads C to size face_counts and
+ * keep.  sparf_mesh_component_faces zeroes and fills face_counts.  sparf_mesh_select_count writes totals [2] = {V', F'}
+ * (device int64) and leaves the output offsets in the workspace; sparf_mesh_select_emit, enqueued after it on the same
+ * stream with the same arguments and workspace, writes vert_ids and faces_out.  Workspace (shared by all calls):
+ * sparf_mesh_components_workspace_bytes(V, F), 4 B per vertex + 4 B per face + scan scratch; 0 for invalid sizes and
+ * where no CUDA device is current (the scratch is sized for the device).  No call synchronises; all are capturable.  No
+ * kernel runs over an empty vertex or face set; the device counts are still written.  Invalid sizes (also C > V) give
+ * SPARF_ERR_INVALID. */
+size_t sparf_mesh_components_workspace_bytes(int64_t n_verts, int64_t n_faces);
+int sparf_mesh_components(const int64_t* faces, int64_t n_faces, int64_t n_verts, int32_t* labels, int64_t* n_components,
+                          void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+int sparf_mesh_component_faces(const int64_t* faces, int64_t n_faces, int64_t n_verts, const int32_t* labels,
+                               int64_t n_components, int64_t* face_counts, sparf_stream_t stream);
+int sparf_mesh_select_count(const int64_t* faces, int64_t n_faces, int64_t n_verts, const int32_t* labels,
+                            const uint8_t* keep, int64_t n_components, int64_t* totals, void* workspace,
+                            size_t workspace_bytes, sparf_stream_t stream);
+int sparf_mesh_select_emit(const int64_t* faces, int64_t n_faces, int64_t n_verts, const int32_t* labels,
+                           const uint8_t* keep, int64_t n_components, int64_t* vert_ids, int64_t* faces_out,
+                           void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+
 /* ---------------------------------------------------------------- occupancy grid
  * Empty-space skipping for inference renders (sparf_b200/occupancy.py): a bitfield over the box [r0, r1]^3 split into
  * res^3 cells, built from the density lattice sigma [res+1]^3 of mesh.density_grid (lattice point (a,b,c) at

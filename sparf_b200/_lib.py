@@ -85,6 +85,11 @@ _SIGNATURES = {
                                            _P]),
     "sparf_tsdf_integrate": (c_int32, [_P, c_int32, c_float, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, _P, _P, _P,
                                        _P]),
+    "sparf_mesh_components_workspace_bytes": (c_size_t, [c_int64, c_int64]),
+    "sparf_mesh_components": (c_int32, [_P, c_int64, c_int64, _P, _P, _P, c_size_t, _P]),
+    "sparf_mesh_component_faces": (c_int32, [_P, c_int64, c_int64, _P, c_int64, _P, _P]),
+    "sparf_mesh_select_count": (c_int32, [_P, c_int64, c_int64, _P, _P, c_int64, _P, _P, c_size_t, _P]),
+    "sparf_mesh_select_emit": (c_int32, [_P, c_int64, c_int64, _P, _P, c_int64, _P, _P, _P, c_size_t, _P]),
     "sparf_occupancy_build": (c_int32, [_P, c_int32, c_float, _P, _P]),
     "sparf_occupancy_workspace_bytes": (c_size_t, [c_int64, c_int32]),
     "sparf_occupancy_count": (c_int32, [c_int64, c_int32, _P, _P, _P, _P, c_int32, c_float, c_float, _P, _P, c_size_t, _P]),

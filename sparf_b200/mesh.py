@@ -1,9 +1,10 @@
 """Mesh extraction from a trained NeRF, BARF's recipe on the device: the density on the lattice of `opt.trimesh`
 (train_settings/default_config.py:267-271), marching cubes (csrc/mcubes.cu), world coordinates, optional normals from
-the density's gradient, and a binary PLY writer.
+the density's gradient, floater removal by connected components (keep_components), and a binary PLY writer.
 
     from sparf_b200 import mesh
     m = mesh.extract_mesh(opt, graph.nerf, normals=True)        # or graph.nerf_fine
+    m = mesh.keep_components(m, largest=1)                      # optional: drop the floaters
     mesh.write_ply("scene.ply", m["vertices"], m["faces"], m["normals"])
 """
 from __future__ import annotations
@@ -186,6 +187,39 @@ def extract_mesh_sparse(opt, nerf, normals: bool = False, engine=None, stats=Non
     out = dict(vertices=to_world(verts, res, rng), faces=faces)
     if normals:
         out["normals"] = density_normals(nerf, out["vertices"], engine=engine)
+    return out
+
+
+VERTEX_KEYS = ("vertices", "normals", "colors")     # the per-vertex entries of the extractors' mesh dicts
+
+
+def keep_components(m: dict, largest=None, min_faces: int = 1, stats=None) -> dict:
+    """Floater removal for a mesh dict of extract_mesh, extract_mesh_sparse or tsdf.extract_mesh: the connected
+    components (ops.mesh_components; two vertices are connected when a face holds both) with at least min_faces faces,
+    and of those, when largest = k, only the k largest by (face count descending, label ascending).  -> a dict with the
+    same keys: the kept faces in their order with renumbered ids, and the kept vertices in their order with their
+    vertices / normals / colors gathered (ops.mesh_select), ready for write_ply.  Other entries are passed on as they
+    are.  stats: an optional dict that receives n_components, n_kept (components kept) and faces_removed."""
+    if largest is not None and (isinstance(largest, bool) or not isinstance(largest, int) or largest < 1):
+        raise ValueError("keep_components: largest must be None or an int >= 1 (got %r)" % (largest,))
+    if isinstance(min_faces, bool) or not isinstance(min_faces, int) or min_faces < 0:
+        raise ValueError("keep_components: min_faces must be an int >= 0 (got %r)" % (min_faces,))
+    faces, n_verts = m["faces"], m["vertices"].shape[0]
+    labels, counts = ops.mesh_components(faces, n_verts)
+    kept = torch.nonzero(counts >= min_faces).flatten()         # increasing labels
+    if largest is not None:
+        order = torch.sort(counts[kept], descending=True, stable=True).indices   # ties: the smaller label first
+        kept = kept[order[:largest]]
+    keep = torch.zeros(counts.numel(), dtype=torch.uint8, device=counts.device)
+    keep[kept] = 1
+    vert_ids, faces_out = ops.mesh_select(faces, n_verts, labels, keep)
+    out = dict(m)
+    out["faces"] = faces_out
+    for k in VERTEX_KEYS:
+        if m.get(k) is not None:
+            out[k] = m[k][vert_ids]
+    if stats is not None:
+        stats.update(n_components=counts.numel(), n_kept=kept.numel(), faces_removed=faces.shape[0] - faces_out.shape[0])
     return out
 
 

@@ -7,6 +7,7 @@ native library is unavailable (no fallback).
 from __future__ import annotations
 
 import ctypes
+import numbers
 from typing import List, Optional, Sequence, Tuple
 
 import torch
@@ -751,6 +752,98 @@ def marching_cubes_sparse(sigma_blocks, res: int, slots, block_ids, iso: float):
     check(L.sparf_mcubes_sparse_emit(_ptr(s), res, _ptr(sl), _ptr(ids), n, float(iso), n_verts, n_faces, _ptr(verts),
                                      _ptr(faces), _ptr(ws), ws.numel(), _stream()), "mcubes_sparse_emit")
     return verts, faces
+
+
+# ------------------------------------------------------------------------------------------------
+# mesh components (no gradient)
+# ------------------------------------------------------------------------------------------------
+MAX_MESH_ELEMENTS = 2 ** 31 - 1     # INT32_MAX: the most vertices and faces sparf_mesh_components takes
+
+
+def _check_faces(faces, n_verts, what):
+    """int(n_verts); ValueError unless faces is a CUDA int64 [F, 3] tensor and 0 <= n_verts, F <= INT32_MAX (no device
+    access)"""
+    if not torch.is_tensor(faces) or faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError("%s: faces must be an int64 tensor [F, 3]" % what)
+    integral = isinstance(n_verts, numbers.Integral) and not isinstance(n_verts, bool)
+    if not integral or not 0 <= n_verts <= MAX_MESH_ELEMENTS:
+        raise ValueError("%s: n_verts must be an int in [0, 2^31 - 1] (got %r)" % (what, n_verts))
+    if faces.shape[0] > MAX_MESH_ELEMENTS or (n_verts == 0 and faces.shape[0]):
+        raise ValueError("%s: %d faces over %d vertices" % (what, faces.shape[0], n_verts))
+    if not faces.is_cuda:
+        raise ValueError("%s: faces must be a CUDA tensor" % what)
+    return int(n_verts)
+
+
+def _check_ids(faces, n_verts, what):
+    """ValueError unless every face id is in [0, n_verts) (one device-to-host copy)"""
+    if faces.numel():
+        lo, hi = torch.aminmax(faces)
+        if lo.item() < 0 or hi.item() >= n_verts:
+            raise ValueError("%s: face ids must lie in [0, %d)" % (what, n_verts))
+
+
+@torch.no_grad()
+@_on_tensor_device
+def mesh_components(faces, n_verts: int):
+    """Connected components of a triangle mesh with faces [F, 3] (int64, CUDA) over n_verts vertices -> (labels
+    [n_verts] int32, face_counts [C] int64), on faces' device (include/sparf_b200.h).  Two vertices are connected when a
+    face holds both; a component's label is the rank of its smallest vertex id, so labels run 0 .. C-1 in order of first
+    vertex; a vertex no face uses is a component with 0 faces.  face_counts counts each face under the label of its first
+    vertex.  Deterministic.  Bad arguments raise ValueError before any library call (one device-to-host copy checks
+    the ids); one more copy reads C."""
+    n_verts = _check_faces(faces, n_verts, "mesh_components")
+    _check_ids(faces, n_verts, "mesh_components")
+    L = _lib.lib()
+    f = faces.contiguous()
+    dev, F = f.device, f.shape[0]
+    labels = torch.empty(n_verts, dtype=torch.int32, device=dev)
+    n_comp = torch.empty(1, dtype=torch.int64, device=dev)
+    ws = torch.empty(max(L.sparf_mesh_components_workspace_bytes(n_verts, F), 1), dtype=torch.uint8, device=dev)
+    check(L.sparf_mesh_components(_ptr(f), F, n_verts, _ptr(labels), _ptr(n_comp), _ptr(ws), ws.numel(), _stream()),
+          "mesh_components")
+    C = int(n_comp.item())
+    counts = torch.empty(C, dtype=torch.int64, device=dev)
+    check(L.sparf_mesh_component_faces(_ptr(f), F, n_verts, _ptr(labels), C, _ptr(counts), _stream()),
+          "mesh_component_faces")
+    return labels, counts
+
+
+@torch.no_grad()
+@_on_tensor_device
+def mesh_select(faces, n_verts: int, labels, keep):
+    """The mesh of the kept components: faces [F, 3] and labels [n_verts] (int32) of mesh_components, keep [C] (bool or
+    uint8, nonzero = kept) -> (vert_ids [V'] int64, the old id of each kept vertex, increasing; faces [F', 3] int64, the
+    kept faces in their original order with renumbered ids).  Gather per-vertex data with vert_ids.  Bad arguments raise
+    ValueError before any library call (device-to-host copies check the ids and labels); one more copy reads V', F'."""
+    what = "mesh_select"
+    n_verts = _check_faces(faces, n_verts, what)
+    if not torch.is_tensor(labels) or labels.dtype != torch.int32 or labels.shape != (n_verts,):
+        raise ValueError("%s: labels must be an int32 tensor [%d]" % (what, n_verts))
+    if not torch.is_tensor(keep) or keep.dtype not in (torch.uint8, torch.bool) or keep.dim() != 1:
+        raise ValueError("%s: keep must be a uint8 or bool tensor [C]" % what)
+    if keep.numel() > max(n_verts, 0) or (n_verts and not keep.numel()):
+        raise ValueError("%s: keep [%d] cannot be a component mask of %d vertices" % (what, keep.numel(), n_verts))
+    if labels.device != faces.device or keep.device != faces.device:
+        raise ValueError("%s: faces, labels and keep must be on one CUDA device" % what)
+    _check_ids(faces, n_verts, what)
+    if n_verts:
+        lo, hi = torch.aminmax(labels)
+        if lo.item() < 0 or hi.item() >= keep.numel():
+            raise ValueError("%s: labels must lie in [0, %d)" % (what, keep.numel()))
+    L = _lib.lib()
+    f, lab, k = faces.contiguous(), labels.contiguous(), keep.contiguous().view(torch.uint8)
+    dev, F, C = f.device, f.shape[0], k.numel()
+    ws = torch.empty(max(L.sparf_mesh_components_workspace_bytes(n_verts, F), 1), dtype=torch.uint8, device=dev)
+    totals = torch.empty(2, dtype=torch.int64, device=dev)
+    args = (_ptr(f), F, n_verts, _ptr(lab), _ptr(k), C)
+    check(L.sparf_mesh_select_count(*args, _ptr(totals), _ptr(ws), ws.numel(), _stream()), "mesh_select_count")
+    n_v, n_f = totals.tolist()
+    vert_ids = torch.empty(n_v, dtype=torch.int64, device=dev)
+    faces_out = torch.empty(n_f, 3, dtype=torch.int64, device=dev)
+    check(L.sparf_mesh_select_emit(*args, _ptr(vert_ids), _ptr(faces_out), _ptr(ws), ws.numel(), _stream()),
+          "mesh_select_emit")
+    return vert_ids, faces_out
 
 
 # ------------------------------------------------------------------------------------------------

@@ -6,6 +6,7 @@ opt.trimesh, on the GPU).
                                  [--range -1.2 1.2] [--thres 25] [--normals] [--barf-c2f START END] [--sparse]
     python tools/extract_mesh.py model.pth.tar --out mesh.ply --tsdf cameras.npz [--res 128] [--range -1.2 1.2]
                                  [--trunc T] [--samples 128] [--samples-fine 128] [--barf-c2f START END]
+    either form takes [--keep-largest K] [--min-faces N]
 
 The snapshot is what the reference's trainer saves (base_trainer.py:196-216): the model dict is ckpt["state_dict"],
 with the Graph's keys nerf.* / nerf_fine.* (or, from a joint pose trainer, those under "nerf_net").  The architecture
@@ -17,6 +18,9 @@ present) renders the views of CAMERAS, a .npz or .pt file with pose_w2c [B,3,4],
 (metric near, far), with --samples / --samples-fine samples per ray; the depth and colour maps are integrated into a TSDF
 volume over --res / --range with truncation --trunc (default tsdf.TRUNC_VOXELS voxels), and the coloured mesh of its
 zero level is written.
+--keep-largest K and --min-faces N remove floaters from any of these meshes (mesh.keep_components): of the connected
+components with at least N faces only the K largest are kept; the tool then also prints the component counts and times
+a components phase.
 Prints V, F and the time of each phase.
 """
 import argparse
@@ -75,6 +79,18 @@ def load_cameras(path):
             tuple(float(x) for x in np.asarray(cams["depth_range"]).reshape(2)))
 
 
+def filter_components(args, m, phase):
+    """mesh.keep_components of the mesh dict m when --keep-largest or --min-faces is given (printing the counts), else m"""
+    if args.keep_largest is None and args.min_faces is None:
+        return m
+    from sparf_b200 import mesh
+    stats = {}
+    min_faces = 1 if args.min_faces is None else args.min_faces
+    m = phase("components", lambda: mesh.keep_components(m, largest=args.keep_largest, min_faces=min_faces, stats=stats))
+    print("components %d, kept %d, faces removed %d" % (stats["n_components"], stats["n_kept"], stats["faces_removed"]))
+    return m
+
+
 def main_tsdf(args):
     from sparf_b200 import mesh, tsdf
     from sparf_b200.renderer import Graph
@@ -105,6 +121,7 @@ def main_tsdf(args):
             break
         phase("integrate", lambda: tsdf.integrate_(vol, batch[0], batch[1], batch[2], rgb=batch[3], valid=batch[4]))
     m = phase("marching_cubes", lambda: tsdf.extract_mesh(vol))
+    m = filter_components(args, m, phase)
     phase("write_ply", lambda: mesh.write_ply(args.out, m["vertices"], m["faces"], colors=m["colors"]))
     print("%s: V %d, F %d (TSDF of %d views %dx%d, res %d, range %s, trunc %g)"
           % (args.out, m["vertices"].shape[0], m["faces"].shape[0], pose.shape[0], H, W, vol.res, list(vol.range),
@@ -112,7 +129,16 @@ def main_tsdf(args):
     print("  " + ", ".join("%s %.3f s" % kv for kv in phases.items()))
 
 
-def main(argv=None):
+def parse_args(ap, argv):
+    args = ap.parse_args(argv)
+    if args.keep_largest is not None and args.keep_largest < 1:
+        ap.error("--keep-largest must be >= 1")
+    if args.min_faces is not None and args.min_faces < 0:
+        ap.error("--min-faces must be >= 0")
+    return args
+
+
+def build_parser():
     ap = argparse.ArgumentParser()
     ap.add_argument("snapshot")
     ap.add_argument("--out", required=True)
@@ -127,7 +153,15 @@ def main(argv=None):
     ap.add_argument("--trunc", type=float, default=None, help="TSDF truncation in world units (--tsdf)")
     ap.add_argument("--samples", type=int, default=128, help="coarse samples per ray of the renders (--tsdf)")
     ap.add_argument("--samples-fine", type=int, default=128, help="fine samples per ray of the renders (--tsdf)")
-    args = ap.parse_args(argv)
+    ap.add_argument("--keep-largest", type=int, default=None, metavar="K",
+                    help="keep only the K connected components with the most faces")
+    ap.add_argument("--min-faces", type=int, default=None, metavar="N",
+                    help="keep only the connected components with at least N faces (default with --keep-largest: 1)")
+    return ap
+
+
+def main(argv=None):
+    args = parse_args(build_parser(), argv)
     assert torch.cuda.is_available(), "extract_mesh.py runs on a GPU"
     if args.tsdf:
         return main_tsdf(args)
@@ -174,6 +208,8 @@ def main(argv=None):
     del sigma
     verts = mesh.to_world(verts, res, rng)
     normals = phase("normals", lambda: mesh.density_normals(nerf, verts)) if args.normals else None
+    m = filter_components(args, dict(vertices=verts, faces=faces, normals=normals), phase)
+    verts, faces, normals = m["vertices"], m["faces"], m["normals"]
     phase("write_ply", lambda: mesh.write_ply(args.out, verts, faces, normals))
     print("%s: V %d, F %d (res %d, range %s, thres %g)" % (args.out, verts.shape[0], faces.shape[0], res, list(rng), thres))
     print("  " + ", ".join("%s %.3f s" % kv for kv in phases.items()))
