@@ -58,7 +58,8 @@ class FlatGradients:
             self._views.append(v)
             p.grad = v
             # this parameter has persistent, contiguous fp32 .grad storage: the MLP backward kernels may accumulate
-            # into it directly (ops.MLPFunction.backward checks the mark on every parameter of the call)
+            # into it directly (every MLP and density pass of ops takes that route when all the parameters of its call
+            # carry the mark: ops._inplace_refs)
             p._sparf_inplace_grad = True
             o += p.numel()
 

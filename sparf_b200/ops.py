@@ -103,6 +103,11 @@ def _ptr(t: Optional[torch.Tensor]) -> ctypes.c_void_p:
     return ctypes.c_void_p(0 if t is None else t.data_ptr())
 
 
+def _row_ptr(t: torch.Tensor, i: int) -> ctypes.c_void_p:
+    """a pointer to element i of a contiguous tensor (a device address; nothing is read)"""
+    return ctypes.c_void_p(t.data_ptr() + i * t.element_size())
+
+
 def _f32c(t: torch.Tensor) -> torch.Tensor:
     assert t.is_cuda, "sparf_b200 ops need CUDA tensors (there is no CPU path)"
     if t.dtype != torch.float32:
@@ -182,9 +187,49 @@ def _workspace(nbytes: int, device) -> torch.Tensor:
     return buf
 
 
+def _inplace_refs(params):
+    """The parameters whose `.grad` a backward may accumulate into (ACCUMULATE_INTO_PARAM_GRAD, or every parameter of
+    the call marked `_sparf_inplace_grad`), else None."""
+    if ACCUMULATE_INTO_PARAM_GRAD[0] or all(getattr(p, "_sparf_inplace_grad", False) for p in params):
+        return params
+    return None
+
+
+def _grad_targets(ctx, params, device):
+    """A backward's view of the network and the destinations of its parameter gradients -> (SparfMLP, the tensors it
+    points at, SparfMLPGrad, parameter gradients to return).  The destinations are the parameters' own `.grad` when the
+    forward opted in (ctx.param_refs) and every one exists (autograd then gets None), else fresh zeroed tensors in one
+    flat buffer."""
+    m, keep = ctx.spec.fill(params, ctx.progress)
+    refs = ctx.param_refs
+    if refs is not None and all(p.grad is not None and p.grad.is_contiguous() and p.grad.dtype == torch.float32 for p in refs):
+        grads, ret = [p.grad for p in refs], [None] * len(params)
+    else:
+        sizes = [p.numel() for p in params]
+        flat = torch.zeros(sum(sizes), device=device, dtype=torch.float32)
+        grads, o = [], 0
+        for p, n in zip(params, sizes):
+            grads.append(flat[o:o + n].view(p.shape))
+            o += n
+        ret = grads
+    return m, keep, ctx.spec.grad_struct(grads), ret
+
+
 # ------------------------------------------------------------------------------------------------
 # MLP: sigma, rgb = NeRF.forward_samples(o, d, t)
 # ------------------------------------------------------------------------------------------------
+# The MLP functions' arguments: (spec, engine, how, origins, dirs, t, noise, progress, *params), where `how` is what
+# differs by pass: grad_mode (dense), grid (grid) or (grid, tau_max, window) (terminated).
+_ORIGINS, _DIRS, _PARAMS = 3, 4, 8
+
+
+def _mlp_grads(d_o, d_d, param_grads):
+    """A backward's return value in the MLP functions' argument layout."""
+    ret = [None] * _PARAMS + list(param_grads)
+    ret[_ORIGINS], ret[_DIRS] = d_o, d_d
+    return tuple(ret)
+
+
 class MLPFunction(torch.autograd.Function):
     @staticmethod
     @_on_tensor_device
@@ -203,7 +248,8 @@ class MLPFunction(torch.autograd.Function):
         # fp32 encodings and activations) so that the backward skips the forward recompute.
         # (grad_mode: autograd is recording at the call site -- under torch.no_grad() nothing is kept)
         EVALS["fwd"] += R * S
-        wants_grad = grad_mode and (any(ctx.needs_input_grad[i] for i in (3, 4)) or any(ctx.needs_input_grad[8:]))
+        needs = ctx.needs_input_grad
+        wants_grad = grad_mode and (needs[_ORIGINS] or needs[_DIRS] or any(needs[_PARAMS:]))
         tape_bytes = L.sparf_mlp_tape_bytes(ctypes.byref(m), engine, R, S) if (wants_grad and USE_TAPE[0]) else 0
         ctx.tape = None
         with _timed("mlp_forward"):
@@ -218,8 +264,7 @@ class MLPFunction(torch.autograd.Function):
         ctx.spec, ctx.engine = spec, engine
         ctx.noise = noise_c
         ctx.progress = progress
-        ctx.param_refs = params if (ACCUMULATE_INTO_PARAM_GRAD[0] or
-                                    all(getattr(p, "_sparf_inplace_grad", False) for p in params)) else None
+        ctx.param_refs = _inplace_refs(params)
         if ctx.tape is not None:
             ctx.save_for_backward(origins, dirs, t, sigma, rgb, *params)
         else:
@@ -234,15 +279,12 @@ class MLPFunction(torch.autograd.Function):
             origins, dirs, t, sigma_f, rgb_f, *params = ctx.saved_tensors
         else:
             origins, dirs, t, *params = ctx.saved_tensors
-        spec = ctx.spec
         R, S = t.shape
         EVALS["bwd"] += R * S
         g_sigma = _f32c(g_sigma) if g_sigma is not None else torch.zeros(R, S, device=t.device)
         g_rgb = _f32c(g_rgb) if g_rgb is not None else torch.zeros(R, S, 3, device=t.device)
-        m, keep = spec.fill(params, ctx.progress)
-        grads, ret = _param_grads(ctx, params, t.device)
-        gs = spec.grad_struct(grads)
-        need_o, need_d = ctx.needs_input_grad[3], ctx.needs_input_grad[4]
+        m, keep, gs, ret = _grad_targets(ctx, params, t.device)
+        need_o, need_d = ctx.needs_input_grad[_ORIGINS], ctx.needs_input_grad[_DIRS]
         d_o = torch.zeros_like(origins) if (need_o or need_d) else None
         d_d = torch.zeros_like(dirs) if (need_o or need_d) else None
         nbytes = L.sparf_mlp_workspace_bytes(ctypes.byref(m), R, S, 2 if ctx.tape is not None else 1, ctx.engine)
@@ -258,7 +300,7 @@ class MLPFunction(torch.autograd.Function):
                 check(L.sparf_mlp_backward(ctypes.byref(m), ctx.engine, R, S, _ptr(origins), _ptr(dirs), _ptr(t),
                                            _ptr(ctx.noise), _ptr(g_sigma), _ptr(g_rgb), ctypes.byref(gs), _ptr(d_o),
                                            _ptr(d_d), _ptr(ws), ws.numel(), _stream()), "mlp_backward")
-        return (None, None, None, d_o if need_o else None, d_d if need_d else None, None, None, None, *ret)
+        return _mlp_grads(d_o if need_o else None, d_d if need_d else None, ret)
 
 
 def mlp_forward(spec: MLPSpec, origins, dirs, t, params: Sequence[torch.Tensor], *, noise=None, progress=None,
@@ -289,7 +331,47 @@ def _grid_compact(grid, o, d, t, K, idx, o_k, d_k, t_k):
               "contracted_emit")
 
 
-class GridMLPFunction(torch.autograd.Function):
+class _CompactedMLPFunction(torch.autograd.Function):
+    """The backward of the passes over a compacted sample set (grid, terminated): the output gradients gathered at the
+    kept rows, one taped backward over them and the per-ray sums of the origin and direction gradients, every row count
+    read on the device.  The forward sets ctx.C = R*S and, unless C = 0, saves (count, idx, o_k, d_k, t_k, sigma_k,
+    rgb_k, *params) and sets ctx.shape, ctx.tape, ctx.rows_at (the kept-row count is count[rows_at]) and
+    ctx.ray_sum(count, idx, src, dst), the ray sum of its layout."""
+
+    @staticmethod
+    @_on_tensor_device
+    def backward(ctx, g_sigma, g_rgb):
+        if ctx.C == 0 or ctx.tape is None:
+            return _mlp_grads(None, None, [None] * (len(ctx.needs_input_grad) - _PARAMS))
+        L = _lib.lib()
+        count, idx, o_k, d_k, t_k, sigma_k, rgb_k, *params = ctx.saved_tensors
+        (R, S), C, dev = ctx.shape, ctx.C, t_k.device
+        rows = _row_ptr(count, ctx.rows_at)
+        g_sigma_k, g_rgb_k = torch.empty(C, 1, device=dev), torch.empty(C, 1, 3, device=dev)
+        check(L.sparf_compact_gather(C, rows, _ptr(idx), 1, _ptr(_f32c(g_sigma)), _ptr(g_sigma_k), _stream()), "compact_gather")
+        check(L.sparf_compact_gather(C, rows, _ptr(idx), 3, _ptr(_f32c(g_rgb)), _ptr(g_rgb_k), _stream()), "compact_gather")
+        m, keep, gs, ret = _grad_targets(ctx, params, dev)
+        need_o, need_d = ctx.needs_input_grad[_ORIGINS], ctx.needs_input_grad[_DIRS]
+        d_o_k = torch.zeros(C, 3, device=dev) if (need_o or need_d) else None
+        d_d_k = torch.zeros(C, 3, device=dev) if (need_o or need_d) else None
+        ws = _workspace(L.sparf_mlp_workspace_bytes(ctypes.byref(m), C, 1, 2, ctx.engine), dev)
+        with _timed("mlp_backward"):
+            check(L.sparf_mlp_backward_tape_rows(ctypes.byref(m), ctx.engine, C, 1, rows, _ptr(o_k), _ptr(d_k), _ptr(t_k),
+                                                 _ptr(sigma_k), _ptr(rgb_k), _ptr(g_sigma_k), _ptr(g_rgb_k), ctypes.byref(gs),
+                                                 _ptr(d_o_k), _ptr(d_d_k), _ptr(ctx.tape), ctx.tape.numel(), _ptr(ws),
+                                                 ws.numel(), _stream()), "mlp_backward_tape_rows")
+        ctx.tape = None
+        d_o = d_d = None
+        if need_o:
+            d_o = torch.empty(R, 3, device=dev)
+            ctx.ray_sum(count, idx, d_o_k, d_o)
+        if need_d:
+            d_d = torch.empty(R, 3, device=dev)
+            ctx.ray_sum(count, idx, d_d_k, d_d)
+        return _mlp_grads(d_o, d_d, ret)
+
+
+class GridMLPFunction(_CompactedMLPFunction):
     """mlp_forward over the samples an occupancy grid keeps, with gradients and without a host round trip: the
     compaction writes the kept count K to device memory, the taped MLP pair with a device row count evaluates the K
     kept samples out of a capacity of R*S, and scatter / gather / ray-sum kernels move rows between the dense and the
@@ -331,46 +413,12 @@ class GridMLPFunction(torch.autograd.Function):
         check(L.sparf_compact_scatter(C, _ptr(K), _ptr(idx), 1, _ptr(sigma_k), _ptr(sigma), _stream()), "compact_scatter")
         check(L.sparf_compact_scatter(C, _ptr(K), _ptr(idx), 3, _ptr(rgb_k), _ptr(rgb), _stream()), "compact_scatter")
         ctx.spec, ctx.engine, ctx.progress, ctx.tape = spec, engine, progress, tape
-        ctx.shape = (R, S)
-        ctx.param_refs = params if (ACCUMULATE_INTO_PARAM_GRAD[0] or
-                                    all(getattr(p, "_sparf_inplace_grad", False) for p in params)) else None
+        ctx.shape, ctx.rows_at = (R, S), 0
+        ctx.ray_sum = lambda K_, idx_, src, dst: check(
+            L.sparf_compact_ray_sum(R, S, C, _ptr(K_), _ptr(idx_), 3, _ptr(src), _ptr(dst), _stream()), "compact_ray_sum")
+        ctx.param_refs = _inplace_refs(params)
         ctx.save_for_backward(K, idx, o_k, d_k, t_k, sigma_k, rgb_k, *params)
         return sigma, rgb
-
-    @staticmethod
-    @_on_tensor_device
-    def backward(ctx, g_sigma, g_rgb):
-        R, S = ctx.shape if ctx.C else (0, 0)
-        if ctx.C == 0 or ctx.tape is None:
-            return (None,) * 8 + tuple(None for _ in ctx.needs_input_grad[8:])
-        L = _lib.lib()
-        K, idx, o_k, d_k, t_k, sigma_k, rgb_k, *params = ctx.saved_tensors
-        C, dev = ctx.C, t_k.device
-        g_sigma_k, g_rgb_k = torch.empty(C, 1, device=dev), torch.empty(C, 1, 3, device=dev)
-        check(L.sparf_compact_gather(C, _ptr(K), _ptr(idx), 1, _ptr(_f32c(g_sigma)), _ptr(g_sigma_k), _stream()),
-              "compact_gather")
-        check(L.sparf_compact_gather(C, _ptr(K), _ptr(idx), 3, _ptr(_f32c(g_rgb)), _ptr(g_rgb_k), _stream()), "compact_gather")
-        m, keep = ctx.spec.fill(params, ctx.progress)
-        grads, ret = _param_grads(ctx, params, dev)
-        gs = ctx.spec.grad_struct(grads)
-        need_o, need_d = ctx.needs_input_grad[3], ctx.needs_input_grad[4]
-        d_o_k = torch.zeros(C, 3, device=dev) if (need_o or need_d) else None
-        d_d_k = torch.zeros(C, 3, device=dev) if (need_o or need_d) else None
-        ws = _workspace(L.sparf_mlp_workspace_bytes(ctypes.byref(m), C, 1, 2, ctx.engine), dev)
-        with _timed("mlp_backward"):
-            check(L.sparf_mlp_backward_tape_rows(ctypes.byref(m), ctx.engine, C, 1, _ptr(K), _ptr(o_k), _ptr(d_k), _ptr(t_k),
-                                                 _ptr(sigma_k), _ptr(rgb_k), _ptr(g_sigma_k), _ptr(g_rgb_k), ctypes.byref(gs),
-                                                 _ptr(d_o_k), _ptr(d_d_k), _ptr(ctx.tape), ctx.tape.numel(), _ptr(ws),
-                                                 ws.numel(), _stream()), "mlp_backward_tape_rows")
-        ctx.tape = None
-        d_o = d_d = None
-        if need_o:
-            d_o = torch.empty(R, 3, device=dev)
-            check(L.sparf_compact_ray_sum(R, S, C, _ptr(K), _ptr(idx), 3, _ptr(d_o_k), _ptr(d_o), _stream()), "compact_ray_sum")
-        if need_d:
-            d_d = torch.empty(R, 3, device=dev)
-            check(L.sparf_compact_ray_sum(R, S, C, _ptr(K), _ptr(idx), 3, _ptr(d_d_k), _ptr(d_d), _stream()), "compact_ray_sum")
-        return (None, None, None, d_o, d_d, None, None, None, *ret)
 
 
 def mlp_forward_grid(spec: MLPSpec, origins, dirs, t, grid, params: Sequence[torch.Tensor], *, noise=None, progress=None,
@@ -385,11 +433,6 @@ def mlp_forward_grid(spec: MLPSpec, origins, dirs, t, grid, params: Sequence[tor
     if eng == _lib.ENGINE_SIMT_FP32:
         raise ValueError("mlp_forward_grid: the simt_fp32 engine has no device-side row count; use tc_3x, tc_1x or tc_3x_w1")
     return GridMLPFunction.apply(spec, eng, grid, origins, dirs, t, noise, progress, *params)
-
-
-def _row_ptr(t: torch.Tensor, i: int) -> ctypes.c_void_p:
-    """a pointer to element i of a contiguous tensor (a device address; nothing is read)"""
-    return ctypes.c_void_p(t.data_ptr() + i * t.element_size())
 
 
 def _window_append(grid, o, d, t, k0, k1, alive, ends, w, idx, o_k, d_k, t_k):
@@ -412,7 +455,7 @@ def _window_append(grid, o, d, t, k0, k1, alive, ends, w, idx, o_k, d_k, t_k):
         check(L.sparf_termination_append(*head, None, 0, 0.0, 1.0, *tail), "termination_append")
 
 
-class TerminatedMLPFunction(torch.autograd.Function):
+class TerminatedMLPFunction(_CompactedMLPFunction):
     """mlp_forward with early ray termination in windows, on top of an optional occupancy grid, with gradients and
     without a host round trip.  Each window appends its kept samples (alive rays, grid-kept samples) to one compacted
     set per pass, rows [ends[w], ends[w+1]), and runs the taped forward over that device-side span into one tape; the
@@ -421,9 +464,9 @@ class TerminatedMLPFunction(torch.autograd.Function):
 
     @staticmethod
     @_on_tensor_device
-    def forward(ctx, spec: MLPSpec, engine: int, grid, tau_max: float, window: int, origins, dirs, t, noise, progress,
-                *params):
+    def forward(ctx, spec: MLPSpec, engine: int, how, origins, dirs, t, noise, progress, *params):
         L = _lib.lib()
+        grid, tau_max, window = how
         o, d, tt = _f32c(origins), _f32c(dirs), _f32c(t)
         R, S = tt.shape
         assert o.shape == (R, 3) and d.shape == (R, 3)
@@ -469,47 +512,13 @@ class TerminatedMLPFunction(torch.autograd.Function):
                 check(L.sparf_termination_update(R, S, k0, k1, _ptr(sigma), _ptr(tt), _ptr(d), float(tau_max), _ptr(tau),
                                                  _ptr(alive), _stream()), "termination_update")
         ctx.spec, ctx.engine, ctx.progress, ctx.tape = spec, engine, progress, tape
-        ctx.shape, ctx.W = (R, S), W
-        ctx.param_refs = params if (ACCUMULATE_INTO_PARAM_GRAD[0] or
-                                    all(getattr(p, "_sparf_inplace_grad", False) for p in params)) else None
+        ctx.shape, ctx.rows_at = (R, S), W          # every window's rows: [0, ends[W])
+        ctx.ray_sum = lambda ends_, idx_, src, dst: check(
+            L.sparf_compact_ray_sum_segments(R, S, W, _ptr(ends_), _ptr(idx_), 3, _ptr(src), _ptr(dst), _stream()),
+            "compact_ray_sum_segments")
+        ctx.param_refs = _inplace_refs(params)
         ctx.save_for_backward(ends, idx, o_k, d_k, t_k, sigma_k, rgb_k, *params)
         return sigma, rgb
-
-    @staticmethod
-    @_on_tensor_device
-    def backward(ctx, g_sigma, g_rgb):
-        if ctx.C == 0 or ctx.tape is None:
-            return (None,) * 10 + tuple(None for _ in ctx.needs_input_grad[10:])
-        L = _lib.lib()
-        ends, idx, o_k, d_k, t_k, sigma_k, rgb_k, *params = ctx.saved_tensors
-        (R, S), W, C, dev = ctx.shape, ctx.W, ctx.C, t_k.device
-        K = _row_ptr(ends, W)       # every window's rows: [0, ends[W])
-        g_sigma_k, g_rgb_k = torch.empty(C, 1, device=dev), torch.empty(C, 1, 3, device=dev)
-        check(L.sparf_compact_gather(C, K, _ptr(idx), 1, _ptr(_f32c(g_sigma)), _ptr(g_sigma_k), _stream()), "compact_gather")
-        check(L.sparf_compact_gather(C, K, _ptr(idx), 3, _ptr(_f32c(g_rgb)), _ptr(g_rgb_k), _stream()), "compact_gather")
-        m, keep = ctx.spec.fill(params, ctx.progress)
-        grads, ret = _param_grads(ctx, params, dev)
-        gs = ctx.spec.grad_struct(grads)
-        need_o, need_d = ctx.needs_input_grad[5], ctx.needs_input_grad[6]
-        d_o_k = torch.zeros(C, 3, device=dev) if (need_o or need_d) else None
-        d_d_k = torch.zeros(C, 3, device=dev) if (need_o or need_d) else None
-        ws = _workspace(L.sparf_mlp_workspace_bytes(ctypes.byref(m), C, 1, 2, ctx.engine), dev)
-        with _timed("mlp_backward"):
-            check(L.sparf_mlp_backward_tape_rows(ctypes.byref(m), ctx.engine, C, 1, K, _ptr(o_k), _ptr(d_k), _ptr(t_k),
-                                                 _ptr(sigma_k), _ptr(rgb_k), _ptr(g_sigma_k), _ptr(g_rgb_k), ctypes.byref(gs),
-                                                 _ptr(d_o_k), _ptr(d_d_k), _ptr(ctx.tape), ctx.tape.numel(), _ptr(ws),
-                                                 ws.numel(), _stream()), "mlp_backward_tape_rows")
-        ctx.tape = None
-        d_o = d_d = None
-        if need_o:
-            d_o = torch.empty(R, 3, device=dev)
-            check(L.sparf_compact_ray_sum_segments(R, S, W, _ptr(ends), _ptr(idx), 3, _ptr(d_o_k), _ptr(d_o), _stream()),
-                  "compact_ray_sum_segments")
-        if need_d:
-            d_d = torch.empty(R, 3, device=dev)
-            check(L.sparf_compact_ray_sum_segments(R, S, W, _ptr(ends), _ptr(idx), 3, _ptr(d_d_k), _ptr(d_d), _stream()),
-                  "compact_ray_sum_segments")
-        return (None,) * 5 + (d_o, d_d) + (None,) * 3 + tuple(ret)
 
 
 def mlp_forward_terminated(spec: MLPSpec, origins, dirs, t, grid, eps: float, window: int, params: Sequence[torch.Tensor], *,
@@ -528,23 +537,8 @@ def mlp_forward_terminated(spec: MLPSpec, origins, dirs, t, grid, eps: float, wi
     if not (0 <= eps < 1) or int(window) != window or window < 1:
         raise ValueError("mlp_forward_terminated: eps %r (0 <= eps < 1), window %r (an integer >= 1)" % (eps, window))
     from .termination import tau_max
-    return TerminatedMLPFunction.apply(spec, eng, grid, tau_max(eps), int(window), origins, dirs, t, noise, progress, *params)
-
-
-def _param_grads(ctx, params, device):
-    """Gradient destinations of a backward: the parameters' own `.grad` when the forward opted in and every one exists
-    (then autograd gets None), else fresh zeroed tensors in one flat buffer.  -> (grads for the C ABI, grads to return)."""
-    inplace = ctx.param_refs is not None and all(
-        p.grad is not None and p.grad.is_contiguous() and p.grad.dtype == torch.float32 for p in ctx.param_refs)
-    if inplace:
-        return [p.grad for p in ctx.param_refs], [None] * len(params)
-    sizes = [p.numel() for p in params]
-    flat = torch.zeros(sum(sizes), device=device, dtype=torch.float32)
-    grads, o = [], 0
-    for p, n in zip(params, sizes):
-        grads.append(flat[o:o + n].view(p.shape))
-        o += n
-    return grads, grads
+    return TerminatedMLPFunction.apply(spec, eng, (grid, tau_max(eps), int(window)), origins, dirs, t, noise, progress,
+                                       *params)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -570,8 +564,7 @@ class DensityFunction(torch.autograd.Function):
         ctx.points_shape = points.shape
         ctx.saved = grad_mode and (ctx.needs_input_grad[4] or any(ctx.needs_input_grad[6:]))
         if ctx.saved:
-            ctx.param_refs = trunk_params if (ACCUMULATE_INTO_PARAM_GRAD[0] or
-                                              all(getattr(p, "_sparf_inplace_grad", False) for p in trunk_params)) else None
+            ctx.param_refs = _inplace_refs(trunk_params)
             ctx.save_for_backward(pts, *trunk_params)
         return raw, feat
 
@@ -586,9 +579,7 @@ class DensityFunction(torch.autograd.Function):
         EVALS["bwd"] += M
         g_raw = _f32c(g_raw) if g_raw is not None else None
         g_feat = _f32c(g_feat) if g_feat is not None else None
-        m, keep = ctx.spec.fill(params, ctx.progress)
-        grads, ret = _param_grads(ctx, params, pts.device)
-        gs = ctx.spec.grad_struct(grads)
+        m, keep, gs, ret = _grad_targets(ctx, params, pts.device)
         d_pts = torch.zeros_like(pts) if ctx.needs_input_grad[4] else None
         ws = _workspace(L.sparf_density_workspace_bytes(ctypes.byref(m), M, 1, ctx.engine), pts.device)
         with _timed("density_backward"):

@@ -2,8 +2,8 @@
 the span forward against the rows forward on the same rows moved to row 0; one backward over the rows of several spans
 against the rows pair on the concatenated rows; the appending compaction and the segment ray sum against their NumPy
 oracles; a training render against the dense render masked by the oracle's kept set (tests/termination_oracle.py, from
-the dense noisy σ); eps = 0; a captured step against the eager one; the engine gate; and a graphed training run that
-converges."""
+the dense noisy σ); eps = 0; a captured step against the eager one; the engine gate; the grid and terminated passes'
+in-place parameter gradients against their returned ones; and a graphed training run that converges."""
 import ctypes
 import os
 import sys
@@ -492,6 +492,42 @@ def test_captured_sparf_step_equals_eager(engine_guard, monkeypatch):
     print("SPARF step with grids and termination: %d terminated passes, losses %s, gradient difference %.2e of max"
           % (calls[0], [float(x) for x in eager], err / scale))
     assert err <= 1e-5 * scale
+
+
+@pytest.mark.parametrize("kind", ["grid", "terminated"])
+def test_inplace_param_grads_equal_returned(kind):
+    """the grid and the terminated pass accumulating into the parameters' own .grad (FlatGradients marks them
+    _sparf_inplace_grad) give the parameter gradients they return otherwise, bit for bit, and return None for them.
+    64 samples fit one row tile, so no gradient element is summed by two CTAs and the bits do not depend on the order of
+    the atomic adds"""
+    from sparf_b200 import ops
+    net, opt, _ = _net()
+    nerf = net.nerf
+    params = nerf.kernel_params()
+    R, S = 4, 16
+    g = torch.Generator(device=DEV).manual_seed(13)
+    o = torch.randn(R, 3, device=DEV, generator=g) * 0.3
+    d = torch.nn.functional.normalize(torch.randn(R, 3, device=DEV, generator=g), dim=-1)
+    t = torch.sort(torch.rand(R, S, device=DEV, generator=g) + 0.1, 1).values
+    w_sigma, w_rgb = torch.randn(R, S, device=DEV, generator=g), torch.randn(R, S, 3, device=DEV, generator=g)
+    grid = _random_grid(16, 0.6, 4)
+
+    def loss():
+        if kind == "grid":
+            sigma, rgb = ops.mlp_forward_grid(nerf._spec(), o, d, t, grid, params, progress=nerf.progress)
+        else:
+            sigma, rgb = ops.mlp_forward_terminated(nerf._spec(), o, d, t, grid, 1e-2, 4, params, progress=nerf.progress)
+        assert 0 < (sigma != 0).sum().item() < R * S
+        return (sigma * w_sigma).sum() + (rgb * w_rgb).sum()
+
+    returned = torch.autograd.grad(loss(), params)
+    for p in params:
+        p._sparf_inplace_grad = True
+        p.grad = torch.zeros_like(p)
+    assert all(x is None for x in torch.autograd.grad(loss(), params, allow_unused=True))
+    assert max(x.abs().max().item() for x in returned) > 0
+    for p, x in zip(params, returned):
+        assert torch.equal(_bits(p.grad), _bits(x))
 
 
 def test_graphed_training_with_termination_converges(engine_guard):
