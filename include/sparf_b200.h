@@ -436,6 +436,51 @@ int sparf_mesh_select_emit(const int64_t* faces, int64_t n_faces, int64_t n_vert
                            const uint8_t* keep, int64_t n_components, int64_t* vert_ids, int64_t* faces_out,
                            void* workspace, size_t workspace_bytes, sparf_stream_t stream);
 
+/* ---------------------------------------------------------------- mesh simplification
+ * Quadric-error edge collapses (Garland-Heckbert) down to a face budget (sparf_b200/mesh.py, simplify), in parallel
+ * rounds whose every decision is a minimum or a sort: the result does not depend on the schedule.
+ *   input:     vertices [V][3] (fp32), faces [F][3] (int64, ids in [0, V): the caller checks), attrs [V][A] (fp32,
+ *              A >= 0, interpolated, not part of the error); V <= INT32_MAX, F <= INT32_MAX / 3.  Open, non-manifold and
+ *              degenerate input is allowed.
+ *   classes:   each round, over the live faces: an edge is interior in exactly 2 of them, boundary in 1, non-manifold in
+ *              3 or more; a vertex is locked on a non-manifold edge or a face with repeated ids, boundary on a boundary
+ *              edge.  Locked vertices never move and are never removed; boundary vertices never move.
+ *   quadrics:  per face, with c = (p1 - p0) x (p2 - p0) in fp64, n = c / |c|, n4 = (n, -n.p0), w = |c| / 2:
+ *              q_ij = (w n4_i) n4_j for ij = 00 01 02 03 11 12 13 22 23 33 (0 when |c| = 0).  Q[v] = the sum over v's
+ *              faces in increasing face id.  Every fp64 operation is rounded on its own (no FMA contraction).
+ *   edges:     indexed by rank among the unique (lo, hi) id pairs of the live faces.  (a, b), a < b, is collapsible when
+ *              interior, neither end locked, not both boundary; valid when also (link condition) its faces abc and abd
+ *              have c != d, a and b have no common neighbour but c and d, and not both acd and bcd are faces; and
+ *              (fold check) every live face around a or b that does not hold both and has a nonzero old normal
+ *              (p1 - p0) x (p2 - p0) keeps a positive dot product of its new (end replaced by v*) and old normals.
+ *   v*:        (fp32) with one boundary end, that end (it survives); else the minimiser of v^T (Q[a] + Q[b]) v by
+ *              Cramer's rule when |det A| > 1e-10 tr(A)^3 and |v* - mid|^2 <= |b - a|^2 (mid = (a + b) / 2); else the
+ *              cheapest of a, b, fp32(mid), ties in that order.  cost = fp32(max(v*^T Q v*, 0)), key = cost bits << 32 | e.
+ *   round:     k = ceil((F_live - target) / 2); the candidates are the k valid edges with the smallest keys (all valid
+ *              edges when fewer).  Each candidate atomicMin's its key onto every vertex of every live face around a or
+ *              b, and wins when it holds all of them.  A winner collapses into s (its boundary end, else a; r the
+ *              other): pos[s] = v*, Q[s] = Q[s] + Q[r], attrs[s] = fp32(attrs[a] + t (attrs[b] - attrs[a])) with t the
+ *              projection of v* on a -> b clamped to [0, 1] (0 when a = b in space); its 2 faces die, r becomes s in
+ *              the others, and the live faces are compacted in their order.
+ *   output:    the vertices never removed, in increasing id (vert_ids [V'] int64, V' = V - the collapses), their
+ *              positions and attrs, and the live faces in input order with renumbered ids (int64).
+ * sparf_mesh_simplify_init copies the input into the workspace and builds the quadrics; counts [2] (device int64) =
+ * {F, 0}.  sparf_mesh_simplify_round (n_live = counts[0] as last read, k >= 1) runs one round and writes counts =
+ * {F_live, winners}; the caller stops when F_live <= target or winners = 0.  sparf_mesh_simplify_emit (n_live = F_live)
+ * writes the output.  With no round the output is the input, byte for byte.  Workspace (one for all three calls):
+ * sparf_mesh_simplify_workspace_bytes(V, F, A) = 110 + 4A B per vertex + 145 B per face + sort / scan scratch over 3F
+ * entries; 0 for invalid sizes and where no CUDA device is current.  No call synchronises; all are capturable.
+ * Invalid sizes or NULL pointers give SPARF_ERR_INVALID. */
+size_t sparf_mesh_simplify_workspace_bytes(int64_t n_verts, int64_t n_faces, int32_t n_attrs);
+int sparf_mesh_simplify_init(const float* vertices, const int64_t* faces, const float* attrs, int64_t n_verts,
+                             int64_t n_faces, int32_t n_attrs, int64_t* counts, void* workspace,
+                             size_t workspace_bytes, sparf_stream_t stream);
+int sparf_mesh_simplify_round(int64_t n_verts, int64_t n_faces, int32_t n_attrs, int64_t n_live, int64_t k,
+                              int64_t* counts, void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+int sparf_mesh_simplify_emit(int64_t n_verts, int64_t n_faces, int32_t n_attrs, int64_t n_live, float* vertices,
+                             float* attrs, int64_t* vert_ids, int64_t* faces, void* workspace, size_t workspace_bytes,
+                             sparf_stream_t stream);
+
 /* ---------------------------------------------------------------- occupancy grid
  * Empty-space skipping for inference renders (sparf_b200/occupancy.py): a bitfield over the box [r0, r1]^3 split into
  * res^3 cells, built from the density lattice sigma [res+1]^3 of mesh.density_grid (lattice point (a,b,c) at

@@ -90,6 +90,10 @@ _SIGNATURES = {
     "sparf_mesh_component_faces": (c_int32, [_P, c_int64, c_int64, _P, c_int64, _P, _P]),
     "sparf_mesh_select_count": (c_int32, [_P, c_int64, c_int64, _P, _P, c_int64, _P, _P, c_size_t, _P]),
     "sparf_mesh_select_emit": (c_int32, [_P, c_int64, c_int64, _P, _P, c_int64, _P, _P, _P, c_size_t, _P]),
+    "sparf_mesh_simplify_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int32]),
+    "sparf_mesh_simplify_init": (c_int32, [_P, _P, _P, c_int64, c_int64, c_int32, _P, _P, c_size_t, _P]),
+    "sparf_mesh_simplify_round": (c_int32, [c_int64, c_int64, c_int32, c_int64, c_int64, _P, _P, c_size_t, _P]),
+    "sparf_mesh_simplify_emit": (c_int32, [c_int64, c_int64, c_int32, c_int64, _P, _P, _P, _P, _P, c_size_t, _P]),
     "sparf_occupancy_build": (c_int32, [_P, c_int32, c_float, _P, _P]),
     "sparf_occupancy_workspace_bytes": (c_size_t, [c_int64, c_int32]),
     "sparf_occupancy_count": (c_int32, [c_int64, c_int32, _P, _P, _P, _P, c_int32, c_float, c_float, _P, _P, c_size_t, _P]),

@@ -223,6 +223,30 @@ def keep_components(m: dict, largest=None, min_faces: int = 1, stats=None) -> di
     return out
 
 
+def simplify(m: dict, target_faces: int, stats=None) -> dict:
+    """Quadric-error simplification (ops.mesh_simplify) of a mesh dict of extract_mesh, extract_mesh_sparse or
+    tsdf.extract_mesh, before or after keep_components, to at most target_faces faces where the edge collapses reach
+    it.  Boundary and non-manifold vertices stay where they are.  normals and colors are interpolated along the
+    collapses; the normals are then made unit again by unit_normals' rule (0 where the length is 0).  Other entries are
+    passed on as they are.  stats: an optional dict that receives rounds, collapses, faces_before, faces_after and
+    reached (faces_after <= target_faces)."""
+    keys = [k for k in VERTEX_KEYS[1:] if m.get(k) is not None]
+    attrs = torch.cat([m[k] for k in keys], dim=1) if keys else None
+    st = {}
+    verts, faces, _, attrs = ops.mesh_simplify(m["vertices"], m["faces"], target_faces, attrs=attrs, stats=st)
+    out = dict(m, vertices=verts, faces=faces)
+    col = 0
+    for k in keys:
+        out[k] = attrs[:, col:col + m[k].shape[1]]
+        col += m[k].shape[1]
+    if "normals" in keys:
+        out["normals"] = unit_normals(-out["normals"])
+    if stats is not None:
+        stats.update(st, faces_before=m["faces"].shape[0], faces_after=faces.shape[0],
+                     reached=faces.shape[0] <= target_faces)
+    return out
+
+
 def write_ply(path, vertices, faces, normals=None, colors=None) -> None:
     """Binary little-endian PLY: float x, y, z (and nx, ny, nz) per vertex, then, when colors [V, 3] is given, uchar
     red, green, blue = round(clamp(c, 0, 1) * 255) (to nearest, ties to even); a uchar-counted int list per face"""

@@ -837,6 +837,63 @@ def mesh_select(faces, n_verts: int, labels, keep):
     return vert_ids, faces_out
 
 
+MAX_SIMPLIFY_FACES = MAX_MESH_ELEMENTS // 3     # sparf_mesh_simplify counts 3 half-edge entries per face in int32
+
+
+@torch.no_grad()
+@_on_tensor_device
+def mesh_simplify(vertices, faces, target_faces: int, attrs=None, stats=None):
+    """Quadric-error edge collapses (include/sparf_b200.h, mesh simplification) of the mesh vertices [V, 3] (fp32, CUDA),
+    faces [F, 3] (int64) with optional per-vertex attrs [V, A] (fp32, interpolated along the collapses) until at most
+    target_faces faces are left or no edge can collapse -> (vertices [V', 3], faces [F', 3] int64, vert_ids [V'] int64,
+    the original id of each kept vertex, increasing; attrs [V', A] or None).  Deterministic; target_faces >= F returns
+    the input's bytes.  Bad arguments raise ValueError before any library call (one device-to-host copy checks the ids);
+    each round reads {F_live, collapses} back.  stats: an optional dict that receives rounds and collapses."""
+    what = "mesh_simplify"
+    if not torch.is_tensor(vertices) or vertices.dtype != torch.float32 or vertices.dim() != 2 or vertices.shape[1] != 3:
+        raise ValueError("%s: vertices must be a float32 tensor [V, 3]" % what)
+    n_verts = vertices.shape[0]
+    _check_faces(faces, n_verts, what)
+    if faces.shape[0] > MAX_SIMPLIFY_FACES:
+        raise ValueError("%s: %d faces (at most %d)" % (what, faces.shape[0], MAX_SIMPLIFY_FACES))
+    if isinstance(target_faces, bool) or not isinstance(target_faces, numbers.Integral) or target_faces < 0:
+        raise ValueError("%s: target_faces must be an int >= 0 (got %r)" % (what, target_faces))
+    if attrs is not None and (not torch.is_tensor(attrs) or attrs.dtype != torch.float32 or attrs.dim() != 2
+                              or attrs.shape[0] != n_verts):
+        raise ValueError("%s: attrs must be None or a float32 tensor [%d, A]" % (what, n_verts))
+    if vertices.device != faces.device or (attrs is not None and attrs.device != faces.device):
+        raise ValueError("%s: vertices, faces and attrs must be on one CUDA device" % what)
+    _check_ids(faces, n_verts, what)
+    L = _lib.lib()
+    v, f = vertices.contiguous(), faces.contiguous()
+    a = attrs.contiguous() if attrs is not None else None
+    dev, F, A = f.device, f.shape[0], 0 if a is None else a.shape[1]
+    ws = torch.empty(max(L.sparf_mesh_simplify_workspace_bytes(n_verts, F, A), 1), dtype=torch.uint8, device=dev)
+    counts = torch.empty(2, dtype=torch.int64, device=dev)
+    check(L.sparf_mesh_simplify_init(_ptr(v), _ptr(f), _ptr(a), n_verts, F, A, _ptr(counts), _ptr(ws), ws.numel(),
+                                     _stream()), "mesh_simplify_init")
+    n_live, rounds, collapses = F, 0, 0
+    while n_live > target_faces:
+        k = (n_live - target_faces + 1) // 2
+        check(L.sparf_mesh_simplify_round(n_verts, F, A, n_live, k, _ptr(counts), _ptr(ws), ws.numel(), _stream()),
+              "mesh_simplify_round")
+        n_live, winners = counts.tolist()
+        rounds += 1
+        collapses += winners
+        if winners == 0:
+            break
+    n_out = n_verts - collapses
+    v_out = torch.empty(n_out, 3, dtype=torch.float32, device=dev)
+    a_out = torch.empty(n_out, A, dtype=torch.float32, device=dev) if a is not None else None
+    vert_ids = torch.empty(n_out, dtype=torch.int64, device=dev)
+    f_out = torch.empty(n_live, 3, dtype=torch.int64, device=dev)
+    check(L.sparf_mesh_simplify_emit(n_verts, F, A, n_live, _ptr(v_out), _ptr(a_out), _ptr(vert_ids), _ptr(f_out),
+                                     _ptr(ws), ws.numel(), _stream()), "mesh_simplify_emit")
+    if stats is not None:
+        stats.update(rounds=rounds, collapses=collapses)
+    return v_out, f_out, vert_ids, a_out
+
+
 # ------------------------------------------------------------------------------------------------
 # occupancy grid (no gradient)
 # ------------------------------------------------------------------------------------------------

@@ -6,7 +6,7 @@ opt.trimesh, on the GPU).
                                  [--range -1.2 1.2] [--thres 25] [--normals] [--barf-c2f START END] [--sparse]
     python tools/extract_mesh.py model.pth.tar --out mesh.ply --tsdf cameras.npz [--res 128] [--range -1.2 1.2]
                                  [--trunc T] [--samples 128] [--samples-fine 128] [--barf-c2f START END]
-    either form takes [--keep-largest K] [--min-faces N]
+    either form takes [--keep-largest K] [--min-faces N] [--simplify F]
 
 The snapshot is what the reference's trainer saves (base_trainer.py:196-216): the model dict is ckpt["state_dict"],
 with the Graph's keys nerf.* / nerf_fine.* (or, from a joint pose trainer, those under "nerf_net").  The architecture
@@ -21,6 +21,9 @@ zero level is written.
 --keep-largest K and --min-faces N remove floaters from any of these meshes (mesh.keep_components): of the connected
 components with at least N faces only the K largest are kept; the tool then also prints the component counts and times
 a components phase.
+--simplify F then simplifies the mesh to at most F faces (mesh.simplify, quadric-error edge collapses; boundaries stay
+put) and prints the rounds and face counts and times a simplify phase.  On the density paths --normals are then
+computed at the simplified vertices; the TSDF colours are interpolated along the collapses.
 Prints V, F and the time of each phase.
 """
 import argparse
@@ -91,6 +94,18 @@ def filter_components(args, m, phase):
     return m
 
 
+def simplify(args, m, phase):
+    """mesh.simplify of the mesh dict m to --simplify faces when given (printing the rounds and faces), else m"""
+    if args.simplify is None:
+        return m
+    from sparf_b200 import mesh
+    stats = {}
+    m = phase("simplify", lambda: mesh.simplify(m, args.simplify, stats=stats))
+    print("simplify: %d rounds, %d collapses, faces %d -> %d%s" % (stats["rounds"], stats["collapses"],
+          stats["faces_before"], stats["faces_after"], "" if stats["reached"] else " (no edge left to collapse)"))
+    return m
+
+
 def main_tsdf(args):
     from sparf_b200 import mesh, tsdf
     from sparf_b200.renderer import Graph
@@ -121,7 +136,7 @@ def main_tsdf(args):
             break
         phase("integrate", lambda: tsdf.integrate_(vol, batch[0], batch[1], batch[2], rgb=batch[3], valid=batch[4]))
     m = phase("marching_cubes", lambda: tsdf.extract_mesh(vol))
-    m = filter_components(args, m, phase)
+    m = simplify(args, filter_components(args, m, phase), phase)
     phase("write_ply", lambda: mesh.write_ply(args.out, m["vertices"], m["faces"], colors=m["colors"]))
     print("%s: V %d, F %d (TSDF of %d views %dx%d, res %d, range %s, trunc %g)"
           % (args.out, m["vertices"].shape[0], m["faces"].shape[0], pose.shape[0], H, W, vol.res, list(vol.range),
@@ -135,6 +150,8 @@ def parse_args(ap, argv):
         ap.error("--keep-largest must be >= 1")
     if args.min_faces is not None and args.min_faces < 0:
         ap.error("--min-faces must be >= 0")
+    if args.simplify is not None and args.simplify < 0:
+        ap.error("--simplify must be >= 0")
     return args
 
 
@@ -157,6 +174,8 @@ def build_parser():
                     help="keep only the K connected components with the most faces")
     ap.add_argument("--min-faces", type=int, default=None, metavar="N",
                     help="keep only the connected components with at least N faces (default with --keep-largest: 1)")
+    ap.add_argument("--simplify", type=int, default=None, metavar="F",
+                    help="simplify the mesh to at most F faces (quadric-error edge collapses)")
     return ap
 
 
@@ -207,9 +226,14 @@ def main(argv=None):
         verts, faces = phase("marching_cubes", lambda: mesh.marching_cubes(sigma, thres))
     del sigma
     verts = mesh.to_world(verts, res, rng)
-    normals = phase("normals", lambda: mesh.density_normals(nerf, verts)) if args.normals else None
-    m = filter_components(args, dict(vertices=verts, faces=faces, normals=normals), phase)
-    verts, faces, normals = m["vertices"], m["faces"], m["normals"]
+    if args.simplify is None:
+        normals = phase("normals", lambda: mesh.density_normals(nerf, verts)) if args.normals else None
+        m = filter_components(args, dict(vertices=verts, faces=faces, normals=normals), phase)
+        verts, faces, normals = m["vertices"], m["faces"], m["normals"]
+    else:       # the normals of the final vertices, not interpolated ones
+        m = simplify(args, filter_components(args, dict(vertices=verts, faces=faces), phase), phase)
+        verts, faces = m["vertices"], m["faces"]
+        normals = phase("normals", lambda: mesh.density_normals(nerf, verts)) if args.normals else None
     phase("write_ply", lambda: mesh.write_ply(args.out, verts, faces, normals))
     print("%s: V %d, F %d (res %d, range %s, thres %g)" % (args.out, verts.shape[0], faces.shape[0], res, list(rng), thres))
     print("  " + ", ".join("%s %.3f s" % kv for kv in phases.items()))
