@@ -481,6 +481,58 @@ int sparf_mesh_simplify_emit(int64_t n_verts, int64_t n_faces, int32_t n_attrs, 
                              float* attrs, int64_t* vert_ids, int64_t* faces, void* workspace, size_t workspace_bytes,
                              sparf_stream_t stream);
 
+/* ---------------------------------------------------------------- mesh distance
+ * Exact closest-point queries against a target surface (sparf_b200/mesh.py, compare: Chamfer distance and F-score):
+ * for each query point the nearest primitive of a triangle mesh or a point cloud, found over a uniform grid.
+ *   target:  vertices [V][3] (fp32, finite) and either faces [F][3] (int64; a triangle target, F >= 0) or n_faces = -1
+ *            (a point target: the primitives are the vertices).  0 <= V, F <= INT32_MAX; F > 0 needs V > 0.  A face with
+ *            an id outside [0, V) is never found (no out-of-bounds access).
+ *   grid:    the box is the target's bounding box (over all V vertices, NaN coordinates skipped) padded on every side
+ *            by max(1e-3 of its largest extent, 1e-6 of its largest |coordinate|, 1e-20), so flat targets get a
+ *            volume.  Cells per axis: given (each >= 1, at most 2^24 cells), or automatic (all 0): with P primitives,
+ *            about T = min(2^24, P^1.5) cubic cells of side h = cbrt(box volume / T), n_a = clamp(ceil(extent_a / h), 1,
+ *            2^24), h grown by 1.25x until at most 2^24 cells.  A surface sampled by P primitives crosses about P^(2/3)
+ *            ... P of such cells, so a crossed cell holds about one point or a few triangle entries.  The cell size
+ *            per axis is extent_a / n_a.  A point is entered in its one cell; a triangle in every cell its bounding box
+ *            overlaps (cell of x = clamp(floor((x - lo) / cell), 0, n - 1) in fp32).  CSR: cell_start [n_cells + 1]
+ *            (int32) and prims [entries] (int32 primitive ids, increasing within a cell); entries <= INT32_MAX.
+ *   query:   points [N][3] (fp32) -> dist [N] (fp32), index [N] (int64), closest [N][3] (fp32): the minimum over every
+ *            primitive of (d, id), d = sqrt(|p - q|^2) with q the primitive's closest point to p, ties to the
+ *            smallest id; a miss (no primitive with d <= max_dist) gives inf / -1 / NaN.  q of a point is the point;
+ *            of a triangle abc the nearest of: the projection onto its plane when n = ab x ac != 0 and the projection
+ *            lies inside (face region; preferred on ties), and the clamped projections onto ab, bc, ca (edge and vertex
+ *            regions; ties in that order), so zero-area, collinear and repeated-vertex triangles are exact too.  Every
+ *            fp32 operation of it is rounded on its own: d and q are one function of (p, primitive), and the result is
+ *            the same bytes for every grid, including 1 x 1 x 1 (brute force).  The search visits Chebyshev shells of
+ *            cells around p's clamped cell and stops once every plane bounding the visited cells lies farther from p
+ *            than min(d_best, max_dist) (strictly, after shrinking the bound by 2^-18 (|p|_inf + the box's largest
+ *            |coordinate|) for rounding), or the whole grid is visited.  max_dist >= 0 (+inf allowed).
+ * sparf_distance_grid_count writes *grid (device) and totals [2] = {entries, n_cells} (device int64) with a workspace of
+ * sparf_distance_grid_workspace_bytes(P, 0); the caller reads the totals to size cell_start and prims, and
+ * sparf_distance_grid_fill, with the same target and grid and a workspace of sparf_distance_grid_workspace_bytes(P,
+ * entries) (8 B per primitive + 12 B per entry + scan / sort scratch; 0 for invalid sizes and where no CUDA device is
+ * current), writes them.  sparf_distance_query reads the target, grid, cell_start and prims and needs no workspace.  No
+ * call synchronises; all are capturable.  An empty target (P = 0) gives an all-zero grid, totals {0, 0}, cell_start
+ * [1] = {0}, and a query of all misses; N = 0 is a no-op; no kernel runs over an empty set.  Invalid sizes, max_dist < 0 or NaN, and NULL pointers
+ * give SPARF_ERR_INVALID. */
+typedef struct SparfDistanceGrid {
+  float lo[3];       /* the padded box's low corner */
+  float cell[3];     /* the cell size per axis */
+  int32_t dims[3];   /* cells per axis (all 0 for an empty target) */
+  int32_t reserved;
+} SparfDistanceGrid;
+size_t sparf_distance_grid_workspace_bytes(int64_t n_prims, int64_t n_entries);
+int sparf_distance_grid_count(const float* vertices, int64_t n_verts, const int64_t* faces, int64_t n_faces,
+                              int32_t cells_x, int32_t cells_y, int32_t cells_z, SparfDistanceGrid* grid,
+                              int64_t* totals, void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+int sparf_distance_grid_fill(const float* vertices, int64_t n_verts, const int64_t* faces, int64_t n_faces,
+                             const SparfDistanceGrid* grid, int64_t n_cells, int64_t n_entries, int32_t* cell_start,
+                             int32_t* prims, void* workspace, size_t workspace_bytes, sparf_stream_t stream);
+int sparf_distance_query(const float* vertices, int64_t n_verts, const int64_t* faces, int64_t n_faces,
+                         const SparfDistanceGrid* grid, const int32_t* cell_start, const int32_t* prims,
+                         const float* points, int64_t n_points, float max_dist, float* dist, int64_t* index,
+                         float* closest, sparf_stream_t stream);
+
 /* ---------------------------------------------------------------- occupancy grid
  * Empty-space skipping for inference renders (sparf_b200/occupancy.py): a bitfield over the box [r0, r1]^3 split into
  * res^3 cells, built from the density lattice sigma [res+1]^3 of mesh.density_grid (lattice point (a,b,c) at

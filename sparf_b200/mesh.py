@@ -1,6 +1,7 @@
 """Mesh extraction from a trained NeRF, BARF's recipe on the device: the density on the lattice of `opt.trimesh`
 (train_settings/default_config.py:267-271), marching cubes (csrc/mcubes.cu), world coordinates, optional normals from
-the density's gradient, floater removal by connected components (keep_components), and a binary PLY writer.
+the density's gradient, floater removal by connected components (keep_components), simplification (simplify),
+measurement against a reference surface (compare: Chamfer distance, F-score), and a PLY writer and reader.
 
     from sparf_b200 import mesh
     m = mesh.extract_mesh(opt, graph.nerf, normals=True)        # or graph.nerf_fine
@@ -244,6 +245,220 @@ def simplify(m: dict, target_faces: int, stats=None) -> dict:
     if stats is not None:
         stats.update(st, faces_before=m["faces"].shape[0], faces_after=faces.shape[0],
                      reached=faces.shape[0] <= target_faces)
+    return out
+
+
+def sample_surface(m: dict, n: int, seed: int = 0) -> torch.Tensor:
+    """n points [n, 3] (fp32) on the triangles of the mesh dict m, uniform over its area: a face by searchsorted of fp64
+    uniforms (scaled to the total) in the fp64 cumulative face areas, a point in it at the barycentrics (1 - sqrt(u1),
+    sqrt(u1) (1 - u2), sqrt(u1) u2).  The uniforms come from a torch.Generator on the mesh's device seeded with seed.
+    A mesh without faces or area gives no points."""
+    if isinstance(n, bool) or not isinstance(n, int) or n < 0:
+        raise ValueError("sample_surface: n must be an int >= 0 (got %r)" % (n,))
+    v, f = m["vertices"], m["faces"]
+    dev = v.device
+    p = v.double()[f] if f.numel() else torch.zeros(0, 3, 3, dtype=torch.float64, device=dev)
+    area = torch.linalg.cross(p[:, 1] - p[:, 0], p[:, 2] - p[:, 0]).norm(dim=1) / 2
+    cum = torch.cumsum(area, 0)
+    if n == 0 or cum.numel() == 0 or not cum[-1].item() > 0:
+        return torch.zeros(0, 3, dtype=torch.float32, device=dev)
+    g = torch.Generator(device=dev)
+    g.manual_seed(seed)
+    u = torch.rand(3, n, generator=g, device=dev, dtype=torch.float64)
+    face = torch.searchsorted(cum, u[0] * cum[-1], right=True).clamp_(max=cum.numel() - 1)
+    s = u[1].sqrt()
+    w = torch.stack([1 - s, s * (1 - u[2]), s * u[2]], 1)
+    return (w[:, :, None] * p[face]).sum(1).float()
+
+
+def distance_metrics(d_acc: torch.Tensor, d_comp: torch.Tensor, threshold: float, max_dist=float("inf")) -> dict:
+    """The metrics of compare from the distances of the pred samples to ref (d_acc) and of the ref samples to pred
+    (d_comp), misses as inf: accuracy / completeness = the fp64 means of min(d, max_dist) (NaN over no samples),
+    chamfer = their mean, precision / recall = the fractions with d < threshold (0 over no samples), fscore = 2PR /
+    (P + R) (0 when P + R = 0), hausdorff = the larger maximum of min(d, max_dist) (of the sides with samples; NaN
+    when neither has any), n_pred, n_ref."""
+    out = dict(n_pred=int(d_acc.numel()), n_ref=int(d_comp.numel()))
+    means, fracs, maxes = [], [], []
+    for d in (d_acc, d_comp):
+        d = d.double().clamp(max=float(max_dist))
+        means.append(d.mean().item() if d.numel() else float("nan"))
+        fracs.append((d < threshold).double().mean().item() if d.numel() else 0.0)
+        if d.numel():
+            maxes.append(d.max().item())
+    P, R = fracs
+    out.update(accuracy=means[0], completeness=means[1], chamfer=(means[0] + means[1]) / 2, precision=P, recall=R,
+               fscore=2 * P * R / (P + R) if P + R > 0 else 0.0, hausdorff=max(maxes) if maxes else float("nan"))
+    return out
+
+
+def _phase(phases, name, fn):
+    """fn(), its synchronised wall time added to phases[name] (s) when phases is a dict"""
+    if phases is None:
+        return fn()
+    import time
+    torch.cuda.synchronize()
+    t = time.perf_counter()
+    out = fn()
+    torch.cuda.synchronize()
+    phases[name] = phases.get(name, 0.0) + time.perf_counter() - t
+    return out
+
+
+def prepare(m: dict, n_samples: int = 1_000_000, seed: int = 0, stats=None) -> dict:
+    """One side of compare, ready to be compared many times: m with "points" (n_samples surface samples of a mesh,
+    sample_surface with seed; the vertices of a point cloud, a dict without faces) and "grid" (ops.distance_grid of its
+    triangles, or of its points).  A dict that already has both is returned as it is.  stats: an optional dict that
+    receives the time of the sample and grid phases (s)."""
+    if m.get("grid") is not None and m.get("points") is not None:
+        return m
+    if m.get("faces") is not None:
+        pts = _phase(stats, "sample", lambda: sample_surface(m, n_samples, seed))
+        grid = _phase(stats, "grid", lambda: ops.distance_grid(m["vertices"], m["faces"]))
+    else:
+        pts = m["vertices"]
+        grid = _phase(stats, "grid", lambda: ops.distance_grid(m["vertices"]))
+    return dict(m, points=pts, grid=grid)
+
+
+def compare(pred: dict, ref: dict, threshold: float, n_samples: int = 1_000_000, max_dist=float("inf"), seed: int = 0,
+            stats=None) -> dict:
+    """How close the mesh dict pred is to the reference ref (a mesh dict, or a point cloud: a dict without faces, such as
+    DTU's reference scans): accuracy = the mean distance of pred's samples to ref, completeness = of ref's samples to
+    pred, chamfer = their mean; precision, recall and their fscore at threshold; hausdorff; n_pred, n_ref
+    (distance_metrics).  A side with faces is sampled with n_samples points (sample_surface, seeds seed for pred and
+    seed + 1 for ref), a point cloud is used as it is; each side's primitives are its triangles, or its points.  The
+    distances are exact (ops.closest_points), capped at max_dist.  Either side may be a prepare()d dict, so that
+    scoring several meshes against one reference samples it and builds its grid once.  Masks and crops are the
+    caller's: filter the points before the call.  stats: an optional dict that receives the time of the sample, grid
+    and query phases (s, synchronised)."""
+    if not threshold > 0:
+        raise ValueError("compare: threshold must be > 0 (got %r)" % (threshold,))
+    if not max_dist >= 0:
+        raise ValueError("compare: max_dist must be >= 0 or inf (got %r)" % (max_dist,))
+    pred = prepare(pred, n_samples, seed, stats)
+    ref = prepare(ref, n_samples, seed + 1, stats)
+    d_acc = _phase(stats, "query", lambda: ops.closest_points(ref["grid"], pred["points"], max_dist)[0])
+    d_comp = _phase(stats, "query", lambda: ops.closest_points(pred["grid"], ref["points"], max_dist)[0])
+    return distance_metrics(d_acc, d_comp, threshold, max_dist)
+
+
+_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2", "ushort": "u2",
+              "uint16": "u2", "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4", "float": "f4", "float32": "f4",
+              "double": "f8", "float64": "f8"}
+
+
+def read_ply(path) -> dict:
+    """A PLY file (ascii or binary_little_endian) as a mesh dict: vertices [V, 3] fp32 from x, y, z; normals from nx,
+    ny, nz and colors (fp32; uchar / 255) from red, green, blue when present; faces [F, 3] int64 from the vertex_indices
+    (or vertex_index) list of the face element, or no faces entry when the file has no face element (a point cloud).
+    Any scalar type; other vertex properties are skipped.  Big-endian files, faces that are not triangles and list
+    properties other than the face list in a binary file raise ValueError.  The tensors are on the CPU."""
+    with open(path, "rb") as fh:
+        data = fh.read()
+    end = data.find(b"end_header")
+    if not data.startswith(b"ply") or end < 0:
+        raise ValueError("read_ply: %s is not a PLY file" % path)
+    body = data.index(b"\n", end) + 1
+    fmt, elements = None, []
+    for line in data[:end].decode("ascii", "replace").splitlines()[1:]:
+        w = line.split()
+        if not w or w[0] in ("comment", "obj_info"):
+            continue
+        if w[0] == "format":
+            fmt = w[1]
+        elif w[0] == "element":
+            elements.append((w[1], int(w[2]), []))
+        elif w[0] == "property" and elements:
+            if w[1] == "list":
+                if w[2] not in _PLY_TYPES or w[3] not in _PLY_TYPES:
+                    raise ValueError("read_ply: unknown list type in %r" % line)
+                elements[-1][2].append((w[4], (_PLY_TYPES[w[2]], _PLY_TYPES[w[3]])))
+            else:
+                if w[1] not in _PLY_TYPES:
+                    raise ValueError("read_ply: unknown property type in %r" % line)
+                elements[-1][2].append((w[2], _PLY_TYPES[w[1]]))
+    if fmt not in ("ascii", "binary_little_endian"):
+        raise ValueError("read_ply: format %r is not supported (ascii or binary_little_endian)" % fmt)
+    arrays = _ply_ascii(data[body:], elements) if fmt == "ascii" else _ply_binary(data[body:], elements)
+    vert = arrays.get("vertex")
+    if vert is None or not all(k in vert for k in "xyz"):
+        raise ValueError("read_ply: %s has no vertex element with x, y, z" % path)
+    cols = lambda names: np.stack([np.asarray(vert[k], np.float64) for k in names], 1)
+    out = dict(vertices=torch.from_numpy(cols("xyz").astype(np.float32)).reshape(-1, 3))
+    if all(k in vert for k in ("nx", "ny", "nz")):
+        out["normals"] = torch.from_numpy(cols(["nx", "ny", "nz"]).astype(np.float32)).reshape(-1, 3)
+    if all(k in vert for k in ("red", "green", "blue")):
+        c = cols(["red", "green", "blue"])
+        if vert["red"].dtype == np.uint8:
+            c = c / 255.0
+        out["colors"] = torch.from_numpy(c.astype(np.float32)).reshape(-1, 3)
+    if "face" in arrays:
+        out["faces"] = torch.from_numpy(arrays["face"]).reshape(-1, 3)
+    return out
+
+
+def _face_list(props):
+    names = [n for n, _ in props]
+    for key in ("vertex_indices", "vertex_index"):
+        if key in names:
+            return key
+    return None
+
+
+def _ply_ascii(text, elements):
+    words = text.split()
+    pos, out = 0, {}
+    for name, count, props in elements:
+        if name == "face" and count and _face_list(props) is None:
+            raise ValueError("read_ply: the face element has no vertex_indices list")
+        cols = {n: [] for n, _ in props}
+        faces = []
+        for _ in range(count):
+            for n, t in props:
+                if isinstance(t, tuple):
+                    k = int(words[pos])
+                    vals = [int(x) for x in words[pos + 1:pos + 1 + k]]
+                    pos += 1 + k
+                    if name == "face" and n == _face_list(props):
+                        if k != 3:
+                            raise ValueError("read_ply: a face with %d vertices (only triangles)" % k)
+                        faces.append(vals)
+                else:
+                    cols[n].append(float(words[pos]))
+                    pos += 1
+        if name == "vertex":
+            out["vertex"] = {n: np.asarray(cols[n], np.float64).astype(t) for n, t in props if not isinstance(t, tuple)}
+        elif name == "face":
+            out["face"] = np.asarray(faces, np.int64).reshape(-1, 3)
+    return out
+
+
+def _ply_binary(buf, elements):
+    pos, out = 0, {}
+    for name, count, props in elements:
+        lists = [(n, t) for n, t in props if isinstance(t, tuple)]
+        if not lists:
+            dt = np.dtype([(n, "<" + t) for n, t in props])
+            arr = np.frombuffer(buf, dt, count, pos)
+            pos += dt.itemsize * count
+            if name == "vertex":
+                out["vertex"] = {n: arr[n] for n, _ in props}
+            continue
+        if name != "face" or len(props) != 1 or _face_list(props) is None:
+            raise ValueError("read_ply: binary list properties are only read as the face element's vertex list")
+        ct, it = np.dtype("<" + props[0][1][0]), np.dtype("<" + props[0][1][1])
+        if count:
+            k = int(np.frombuffer(buf, ct, 1, pos)[0])
+            if k != 3:
+                raise ValueError("read_ply: a face with %d vertices (only triangles)" % k)
+            rec = np.dtype([("n", ct), ("v", it, (3,))])
+            arr = np.frombuffer(buf, rec, count, pos)
+            if (arr["n"] != 3).any():
+                raise ValueError("read_ply: a face that is not a triangle")
+            pos += rec.itemsize * count
+            out["face"] = arr["v"].astype(np.int64)
+        else:
+            out["face"] = np.zeros((0, 3), np.int64)
     return out
 
 

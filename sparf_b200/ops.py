@@ -895,6 +895,124 @@ def mesh_simplify(vertices, faces, target_faces: int, attrs=None, stats=None):
 
 
 # ------------------------------------------------------------------------------------------------
+# mesh distance (no gradient)
+# ------------------------------------------------------------------------------------------------
+GRID_BYTES = 40                 # sizeof(SparfDistanceGrid)
+MAX_GRID_CELLS = 1 << 24
+
+
+class DistanceGrid:
+    """A uniform grid over a target surface (distance_grid; include/sparf_b200.h, mesh distance): the target (vertices
+    [V, 3] fp32, faces [F, 3] int64 or None for a point cloud), the device grid description (params, the 40 bytes of
+    SparfDistanceGrid), the CSR lists cell_start [n_cells + 1] and prims [entries] (int32), and on the host the cells
+    per axis (dims) and the entry count.  Build it once, query it with closest_points as often as needed."""
+
+    def __init__(self, vertices, faces, params, cell_start, prims, dims, entries):
+        self.vertices, self.faces, self.params = vertices, faces, params
+        self.cell_start, self.prims, self.dims, self.entries = cell_start, prims, dims, entries
+
+    @property
+    def n_prims(self) -> int:
+        return self.vertices.shape[0] if self.faces is None else self.faces.shape[0]
+
+    def _target(self):
+        F = -1 if self.faces is None else self.faces.shape[0]
+        return (_ptr(self.vertices), self.vertices.shape[0], _ptr(self.faces), F)
+
+
+def _check_cells(cells_per_axis, what):
+    """(cx, cy, cz): (0, 0, 0) for None (automatic), else the given int or three ints, each >= 1, at most 2^24 cells"""
+    if cells_per_axis is None:
+        return (0, 0, 0)
+    if isinstance(cells_per_axis, numbers.Integral):
+        c = (cells_per_axis,) * 3
+    elif isinstance(cells_per_axis, (tuple, list)):
+        c = tuple(cells_per_axis)
+    else:
+        c = ()
+    if (len(c) != 3 or any(isinstance(x, bool) or not isinstance(x, numbers.Integral) or x < 1 for x in c)
+            or c[0] * c[1] * c[2] > MAX_GRID_CELLS):
+        raise ValueError("%s: cells_per_axis must be None, an int or three ints, each >= 1, with at most 2^24 cells "
+                         "(got %r)" % (what, cells_per_axis))
+    return tuple(int(x) for x in c)
+
+
+@torch.no_grad()
+@_on_tensor_device
+def distance_grid(vertices, faces=None, cells_per_axis=None) -> DistanceGrid:
+    """The uniform grid of closest_points over a triangle mesh (vertices [V, 3] fp32, faces [F, 3] int64, CUDA) or, with
+    faces None, over the point cloud vertices (include/sparf_b200.h, mesh distance).  cells_per_axis: None (automatic:
+    about min(2^24, P^1.5) cells for P primitives), an int or three ints; the query results do not depend on it.  Bad
+    arguments raise ValueError before any library call (with faces, one device-to-host copy checks the ids); one more
+    copy reads the entry and cell counts."""
+    what = "distance_grid"
+    if not torch.is_tensor(vertices) or vertices.dtype != torch.float32 or vertices.dim() != 2 or vertices.shape[1] != 3:
+        raise ValueError("%s: vertices must be a float32 tensor [V, 3]" % what)
+    n_verts = vertices.shape[0]
+    if n_verts > MAX_MESH_ELEMENTS:
+        raise ValueError("%s: %d vertices (at most 2^31 - 1)" % (what, n_verts))
+    cells = _check_cells(cells_per_axis, what)
+    if faces is not None:
+        _check_faces(faces, n_verts, what)
+        if faces.device != vertices.device:
+            raise ValueError("%s: vertices and faces must be on one CUDA device" % what)
+    if not vertices.is_cuda:
+        raise ValueError("%s: vertices must be a CUDA tensor" % what)
+    if faces is not None:
+        _check_ids(faces, n_verts, what)
+    L = _lib.lib()
+    v = vertices.contiguous()
+    f = faces.contiguous() if faces is not None else None
+    dev = v.device
+    P = n_verts if f is None else f.shape[0]
+    target = (_ptr(v), n_verts, _ptr(f), -1 if f is None else f.shape[0])
+    params = torch.empty(GRID_BYTES, dtype=torch.uint8, device=dev)
+    totals = torch.empty(2, dtype=torch.int64, device=dev)
+    ws = torch.empty(max(L.sparf_distance_grid_workspace_bytes(P, 0), 1), dtype=torch.uint8, device=dev)
+    check(L.sparf_distance_grid_count(*target, *cells, _ptr(params), _ptr(totals), _ptr(ws), ws.numel(), _stream()),
+          "distance_grid_count")
+    entries, n_cells, *dims = torch.cat([totals, params.view(torch.int32)[6:9].long()]).tolist()
+    if entries > MAX_MESH_ELEMENTS:
+        raise RuntimeError("%s: %d grid entries (at most 2^31 - 1): give fewer cells_per_axis" % (what, entries))
+    ws = torch.empty(max(L.sparf_distance_grid_workspace_bytes(P, entries), 1), dtype=torch.uint8, device=dev)
+    cell_start = torch.empty(n_cells + 1, dtype=torch.int32, device=dev)
+    prims = torch.empty(entries, dtype=torch.int32, device=dev)
+    check(L.sparf_distance_grid_fill(*target, _ptr(params), n_cells, entries, _ptr(cell_start), _ptr(prims), _ptr(ws),
+                                     ws.numel(), _stream()), "distance_grid_fill")
+    return DistanceGrid(v, f, params, cell_start, prims, tuple(dims), entries)
+
+
+@torch.no_grad()
+@_on_tensor_device
+def closest_points(grid: DistanceGrid, points, max_dist: float = float("inf")):
+    """The nearest primitive of grid's target to each of points [N, 3] (fp32, CUDA) -> (dist [N] fp32, index [N] int64,
+    closest [N, 3] fp32): the exact minimum over all primitives (ties to the smallest id), the same bytes for every
+    grid; inf / -1 / NaN where no primitive lies within max_dist (>= 0, inf allowed).  No host synchronisation, so it
+    can be captured in a CUDA graph.  Bad arguments raise ValueError before any library call."""
+    what = "closest_points"
+    if not isinstance(grid, DistanceGrid):
+        raise ValueError("%s: grid must be a DistanceGrid of distance_grid" % what)
+    if not torch.is_tensor(points) or points.dtype != torch.float32 or points.dim() != 2 or points.shape[1] != 3:
+        raise ValueError("%s: points must be a float32 tensor [N, 3]" % what)
+    if points.shape[0] > MAX_MESH_ELEMENTS:
+        raise ValueError("%s: %d points (at most 2^31 - 1)" % (what, points.shape[0]))
+    if points.device != grid.vertices.device:
+        raise ValueError("%s: points must be on the grid's CUDA device" % what)
+    if not isinstance(max_dist, numbers.Real) or not max_dist >= 0:
+        raise ValueError("%s: max_dist must be a number >= 0 or inf (got %r)" % (what, max_dist))
+    L = _lib.lib()
+    p = points.contiguous()
+    N, dev = p.shape[0], p.device
+    dist = torch.empty(N, dtype=torch.float32, device=dev)
+    index = torch.empty(N, dtype=torch.int64, device=dev)
+    closest = torch.empty(N, 3, dtype=torch.float32, device=dev)
+    check(L.sparf_distance_query(*grid._target(), _ptr(grid.params), _ptr(grid.cell_start), _ptr(grid.prims), _ptr(p),
+                                 N, float(max_dist), _ptr(dist), _ptr(index), _ptr(closest), _stream()),
+          "distance_query")
+    return dist, index, closest
+
+
+# ------------------------------------------------------------------------------------------------
 # occupancy grid (no gradient)
 # ------------------------------------------------------------------------------------------------
 @torch.no_grad()
