@@ -533,6 +533,35 @@ int sparf_distance_query(const float* vertices, int64_t n_verts, const int64_t* 
                          const float* points, int64_t n_points, float max_dist, float* dist, int64_t* index,
                          float* closest, sparf_stream_t stream);
 
+/* ---------------------------------------------------------------- mesh ray cast
+ * First hits of rays on a triangle mesh (sparf_b200/mesh.py: render, visible_faces, cull) over the grid, cell_start and
+ * prims of sparf_distance_grid_count / _fill for that mesh (n_faces >= 0; a point grid is refused).
+ *   rays:    origins [N][3], dirs [N][3] (fp32; d need not be unit: t is in units of d, so a pixel ray of raygen with
+ *            camera-space z = 1 gives t = camera z-depth) -> t [N] (fp32), face [N] (int64), bary [N][3] (fp32): the
+ *            minimum over every triangle of (t, id) with t_min <= t <= t_max, ties to the smallest id, and the hit's
+ *            barycentrics (U, V, W) / det of the face's vertices 0, 1, 2 (each in [0, 1], summing to 1 up to rounding).
+ *            A miss gives inf / -1 / NaN; so does a ray with a non-finite component or d = 0.
+ *   hit:     the watertight test of Woop, Benthin and Wald (JCGT 2013): k = the axis of the largest |d| (the first on
+ *            ties), kx = k + 1, ky = k + 2 (mod 3); per vertex A = v - o, Ax = A[kx] - (d[kx] / d[k]) A[k], Ay likewise,
+ *            Az = (1 / d[k]) A[k]; U = Cx By - Cy Bx, V = Ax Cy - Ay Cx, W = Bx Ay - By Ax,
+ *            recomputed in fp64 from the same fp32 Ax .. Cy when any is exactly 0; a hit when U, V, W are all >= 0 or
+ *            all <= 0, det = U + V + W != 0 and (b - a) x (c - a) != 0 exactly (in fp64: a zero-area triangle is never
+ *            hit); t = (U Az + V Bz + W Cz) / det.  Every fp32 operation is rounded on its own (no contraction): the hit
+ *            is one function of (ray, triangle), and a shared edge gives exactly opposite edge functions in its two
+ *            triangles, so a ray through an edge or vertex of a closed mesh cannot pass between them.  Triangles are
+ *            two-sided.  A face with an id outside [0, V) is never hit.
+ *   walk:    the slabs of cells perpendicular to k in ray order, clipped to [t_min, t_max] and the grid's box; in each,
+ *            the cells the ray's segment in the slab covers (padded by 2^-18 (|o|_inf + the box's largest
+ *            |coordinate|)); after each slab it stops once the slab's far plane, moved back by 2^-14 of that scale, gives
+ *            a t that, shrunk by 2^-20 of itself, is strictly greater than the best.  The result is the same bytes for every grid, including 1
+ *            x 1 x 1 (brute force); DESIGN §3.1.15 gives the argument.
+ * No workspace.  No call synchronises; it is capturable.  N = 0 is a no-op; an empty mesh (F = 0) gives all misses.
+ * Invalid sizes, t_min < 0, t_max < t_min, NaN bounds and NULL pointers give SPARF_ERR_INVALID. */
+int sparf_raycast(const float* vertices, int64_t n_verts, const int64_t* faces, int64_t n_faces,
+                  const SparfDistanceGrid* grid, const int32_t* cell_start, const int32_t* prims,
+                  const float* origins, const float* dirs, int64_t n_rays, float t_min, float t_max, float* t,
+                  int64_t* face, float* bary, sparf_stream_t stream);
+
 /* ---------------------------------------------------------------- occupancy grid
  * Empty-space skipping for inference renders (sparf_b200/occupancy.py): a bitfield over the box [r0, r1]^3 split into
  * res^3 cells, built from the density lattice sigma [res+1]^3 of mesh.density_grid (lattice point (a,b,c) at

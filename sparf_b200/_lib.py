@@ -99,6 +99,8 @@ _SIGNATURES = {
                                             _P]),
     "sparf_distance_grid_fill": (c_int32, [_P, c_int64, _P, c_int64, _P, c_int64, c_int64, _P, _P, _P, c_size_t, _P]),
     "sparf_distance_query": (c_int32, [_P, c_int64, _P, c_int64, _P, _P, _P, _P, c_int64, c_float, _P, _P, _P, _P]),
+    "sparf_raycast": (c_int32, [_P, c_int64, _P, c_int64, _P, _P, _P, _P, _P, c_int64, c_float, c_float, _P, _P, _P,
+                                _P]),
     "sparf_occupancy_build": (c_int32, [_P, c_int32, c_float, _P, _P]),
     "sparf_occupancy_workspace_bytes": (c_size_t, [c_int64, c_int32]),
     "sparf_occupancy_count": (c_int32, [c_int64, c_int32, _P, _P, _P, _P, c_int32, c_float, c_float, _P, _P, c_size_t, _P]),

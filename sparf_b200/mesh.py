@@ -1,7 +1,8 @@
 """Mesh extraction from a trained NeRF, BARF's recipe on the device: the density on the lattice of `opt.trimesh`
 (train_settings/default_config.py:267-271), marching cubes (csrc/mcubes.cu), world coordinates, optional normals from
 the density's gradient, floater removal by connected components (keep_components), simplification (simplify),
-measurement against a reference surface (compare: Chamfer distance, F-score), and a PLY writer and reader.
+measurement against a reference surface (compare: Chamfer distance, F-score), ray casting (render: mesh depth maps;
+visible_faces and cull: the part of a mesh that cameras see), and a PLY writer and reader.
 
     from sparf_b200 import mesh
     m = mesh.extract_mesh(opt, graph.nerf, normals=True)        # or graph.nerf_fine
@@ -340,6 +341,131 @@ def compare(pred: dict, ref: dict, threshold: float, n_samples: int = 1_000_000,
     d_acc = _phase(stats, "query", lambda: ops.closest_points(ref["grid"], pred["points"], max_dist)[0])
     d_comp = _phase(stats, "query", lambda: ops.closest_points(pred["grid"], ref["points"], max_dist)[0])
     return distance_metrics(d_acc, d_comp, threshold, max_dist)
+
+
+def _check_views(m, pose_w2c, intr, H, W, masks, grid, what, near=0.0, far=float("inf")):
+    """(B, the ray-cast grid or None when it is to be built) after ValueError checks that need no library call"""
+    real = lambda x: isinstance(x, (int, float)) and not isinstance(x, bool)
+    if not real(near) or not real(far) or not 0 <= near <= far:
+        raise ValueError("%s: need 0 <= near <= far (inf allowed), got %r, %r" % (what, near, far))
+    if not isinstance(m, dict) or not torch.is_tensor(m.get("vertices")) or not torch.is_tensor(m.get("faces")):
+        raise ValueError("%s: m must be a mesh dict with vertices and faces" % what)
+    if not torch.is_tensor(pose_w2c) or pose_w2c.dtype != torch.float32 or pose_w2c.dim() != 3 \
+            or tuple(pose_w2c.shape[1:]) != (3, 4) or pose_w2c.shape[0] < 1:
+        raise ValueError("%s: pose_w2c must be a float32 tensor [B, 3, 4] with B >= 1" % what)
+    B = pose_w2c.shape[0]
+    if not torch.is_tensor(intr) or intr.dtype != torch.float32 or tuple(intr.shape) not in ((3, 3), (B, 3, 3)):
+        raise ValueError("%s: intr must be a float32 tensor [3, 3] or [%d, 3, 3]" % (what, B))
+    for name, n in (("H", H), ("W", W)):
+        if isinstance(n, bool) or not isinstance(n, int) or n < 1:
+            raise ValueError("%s: %s must be an int >= 1 (got %r)" % (what, name, n))
+    if masks is not None and (not torch.is_tensor(masks) or masks.dtype not in (torch.bool, torch.uint8)
+                              or tuple(masks.shape) != (B, H, W)):
+        raise ValueError("%s: masks must be None or a bool / uint8 tensor [%d, %d, %d]" % (what, B, H, W))
+    dev = m["vertices"].device
+    if dev.type != "cuda" or any(x is not None and x.device != dev for x in (m["faces"], pose_w2c, intr, masks)):
+        raise ValueError("%s: the mesh, cameras and masks must be on one CUDA device" % what)
+    grid = grid if grid is not None else m.get("grid")
+    if grid is not None and (not isinstance(grid, ops.DistanceGrid) or grid.faces is None):
+        raise ValueError("%s: grid must be an ops.DistanceGrid of the mesh's triangles" % what)
+    return B, grid
+
+
+def _cast_views(m, pose_w2c, intr, H, W, near, far, grid):
+    """ops.raycast of the pixel-centre rays of every view (camera.get_center_and_ray) in chunks of about
+    tsdf.BATCH_PIXELS rays: yields (b0, b1, p0, p1, t, face, bary), the results for views b0..b1-1 and pixels p0..p1-1
+    as [b1 - b0, p1 - p0] (bary [..., 3])"""
+    from . import camera, tsdf
+    grid = grid if grid is not None else ops.distance_grid(m["vertices"], m["faces"])
+    B, HW = pose_w2c.shape[0], H * W
+    intr = intr.expand(B, 3, 3) if intr.dim() == 2 else intr
+    per_view = max(1, tsdf.BATCH_PIXELS // HW)
+    pix = min(HW, tsdf.BATCH_PIXELS)
+    for b0 in range(0, B, per_view):
+        b1 = min(B, b0 + per_view)
+        for p0 in range(0, HW, pix):
+            p1 = min(HW, p0 + pix)
+            idx = torch.arange(p0, p1, device=pose_w2c.device)
+            o, d = camera.get_center_and_ray(pose_w2c[b0:b1], H, W, intr[b0:b1], ray_idx=idx)
+            t, face, bary = ops.raycast(grid, o.reshape(-1, 3), d.reshape(-1, 3), near, far)
+            n = p1 - p0
+            yield b0, b1, p0, p1, t.view(-1, n), face.view(-1, n), bary.view(-1, n, 3)
+
+
+@torch.no_grad()
+def render(m: dict, pose_w2c, intr, H: int, W: int, near: float = 0.0, far: float = float("inf"), grid=None) -> dict:
+    """Depth maps of the mesh dict m from B views, pose_w2c [B, 3, 4] and intr [B, 3, 3] or [3, 3] (fp32, on the
+    mesh's CUDA device), H x W pixels: the first hit (ops.raycast, t in [near, far]) of each pixel-centre ray of
+    camera.get_center_and_ray.  -> dict(depth [B, H, W] fp32: t, the camera z-depth as in tsdf.render_maps, inf at
+    misses; face [B, H, W] int64, -1 at misses; bary [B, H, W, 3] fp32, NaN at misses), plus for each per-vertex entry
+    of m (normals, colors) its barycentric interpolation at the hit [B, H, W, C], NaN at misses.  The grid is grid if
+    given, else m["grid"] of a prepare()d dict, else ops.distance_grid of m's triangles.  ValueError for bad arguments
+    before any library call."""
+    B, grid = _check_views(m, pose_w2c, intr, H, W, None, grid, "render", near, far)
+    dev = m["vertices"].device
+    out = dict(depth=torch.empty(B, H * W, device=dev), face=torch.empty(B, H * W, dtype=torch.int64, device=dev),
+               bary=torch.empty(B, H * W, 3, device=dev))
+    for b0, b1, p0, p1, t, face, bary in _cast_views(m, pose_w2c, intr, H, W, near, far, grid):
+        out["depth"][b0:b1, p0:p1] = t
+        out["face"][b0:b1, p0:p1] = face
+        out["bary"][b0:b1, p0:p1] = bary
+    f = m["faces"]
+    for k in VERTEX_KEYS[1:]:
+        if m.get(k) is None:
+            continue
+        a = m[k]
+        if f.shape[0] == 0:
+            out[k] = torch.full((B, H * W, a.shape[1]), float("nan"), device=dev)
+            continue
+        corners = a[f[out["face"].clamp(min=0)]]                       # [B, HW, 3, C]
+        out[k] = (out["bary"][..., None] * corners).sum(-2)            # NaN barycentrics at misses give NaN
+    for k, v in out.items():
+        out[k] = v.view(B, H, W, *v.shape[2:])
+    return out
+
+
+@torch.no_grad()
+def visible_faces(m: dict, pose_w2c, intr, H: int, W: int, masks=None, grid=None) -> torch.Tensor:
+    """bool [F]: the faces of the mesh dict m that are the first hit (render's) of the pixel-centre ray of at least one
+    pixel of at least one view, counting only the pixels inside masks [B, H, W] (bool / uint8) when given.  Visibility
+    is sampled at pixel centres, as a rasterizer samples coverage: a face that no pixel centre hits first (smaller than
+    a pixel, or seen only edge-on) is not visible."""
+    B, grid = _check_views(m, pose_w2c, intr, H, W, masks, grid, "visible_faces")
+    F = m["faces"].shape[0]
+    vis = torch.zeros(F, dtype=torch.bool, device=m["vertices"].device)
+    flat = masks.reshape(B, H * W) if masks is not None else None
+    for b0, b1, p0, p1, _, face, _ in _cast_views(m, pose_w2c, intr, H, W, 0.0, float("inf"), grid):
+        keep = face >= 0
+        if flat is not None:
+            keep &= flat[b0:b1, p0:p1].bool()
+        vis[face[keep]] = True
+    return vis
+
+
+@torch.no_grad()
+def cull(m: dict, pose_w2c, intr, H: int, W: int, masks=None, stats=None) -> dict:
+    """The part of the mesh dict m that the views see (visible_faces, with masks [B, H, W] when given): the visible
+    faces in their order with renumbered ids, and the vertices they use in their order with their vertices / normals /
+    colors gathered; other entries are passed on as they are (the output of keep_components, so cull, keep_components,
+    simplify and compare chain), except the points and grid of a prepare()d dict, which describe the uncut mesh and are
+    dropped.  DTU's evaluation culls a predicted mesh this way before scoring it.  stats: an optional dict that receives
+    faces_before, faces_after, views and pixels (the rays cast)."""
+    B, _ = _check_views(m, pose_w2c, intr, H, W, masks, None, "cull")
+    faces = m["faces"]
+    vis = visible_faces(m, pose_w2c, intr, H, W, masks=masks)
+    kept = faces[vis]
+    used = torch.zeros(m["vertices"].shape[0], dtype=torch.bool, device=faces.device)
+    used[kept.reshape(-1)] = True
+    new_id = torch.cumsum(used, 0) - 1
+    out = {k: v for k, v in m.items() if k not in ("points", "grid")}
+    out["faces"] = new_id[kept]
+    vert_ids = torch.nonzero(used).flatten()
+    for k in VERTEX_KEYS:
+        if m.get(k) is not None:
+            out[k] = m[k][vert_ids]
+    if stats is not None:
+        stats.update(faces_before=faces.shape[0], faces_after=kept.shape[0], views=B, pixels=B * H * W)
+    return out
 
 
 _PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2", "ushort": "u2",

@@ -1012,6 +1012,41 @@ def closest_points(grid: DistanceGrid, points, max_dist: float = float("inf")):
     return dist, index, closest
 
 
+@torch.no_grad()
+@_on_tensor_device
+def raycast(grid: DistanceGrid, origins, dirs, t_min: float = 0.0, t_max: float = float("inf")):
+    """The first triangle of grid's mesh that each ray o + t d meets, origins and dirs [N, 3] (fp32, CUDA) ->
+    (t [N] fp32, face [N] int64, bary [N, 3] fp32): the exact minimum over all triangles of (t, id) with t in [t_min,
+    t_max] (ties to the smallest id) by a watertight, two-sided hit test, the same bytes for every grid, and the hit's
+    barycentrics of the face's vertices; inf / -1 / NaN for a miss (include/sparf_b200.h, mesh ray cast).  t is in
+    units of d: a pixel ray of raygen (camera-space z = 1) gives the camera z-depth.  No host synchronisation, so it
+    can be captured in a CUDA graph.  Bad arguments raise ValueError before any library call."""
+    what = "raycast"
+    if not isinstance(grid, DistanceGrid) or grid.faces is None:
+        raise ValueError("%s: grid must be a DistanceGrid of a triangle mesh (distance_grid with faces)" % what)
+    for name, x in (("origins", origins), ("dirs", dirs)):
+        if not torch.is_tensor(x) or x.dtype != torch.float32 or x.dim() != 2 or x.shape[1] != 3:
+            raise ValueError("%s: %s must be a float32 tensor [N, 3]" % (what, name))
+        if x.device != grid.vertices.device:
+            raise ValueError("%s: %s must be on the grid's CUDA device" % (what, name))
+    if origins.shape != dirs.shape:
+        raise ValueError("%s: origins %s and dirs %s differ" % (what, list(origins.shape), list(dirs.shape)))
+    if origins.shape[0] > MAX_MESH_ELEMENTS:
+        raise ValueError("%s: %d rays (at most 2^31 - 1)" % (what, origins.shape[0]))
+    real = lambda x: isinstance(x, numbers.Real) and not isinstance(x, bool)
+    if not real(t_min) or not real(t_max) or not 0 <= t_min <= t_max:
+        raise ValueError("%s: need 0 <= t_min <= t_max (inf allowed), got %r, %r" % (what, t_min, t_max))
+    L = _lib.lib()
+    o, d = origins.contiguous(), dirs.contiguous()
+    N, dev = o.shape[0], o.device
+    t = torch.empty(N, dtype=torch.float32, device=dev)
+    face = torch.empty(N, dtype=torch.int64, device=dev)
+    bary = torch.empty(N, 3, dtype=torch.float32, device=dev)
+    check(L.sparf_raycast(*grid._target(), _ptr(grid.params), _ptr(grid.cell_start), _ptr(grid.prims), _ptr(o), _ptr(d),
+                          N, float(t_min), float(t_max), _ptr(t), _ptr(face), _ptr(bary), _stream()), "raycast")
+    return t, face, bary
+
+
 # ------------------------------------------------------------------------------------------------
 # occupancy grid (no gradient)
 # ------------------------------------------------------------------------------------------------

@@ -2,13 +2,16 @@
 """Measure a mesh against a reference surface on the GPU (sparf_b200.mesh.compare): Chamfer accuracy and completeness,
 precision, recall and F-score at a distance threshold, and the Hausdorff distance.
 
-    python tools/compare_mesh.py PRED.ply REF.ply --threshold T [--samples N] [--max-dist D] [--seed S]
+    python tools/compare_mesh.py PRED.ply REF.ply --threshold T [--samples N] [--max-dist D] [--seed S] [--cull CAMERAS]
 
 Both files are read with mesh.read_ply (ascii or binary little-endian).  A file with faces is sampled with N points
 (default 1 000 000) uniformly over its area; a file without a face element is a point cloud (such as DTU's reference
 scans) and its points are used as they are.  Distances are exact closest-point distances to the other side's
 triangles (or points), capped at D.  Masks and crops are the caller's: filter the points before writing the files.
-Prints the metrics, V and F of each side, and the time of each phase (load, sample, grid, query).
+--cull CAMERAS first keeps only the faces of PRED that the views of CAMERAS see (mesh.cull; a .npz or .pt file with
+pose_w2c [B,3,4], intr [B,3,3], H, W and optionally mask [B,H,W], as tools/extract_mesh.py reads it), as DTU's
+evaluation culls a predicted mesh; the reference is not culled.
+Prints the metrics, V and F of each side, and the time of each phase (load, [cull,] sample, grid, query).
 """
 import argparse
 import math
@@ -30,6 +33,8 @@ def build_parser():
     ap.add_argument("--samples", type=int, default=1_000_000, help="surface samples of a side with faces")
     ap.add_argument("--max-dist", type=float, default=float("inf"), help="cap of every distance (default: none)")
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--cull", metavar="CAMERAS", default=None,
+                    help="score only the faces of PRED these cameras see (.npz / .pt, optional mask)")
     return ap
 
 
@@ -55,6 +60,10 @@ def main(argv=None):
         sides.append({k: v.cuda() for k, v in m.items()})
     torch.cuda.synchronize()
     phases = {"load": time.perf_counter() - t0}
+    if args.cull:
+        assert sides[0].get("faces") is not None, "--cull needs a PRED with faces"
+        from extract_mesh import cull_mesh
+        sides[0] = cull_mesh(args.cull, sides[0], lambda name, fn: mesh._phase(phases, name, fn))
     res = mesh.compare(sides[0], sides[1], args.threshold, n_samples=args.samples, max_dist=args.max_dist,
                        seed=args.seed, stats=phases)
     for name, path, m in (("pred", args.pred, sides[0]), ("ref", args.ref, sides[1])):

@@ -6,7 +6,7 @@ opt.trimesh, on the GPU).
                                  [--range -1.2 1.2] [--thres 25] [--normals] [--barf-c2f START END] [--sparse]
     python tools/extract_mesh.py model.pth.tar --out mesh.ply --tsdf cameras.npz [--res 128] [--range -1.2 1.2]
                                  [--trunc T] [--samples 128] [--samples-fine 128] [--barf-c2f START END]
-    either form takes [--keep-largest K] [--min-faces N] [--simplify F]
+    either form takes [--cull CAMERAS] [--keep-largest K] [--min-faces N] [--simplify F]
 
 The snapshot is what the reference's trainer saves (base_trainer.py:196-216): the model dict is ckpt["state_dict"],
 with the Graph's keys nerf.* / nerf_fine.* (or, from a joint pose trainer, those under "nerf_net").  The architecture
@@ -18,6 +18,9 @@ present) renders the views of CAMERAS, a .npz or .pt file with pose_w2c [B,3,4],
 (metric near, far), with --samples / --samples-fine samples per ray; the depth and colour maps are integrated into a TSDF
 volume over --res / --range with truncation --trunc (default tsdf.TRUNC_VOXELS voxels), and the coloured mesh of its
 zero level is written.
+--cull CAMERAS first keeps only the faces that the views of CAMERAS see (mesh.cull: the first hit of some pixel-centre
+ray, inside the view's mask when the file has mask [B,H,W]; depth_range is not needed), prints the faces removed and
+times a cull phase; on the density paths --normals are then computed at the kept vertices.
 --keep-largest K and --min-faces N remove floaters from any of these meshes (mesh.keep_components): of the connected
 components with at least N faces only the K largest are kept; the tool then also prints the component counts and times
 a components phase.
@@ -70,7 +73,8 @@ def graph_opt_from_state_dict(sd, barf_c2f, depth_range, samples, samples_fine):
 
 
 def load_cameras(path):
-    """pose_w2c [B,3,4], intr [B,3,3] (fp32 tensors), H, W, depth_range (near, far) of a .npz or .pt camera file"""
+    """pose_w2c [B,3,4], intr [B,3,3] (fp32 tensors), H, W, depth_range (near, far) or None where the file has none, and
+    mask [B,H,W] (bool tensor) or None, of a .npz or .pt camera file"""
     import numpy as np
     if path.endswith(".npz"):
         with np.load(path) as z:
@@ -78,8 +82,24 @@ def load_cameras(path):
     else:
         cams = torch.load(path, map_location="cpu", weights_only=False)
     t = lambda x: torch.as_tensor(np.asarray(x), dtype=torch.float32)
+    depth_range = cams.get("depth_range")
+    mask = cams.get("mask")
     return (t(cams["pose_w2c"]), t(cams["intr"]), int(cams["H"]), int(cams["W"]),
-            tuple(float(x) for x in np.asarray(cams["depth_range"]).reshape(2)))
+            None if depth_range is None else tuple(float(x) for x in np.asarray(depth_range).reshape(2)),
+            None if mask is None else torch.as_tensor(np.asarray(mask)).bool())
+
+
+def cull_mesh(path, m, phase):
+    """mesh.cull of the mesh dict m to the views (and masks) of the camera file path, printing the faces removed"""
+    from sparf_b200 import mesh
+    pose, intr, H, W, _, mask = load_cameras(path)
+    dev = m["vertices"].device
+    stats = {}
+    m = phase("cull", lambda: mesh.cull(m, pose.to(dev), intr.to(dev), H, W,
+                                        masks=None if mask is None else mask.to(dev), stats=stats))
+    print("cull: %d views %dx%d%s, faces %d -> %d (removed %d)" % (stats["views"], H, W, ", masked" if mask is not None
+          else "", stats["faces_before"], stats["faces_after"], stats["faces_before"] - stats["faces_after"]))
+    return m
 
 
 def filter_components(args, m, phase):
@@ -113,7 +133,8 @@ def main_tsdf(args):
     sd = torch.load(args.snapshot, map_location="cpu", weights_only=False)["state_dict"]
     sd = sd.get("nerf_net", sd)
     assert any(k.startswith("nerf.") for k in sd), "the snapshot has no nerf.* tensors"
-    pose, intr, H, W, depth_range = load_cameras(args.tsdf)
+    pose, intr, H, W, depth_range, _ = load_cameras(args.tsdf)
+    assert depth_range is not None, "--tsdf needs depth_range in the camera file"
     opt = graph_opt_from_state_dict(sd, args.barf_c2f, depth_range, args.samples, args.samples_fine)
     graph = Graph(opt, torch.device("cuda"))
     graph.load_state_dict({k: v for k, v in sd.items() if k.startswith(("nerf.", "nerf_fine."))})
@@ -136,6 +157,8 @@ def main_tsdf(args):
             break
         phase("integrate", lambda: tsdf.integrate_(vol, batch[0], batch[1], batch[2], rgb=batch[3], valid=batch[4]))
     m = phase("marching_cubes", lambda: tsdf.extract_mesh(vol))
+    if args.cull:
+        m = cull_mesh(args.cull, m, phase)
     m = simplify(args, filter_components(args, m, phase), phase)
     phase("write_ply", lambda: mesh.write_ply(args.out, m["vertices"], m["faces"], colors=m["colors"]))
     print("%s: V %d, F %d (TSDF of %d views %dx%d, res %d, range %s, trunc %g)"
@@ -170,6 +193,8 @@ def build_parser():
     ap.add_argument("--trunc", type=float, default=None, help="TSDF truncation in world units (--tsdf)")
     ap.add_argument("--samples", type=int, default=128, help="coarse samples per ray of the renders (--tsdf)")
     ap.add_argument("--samples-fine", type=int, default=128, help="fine samples per ray of the renders (--tsdf)")
+    ap.add_argument("--cull", metavar="CAMERAS", default=None,
+                    help="keep only the faces these cameras (.npz / .pt, optional mask) see (mesh.cull)")
     ap.add_argument("--keep-largest", type=int, default=None, metavar="K",
                     help="keep only the K connected components with the most faces")
     ap.add_argument("--min-faces", type=int, default=None, metavar="N",
@@ -225,13 +250,16 @@ def main(argv=None):
         sigma = phase("density_grid", lambda: mesh.density_grid(opt, nerf))
         verts, faces = phase("marching_cubes", lambda: mesh.marching_cubes(sigma, thres))
     del sigma
-    verts = mesh.to_world(verts, res, rng)
+    m = dict(vertices=mesh.to_world(verts, res, rng), faces=faces)
+    if args.cull:
+        m = cull_mesh(args.cull, m, phase)
+    verts = m["vertices"]
     if args.simplify is None:
         normals = phase("normals", lambda: mesh.density_normals(nerf, verts)) if args.normals else None
-        m = filter_components(args, dict(vertices=verts, faces=faces, normals=normals), phase)
+        m = filter_components(args, dict(m, normals=normals), phase)
         verts, faces, normals = m["vertices"], m["faces"], m["normals"]
     else:       # the normals of the final vertices, not interpolated ones
-        m = simplify(args, filter_components(args, dict(vertices=verts, faces=faces), phase), phase)
+        m = simplify(args, filter_components(args, m, phase), phase)
         verts, faces = m["vertices"], m["faces"]
         normals = phase("normals", lambda: mesh.density_normals(nerf, verts)) if args.normals else None
     phase("write_ply", lambda: mesh.write_ply(args.out, verts, faces, normals))
