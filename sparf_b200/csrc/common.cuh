@@ -51,6 +51,58 @@ extern unsigned long long g_launch_count;
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// the blocks of `threads` threads that cover n items, and the item of the calling thread
+static inline unsigned grid_of(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
+__device__ __forceinline__ long long thread_index() { return (long long)blockIdx.x * blockDim.x + threadIdx.x; }
+
+// The layout of a caller's workspace: each take<T>(count) starts at the next multiple of 256 B and returns a typed
+// pointer (NULL when the base is NULL: the carve only measures).  end = the last piece's offset plus its size.
+struct WsCarver {
+  char* base;
+  size_t end = 0;
+  explicit WsCarver(void* ws) : base((char*)ws) {}
+  template <typename T>
+  T* take(size_t count) {
+    const size_t o = align_up(end, 256);
+    end = o + count * sizeof(T);
+    return base ? (T*)(base + o) : nullptr;
+  }
+};
+
+// The largest scratch of a set of cub size queries.  cub sizes its scratch for the current device: without one a query
+// fails, its error is cleared, ok turns false and the later queries are skipped.
+struct CubScratch {
+  size_t bytes = 0;
+  bool ok = true;
+  // query: cudaError_t (size_t& bytes), one cub call with a NULL scratch pointer
+  template <typename Query>
+  void add(Query query) {
+    if (!ok) return;
+    size_t b = 0;
+    if (query(b) != cudaSuccess) {
+      cudaGetLastError();
+      ok = false;
+    } else if (b > bytes) {
+      bytes = b;
+    }
+  }
+};
+
+// A call's workspace ws of `have` bytes against the `need` bytes its carve measured: SPARF_ERR_INVALID for a NULL ws,
+// SPARF_ERR_CUDA for need = 0 (cub could not size its scratch), SPARF_ERR_WORKSPACE when have < need.
+static inline int check_workspace(const char* what, const void* ws, size_t have, size_t need) {
+  SPARF_REQUIRE(ws, "%s: NULL workspace", what);
+  if (need == 0) {
+    set_error("%s: no current CUDA device to size the cub scratch for", what);
+    return SPARF_ERR_CUDA;
+  }
+  if (have < need) {
+    set_error("%s: workspace %zu B < %zu B", what, have, need);
+    return SPARF_ERR_WORKSPACE;
+  }
+  return SPARF_OK;
+}
+
 // A row count read on the device (the *_rows and *_span MLP entry points): of the cap rows a kernel is sized for,
 // starting at row m0 of the call, it processes min(cap, max(0, *rows - s - m0)), s = *start (start NULL: s = 0).  The
 // span forward (start != NULL) adds s to the row of every global input, output and tape buffer it touches; workspace

@@ -149,10 +149,10 @@ struct Carve {
 // the workspace of a compaction over n = R * S samples
 size_t carve(int64_t R, int32_t S, void* ws, Carve* c) {
   const long long ntiles = ((long long)R * S + kOcTile - 1) / kOcTile;
-  const size_t a = align_up((size_t)ntiles * kOcThreads * 4, 256);
-  char* b = (char*)ws;
-  if (c) *c = Carve{(uint32_t*)b, (long long*)(b + a), ntiles};
-  return a + (size_t)ntiles * sizeof(long long);
+  WsCarver w(ws);
+  const Carve k{w.take<uint32_t>(ntiles * kOcThreads), w.take<long long>(ntiles), ntiles};
+  if (c) *c = k;
+  return w.end;
 }
 
 Lookup make_lookup(int64_t R, int32_t S, const float* origins, const float* dirs, const float* t, const uint32_t* bits,

@@ -62,10 +62,10 @@ struct SampleCarve {
 size_t sample_carve(int32_t res, void* ws, SampleCarve* c) {
   const long long words = ((long long)res * res * res + 31) / 32;
   const long long ntiles = (words + kOcTile - 1) / kOcTile;
-  const size_t a = align_up((size_t)words * 4, 256), b = align_up((size_t)ntiles * 8, 256);
-  char* p = (char*)ws;
-  if (c) *c = SampleCarve{(uint32_t*)p, (long long*)(p + a), (int64_t*)(p + a + b), words, ntiles};
-  return a + b + sizeof(int64_t);
+  WsCarver w(ws);
+  const SampleCarve k{w.take<uint32_t>(words), w.take<long long>(ntiles), w.take<int64_t>(1), words, ntiles};
+  if (c) *c = k;
+  return w.end;
 }
 
 size_t ema_bytes(int32_t res) { return (size_t)res * res * res * 4; }
@@ -229,11 +229,7 @@ extern "C" int sparf_occupancy_sample(int32_t res, const uint32_t* bits, float r
   if (n == 0) return SPARF_OK;
   SPARF_REQUIRE(bits && u_cell && u_jit && cells && points && workspace, "occupancy_sample: NULL pointer");
   SampleCarve c;
-  const size_t need = sample_carve(res, workspace, &c);
-  if (workspace_bytes < need) {
-    set_error("occupancy_sample: workspace %zu B < %zu B", workspace_bytes, need);
-    return SPARF_ERR_WORKSPACE;
-  }
+  SPARF_TRY(check_workspace("occupancy_sample", workspace, workspace_bytes, sample_carve(res, workspace, &c)));
   cudaStream_t s = (cudaStream_t)stream;
   const GridShape G = make_shape(res, contracted);
   grid_count_kernel<<<(unsigned)c.ntiles, kOcThreads, 0, s>>>(G, bits, c.words, c.local, c.tiles);
@@ -257,10 +253,7 @@ extern "C" int sparf_occupancy_ema(int32_t res, int32_t contracted, int64_t n, c
   SPARF_REQUIRE(n >= 0 && n <= (1ll << 31), "occupancy_ema: n %lld (0 ... 2^31)", (long long)n);
   SPARF_REQUIRE(decay > 0.f && decay <= 1.f, "occupancy_ema: decay %g (0 < decay <= 1)", (double)decay);
   SPARF_REQUIRE(density && bits && workspace && (n == 0 || (cells && sigma)), "occupancy_ema: NULL pointer");
-  if (workspace_bytes < ema_bytes(res)) {
-    set_error("occupancy_ema: workspace %zu B < %zu B", workspace_bytes, ema_bytes(res));
-    return SPARF_ERR_WORKSPACE;
-  }
+  SPARF_TRY(check_workspace("occupancy_ema", workspace, workspace_bytes, ema_bytes(res)));
   cudaStream_t s = (cudaStream_t)stream;
   const GridShape G = make_shape(res, contracted != 0);
   int* smax = (int*)workspace;

@@ -311,10 +311,10 @@ struct Carve {
 size_t carve(int64_t nx, int64_t ny, int64_t nz, void* ws, Carve* c) {
   const long long n = (long long)nx * ny * nz;
   const long long ntiles = (n + kMcTile - 1) / kMcTile;
-  const size_t a = align_up((size_t)n * 4, 256);
-  char* b = (char*)ws;
-  if (c) *c = Carve{(uint32_t*)b, (uint32_t*)(b + a), (longlong2*)(b + 2 * a), ntiles};
-  return 2 * a + (size_t)ntiles * sizeof(longlong2);
+  WsCarver w(ws);
+  const Carve k{w.take<uint32_t>(n), w.take<uint32_t>(n), w.take<longlong2>(ntiles), ntiles};
+  if (c) *c = k;
+  return w.end;
 }
 
 Vol make_vol(const float* vol, int64_t nx, int64_t ny, int64_t nz, float iso) {
@@ -328,11 +328,7 @@ int mcubes_count(const char* what, const float* vol, int64_t nx, int64_t ny, int
                 (long long)nx, (long long)ny, (long long)nz);
   SPARF_REQUIRE(vol && totals && workspace, "%s: NULL pointer", what);
   Carve c;
-  const size_t need = carve(nx, ny, nz, workspace, &c);
-  if (workspace_bytes < need) {
-    set_error("%s: workspace %zu B < %zu B", what, workspace_bytes, need);
-    return SPARF_ERR_WORKSPACE;
-  }
+  SPARF_TRY(check_workspace(what, workspace, workspace_bytes, carve(nx, ny, nz, workspace, &c)));
   SPARF_REQUIRE(c.ntiles < (1ll << 31), "%s: volume too large", what);
   cudaStream_t s = (cudaStream_t)stream;
   const Vol V = make_vol(vol, nx, ny, nz, iso);
@@ -351,11 +347,7 @@ int mcubes_emit(const char* what, const float* vol, int64_t nx, int64_t ny, int6
                 (long long)nx, (long long)ny, (long long)nz);
   SPARF_REQUIRE(vol && workspace, "%s: NULL pointer", what);
   Carve c;
-  const size_t need = carve(nx, ny, nz, workspace, &c);
-  if (workspace_bytes < need) {
-    set_error("%s: workspace %zu B < %zu B", what, workspace_bytes, need);
-    return SPARF_ERR_WORKSPACE;
-  }
+  SPARF_TRY(check_workspace(what, workspace, workspace_bytes, carve(nx, ny, nz, workspace, &c)));
   SPARF_REQUIRE(c.ntiles < (1ll << 31), "%s: volume too large", what);
   mcubes_emit_kernel<kMasked><<<(unsigned)c.ntiles, kMcThreads, 0, (cudaStream_t)stream>>>(
       make_vol(vol, nx, ny, nz, iso), c.vpack, c.tloc, c.tiles, verts, faces);

@@ -297,56 +297,49 @@ struct Carve {
   int64_t *keys_out, *idx_out;
 };
 
-// layout: counts (n_active), sort buffers (max_verts), then scratch; classification uses flags + scratch
+// layout: counts (n_active), sort buffers (max_verts), then scratch; classification's flags share offset 0 with the
+// counts, and the scratch starts after the larger of the two
 size_t carve(int32_t res, long long n_active, long long max_verts, void* ws, Carve* c) {
   const long long nb = res / kB, nblocks = nb * nb * nb;
-  // cub sizes its scratch for the current device; without one the queries fail and so does this (0)
-  size_t scan_cls = 0, scan_v = 0, scan_s = 0, sort = 0;
-  bool ok = cub::DeviceScan::ExclusiveSum(nullptr, scan_cls, (const int*)nullptr, (int*)nullptr, (int)nblocks) ==
-            cudaSuccess;
+  CubScratch tmp;
+  tmp.add([&](size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(nullptr, b, (const int*)nullptr, (int*)nullptr, (int)nblocks);
+  });
   if (n_active > 0) {
-    ok = ok && cub::DeviceScan::ExclusiveSum(nullptr, scan_v, (const int64_t*)nullptr, (int64_t*)nullptr,
-                                             (int)n_active) == cudaSuccess;
-    ok = ok && cub::DeviceScan::ExclusiveSum(nullptr, scan_s, (const int64_t*)nullptr, (int64_t*)nullptr,
-                                             (int)(kSegs * n_active)) == cudaSuccess;
+    tmp.add([&](size_t& b) {
+      return cub::DeviceScan::ExclusiveSum(nullptr, b, (const int64_t*)nullptr, (int64_t*)nullptr, (int)n_active);
+    });
+    tmp.add([&](size_t& b) {
+      return cub::DeviceScan::ExclusiveSum(nullptr, b, (const int64_t*)nullptr, (int64_t*)nullptr,
+                                           (int)(kSegs * n_active));
+    });
   }
   if (max_verts > 0)
-    ok = ok && cub::DeviceRadixSort::SortPairs(nullptr, sort, (const int64_t*)nullptr, (int64_t*)nullptr,
-                                               (const int64_t*)nullptr, (int64_t*)nullptr, (int)max_verts, 0,
-                                               key_bits(res)) == cudaSuccess;
-  if (!ok) {
-    cudaGetLastError();
-    return 0;
-  }
-  char* base = (char*)ws;
-  size_t o = 0;
-  auto take = [&](size_t bytes) {
-    char* p = base ? base + o : nullptr;
-    o += align_up(bytes, 256);
-    return p;
-  };
+    tmp.add([&](size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(nullptr, b, (const int64_t*)nullptr, (int64_t*)nullptr,
+                                             (const int64_t*)nullptr, (int64_t*)nullptr, (int)max_verts, 0,
+                                             key_bits(res));
+    });
+  if (!tmp.ok) return 0;
   Carve k{};
-  k.flag = (int*)take(4 * (size_t)nblocks);
-  const size_t cls_end = o;
-  o = 0;
-  k.C.vcnt = (int64_t*)take(8 * (size_t)n_active);
-  k.C.voff = (int64_t*)take(8 * (size_t)n_active);
-  k.C.scnt = (int64_t*)take(8 * (size_t)kSegs * n_active);
-  k.C.soff = (int64_t*)take(8 * (size_t)kSegs * n_active);
-  k.C.totals = (int64_t*)take(16);
-  k.E.keys = (int64_t*)take(8 * (size_t)max_verts);
-  k.keys_out = (int64_t*)take(8 * (size_t)max_verts);
-  k.E.idx = (int64_t*)take(8 * (size_t)max_verts);
-  k.idx_out = (int64_t*)take(8 * (size_t)max_verts);
-  k.E.pos = (float*)take(12 * (size_t)max_verts);
+  WsCarver cls(ws), w(ws);
+  k.flag = cls.take<int>(nblocks);
+  k.C.vcnt = w.take<int64_t>(n_active);
+  k.C.voff = w.take<int64_t>(n_active);
+  k.C.scnt = w.take<int64_t>(kSegs * n_active);
+  k.C.soff = w.take<int64_t>(kSegs * n_active);
+  k.C.totals = w.take<int64_t>(2);
+  k.E.keys = w.take<int64_t>(max_verts);
+  k.keys_out = w.take<int64_t>(max_verts);
+  k.E.idx = w.take<int64_t>(max_verts);
+  k.idx_out = w.take<int64_t>(max_verts);
+  k.E.pos = w.take<float>(3 * max_verts);
   k.E.max_verts = max_verts;
-  o = o > cls_end ? o : cls_end;
-  k.tmp_bytes = scan_cls > scan_v ? scan_cls : scan_v;
-  k.tmp_bytes = k.tmp_bytes > scan_s ? k.tmp_bytes : scan_s;
-  k.tmp_bytes = k.tmp_bytes > sort ? k.tmp_bytes : sort;
-  k.tmp = take(k.tmp_bytes);
+  w.end = w.end > cls.end ? w.end : cls.end;
+  k.tmp_bytes = tmp.bytes;
+  k.tmp = w.take<char>(tmp.bytes);
   if (c) *c = k;
-  return o;
+  return w.end;
 }
 
 // every scanned or sorted length fits cub's int item count
@@ -355,18 +348,6 @@ bool sizes_ok(int32_t res, int64_t n_active, int64_t max_verts) {
   const long long nb = res / kB;
   return n_active >= 0 && n_active <= nb * nb * nb && kSegs * n_active < (1ll << 31) && max_verts >= 0 &&
          max_verts < (1ll << 31);
-}
-
-unsigned grid_of(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
-
-int need_ws(const char* what, size_t have, size_t need) {
-  if (need == 0) {
-    set_error("%s: no current CUDA device to size the scan / sort scratch for", what);
-    return SPARF_ERR_CUDA;
-  }
-  if (have >= need) return SPARF_OK;
-  set_error("%s: workspace %zu B < %zu B", what, have, need);
-  return SPARF_ERR_WORKSPACE;
 }
 
 // count and emit share this: the per-block pass and the two scans
@@ -397,7 +378,7 @@ extern "C" int sparf_mcubes_sparse_classify(const float* coarse, int32_t res, fl
   SPARF_REQUIRE(res_ok(res), "mcubes_sparse_classify: res %d (a multiple of %d in [%d, %d])", res, kB, kB, kMaxRes);
   SPARF_REQUIRE(coarse && slots && n_active && workspace, "mcubes_sparse_classify: NULL pointer");
   Carve c;
-  SPARF_TRY(need_ws("mcubes_sparse_classify", workspace_bytes, carve(res, 0, 0, workspace, &c)));
+  SPARF_TRY(check_workspace("mcubes_sparse_classify", workspace, workspace_bytes, carve(res, 0, 0, workspace, &c)));
   cudaStream_t s = (cudaStream_t)stream;
   const int nb = res / kB;
   const long long nblocks = (long long)nb * nb * nb;
@@ -445,7 +426,7 @@ extern "C" int sparf_mcubes_sparse_count(const float* sigma_blocks, int32_t res,
   }
   SPARF_REQUIRE(sigma_blocks && slots && block_ids, "mcubes_sparse_count: NULL pointer");
   Carve c;
-  SPARF_TRY(need_ws("mcubes_sparse_count", workspace_bytes, carve(res, n_active, 0, workspace, &c)));
+  SPARF_TRY(check_workspace("mcubes_sparse_count", workspace, workspace_bytes, carve(res, n_active, 0, workspace, &c)));
   const Sparse S{sigma_blocks, slots, block_ids, n_active, res / kB, res + 1, iso};
   c.C.totals = totals;
   return count_pass(S, c, s);
@@ -464,7 +445,8 @@ extern "C" int sparf_mcubes_sparse_emit(const float* sigma_blocks, int32_t res, 
   SPARF_REQUIRE(sigma_blocks && slots && block_ids && workspace && (verts || !max_verts) && (faces || !max_faces),
                 "mcubes_sparse_emit: NULL pointer");
   Carve c;
-  SPARF_TRY(need_ws("mcubes_sparse_emit", workspace_bytes, carve(res, n_active, max_verts, workspace, &c)));
+  SPARF_TRY(check_workspace("mcubes_sparse_emit", workspace, workspace_bytes,
+                            carve(res, n_active, max_verts, workspace, &c)));
   cudaStream_t s = (cudaStream_t)stream;
   const Sparse S{sigma_blocks, slots, block_ids, n_active, res / kB, res + 1, iso};
   SPARF_TRY(count_pass(S, c, s));

@@ -54,8 +54,6 @@ __device__ __forceinline__ void unite(int* parent, int a, int b) {
 
 __device__ __forceinline__ bool id_ok(long long x, long long n) { return x >= 0 && x < n; }
 
-__device__ __forceinline__ long long thread_index() { return (long long)blockIdx.x * blockDim.x + threadIdx.x; }
-
 __global__ void __launch_bounds__(kCcThreads) cc_init_kernel(int n_verts, int* __restrict__ parent) {
   const long long v = thread_index();
   if (v < n_verts) parent[v] = (int)v;
@@ -172,36 +170,16 @@ struct Carve {
 };
 
 size_t carve(int64_t n_verts, int64_t n_faces, void* ws, Carve* c) {
-  // cub sizes its scratch for the current device; without one the queries fail and so does this (0)
-  size_t tv = 0, tf = 0;
-  bool ok = true;
-  if (n_verts > 0) ok = cub::DeviceScan::ExclusiveSum(nullptr, tv, (int*)nullptr, (int)n_verts) == cudaSuccess;
-  if (n_faces > 0) ok = ok && cub::DeviceScan::ExclusiveSum(nullptr, tf, (int*)nullptr, (int)n_faces) == cudaSuccess;
-  if (!ok) {
-    cudaGetLastError();
-    return 0;
-  }
-  char* b = (char*)ws;
-  const size_t av = align_up(4 * (size_t)n_verts, 256), af = align_up(4 * (size_t)n_faces, 256);
-  const size_t tmp = tv > tf ? tv : tf;
-  if (c) *c = Carve{(int*)b, (int*)(b + av), b + av + af, tmp};
-  return av + af + (tmp > 0 ? tmp : 1);
-}
-
-unsigned grid_of(long long n) { return (unsigned)((n + kCcThreads - 1) / kCcThreads); }
-
-int check_ws(const char* what, int64_t n_verts, int64_t n_faces, void* ws, size_t ws_bytes, Carve* c) {
-  SPARF_REQUIRE(ws, "%s: NULL workspace", what);
-  const size_t need = carve(n_verts, n_faces, ws, c);
-  if (need == 0) {
-    set_error("%s: no current CUDA device to size the scan scratch for", what);
-    return SPARF_ERR_CUDA;
-  }
-  if (ws_bytes < need) {
-    set_error("%s: workspace %zu B < %zu B", what, ws_bytes, need);
-    return SPARF_ERR_WORKSPACE;
-  }
-  return SPARF_OK;
+  CubScratch tmp;
+  if (n_verts > 0)
+    tmp.add([&](size_t& b) { return cub::DeviceScan::ExclusiveSum(nullptr, b, (int*)nullptr, (int)n_verts); });
+  if (n_faces > 0)
+    tmp.add([&](size_t& b) { return cub::DeviceScan::ExclusiveSum(nullptr, b, (int*)nullptr, (int)n_faces); });
+  if (!tmp.ok) return 0;
+  WsCarver w(ws);
+  const Carve k{w.take<int>(n_verts), w.take<int>(n_faces), w.take<char>(tmp.bytes > 0 ? tmp.bytes : 1), tmp.bytes};
+  if (c) *c = k;
+  return w.end;
 }
 
 #define SPARF_CC_REQUIRE_SIZES(what, V, F)                                                                        \
@@ -228,19 +206,19 @@ extern "C" int sparf_mesh_components(const int64_t* faces, int64_t n_faces, int6
     return SPARF_OK;
   }
   Carve c;
-  SPARF_TRY(check_ws("mesh_components", n_verts, n_faces, workspace, workspace_bytes, &c));
+  SPARF_TRY(check_workspace("mesh_components", workspace, workspace_bytes, carve(n_verts, n_faces, workspace, &c)));
   const int V = (int)n_verts;
-  cc_init_kernel<<<grid_of(V), kCcThreads, 0, s>>>(V, labels);
+  cc_init_kernel<<<grid_of(V, kCcThreads), kCcThreads, 0, s>>>(V, labels);
   SPARF_CHECK_LAUNCH("cc_init_kernel");
   if (n_faces > 0) {
-    cc_hook_kernel<<<grid_of(n_faces), kCcThreads, 0, s>>>(faces, n_faces, V, labels);
+    cc_hook_kernel<<<grid_of(n_faces, kCcThreads), kCcThreads, 0, s>>>(faces, n_faces, V, labels);
     SPARF_CHECK_LAUNCH("cc_hook_kernel");
   }
-  cc_compress_kernel<<<grid_of(V), kCcThreads, 0, s>>>(V, labels, c.rank);
+  cc_compress_kernel<<<grid_of(V, kCcThreads), kCcThreads, 0, s>>>(V, labels, c.rank);
   SPARF_CHECK_LAUNCH("cc_compress_kernel");
   size_t t = c.tmp_bytes;
   SPARF_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(c.tmp, t, c.rank, V, s));
-  cc_label_kernel<<<grid_of(V), kCcThreads, 0, s>>>(V, labels, c.rank, n_components);
+  cc_label_kernel<<<grid_of(V, kCcThreads), kCcThreads, 0, s>>>(V, labels, c.rank, n_components);
   SPARF_CHECK_LAUNCH("cc_label_kernel");
   return SPARF_OK;
 }
@@ -256,8 +234,9 @@ extern "C" int sparf_mesh_component_faces(const int64_t* faces, int64_t n_faces,
   cudaStream_t s = (cudaStream_t)stream;
   SPARF_CHECK_CUDA(cudaMemsetAsync(face_counts, 0, sizeof(int64_t) * (size_t)n_components, s));
   if (n_faces == 0) return SPARF_OK;
-  cc_face_count_kernel<<<grid_of(n_faces), kCcThreads, 0, s>>>(faces, n_faces, n_verts, labels, n_components,
-                                                               (unsigned long long*)face_counts);
+  cc_face_count_kernel<<<grid_of(n_faces, kCcThreads), kCcThreads, 0, s>>>(faces, n_faces, n_verts, labels,
+                                                                           n_components,
+                                                                           (unsigned long long*)face_counts);
   SPARF_CHECK_LAUNCH("cc_face_count_kernel");
   return SPARF_OK;
 }
@@ -285,9 +264,9 @@ extern "C" int sparf_mesh_select_count(const int64_t* faces, int64_t n_faces, in
     return SPARF_OK;
   }
   Carve c;
-  SPARF_TRY(check_ws("mesh_select_count", n_verts, n_faces, workspace, workspace_bytes, &c));
+  SPARF_TRY(check_workspace("mesh_select_count", workspace, workspace_bytes, carve(n_verts, n_faces, workspace, &c)));
   const Select S{faces, n_faces, n_verts, labels, keep, n_components, c.rank, c.foff};
-  select_flag_kernel<<<grid_of(n_verts > n_faces ? n_verts : n_faces), kCcThreads, 0, s>>>(S);
+  select_flag_kernel<<<grid_of(n_verts > n_faces ? n_verts : n_faces, kCcThreads), kCcThreads, 0, s>>>(S);
   SPARF_CHECK_LAUNCH("select_flag_kernel");
   size_t t = c.tmp_bytes;
   SPARF_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(c.tmp, t, c.rank, (int)n_verts, s));
@@ -306,10 +285,10 @@ extern "C" int sparf_mesh_select_emit(const int64_t* faces, int64_t n_faces, int
   SPARF_TRY(select_args("mesh_select_emit", faces, n_faces, n_verts, labels, keep, n_components));
   if (n_verts == 0) return SPARF_OK;
   Carve c;
-  SPARF_TRY(check_ws("mesh_select_emit", n_verts, n_faces, workspace, workspace_bytes, &c));
+  SPARF_TRY(check_workspace("mesh_select_emit", workspace, workspace_bytes, carve(n_verts, n_faces, workspace, &c)));
   const Select S{faces, n_faces, n_verts, labels, keep, n_components, c.rank, c.foff};
-  select_emit_kernel<<<grid_of(n_verts > n_faces ? n_verts : n_faces), kCcThreads, 0, (cudaStream_t)stream>>>(
-      S, vert_ids, faces_out);
+  select_emit_kernel<<<grid_of(n_verts > n_faces ? n_verts : n_faces, kCcThreads), kCcThreads, 0,
+                       (cudaStream_t)stream>>>(S, vert_ids, faces_out);
   SPARF_CHECK_LAUNCH("select_emit_kernel");
   return SPARF_OK;
 }

@@ -15,7 +15,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
-#include "common.cuh"
+#include "distance_grid.cuh"
 
 namespace sparf {
 namespace {
@@ -24,11 +24,6 @@ constexpr int kMdThreads = 256;
 constexpr int kQueryThreads = 128;
 constexpr long long kMaxCells = 1ll << 24;
 
-struct V3 {
-  float x, y, z;
-};
-
-__device__ __forceinline__ V3 sub(V3 a, V3 b) { return {__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y), __fsub_rn(a.z, b.z)}; }
 __device__ __forceinline__ V3 axpy(float t, V3 d, V3 a) {   // a + t d
   return {__fadd_rn(a.x, __fmul_rn(t, d.x)), __fadd_rn(a.y, __fmul_rn(t, d.y)), __fadd_rn(a.z, __fmul_rn(t, d.z))};
 }
@@ -54,7 +49,6 @@ __device__ __forceinline__ float dist2(V3 a, V3 b) {
   const V3 d = sub(a, b);
   return dot(d, d);
 }
-__device__ __forceinline__ V3 load3(const float* v, long long i) { return {v[3 * i], v[3 * i + 1], v[3 * i + 2]}; }
 
 // the closest point of the segment a -> b to p: the projection's parameter clamped to [0, 1] (0 when a = b)
 __device__ __forceinline__ V3 closest_on_segment(V3 p, V3 a, V3 b) {
@@ -92,26 +86,12 @@ __device__ __forceinline__ V3 closest_on_triangle(V3 p, V3 a, V3 b, V3 c, float*
   return q;
 }
 
-__device__ __forceinline__ bool tri_ids(const int64_t* faces, long long f, long long n_verts, long long* id) {
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    id[c] = faces[3 * f + c];
-    if (id[c] < 0 || id[c] >= n_verts) return false;
-  }
-  return true;
-}
-
 // float <-> int keys whose int order is the float order (atomicMin / atomicMax on floats; NaN is never stored)
 __device__ __forceinline__ int fkey(float f) {
   const int i = __float_as_int(f);
   return i >= 0 ? i : i ^ 0x7fffffff;
 }
 __device__ __forceinline__ float fkey_inv(int k) { return __int_as_float(k >= 0 ? k : k ^ 0x7fffffff); }
-
-__device__ __forceinline__ int cell_of(float x, float lo, float h, int n) {
-  const float t = floorf(__fdiv_rn(__fsub_rn(x, lo), h));
-  return (int)fminf(fmaxf(t, 0.f), (float)(n - 1));    // NaN -> 0
-}
 
 struct Target {
   const float* verts;
@@ -146,8 +126,6 @@ __device__ __forceinline__ long long prim_count(const Target& T, const SparfDist
   if (!prim_cells(T, g, i, lo, hi)) return 0;
   return (long long)(hi[0] - lo[0] + 1) * (hi[1] - lo[1] + 1) * (hi[2] - lo[2] + 1);
 }
-
-__device__ __forceinline__ long long thread_index() { return (long long)blockIdx.x * blockDim.x + threadIdx.x; }
 
 // box[0..2] = fkey(min), box[3..5] = fkey(max) over the finite-or-infinite (non-NaN) vertex coordinates
 __global__ void __launch_bounds__(kMdThreads) bbox_kernel(const float* __restrict__ verts, long long n_verts,
@@ -365,8 +343,6 @@ __global__ void __launch_bounds__(kMdThreads) miss_kernel(long long n, float* di
   closest[3 * i] = closest[3 * i + 1] = closest[3 * i + 2] = NAN;
 }
 
-unsigned grid_of(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
-
 // V, F in [0, INT32_MAX]; F = -1 is a point target; triangles need vertices
 bool sizes_ok(int64_t n_verts, int64_t n_faces) {
   return n_verts >= 0 && n_verts <= INT32_MAX && n_faces >= -1 && n_faces <= INT32_MAX && (n_verts > 0 || n_faces <= 0);
@@ -390,49 +366,22 @@ struct Ws {
 
 // 0 when cub cannot size its scratch (no current device)
 size_t carve(long long n_prims, long long n_entries, void* ws, Ws* out) {
-  size_t t_scan = 0, t_sort = 0;
-  bool ok = true;
+  CubScratch tmp;
   if (n_prims > 0)
-    ok = cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (long long*)nullptr, (long long*)nullptr, (int)n_prims) ==
-         cudaSuccess;
+    tmp.add([&](size_t& b) {
+      return cub::DeviceScan::ExclusiveSum(nullptr, b, (long long*)nullptr, (long long*)nullptr, (int)n_prims);
+    });
   if (n_entries > 0)
-    ok = ok && cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (int*)nullptr, (int*)nullptr, (int*)nullptr,
-                                               (int*)nullptr, (int)n_entries, 0, 24) == cudaSuccess;
-  if (!ok) {
-    cudaGetLastError();
-    return 0;
-  }
-  char* b = (char*)ws;
-  size_t o = 0;
-  auto take = [&](size_t bytes) {
-    char* p = b + o;
-    o += align_up(bytes, 256);
-    return p;
-  };
-  Ws w;
-  w.box = (int*)take(6 * sizeof(int));
-  w.offs = (long long*)take(8 * (size_t)n_prims);
-  w.keys_in = (int*)take(4 * (size_t)n_entries);
-  w.keys = (int*)take(4 * (size_t)n_entries);
-  w.ids_in = (int*)take(4 * (size_t)n_entries);
-  w.tmp_bytes = t_scan > t_sort ? t_scan : t_sort;
-  w.tmp = take(w.tmp_bytes > 0 ? w.tmp_bytes : 1);
+    tmp.add([&](size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(nullptr, b, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int*)nullptr,
+                                             (int)n_entries, 0, 24);
+    });
+  if (!tmp.ok) return 0;
+  WsCarver c(ws);
+  const Ws w{c.take<int>(6), c.take<long long>(n_prims), c.take<int>(n_entries), c.take<int>(n_entries),
+             c.take<int>(n_entries), c.take<char>(tmp.bytes > 0 ? tmp.bytes : 1), tmp.bytes};
   if (out) *out = w;
-  return o;
-}
-
-int check_ws(const char* what, long long n_prims, long long n_entries, void* ws, size_t ws_bytes, Ws* w) {
-  SPARF_REQUIRE(ws, "%s: NULL workspace", what);
-  const size_t need = carve(n_prims, n_entries, ws, w);
-  if (need == 0) {
-    set_error("%s: no current CUDA device to size the scan and sort scratch for", what);
-    return SPARF_ERR_CUDA;
-  }
-  if (ws_bytes < need) {
-    set_error("%s: workspace %zu B < %zu B", what, ws_bytes, need);
-    return SPARF_ERR_WORKSPACE;
-  }
-  return SPARF_OK;
+  return c.end;
 }
 
 // the per-primitive counts of the grid g, scanned in place into w.offs
@@ -478,7 +427,7 @@ extern "C" int sparf_distance_grid_count(const float* vertices, int64_t n_verts,
     return SPARF_OK;
   }
   Ws w;
-  SPARF_TRY(check_ws(what, P, 0, workspace, workspace_bytes, &w));
+  SPARF_TRY(check_workspace(what, workspace, workspace_bytes, carve(P, 0, workspace, &w)));
   SPARF_CHECK_CUDA(cudaMemsetAsync(w.box, 0x7f, 3 * sizeof(int), s));     // fkey(3.4e38)
   SPARF_CHECK_CUDA(cudaMemsetAsync(w.box + 3, 0x80, 3 * sizeof(int), s)); // fkey(-3.4e38)
   const unsigned nb = min(grid_of(n_verts, kMdThreads), 4u * (unsigned)num_sms());
@@ -513,7 +462,7 @@ extern "C" int sparf_distance_grid_fill(const float* vertices, int64_t n_verts, 
     return SPARF_OK;
   }
   Ws w;
-  SPARF_TRY(check_ws(what, P, n_entries, workspace, workspace_bytes, &w));
+  SPARF_TRY(check_workspace(what, workspace, workspace_bytes, carve(P, n_entries, workspace, &w)));
   const Target T{vertices, n_faces < 0 ? nullptr : faces, n_verts, P};
   if (n_entries > 0) {
     SPARF_TRY(count_and_scan(T, grid, w, s));

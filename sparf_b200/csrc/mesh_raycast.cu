@@ -10,7 +10,7 @@
 //             slab's far plane, shrunk for rounding, lies strictly beyond the best hit.  DESIGN §3.1.15 gives the
 //             argument that no grid changes the result.
 // No workspace.
-#include "common.cuh"
+#include "distance_grid.cuh"
 
 namespace sparf {
 namespace {
@@ -18,21 +18,10 @@ namespace {
 constexpr int kRcThreads = 128;
 constexpr int kMissThreads = 256;
 
-struct V3 {
-  float x, y, z;
-};
-
-__device__ __forceinline__ V3 load3(const float* v, long long i) { return {v[3 * i], v[3 * i + 1], v[3 * i + 2]}; }
 __device__ __forceinline__ float comp(V3 v, int a) { return a == 0 ? v.x : (a == 1 ? v.y : v.z); }
 // element a of a per-axis array by selects (a runtime index would put the array in local memory)
 template <typename T>
 __device__ __forceinline__ T pick(const T (&v)[3], int a) { return a == 0 ? v[0] : (a == 1 ? v[1] : v[2]); }
-
-// the same cell assignment as the grid build (mesh_distance.cu)
-__device__ __forceinline__ int cell_of(float x, float lo, float h, int n) {
-  const float t = floorf(__fdiv_rn(__fsub_rn(x, lo), h));
-  return (int)fminf(fmaxf(t, 0.f), (float)(n - 1));    // NaN -> 0
-}
 
 // the ray in the sheared frame of the watertight test
 struct Shear {
@@ -46,7 +35,7 @@ struct Sheared {
 };
 
 __device__ __forceinline__ Sheared shear(const Shear& S, V3 v) {
-  const V3 a = {__fsub_rn(v.x, S.o.x), __fsub_rn(v.y, S.o.y), __fsub_rn(v.z, S.o.z)};
+  const V3 a = sub(v, S.o);
   const float az = comp(a, S.kz);
   return {__fsub_rn(comp(a, S.kx), __fmul_rn(S.sx, az)), __fsub_rn(comp(a, S.ky), __fmul_rn(S.sy, az)), az};
 }
@@ -90,11 +79,7 @@ struct Best {
 // the hit of triangle id, if any, replaces *B when (t, id) is smaller
 __device__ __forceinline__ void test_triangle(const Cast& C, const Shear& S, int id, Best* B) {
   long long ix[3];
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    ix[c] = C.faces[3 * (long long)id + c];
-    if (ix[c] < 0 || ix[c] >= C.n_verts) return;
-  }
+  if (!tri_ids(C.faces, id, C.n_verts, ix)) return;
   const V3 a = load3(C.verts, ix[0]), b = load3(C.verts, ix[1]), c = load3(C.verts, ix[2]);
   const Sheared A = shear(S, a), Bv = shear(S, b), Cv = shear(S, c);
   float U = edge32(Cv, Bv), V = edge32(A, Cv), W = edge32(Bv, A);
@@ -221,8 +206,6 @@ __global__ void __launch_bounds__(kMissThreads) miss_kernel(long long n, float* 
   face[i] = -1;
   bary[3 * i] = bary[3 * i + 1] = bary[3 * i + 2] = NAN;
 }
-
-unsigned grid_of(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
 }  // namespace
 }  // namespace sparf

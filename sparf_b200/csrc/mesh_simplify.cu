@@ -148,9 +148,6 @@ struct Ws {
   size_t tmp_bytes;
 };
 
-__device__ __forceinline__ long long thread_index() { return (long long)blockIdx.x * blockDim.x + threadIdx.x; }
-unsigned grid_of(long long n) { return (unsigned)((n + kMsThreads - 1) / kMsThreads); }
-
 int id_bits(int64_t n_verts) {
   int nb = 1;
   while (nb < 31 && ((int64_t)1 << nb) < n_verts) ++nb;
@@ -453,12 +450,6 @@ bool sizes_ok(int64_t n_verts, int64_t n_faces, int32_t n_attrs) {
          (n_verts > 0 || n_faces == 0) && n_attrs >= 0;
 }
 
-size_t take(char** p, size_t bytes) {
-  const size_t a = align_up(bytes, 256);
-  *p += a;
-  return a;
-}
-
 // Layout (bytes): per vertex pos 12, attrs 4A, Q 80, ren 4, boundary and locked flags 2, claim 8, vstart 4 (+4);
 // per face the live faces 12 and the dead flags 1; per half-edge entry (3 per face) the two sorts' keys and values in
 // and out (8 + 8 + 4 + 4 and 4 + 4 + 4 + 4) and estart 4 (+4).  The sort inputs are dead once both sorts ran: the
@@ -467,69 +458,52 @@ size_t take(char** p, size_t bytes) {
 // largest cub scratch of the sorts and scans over 3F entries.
 size_t carve(int64_t n_verts, int64_t n_faces, int32_t n_attrs, void* ws, Ws* out) {
   const int n3 = (int)(3 * n_faces), nv = (int)n_verts;
-  size_t t_sort = 0, t_vsort = 0, t_scan = 0, t_vscan = 0;
-  bool ok = true;
+  CubScratch tmp;
   if (n3 > 0) {
-    ok = cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                         (int*)nullptr, (int*)nullptr, n3) == cudaSuccess;
-    ok = ok && cub::DeviceRadixSort::SortPairs(nullptr, t_vsort, (int*)nullptr, (int*)nullptr, (int*)nullptr,
-                                               (int*)nullptr, n3) == cudaSuccess;
-    ok = ok && cub::DeviceScan::InclusiveSum(nullptr, t_scan, (int*)nullptr, n3) == cudaSuccess;
+    tmp.add([&](size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(nullptr, b, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                             (int*)nullptr, (int*)nullptr, n3);
+    });
+    tmp.add([&](size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(nullptr, b, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int*)nullptr,
+                                             n3);
+    });
+    tmp.add([&](size_t& b) { return cub::DeviceScan::InclusiveSum(nullptr, b, (int*)nullptr, n3); });
   }
-  if (nv > 0) ok = ok && cub::DeviceScan::ExclusiveSum(nullptr, t_vscan, (int*)nullptr, nv) == cudaSuccess;
-  if (!ok) {
-    cudaGetLastError();
-    return 0;
-  }
-  size_t tmp = t_sort;
-  for (size_t t : {t_vsort, t_scan, t_vscan}) tmp = t > tmp ? t : tmp;
-  char* base = (char*)ws;
-  char* p = base;
+  if (nv > 0) tmp.add([&](size_t& b) { return cub::DeviceScan::ExclusiveSum(nullptr, b, (int*)nullptr, nv); });
+  if (!tmp.ok) return 0;
   const size_t V = (size_t)n_verts, F = (size_t)n_faces, H = 3 * F;
+  WsCarver c(ws);
   Ws w;
-  w.pos = (float*)p;                 take(&p, 12 * V);
-  w.attrs = (float*)p;               take(&p, 4 * (size_t)n_attrs * V);
-  w.q = (double*)p;                  take(&p, 80 * V);
-  w.ren = (int*)p;                   take(&p, 4 * V);
-  w.bnd = (uint8_t*)p;               take(&p, V);
-  w.lock = (uint8_t*)p;              take(&p, V);
-  w.claim = (unsigned long long*)p;  take(&p, 8 * V);
-  w.vstart = (int*)p;                take(&p, 4 * (V + 1));
-  w.faces = (int*)p;                 take(&p, 12 * F);
-  w.dead = (uint8_t*)p;              take(&p, F);
-  w.ekeys_in = (unsigned long long*)p;  take(&p, 8 * H);
-  w.ekeys = (unsigned long long*)p;     take(&p, 8 * H);
-  w.evals_in = (int*)p;              take(&p, 4 * H);
-  w.evals = (int*)p;                 take(&p, 4 * H);
-  w.vkeys_in = (int*)p;              take(&p, 4 * (H > V ? H : V));   // faces_tmp / vertex offsets
-  w.vkeys = (int*)p;                 take(&p, 4 * H);
-  w.vvals_in = (int*)p;              take(&p, 4 * (H > V ? H : V));   // face / vertex offsets
-  w.vvals = (int*)p;                 take(&p, 4 * H);
-  w.estart = (int*)p;                take(&p, 4 * (H + 1));
-  w.sel = (unsigned long long*)p;    take(&p, 8 * 5);
-  w.hist = (unsigned*)p;             take(&p, 4 * 256);
-  w.tmp = p;
-  w.tmp_bytes = tmp;
+  w.pos = c.take<float>(3 * V);
+  w.attrs = c.take<float>((size_t)n_attrs * V);
+  w.q = c.take<double>(10 * V);
+  w.ren = c.take<int>(V);
+  w.bnd = c.take<uint8_t>(V);
+  w.lock = c.take<uint8_t>(V);
+  w.claim = c.take<unsigned long long>(V);
+  w.vstart = c.take<int>(V + 1);
+  w.faces = c.take<int>(3 * F);
+  w.dead = c.take<uint8_t>(F);
+  w.ekeys_in = c.take<unsigned long long>(H);
+  w.ekeys = c.take<unsigned long long>(H);
+  w.evals_in = c.take<int>(H);
+  w.evals = c.take<int>(H);
+  w.vkeys_in = c.take<int>(H > V ? H : V);   // faces_tmp / vertex offsets
+  w.vkeys = c.take<int>(H);
+  w.vvals_in = c.take<int>(H > V ? H : V);   // face / vertex offsets
+  w.vvals = c.take<int>(H);
+  w.estart = c.take<int>(H + 1);
+  w.sel = c.take<unsigned long long>(5);
+  w.hist = c.take<unsigned>(256);
+  w.tmp = c.take<char>(tmp.bytes > 0 ? tmp.bytes : 1);
+  w.tmp_bytes = tmp.bytes;
   w.ckey = w.ekeys_in;
   w.eid = w.evals_in;
   w.faces_tmp = w.vkeys_in;
   w.foff = w.vvals_in;
   if (out) *out = w;
-  return (size_t)(p - base) + (tmp > 0 ? tmp : 1);
-}
-
-int check_ws(const char* what, int64_t n_verts, int64_t n_faces, int32_t n_attrs, void* ws, size_t ws_bytes, Ws* w) {
-  SPARF_REQUIRE(ws, "%s: NULL workspace", what);
-  const size_t need = carve(n_verts, n_faces, n_attrs, ws, w);
-  if (need == 0) {
-    set_error("%s: no current CUDA device to size the sort and scan scratch for", what);
-    return SPARF_ERR_CUDA;
-  }
-  if (ws_bytes < need) {
-    set_error("%s: workspace %zu B < %zu B", what, ws_bytes, need);
-    return SPARF_ERR_WORKSPACE;
-  }
-  return SPARF_OK;
+  return c.end;
 }
 
 // the vertex CSR of the live faces (sorted vertex entries, vstart); build must have run
@@ -537,7 +511,7 @@ int vertex_csr(Ws& w, int n_live, int n_verts, int nb, cudaStream_t s) {
   size_t t = w.tmp_bytes;
   SPARF_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(w.tmp, t, w.vkeys_in, w.vkeys, w.vvals_in, w.vvals, 3 * n_live, 0,
                                                    nb, s));
-  ms_vstart_kernel<<<grid_of(n_verts + 1), kMsThreads, 0, s>>>(n_verts, 3 * n_live, w);
+  ms_vstart_kernel<<<grid_of(n_verts + 1, kMsThreads), kMsThreads, 0, s>>>(n_verts, 3 * n_live, w);
   SPARF_CHECK_LAUNCH("ms_vstart_kernel");
   return SPARF_OK;
 }
@@ -568,22 +542,23 @@ extern "C" int sparf_mesh_simplify_init(const float* vertices, const int64_t* fa
     return SPARF_OK;
   }
   Ws w;
-  SPARF_TRY(check_ws("mesh_simplify_init", n_verts, n_faces, n_attrs, workspace, workspace_bytes, &w));
+  SPARF_TRY(check_workspace("mesh_simplify_init", workspace, workspace_bytes,
+                            carve(n_verts, n_faces, n_attrs, workspace, &w)));
   const int V = (int)n_verts, F = (int)n_faces;
   SPARF_CHECK_CUDA(cudaMemcpyAsync(w.pos, vertices, 12 * (size_t)V, cudaMemcpyDeviceToDevice, s));
   if (n_attrs > 0)
     SPARF_CHECK_CUDA(cudaMemcpyAsync(w.attrs, attrs, 4 * (size_t)n_attrs * V, cudaMemcpyDeviceToDevice, s));
-  ms_init_kernel<<<grid_of(3ll * F > V ? 3ll * F : V), kMsThreads, 0, s>>>(faces, F, V, w, counts);
+  ms_init_kernel<<<grid_of(3ll * F > V ? 3ll * F : V, kMsThreads), kMsThreads, 0, s>>>(faces, F, V, w, counts);
   SPARF_CHECK_LAUNCH("ms_init_kernel");
   const int nb = id_bits(V);
   if (F > 0) {
-    ms_build_kernel<<<grid_of(F), kMsThreads, 0, s>>>(F, nb, w);
+    ms_build_kernel<<<grid_of(F, kMsThreads), kMsThreads, 0, s>>>(F, nb, w);
     SPARF_CHECK_LAUNCH("ms_build_kernel");
     SPARF_TRY(vertex_csr(w, F, V, nb, s));
   } else {
     SPARF_CHECK_CUDA(cudaMemsetAsync(w.vstart, 0, 4 * ((size_t)V + 1), s));
   }
-  ms_quadric_kernel<<<grid_of(V), kMsThreads, 0, s>>>(V, w);
+  ms_quadric_kernel<<<grid_of(V, kMsThreads), kMsThreads, 0, s>>>(V, w);
   SPARF_CHECK_LAUNCH("ms_quadric_kernel");
   return SPARF_OK;
 }
@@ -601,7 +576,8 @@ extern "C" int sparf_mesh_simplify_round(int64_t n_verts, int64_t n_faces, int32
     return SPARF_OK;
   }
   Ws w;
-  SPARF_TRY(check_ws("mesh_simplify_round", n_verts, n_faces, n_attrs, workspace, workspace_bytes, &w));
+  SPARF_TRY(check_workspace("mesh_simplify_round", workspace, workspace_bytes,
+                            carve(n_verts, n_faces, n_attrs, workspace, &w)));
   const int V = (int)n_verts, n = (int)n_live, H = 3 * n, nb = id_bits(V);
   SPARF_CHECK_CUDA(cudaMemsetAsync(w.bnd, 0, (size_t)V, s));
   SPARF_CHECK_CUDA(cudaMemsetAsync(w.lock, 0, (size_t)V, s));
@@ -609,38 +585,38 @@ extern "C" int sparf_mesh_simplify_round(int64_t n_verts, int64_t n_faces, int32
   SPARF_CHECK_CUDA(cudaMemsetAsync(w.dead, 0, (size_t)n, s));
   ms_round_begin_kernel<<<1, 1, 0, s>>>(w, k, counts);
   SPARF_CHECK_LAUNCH("ms_round_begin_kernel");
-  ms_build_kernel<<<grid_of(n), kMsThreads, 0, s>>>(n, nb, w);
+  ms_build_kernel<<<grid_of(n, kMsThreads), kMsThreads, 0, s>>>(n, nb, w);
   SPARF_CHECK_LAUNCH("ms_build_kernel");
   size_t t = w.tmp_bytes;
   SPARF_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(w.tmp, t, w.ekeys_in, w.ekeys, w.evals_in, w.evals, H, 0, 2 * nb, s));
   SPARF_TRY(vertex_csr(w, n, V, nb, s));
-  ms_head_kernel<<<grid_of(H), kMsThreads, 0, s>>>(H, w);
+  ms_head_kernel<<<grid_of(H, kMsThreads), kMsThreads, 0, s>>>(H, w);
   SPARF_CHECK_LAUNCH("ms_head_kernel");
   t = w.tmp_bytes;
   SPARF_CHECK_CUDA(cub::DeviceScan::InclusiveSum(w.tmp, t, w.eid, w.eid, H, s));
-  ms_edge_start_kernel<<<grid_of(H), kMsThreads, 0, s>>>(H, w);
+  ms_edge_start_kernel<<<grid_of(H, kMsThreads), kMsThreads, 0, s>>>(H, w);
   SPARF_CHECK_LAUNCH("ms_edge_start_kernel");
   // the kernels over edges run over H >= E threads and read E on the device
-  ms_classify_kernel<<<grid_of(H), kMsThreads, 0, s>>>(nb, w);
+  ms_classify_kernel<<<grid_of(H, kMsThreads), kMsThreads, 0, s>>>(nb, w);
   SPARF_CHECK_LAUNCH("ms_classify_kernel");
-  ms_key_kernel<<<grid_of(H), kMsThreads, 0, s>>>(nb, w);
+  ms_key_kernel<<<grid_of(H, kMsThreads), kMsThreads, 0, s>>>(nb, w);
   SPARF_CHECK_LAUNCH("ms_key_kernel");
-  const unsigned hist_grid = grid_of(H) < 1024 ? grid_of(H) : 1024;
+  const unsigned hist_grid = min(grid_of(H, kMsThreads), 1024u);
   for (int pass = 0; pass < 8; ++pass) {
     ms_hist_kernel<<<hist_grid, kMsThreads, 0, s>>>(pass, w);
     SPARF_CHECK_LAUNCH("ms_hist_kernel");
     ms_pick_kernel<<<1, 1, 0, s>>>(pass, w);
     SPARF_CHECK_LAUNCH("ms_pick_kernel");
   }
-  ms_claim_kernel<<<grid_of(H), kMsThreads, 0, s>>>(nb, w);
+  ms_claim_kernel<<<grid_of(H, kMsThreads), kMsThreads, 0, s>>>(nb, w);
   SPARF_CHECK_LAUNCH("ms_claim_kernel");
-  ms_win_kernel<<<grid_of(H), kMsThreads, 0, s>>>(nb, n_attrs, w, counts);
+  ms_win_kernel<<<grid_of(H, kMsThreads), kMsThreads, 0, s>>>(nb, n_attrs, w, counts);
   SPARF_CHECK_LAUNCH("ms_win_kernel");
-  ms_face_flag_kernel<<<grid_of(n), kMsThreads, 0, s>>>(n, w);
+  ms_face_flag_kernel<<<grid_of(n, kMsThreads), kMsThreads, 0, s>>>(n, w);
   SPARF_CHECK_LAUNCH("ms_face_flag_kernel");
   t = w.tmp_bytes;
   SPARF_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(w.tmp, t, w.foff, w.foff, n, s));
-  ms_face_emit_kernel<<<grid_of(n), kMsThreads, 0, s>>>(n, w, counts);
+  ms_face_emit_kernel<<<grid_of(n, kMsThreads), kMsThreads, 0, s>>>(n, w, counts);
   SPARF_CHECK_LAUNCH("ms_face_emit_kernel");
   SPARF_CHECK_CUDA(cudaMemcpyAsync(w.faces, w.faces_tmp, 12 * (size_t)n, cudaMemcpyDeviceToDevice, s));
   return SPARF_OK;
@@ -656,14 +632,16 @@ extern "C" int sparf_mesh_simplify_emit(int64_t n_verts, int64_t n_faces, int32_
                 "mesh_simplify_emit: NULL pointer");
   if (n_verts == 0) return SPARF_OK;
   Ws w;
-  SPARF_TRY(check_ws("mesh_simplify_emit", n_verts, n_faces, n_attrs, workspace, workspace_bytes, &w));
+  SPARF_TRY(check_workspace("mesh_simplify_emit", workspace, workspace_bytes,
+                            carve(n_verts, n_faces, n_attrs, workspace, &w)));
   cudaStream_t s = (cudaStream_t)stream;
   const int V = (int)n_verts, n = (int)n_live;
-  ms_vert_flag_kernel<<<grid_of(V), kMsThreads, 0, s>>>(V, w);
+  ms_vert_flag_kernel<<<grid_of(V, kMsThreads), kMsThreads, 0, s>>>(V, w);
   SPARF_CHECK_LAUNCH("ms_vert_flag_kernel");
   size_t t = w.tmp_bytes;
   SPARF_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(w.tmp, t, w.foff, w.foff, V, s));
-  ms_emit_kernel<<<grid_of(V > n ? V : n), kMsThreads, 0, s>>>(V, n, n_attrs, w, vertices, attrs, vert_ids, faces);
+  ms_emit_kernel<<<grid_of(V > n ? V : n, kMsThreads), kMsThreads, 0, s>>>(V, n, n_attrs, w, vertices, attrs, vert_ids,
+                                                                         faces);
   SPARF_CHECK_LAUNCH("ms_emit_kernel");
   return SPARF_OK;
 }

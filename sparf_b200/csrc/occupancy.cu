@@ -112,11 +112,7 @@ extern "C" int sparf_occupancy_count(int64_t R, int32_t S, const float* origins,
     return SPARF_OK;
   }
   Carve c;
-  const size_t need = carve(R, S, workspace, &c);
-  if (workspace_bytes < need) {
-    set_error("occupancy_count: workspace %zu B < %zu B", workspace_bytes, need);
-    return SPARF_ERR_WORKSPACE;
-  }
+  SPARF_TRY(check_workspace("occupancy_count", workspace, workspace_bytes, carve(R, S, workspace, &c)));
   SPARF_REQUIRE(c.ntiles < (1ll << 31), "occupancy_count: too many samples");
   const Lookup Q = make_lookup(R, S, origins, dirs, t, bits, res, r0, r1);
   occupancy_count_kernel<<<(unsigned)c.ntiles, kOcThreads, 0, s>>>(Q, c.local, c.tiles);
@@ -136,11 +132,7 @@ extern "C" int sparf_occupancy_emit(int64_t R, int32_t S, const float* origins, 
   if (R == 0) return SPARF_OK;
   SPARF_REQUIRE(origins && dirs && t && bits && workspace, "occupancy_emit: NULL pointer");
   Carve c;
-  const size_t need = carve(R, S, workspace, &c);
-  if (workspace_bytes < need) {
-    set_error("occupancy_emit: workspace %zu B < %zu B", workspace_bytes, need);
-    return SPARF_ERR_WORKSPACE;
-  }
+  SPARF_TRY(check_workspace("occupancy_emit", workspace, workspace_bytes, carve(R, S, workspace, &c)));
   SPARF_REQUIRE(c.ntiles < (1ll << 31), "occupancy_emit: too many samples");
   occupancy_emit_kernel<<<(unsigned)c.ntiles, kOcThreads, 0, (cudaStream_t)stream>>>(
       make_lookup(R, S, origins, dirs, t, bits, res, r0, r1), c.local, c.tiles, sample_idx, origins_k, dirs_k, t_k);

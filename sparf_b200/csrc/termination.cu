@@ -125,11 +125,7 @@ static int window_setup(const char* name, int64_t R, int32_t S, int32_t k0, int3
   SPARF_TRY(grid_ok());
   if (R == 0) return SPARF_OK;
   SPARF_REQUIRE(origins && dirs && t && workspace, "%s: NULL pointer", name);
-  const size_t need = carve(R, k1 - k0, workspace, c);
-  if (workspace_bytes < need) {
-    set_error("%s: workspace %zu B < %zu B", name, workspace_bytes, need);
-    return SPARF_ERR_WORKSPACE;
-  }
+  SPARF_TRY(check_workspace(name, workspace, workspace_bytes, carve(R, k1 - k0, workspace, c)));
   SPARF_REQUIRE(c->ntiles < (1ll << 31), "%s: too many samples", name);
   wn->alive = alive;
   wn->n = (long long)R * (k1 - k0);
