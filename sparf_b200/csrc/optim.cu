@@ -132,6 +132,12 @@ extern "C" int sparf_adam_step(int64_t n, float* param, float* grad, float* exp_
 // ray; along a ray the mid-points u are monotone, so the pair sum collapses to prefix sums:
 //   sum_ij a_i a_j |u_i - u_j| = 2 sum_i a_i (u_i A_i - M_i),  A_i = sum_{j<i} a_j,  M_i = sum_{j<i} a_j u_j
 // with a_i = w_{i+1}, u_i = (t_{i+1} + t_i) / 2, i = 0..S-2; plus sum_i a_i^2 (t_{i+1} - t_i) / 3.
+// The terms u_i A_i and M_i cancel when the weight mass sits far from u = 0 compared with its spread (a far scene, or
+// fine samples clustered at a surface): in fp32 that costs up to 10-50x the literal form's error
+// (tests/test_distortion_fp64.py).  The pair term is invariant under u -> u - c, so every pass after the first works on
+// mid-points centred at the ray's weighted mean c = sum a u / sum a (u_0 when sum a = 0), formed as
+// ((t_{i+1} - c) + (t_i - c)) / 2 so the shift is exact for t near c.  c is a constant of the formula, not a function
+// of the inputs: d_w and d_t are those of the uncentred sums.
 // One warp per ray, shuffle scans (like compositing).  loss += scale * mean over rays; d_w, d_t are written.
 // ------------------------------------------------------------------------------------------------
 namespace sparf {
@@ -160,12 +166,24 @@ __global__ void __launch_bounds__(128) distortion_kernel(int R, int S, const flo
   const int n = S - 1;
   // orientation: inverse-depth samples decrease along the ray; the pair term only needs monotone mid-points
   const float sgn = tr[S - 1] >= tr[0] ? 1.f : -1.f;
-  // pass 1: totals (for the suffix sums) and the loss
+  // pass 0: the centre c (in t, unoriented)
   float A_tot = 0.f, M_tot = 0.f;
   for (int i0 = 0; i0 < n; i0 += 32) {
     const int i = i0 + lane;
     const float a = i < n ? wr[i + 1] : 0.f;
-    const float u = i < n ? sgn * 0.5f * (tr[i + 1] + tr[i]) : 0.f;
+    const float m = i < n ? 0.5f * (tr[i + 1] + tr[i]) : 0.f;
+    float sa = a, sm = a * m;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { sa += __shfl_xor_sync(0xffffffffu, sa, o); sm += __shfl_xor_sync(0xffffffffu, sm, o); }
+    A_tot += sa; M_tot += sm;
+  }
+  const float c = A_tot > 0.f ? M_tot / A_tot : 0.5f * (tr[1] + tr[0]);
+  // pass 1: totals (for the suffix sums) and the loss
+  A_tot = 0.f; M_tot = 0.f;
+  for (int i0 = 0; i0 < n; i0 += 32) {
+    const int i = i0 + lane;
+    const float a = i < n ? wr[i + 1] : 0.f;
+    const float u = i < n ? sgn * 0.5f * ((tr[i + 1] - c) + (tr[i] - c)) : 0.f;
     float sa = a, sm = a * u;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) { sa += __shfl_xor_sync(0xffffffffu, sa, o); sm += __shfl_xor_sync(0xffffffffu, sm, o); }
@@ -178,7 +196,7 @@ __global__ void __launch_bounds__(128) distortion_kernel(int R, int S, const flo
     const bool ok = i < n;
     const float a = ok ? wr[i + 1] : 0.f;
     const float t0 = ok ? tr[i] : 0.f, t1 = ok ? tr[i + 1] : 0.f;
-    const float u = sgn * 0.5f * (t1 + t0), dt = t1 - t0;
+    const float u = sgn * 0.5f * ((t1 - c) + (t0 - c)), dt = t1 - t0;
     float ta, tm;
     const float A = A_run + warp_excl_scan(a, lane, ta);
     const float M = M_run + warp_excl_scan(a * u, lane, tm);
