@@ -17,11 +17,11 @@
 //     gradients are never packed from fp32;
 //   staged weight-gradient gemm: the same walk, ring and MMAs, with B read as fp32 rows by bulk copies and split in
 //     shared memory by a fourth (converter) warpgroup, so the weight gradient's activation operand is never packed.
-//   trunk chain: the trunk forward at width 256 in one persistent kernel.  A tile of 64 rows goes through every layer
-//     with its activations in shared memory (each layer's epilogue splits its output over its input), the two consumer
-//     warpgroups splitting N; only the weights stream through the ring, and global memory gets the fp32 activations
-//     that are asked for and the last layer's row image.  Same MMA order and epilogue arithmetic per output element as
-//     the gemm, so the same bytes.
+//   trunk chain: the trunk forward at width 256 in one persistent kernel.  A tile of 128 rows goes through every layer
+//     with its activations in shared memory (each layer's epilogue splits its output over its input), each consumer
+//     warpgroup on its own 64 rows, a quarter of the columns at a time; only the weights stream through the ring, one
+//     stage feeding both warpgroups, and global memory gets the fp32 activations that are asked for and the last
+//     layer's row image.  Same MMA order and epilogue arithmetic per output element as the gemm, so the same bytes.
 #include <cuda_bf16.h>
 #include <cudaTypedefs.h>
 #include <cuda_fp16.h>
@@ -77,6 +77,30 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, ui
     asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
                  "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " SPARF_WG_REGS ", %64, %65, p, 1, 1, 0, 0;\n}\n"
                  : SPARF_WG_D64
+                 : "l"(da), "l"(db), "r"(1));
+  }
+}
+
+#define SPARF_WG_D32                                                                                                        \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),   \
+      "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),  \
+      "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),  \
+      "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+#define SPARF_WG_REGS32                                                                                                     \
+  "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}"
+
+// D[64 x 64] += A[64 x 16] B[64 x 16]^T, both K-major in shared memory (the fused trunk chains' column quarters)
+template <bool F16>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db) {
+  if constexpr (F16) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " SPARF_WG_REGS32 ", %32, %33, p, 1, 1, 0, 0;\n}\n"
+                 : SPARF_WG_D32
+                 : "l"(da), "l"(db), "r"(1));
+  } else {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " SPARF_WG_REGS32 ", %32, %33, p, 1, 1, 0, 0;\n}\n"
+                 : SPARF_WG_D32
                  : "l"(da), "l"(db), "r"(1));
   }
 }
@@ -177,7 +201,9 @@ struct TnB {
 // contiguous dimension (KFAST); the split tile is assembled in shared memory and leaves in 16-byte vectors.
 // DYN (Rows only): f.M is a capacity, of which live_rows rows are packed; row tiles past them are not written.  f.X's
 // rows start at row_start (the span forward's global rows); the image's at 0.
-template <bool F16, int PASSES, bool KFAST, class F, bool DYN = false>
+// QUARTERS (the fused trunk chains' weight images): the image is laid out per 64-row quarter instead, 4 KB [64 x 32]
+// blocks at ((quarter * ksteps + kt) * PASSES' halves + half) * 2048 elements, so that a quarter's k-steps are contiguous.
+template <bool F16, int PASSES, bool KFAST, class F, bool DYN = false, bool QUARTERS = false>
 __global__ void __launch_bounds__(256) pack_kernel(F f, int ksteps, uint16_t* __restrict__ img, RowCount rc) {
   __shared__ __align__(16) uint16_t t[2 * TILE_ELEMS];
   const int kt = blockIdx.x, rt = blockIdx.y;
@@ -219,11 +245,22 @@ __global__ void __launch_bounds__(256) pack_kernel(F f, int ksteps, uint16_t* __
     if (PASSES == 3) t[TILE_ELEMS + o] = lo;
   }
   __syncthreads();
-  uint4* dst = reinterpret_cast<uint4*>(img + ((size_t)rt * ksteps + kt) * 2 * TILE_ELEMS);
   const uint4* src = reinterpret_cast<const uint4*>(t);
-  constexpr int NV = (PASSES == 3 ? 2 : 1) * TILE_ELEMS * 2 / 16;
+  constexpr int HB = PASSES == 3 ? 2 : 1;
+  constexpr int NV = HB * TILE_ELEMS * 2 / 16;
+  if constexpr (QUARTERS) {
+    constexpr int QV = TILE_ELEMS / 16;     // 16-byte vectors of a [64 x 32] half: rows 0-63 of a tile half come first
+    uint4* dst = reinterpret_cast<uint4*>(img);
 #pragma unroll
-  for (int i = threadIdx.x; i < NV; i += 256) dst[i] = src[i];
+    for (int i = threadIdx.x; i < NV; i += 256) {
+      const int h = i / (2 * QV), v = i % (2 * QV);
+      dst[(((size_t)(2 * rt + v / QV) * ksteps + kt) * HB + h) * QV + v % QV] = src[i];
+    }
+  } else {
+    uint4* dst = reinterpret_cast<uint4*>(img + ((size_t)rt * ksteps + kt) * 2 * TILE_ELEMS);
+#pragma unroll
+    for (int i = threadIdx.x; i < NV; i += 256) dst[i] = src[i];
+  }
 }
 
 // The colour-head backward of the tensor-core engines, one CTA per 128-row tile (rows m0 + r):
@@ -1098,22 +1135,26 @@ __global__ void __launch_bounds__(STAGED_THREADS, 1) wg_gemm_staged_kernel(Opnd 
   }
 }
 
-// ---- The fused trunk forward: one tile of 64 rows goes through every trunk layer without leaving the SM.
-constexpr int CH_W = 256;                     // the trunk width it is built for: one 128-column N tile per warpgroup
-constexpr int CH_M = 64;                      // rows per tile
+// ---- The fused trunk forward: one tile of 128 rows goes through every trunk layer without leaving the SM.
+constexpr int CH_W = 256;                     // the trunk width it is built for
+constexpr int CH_M = TM;                      // rows per tile: 64 per consumer warpgroup
 constexpr int CH_KS = CH_W / TK;              // k-steps of a layer's activation input
 constexpr int CH_ENC_KS = 2;                  // k-steps of the encoding at most (64 columns)
-constexpr int CH_HALF = CH_M * TK * 2;        // one 16-bit half of a [64 x 32] k-step of A, 4 KB
-constexpr int CH_STAGES = 4;                  // weight ring: per stage the k-step's two [128 x 32] B tiles (hi, lo each)
-constexpr int CH_ENC = CH_KS * 2 * CH_HALF;               // byte offsets in shared memory: activations at 0 (64 KB),
-constexpr int CH_RING = CH_ENC + CH_ENC_KS * 2 * CH_HALF; // the encoding (16 KB), the ring (128 KB),
-constexpr int CH_BAR = CH_RING + CH_STAGES * STAGE_BYTES; // full[4], empty[4], enc_full, enc_empty, rd[2], wr[2]
-constexpr int CH_SMEM = CH_BAR + (2 * CH_STAGES + 6) * 8;
+constexpr int CH_Q = 4;                       // a layer's output columns are computed in quarters of 64
+constexpr int CH_QHALF = CH_W / CH_Q * TK * 2;             // one 16-bit half of a quarter's k-step of B, [64 x 32], 4 KB
+constexpr int CH_STAGE_KS = 2;                // weight ring: per stage two k-steps of one quarter (hi, lo each), 16 KB
+constexpr int CH_STAGE = CH_STAGE_KS * 2 * CH_QHALF;
+constexpr int CH_STAGES = 4;
+constexpr int CH_ENC = CH_KS * 2 * TILE_BYTES;            // byte offsets in shared memory: activations at 0 (128 KB),
+constexpr int CH_RING = CH_ENC + CH_ENC_KS * 2 * TILE_BYTES;  // the encoding (32 KB), the ring (64 KB),
+constexpr int CH_BAR = CH_RING + CH_STAGES * CH_STAGE;    // full[4], empty[4], enc_full, enc_empty
+constexpr int CH_SMEM = CH_BAR + (2 * CH_STAGES + 2) * 8;
+static_assert(CH_SMEM <= 232448, "the fused chains' shared memory exceeds an H100 SM's 227 KB");
 
 // Its own parameter struct (not Epi: see the note there).  Layer l < nl computes H[l] = relu(in_l W_l^T + bias[l]), in_0 =
-// enc, in_l = H[l-1] ( | enc at l == skip), from the weight image w[l] (256 rows, chain_ks(l) k-steps, as pack_kernel<NtB>
-// makes it).  H[l] == NULL: not written to global memory.  last (may be NULL): the row image of H[nl-1].  bits[l] (may
-// be NULL): the ReLU mask H[l] > 0, 8 words per row (trunk_chain_kernel's BITS instantiations only).
+// enc, in_l = H[l-1] ( | enc at l == skip), from the weight image w[l] (256 rows, chain_ks(l) k-steps, as tc_pack_nt
+// makes it: per quarter).  H[l] == NULL: not written to global memory.  last (may be NULL): the row image of H[nl-1].
+// bits[l] (may be NULL): the ReLU mask H[l] > 0, 8 words per row (trunk_chain_kernel's BITS instantiations only).
 struct Chain {
   int M, nl, skip, enc_ks;
   const uint16_t* enc;
@@ -1128,140 +1169,154 @@ __host__ __device__ __forceinline__ int chain_ks(int l, int skip, int enc_ks) {
   return l == 0 ? enc_ks : CH_KS + (l == skip ? enc_ks : 0);
 }
 
-// The producer (one thread) walks (tile, layer, k-step): the tile's 64 rows of the encoding image once per tile (they
-// stay for layer 0 and the skip layer; the buffer is free once the previous tile's last reader has retired), and per
-// k-step both B tiles of the layer's weight image into a ring that runs on across layers and tiles.
+// The weight stages of one layer of nk k-steps into the ring (position it, advanced): per quarter its k-steps,
+// CH_STAGE_KS to a stage (the last one of an odd count alone), each stage one copy, since the image holds a quarter's
+// k-steps one after another.
 template <int PASSES>
-__device__ __forceinline__ void chain_produce(const Chain& c, int M, int tiles, uint64_t* full, uint64_t* empty, uint64_t* enc_full,
-                                              uint64_t* enc_empty) {
+__device__ __forceinline__ void chain_stream(const uint16_t* w, int nk, int& it, uint64_t* full, uint64_t* empty) {
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr int HB = PASSES == 3 ? 2 : 1;     // halves copied
+  for (int q = 0; q < CH_Q; ++q)
+    for (int j0 = 0; j0 < nk; j0 += CH_STAGE_KS, ++it) {
+      const int s = it % CH_STAGES;
+      mbar_wait(&empty[s], ((it / CH_STAGES) & 1) ^ 1);
+      const uint32_t bytes = (nk - j0 < CH_STAGE_KS ? nk - j0 : CH_STAGE_KS) * HB * CH_QHALF;
+      mbar_expect_tx(&full[s], bytes);
+      bulk_g2s(smem + CH_RING + s * CH_STAGE, w + ((size_t)q * nk + j0) * HB * (CH_QHALF / 2), bytes, &full[s]);
+    }
+}
+
+// A 128-row tile of a row image (row tile t, ks k-steps) into shared memory at dst, one copy per k-step and half
+template <int PASSES>
+__device__ __forceinline__ void chain_load_rows(uint8_t* dst, const uint16_t* img, int t, int ks, uint64_t* bar) {
+  constexpr int HB = PASSES == 3 ? 2 : 1;
+  mbar_expect_tx(bar, ks * HB * TILE_BYTES);
+  for (int kt = 0; kt < ks; ++kt)
+    for (int h = 0; h < HB; ++h)
+      bulk_g2s(dst + (kt * 2 + h) * TILE_BYTES, img + (((size_t)t * ks + kt) * 2 + h) * TILE_ELEMS, TILE_BYTES, bar);
+}
+
+// The producer (one thread) walks (tile, layer, quarter, k-step): the tile's rows of the encoding image once per tile
+// (they stay for layer 0 and the skip layer; the buffer is free once the previous tile's last reader has retired), and
+// the layers' weights into a ring that runs on across quarters, layers and tiles.
+template <int PASSES>
+__device__ __forceinline__ void chain_produce(const Chain& c, int tiles, uint64_t* full, uint64_t* empty, uint64_t* enc_full,
+                                              uint64_t* enc_empty) {
+  extern __shared__ __align__(1024) uint8_t smem[];
   int it = 0, n = 0;
   for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
-    if (t * CH_M >= M) continue;
     mbar_wait(enc_empty, (n & 1) ^ 1);
     ++n;
-    mbar_expect_tx(enc_full, c.enc_ks * HB * CH_HALF);
-    for (int kt = 0; kt < c.enc_ks; ++kt)
-      for (int h = 0; h < HB; ++h)    // rows 64 (t & 1) ... + 63 of a half tile: its first or second 4 KB
-        bulk_g2s(smem + CH_ENC + (kt * 2 + h) * CH_HALF,
-                 c.enc + (((size_t)(t >> 1) * c.enc_ks + kt) * 2 + h) * TILE_ELEMS + (t & 1) * (CH_M * TK), CH_HALF, enc_full);
-    for (int l = 0; l < c.nl; ++l) {
-      const int nk = chain_ks(l, c.skip, c.enc_ks);
-      for (int kt = 0; kt < nk; ++kt, ++it) {
-        const int s = it % CH_STAGES;
-        mbar_wait(&empty[s], ((it / CH_STAGES) & 1) ^ 1);
-        uint8_t* st = smem + CH_RING + s * STAGE_BYTES;
-        mbar_expect_tx(&full[s], 2 * HB * TILE_BYTES);
-        for (int g = 0; g < 2; ++g)
-          bulk_g2s(st + g * 2 * TILE_BYTES, c.w[l] + ((size_t)g * nk + kt) * 2 * TILE_ELEMS, HB * TILE_BYTES, &full[s]);
-      }
-    }
+    chain_load_rows<PASSES>(smem + CH_ENC, c.enc, t, c.enc_ks, enc_full);
+    for (int l = 0; l < c.nl; ++l) chain_stream<PASSES>(c.w[l], chain_ks(l, c.skip, c.enc_ks), it, full, empty);
   }
 }
 
-// The hand-offs of the activation buffer between the two warpgroups.  Half h of the buffer (k-steps [4 h, 4 h + 4), the
-// layer's output columns [128 h, 128 h + 128)) is written by warpgroup h and read by both.  rd[h] completes once all 8
-// consumer warps have retired their MMAs on half h (warpgroup h may then overwrite it), wr[h] once warpgroup h's 4 warps
-// have stored and proxy-fenced its split there (the MMAs on it may then start).  Each warpgroup waits only for the half
-// it is about to touch, so the two drift apart by up to the weight ring's depth instead of meeting twice per layer.
-// Both complete once per generation of the buffer, in the same order on every thread; a wait takes the parity of the
-// generation's index, which is never more than one phase from where the barrier stands.
-struct Halves {
-  uint64_t* rd;
-  uint64_t* wr;
-};
-
-// The MMAs of one layer for this warpgroup's 128 output columns of the tile's 64 rows: mma_unit's instruction sequence
-// per k-step (so every output element sums in the same order), nk k-steps of A, the first na (0 or CH_KS) from the
-// activation buffer and the rest from the encoding's (the skip layer; the encoding alone at layer 0), B this warpgroup's
-// tile of the stage.  wr_parity >= 0: the buffer holds a generation the epilogues wrote, waited for half by half in front
-// of the half's first k-step.  rd_arrive: arrive on rd[h] as soon as half h's MMAs have retired.
+// The MMAs of one quarter of a layer for this warpgroup's 64 rows of the tile: nk k-steps of A, the first na (0 or
+// CH_KS) from the activation buffer and the rest from the encoding's (the skip layer; the encoding alone at layer 0), B
+// the quarter's k-steps from the ring.  Per k-step mma_unit's instruction sequence, so every output element sums in the
+// same order as the GEMMs'.  Warpgroup g's A is rows [64 g, 64 g + 64) of each [128 x 32] k-step, its second 4 KB.  One
+// MMA group (a stage) stays in flight; each warp releases a stage once the group that read it has retired.
 template <bool F16, int PASSES>
-__device__ __forceinline__ void chain_mma(float (&acc)[64], int nk, int na, int& it, uint64_t* full, uint64_t* empty,
-                                          Halves hv, int wr_parity, bool rd_arrive) {
+__device__ __forceinline__ void chain_mma(float (&acc)[32], int nk, int na, int& it, uint64_t* full, uint64_t* empty) {
   extern __shared__ __align__(1024) uint8_t smem[];
+  constexpr int HB = PASSES == 3 ? 2 : 1;
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
-  float acc_lo[PASSES == 3 ? 64 : 1];
+  float acc_lo[PASSES == 3 ? 32 : 1];
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
 #pragma unroll
-  for (int i = 0; i < (PASSES == 3 ? 64 : 1); ++i) acc_lo[i] = 0.f;
-  for (int j = 0; j < nk; ++j, ++it) {
+  for (int i = 0; i < (PASSES == 3 ? 32 : 1); ++i) acc_lo[i] = 0.f;
+  for (int j0 = 0; j0 < nk; j0 += CH_STAGE_KS, ++it) {
     const int s = it % CH_STAGES;
-    if (wr_parity >= 0 && j < na && j % (CH_KS / 2) == 0) mbar_wait(&hv.wr[j / (CH_KS / 2)], wr_parity);
     mbar_wait(&full[s], (it / CH_STAGES) & 1);
-    const uint8_t* a = j < na ? smem + j * 2 * CH_HALF : smem + CH_ENC + (j - na) * 2 * CH_HALF;
-    const uint8_t* b = smem + CH_RING + s * STAGE_BYTES + wg * 2 * TILE_BYTES;
+    const uint8_t* st = smem + CH_RING + s * CH_STAGE;
     wgmma_fence();
 #pragma unroll
-    for (int ks = 0; ks < TK / 16; ++ks) {
-      const uint64_t ahi = smem_desc(a + ks * 256), bhi = smem_desc(b + ks * 256);
-      if constexpr (PASSES == 3) {
-        wgmma_m64n128k16<F16>(acc_lo, smem_desc(a + CH_HALF + ks * 256), bhi);
-        wgmma_m64n128k16<F16>(acc_lo, ahi, smem_desc(b + TILE_BYTES + ks * 256));
+    for (int jj = 0; jj < CH_STAGE_KS; ++jj) {
+      const int j = j0 + jj;
+      if (j >= nk) break;
+      const uint8_t* a = (j < na ? smem + j * 2 * TILE_BYTES : smem + CH_ENC + (j - na) * 2 * TILE_BYTES) + wg * (TILE_BYTES / 2);
+      const uint8_t* b = st + jj * HB * CH_QHALF;
+#pragma unroll
+      for (int ks = 0; ks < TK / 16; ++ks) {
+        const uint64_t ahi = smem_desc(a + ks * 256), bhi = smem_desc(b + ks * 256);
+        if constexpr (PASSES == 3) {
+          wgmma_m64n64k16<F16>(acc_lo, smem_desc(a + TILE_BYTES + ks * 256), bhi);
+          wgmma_m64n64k16<F16>(acc_lo, ahi, smem_desc(b + CH_QHALF + ks * 256));
+        }
+        wgmma_m64n64k16<F16>(acc, ahi, bhi);
       }
-      wgmma_m64n128k16<F16>(acc, ahi, bhi);
     }
     wgmma_commit();
-    wgmma_wait_1();             // k-steps 0 ... j - 1 have retired
-    if (j > 0 && lane == 0) mbar_arrive(&empty[(it + CH_STAGES - 1) % CH_STAGES]);
-    if (rd_arrive && lane == 0 && j > 0 && j <= na && j % (CH_KS / 2) == 0) mbar_arrive(&hv.rd[j / (CH_KS / 2) - 1]);
+    wgmma_wait_1();             // the stages before this one have retired
+    if (j0 > 0 && lane == 0) mbar_arrive(&empty[(it + CH_STAGES - 1) % CH_STAGES]);
   }
   wgmma_wait_all();
   if (lane == 0) mbar_arrive(&empty[(it + CH_STAGES - 1) % CH_STAGES]);
-  if (rd_arrive && lane == 0 && nk == na) mbar_arrive(&hv.rd[1]);
   if constexpr (PASSES == 3) {
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] += lo_unscale(acc_lo[i]);
+    for (int i = 0; i < 32; ++i) acc[i] += lo_unscale(acc_lo[i]);
   }
 }
 
-// this warpgroup's 4 warps have stored and proxy-fenced their part of half wg of the buffer
-__device__ __forceinline__ void chain_written(Halves hv) {
-  fence_proxy_async();          // the stores into the activation buffer, before the MMAs that read them
-  __syncwarp();
-  if ((threadIdx.x & 31) == 0) mbar_arrive(&hv.wr[threadIdx.x >> 7]);
+// A quarter's fragment: acc[4 j + 2 h + c] is row 64 wg + 16 wq + lane / 4 + 8 h of the tile, column 64 q + 8 j +
+// 2 (lane % 4) + c of the layer.
+__device__ __forceinline__ int chain_row(int t, int h) {
+  return t * CH_M + (threadIdx.x >> 5) * 16 + ((threadIdx.x & 31) >> 2) + 8 * h;
 }
 
-// the tile's split (PASSES halves) of this warpgroup's columns as a row image at img: k-step stride kstride, lo half
-// lo_off after the hi half (16-bit elements); the fragment of (j, h) is one core matrix, this lane's pair its 32-bit
-// word `lane`
+// The split of a quarter's values (split2: the bytes a row image holds of them): s[2 j + h] the hi pair of (j, h), the
+// lo pair 16 words further on (PASSES == 3)
+template <int PASSES>
+using ChainSplit = uint32_t[PASSES == 3 ? 32 : 16];
+
 template <bool F16, int PASSES>
-__device__ __forceinline__ void chain_split(const float (&acc)[64], uint16_t* img, int kstride, int lo_off) {
-  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+__device__ __forceinline__ void chain_split(const float (&acc)[32], ChainSplit<PASSES>& s) {
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    uint16_t* kt = img + (size_t)(4 * wg + (j >> 2)) * kstride;
+  for (int j = 0; j < 8; ++j)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       uint32_t hi, lo;
       split2<F16>(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], hi, lo);
-      const int core = (2 * wq + h) * (TK / 8) + (j & 3);
-      reinterpret_cast<uint32_t*>(kt + core * 64)[lane] = hi;
-      if (PASSES == 3) reinterpret_cast<uint32_t*>(kt + lo_off + core * 64)[lane] = lo;
+      s[2 * j + h] = hi;
+      if (PASSES == 3) s[16 + 2 * j + h] = lo;
+    }
+}
+
+// quarter q's split as part of a 128-row tile of a row image at img (k-step stride kstride, the lo half lo_off after
+// the hi half, 16-bit elements): the fragment of (j, h) is one core matrix, this lane's pair its 32-bit word `lane`
+template <int PASSES>
+__device__ __forceinline__ void chain_put(const ChainSplit<PASSES>& s, int q, uint16_t* img, int kstride, int lo_off) {
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    uint16_t* kt = img + (size_t)(2 * q + (j >> 2)) * kstride;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int core = (2 * w + h) * (TK / 8) + (j & 3);
+      reinterpret_cast<uint32_t*>(kt + core * 64)[lane] = s[2 * j + h];
+      if (PASSES == 3) reinterpret_cast<uint32_t*>(kt + lo_off + core * 64)[lane] = s[16 + 2 * j + h];
     }
   }
 }
 
-// this thread's bias pairs of layer l, columns wg 128 + 8 j + 2 (lane % 4) + {0, 1}; loaded before the layer's MMAs.
-// Two scalar loads per pair: a bias in a flat parameter bank may start at an odd float.
-__device__ __forceinline__ void chain_bias(float2 (&bv)[16], const float* bias) {
-  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
+// this thread's bias pairs of quarter q of layer l, columns 64 q + 8 j + 2 (lane % 4) + {0, 1}; loaded before the
+// quarter's MMAs.  Two scalar loads per pair: a bias in a flat parameter bank may start at an odd float.
+__device__ __forceinline__ void chain_bias(float2 (&bv)[8], const float* bias, int q) {
+  const int lane = threadIdx.x & 31;
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    const float* b = bias + wg * TN + j * 8 + (lane & 3) * 2;
+  for (int j = 0; j < 8; ++j) {
+    const float* b = bias + q * 64 + j * 8 + (lane & 3) * 2;
     bv[j] = make_float2(b[0], b[1]);
   }
 }
 
-// Layer l's bias and ReLU of tile t as epilogue_values kind 0: acc becomes the layer's output, zero past M.
-__device__ __forceinline__ void chain_bias_relu(float (&acc)[64], const float2 (&bv)[16], int M, int t) {
-  const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+// The bias and ReLU of a quarter as epilogue_values kind 0: acc becomes the layer's output, zero past M.
+__device__ __forceinline__ void chain_bias_relu(float (&acc)[32], const float2 (&bv)[8], int M, int t) {
 #pragma unroll
-  for (int i = 0; i < 64; i += 2) {
-    const int m = t * CH_M + wq * 16 + (lane >> 2) + ((i >> 1) & 1) * 8;
-    if (m >= M) {
+  for (int i = 0; i < 32; i += 2) {
+    if (chain_row(t, (i >> 1) & 1) >= M) {
       acc[i] = acc[i + 1] = 0.f;
       continue;
     }
@@ -1270,66 +1325,66 @@ __device__ __forceinline__ void chain_bias_relu(float (&acc)[64], const float2 (
   }
 }
 
-// The fp32 output of layer l (acc after chain_bias_relu) to H[l].  It runs after the proxy fence that follows the stores
-// into the activation buffer: a fence issued behind these global stores waits for them too, once per layer with no MMA
-// in flight; issued after it, they drain while the next layer's MMAs run.
-__device__ __forceinline__ void chain_store(const float (&acc)[64], float* H, int M, int t) {
-  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+// The fp32 output of quarter q (acc after chain_bias_relu) to H[l].  Quarter 3's runs after the proxy fence that follows
+// the stores into the activation buffer: a fence issued behind these global stores waits for them too, once per layer
+// with no MMA in flight; issued after it, they drain while the next layer's MMAs run.
+__device__ __forceinline__ void chain_store(const float (&acc)[32], float* H, int M, int t, int q) {
+  const int lane = threadIdx.x & 31;
 #pragma unroll
-  for (int i = 0; i < 64; i += 2) {
-    const int m = t * CH_M + wq * 16 + (lane >> 2) + ((i >> 1) & 1) * 8, n = wg * TN + (i >> 2) * 8 + (lane & 3) * 2;
+  for (int i = 0; i < 32; i += 2) {
+    const int m = chain_row(t, (i >> 1) & 1), n = q * 64 + (i >> 2) * 8 + (lane & 3) * 2;
     if (m < M) *reinterpret_cast<float2*>(H + (size_t)m * CH_W + n) = make_float2(acc[i], acc[i + 1]);
   }
 }
 
-// The ReLU mask of layer l's output as tc_gemm_tn writes it, bit n & 31 of word [m][n >> 5] = H[m][n] > 0 (the predicate
-// the fp32 mask applies, so NaN and -0 give 0): a lane's 8 values of a 32-column word (4 j x 2 columns) go to its bits
-// 2 (lane % 4) + 8 (j % 4) + {0, 1}, the quad ORs them together, and lane % 4 stores word lane % 4 of its warpgroup's
-// four.  Like chain_store, it runs after the proxy fence.
-__device__ __forceinline__ void chain_store_bits(const float (&acc)[64], uint32_t* bits, int M, int t) {
-  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+// The ReLU mask of quarter q as tc_gemm_tn writes it, bit n & 31 of word [m][n >> 5] = H[m][n] > 0 (the predicate the
+// fp32 mask applies, so NaN and -0 give 0): a lane's 8 values of a 32-column word (4 j x 2 columns) go to its bits
+// 2 (lane % 4) + 8 (j % 4) + {0, 1}, the quad ORs them together, and lanes with lane % 4 < 2 store word lane % 4 of the
+// quarter's two.  Like chain_store, quarter 3's runs after the proxy fence.
+__device__ __forceinline__ void chain_store_bits(const float (&acc)[32], uint32_t* bits, int M, int t, int q) {
+  const int lane = threadIdx.x & 31;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     uint32_t mine = 0;
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {
+    for (int wd = 0; wd < 2; ++wd) {
       uint32_t w = 0;
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj) {
-        const int i = 4 * (4 * q + jj) + 2 * h, b = 8 * jj + 2 * (lane & 3);
+        const int i = 4 * (4 * wd + jj) + 2 * h, b = 8 * jj + 2 * (lane & 3);
         w |= (uint32_t)(acc[i] > 0.f) << b | (uint32_t)(acc[i + 1] > 0.f) << (b + 1);
       }
       w |= __shfl_xor_sync(0xffffffffu, w, 1);
       w |= __shfl_xor_sync(0xffffffffu, w, 2);
-      if ((lane & 3) == q) mine = w;
+      if ((lane & 3) == wd) mine = w;
     }
-    const int m = t * CH_M + wq * 16 + (lane >> 2) + 8 * h;
-    if (m < M) bits[(size_t)m * (CH_W / 32) + wg * 4 + (lane & 3)] = mine;
+    const int m = chain_row(t, h);
+    if (m < M && (lane & 3) < 2) bits[(size_t)m * (CH_W / 32) + 2 * q + (lane & 3)] = mine;
   }
 }
 
 // Persistent and warp-specialized like wg_gemm_kernel (thread 256 produces, warps 0-7 consume, the same register
-// hand-back), but the two consumer warpgroups split N: warpgroup g computes columns [128 g, 128 g + 128) of the tile's 64
-// rows from the same A.  Each warpgroup overwrites its half of the layer's input with its half of the output (the same
-// split2 as a row image's) once every warp's MMAs on that half have retired, and the next layer's MMAs on a half start
-// once its stores are fenced for the async proxy (Halves).  So one warpgroup's epilogue runs while the other's MMAs do;
-// the last layer's split goes to its row image in global memory instead, where asked.
-// Tiles: 2 ceil(M / 128), so that the last image's 128-row tiles are written whole; a tile wholly past M only zeroes its
-// half of them.  DYN: c.M is a capacity, of which live_rows rows (M) are computed.  SPAN (with DYN; the span forward): H
-// and bits take their rows from row_start on (the last image's rows start at 0); without it rc.start is never read.
-// BITS: c.bits[l] are written where
-// not NULL (the other instantiations never read them).
+// hand-back), on tiles of 128 rows: warpgroup g computes every column of rows [64 g, 64 g + 64) of the tile, a quarter
+// of 64 columns at a time, and never reads the other warpgroup's rows; the two share only the weight ring, each stage of
+// which both consume.  A quarter's split stays in registers until the layer's last quarter has retired its MMAs; then
+// the warpgroup overwrites its rows of the layer's input in the activation buffer with all four (the same split2 as a
+// row image's), fences them for the async proxy and meets its own 4 warps at a named barrier before the next layer's
+// MMAs.  The last layer's split goes to its row image in global memory instead, where asked.
+// Tiles: ceil(M / 128), so that the last image's 128-row tiles are written whole; a warpgroup whose rows all lie past M
+// still runs (and releases) every stage, and its epilogue zeroes them.  DYN: c.M is a capacity, of which live_rows rows
+// (M) are computed.  SPAN (with DYN; the span forward): H and bits take their rows from row_start on (the last image's
+// rows start at 0); without it rc.start is never read.  BITS: c.bits[l] are written where not NULL (the other
+// instantiations never read them).
 template <bool F16, int PASSES, bool DYN = false, bool BITS = false, bool SPAN = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) trunk_chain_kernel(const Chain c, RowCount rc) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const int M = (int)live_rows<DYN, SPAN>(c.M, rc);
   if (DYN && M == 0) return;
-  const int tiles = (M + TM - 1) / TM * 2;
+  const int tiles = (M + CH_M - 1) / CH_M;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + CH_BAR);
   uint64_t* empty = full + CH_STAGES;
   uint64_t* enc_full = empty + CH_STAGES;
   uint64_t* enc_empty = enc_full + 1;
-  const Halves hv{enc_empty + 1, enc_empty + 3};
   if (threadIdx.x == 0) {
     for (int i = 0; i < CH_STAGES; ++i) {
       mbar_init(&full[i], 1);
@@ -1337,55 +1392,53 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) trunk_chain_kernel(const Chai
     }
     mbar_init(enc_full, 1);
     mbar_init(enc_empty, CONSUMERS / 32);
-    for (int h = 0; h < 2; ++h) {
-      mbar_init(&hv.rd[h], CONSUMERS / 32);
-      mbar_init(&hv.wr[h], 4);
-    }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   __syncthreads();
   if (threadIdx.x >= CONSUMERS) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
-    if (threadIdx.x == CONSUMERS) chain_produce<PASSES>(c, M, tiles, full, empty, enc_full, enc_empty);
+    if (threadIdx.x == CONSUMERS) chain_produce<PASSES>(c, tiles, full, empty, enc_full, enc_empty);
     return;
   }
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
   const int enc_last = c.skip > 0 && c.skip < c.nl ? c.skip : 0;   // the last layer that reads the encoding
   const long long s0 = row_start<SPAN>(rc);   // the span forward: H and bits at global rows s0 + m; 0 otherwise
-  const int wg = threadIdx.x >> 7;
-  // p: generations of the activation buffer written so far.  Every layer l > 0 reads generation p - 1 (layer l - 1's
-  // output) and every layer but the last writes generation p over it, after the reads of generation p - 1: the same
-  // tile's at l > 0, the previous tile's last layer at l == 0.
-  int it = 0, n = 0, p = 0;
+  int it = 0, n = 0;
   for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
-    if (t * CH_M >= M) {
-      if (c.last)
-        for (int i = 0; i < CH_KS * (PASSES == 3 ? 2 : 1); ++i)
-          reinterpret_cast<uint4*>(c.last + ((size_t)(t >> 1) * CH_KS * 2 + (PASSES == 3 ? i : 2 * i)) * TILE_ELEMS +
-                                   (t & 1) * (CH_M * TK))[threadIdx.x] = make_uint4(0, 0, 0, 0);
-      continue;
-    }
     mbar_wait(enc_full, n & 1);
     ++n;
     for (int l = 0; l < c.nl; ++l) {
-      float2 bv[16];
-      chain_bias(bv, c.bias[l]);
-      float acc[64];
-      chain_mma<F16, PASSES>(acc, chain_ks(l, c.skip, c.enc_ks), l == 0 ? 0 : CH_KS, it, full, empty, hv,
-                             l == 0 ? -1 : (p - 1) & 1, l > 0);
-      if (l == enc_last && (threadIdx.x & 31) == 0) mbar_arrive(enc_empty);
-      chain_bias_relu(acc, bv, M, t);
-      if (l + 1 < c.nl) {
-        if (p > 0) mbar_wait(&hv.rd[wg], (p - 1) & 1);    // every warp has read generation p - 1 of this half
-        chain_split<F16, PASSES>(acc, reinterpret_cast<uint16_t*>(smem), CH_HALF, CH_HALF / 2);
-        chain_written(hv);
-        ++p;
-      } else if (c.last) {
-        chain_split<F16, PASSES>(acc, c.last + (size_t)(t >> 1) * CH_KS * 2 * TILE_ELEMS + (t & 1) * (CH_M * TK),
-                                 2 * TILE_ELEMS, TILE_ELEMS);
+      const int nk = chain_ks(l, c.skip, c.enc_ks), na = l == 0 ? 0 : CH_KS;
+      ChainSplit<PASSES> held[CH_Q - 1];
+#pragma unroll
+      for (int q = 0; q < CH_Q; ++q) {
+        float2 bv[8];
+        chain_bias(bv, c.bias[l], q);
+        float acc[32];
+        chain_mma<F16, PASSES>(acc, nk, na, it, full, empty);
+        if (q == CH_Q - 1 && l == enc_last && (threadIdx.x & 31) == 0) mbar_arrive(enc_empty);
+        chain_bias_relu(acc, bv, M, t);
+        if (l + 1 < c.nl) {
+          if (q < CH_Q - 1) {
+            chain_split<F16, PASSES>(acc, held[q]);
+          } else {      // every MMA on this warpgroup's rows of the layer's input has retired
+            ChainSplit<PASSES> s;
+            chain_split<F16, PASSES>(acc, s);
+            uint16_t* buf = reinterpret_cast<uint16_t*>(smem);
+#pragma unroll
+            for (int p = 0; p < CH_Q - 1; ++p) chain_put<PASSES>(held[p], p, buf, 2 * TILE_ELEMS, TILE_ELEMS);
+            chain_put<PASSES>(s, CH_Q - 1, buf, 2 * TILE_ELEMS, TILE_ELEMS);
+            fence_proxy_async();      // the stores into the activation buffer, before the MMAs that read them
+            warpgroup_sync();
+          }
+        } else if (c.last) {
+          ChainSplit<PASSES> s;
+          chain_split<F16, PASSES>(acc, s);
+          chain_put<PASSES>(s, q, c.last + (size_t)t * CH_KS * 2 * TILE_ELEMS, 2 * TILE_ELEMS, TILE_ELEMS);
+        }
+        if (c.H[l]) chain_store(acc, c.H[l] + s0 * CH_W, M, t, q);
+        if (BITS && c.bits[l]) chain_store_bits(acc, c.bits[l] + s0 * (CH_W / 32), M, t, q);
       }
-      if (c.H[l]) chain_store(acc, c.H[l] + s0 * CH_W, M, t);
-      if (BITS && c.bits[l]) chain_store_bits(acc, c.bits[l] + s0 * (CH_W / 32), M, t);
     }
   }
 }
@@ -1404,17 +1457,17 @@ static int launch_chain(const Chain& c, int ctas, RowCount rc, cudaStream_t st) 
     kernel = trunk_chain_kernel<F16, PASSES, true, true, true>;
   }
   SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM));
-  kernel<<<std::min(2 * ceil_div(c.M, TM), ctas), GEMM_THREADS, CH_SMEM, st>>>(c, rc);
+  kernel<<<std::min(ceil_div(c.M, CH_M), ctas), GEMM_THREADS, CH_SMEM, st>>>(c, rc);
   SPARF_CHECK_LAUNCH("trunk_chain_kernel");
   return SPARF_OK;
 }
 
 // ---- The trunk backward's input gradients in one persistent kernel, the same walk as trunk_chain_kernel.  Layer l
 // (top >= l >= 1) computes G[l-1] = mask_l * (G[l] W_l), W_l's [256 x 256] part over H[l-1], from its weight image w[l]
-// (256 rows, CH_KS k-steps, as tc_gemm_nn packs it: tc_pack_nn); mask_l = bits[l] (H[l-1] > 0, 8 words per row).  G[top]
-// comes in as its row image, and a tile's gradient stays in the activation buffer from layer to layer.  G[l-1] leaves as
-// its transposed image tr[l] (tr_ks k-steps per row tile), its column sums (db[l] +=) and, where row[l] is not NULL, its
-// row image.  Shared memory as trunk_chain_kernel's, with the column-sum reduction where the encoding would be.
+// (256 rows, CH_KS k-steps, as tc_pack_nn packs it: per quarter); mask_l = bits[l] (H[l-1] > 0, 8 words per row).
+// G[top] comes in as its row image, and a tile's gradient stays in the activation buffer from layer to layer.  G[l-1]
+// leaves as its transposed image tr[l] (tr_ks k-steps per row tile), its column sums (db[l] +=) and, where row[l] is not
+// NULL, its row image.  Shared memory as trunk_chain_kernel's, with the column sums' partials where the encoding would be.
 struct DgChain {
   int M, top, tr_ks;
   const uint16_t* in;
@@ -1425,84 +1478,70 @@ struct DgChain {
   uint16_t* row[SPARF_MAX_TRUNK];
 };
 
-// The producer (one thread) walks (tile, layer, k-step): the tile's 64 rows of the input image once per tile, once the
-// previous tile's last MMAs have retired (act_empty), and the weights as chain_produce streams them.
+// The producer (one thread) walks (tile, layer, quarter, k-step): the tile's rows of the input image once per tile,
+// once the previous tile's last MMAs have retired (act_empty), and the weights as chain_produce streams them.
 template <int DP>
-__device__ __forceinline__ void dg_produce(const DgChain& c, int M, int tiles, uint64_t* full, uint64_t* empty, uint64_t* act_full,
+__device__ __forceinline__ void dg_produce(const DgChain& c, int tiles, uint64_t* full, uint64_t* empty, uint64_t* act_full,
                                            uint64_t* act_empty) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  constexpr int HB = DP == 3 ? 2 : 1;
   int it = 0, n = 0;
   for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
-    if (t * CH_M >= M) continue;
     mbar_wait(act_empty, (n & 1) ^ 1);
     ++n;
-    mbar_expect_tx(act_full, CH_KS * HB * CH_HALF);
-    for (int kt = 0; kt < CH_KS; ++kt)
-      for (int h = 0; h < HB; ++h)
-        bulk_g2s(smem + (kt * 2 + h) * CH_HALF,
-                 c.in + (((size_t)(t >> 1) * CH_KS + kt) * 2 + h) * TILE_ELEMS + (t & 1) * (CH_M * TK), CH_HALF, act_full);
-    for (int l = c.top; l >= 1; --l)
-      for (int kt = 0; kt < CH_KS; ++kt, ++it) {
-        const int s = it % CH_STAGES;
-        mbar_wait(&empty[s], ((it / CH_STAGES) & 1) ^ 1);
-        uint8_t* st = smem + CH_RING + s * STAGE_BYTES;
-        mbar_expect_tx(&full[s], 2 * HB * TILE_BYTES);
-        for (int g = 0; g < 2; ++g)
-          bulk_g2s(st + g * 2 * TILE_BYTES, c.w[l] + ((size_t)g * CH_KS + kt) * 2 * TILE_ELEMS, HB * TILE_BYTES, &full[s]);
-      }
+    chain_load_rows<DP>(smem, c.in, t, CH_KS, act_full);
+    for (int l = c.top; l >= 1; --l) chain_stream<DP>(c.w[l], CH_KS, it, full, empty);
   }
 }
 
-// this thread's two rows of its warpgroup's four mask words (one 16-byte load each); rows past M get none
-__device__ __forceinline__ void dg_mask_words(uint4 (&wd)[2], const uint32_t* bits, int M, int t) {
-  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+// this thread's two rows' mask words of quarter q (one 8-byte load each); rows past M get none, so they are zero
+__device__ __forceinline__ void dg_mask_words(uint2 (&wd)[2], const uint32_t* bits, int M, int t, int q) {
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int m = t * CH_M + wq * 16 + (lane >> 2) + 8 * h;
-    wd[h] = m < M ? *reinterpret_cast<const uint4*>(bits + (size_t)m * (CH_W / 32) + wg * 4) : make_uint4(0, 0, 0, 0);
+    const int m = chain_row(t, h);
+    wd[h] = m < M ? *reinterpret_cast<const uint2*>(bits + (size_t)m * (CH_W / 32) + 2 * q) : make_uint2(0, 0);
   }
 }
 
-// A tile wholly past M writes zeros where the layer-by-layer GEMMs' 128-row tiles would: its half of the row images, and
-// the transposed images' k-steps of its rows below tr_ks (a capacity's, with a device row count).
-template <int DP, int TP>
-__device__ __forceinline__ void dg_zero_tile(const DgChain& c, int t) {
-  const uint4 z = make_uint4(0, 0, 0, 0);
-  for (int l = c.top; l >= 1; --l) {
-    if (c.row[l])
-      for (int i = 0; i < CH_KS * (DP == 3 ? 2 : 1); ++i)
-        reinterpret_cast<uint4*>(c.row[l] + ((size_t)(t >> 1) * CH_KS * 2 + (DP == 3 ? i : 2 * i)) * TILE_ELEMS +
-                                 (t & 1) * (CH_M * TK))[threadIdx.x] = z;
-    for (int g = 0; g < 2; ++g)
-      for (int kt = 2 * t; kt < 2 * t + 2 && kt < c.tr_ks; ++kt)
-        for (int h = 0; h < (TP == 3 ? 2 : 1); ++h)
-          for (int i = threadIdx.x; i < TILE_ELEMS / 8; i += CONSUMERS)
-            reinterpret_cast<uint4*>(c.tr[l] + (((size_t)g * c.tr_ks + kt) * 2 + h) * TILE_ELEMS)[i] = z;
-  }
+// quarter q's split as the transposed image's (epilogue<..., TRP>'s): rows n (row tile q / 2), k = m (k-step 4 t + m / 32
+// of the tile's rows); each 8 x 8 block is transposed in registers
+template <int TP, int DP>
+__device__ __forceinline__ void dg_put_tr(const ChainSplit<DP>& s, int q, uint16_t* tr, int tr_ks, int t) {
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int kt = 4 * t + (w >> 1);
+  if (kt >= tr_ks) return;
+  uint16_t* tp = tr + ((size_t)(q >> 1) * tr_ks + kt) * 2 * TILE_ELEMS;
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int core = (8 * (q & 1) + j) * (TK / 8) + 2 * (w & 1) + h;
+      reinterpret_cast<uint32_t*>(tp + core * 64)[lane] = movmatrix_trans(s[2 * j + h]);
+      if (TP == 3) reinterpret_cast<uint32_t*>(tp + TILE_ELEMS + core * 64)[lane] = movmatrix_trans(s[16 + 2 * j + h]);
+    }
 }
 
-// Persistent and warp-specialized as trunk_chain_kernel (tiles, ring, register hand-back, the two warpgroups splitting
-// N, each on its half of the activation buffer through Halves), with the mask words of a layer loaded before its MMAs.
-// Per layer and tile: MMAs (tc_gemm_nn's per output element); the mask (rows past M have no bits, so they are zero),
-// the column sums' per-warp partials, the split over this warpgroup's half of the layer's input in the activation
-// buffer (not after layer 1) once every warp has read that half; then, past a barrier of the warpgroup's own 4 warps,
-// the column sums' atomics and the global stores, which drain while the next layer's MMAs run.  The values and the
-// images' bytes are tc_gemm_nn's; the column sums add 64-row tiles instead of 128-row ones.
+// Persistent and warp-specialized as trunk_chain_kernel (128-row tiles, each warpgroup on its own 64 rows a quarter of
+// the columns at a time, the ring, register hand-back), with a quarter's mask words loaded before its MMAs.  Per quarter:
+// MMAs (tc_gemm_nn's per output element), the mask (rows past M have no bits, so they are zero), the column sums'
+// per-warp partials, the split, and from it the transposed image and the row image, which drain while the next
+// quarter's MMAs run.  After quarter 3 the warpgroup writes the four splits over its rows of the layer's input in the
+// activation buffer (not after layer 1), fences them and meets its own 4 warps at a named barrier; then come the column
+// sums' atomics (one per column per 64 rows) and quarter 3's global stores.  The values and the images' bytes are
+// tc_gemm_nn's; the column sums add 64-row blocks instead of 128-row tiles.
 // DP: the activation buffer's and row images' passes (the input gradients'), TP: the transposed images' (the weight
-// gradients').  DYN: c.M is a capacity, of which live_rows rows are computed.
+// gradients'), TP <= DP.  DYN: c.M is a capacity, of which live_rows rows are computed.
 template <int DP, int TP, bool DYN = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) dgrad_chain_kernel(const DgChain c, RowCount rc) {
+  static_assert(TP <= DP, "the transposed images are written from the activation buffer's split");
   extern __shared__ __align__(1024) uint8_t smem[];
   const int M = (int)live_rows<DYN, false>(c.M, rc);
   if (DYN && M == 0) return;
-  const int tiles = (M + TM - 1) / TM * 2;
+  const int tiles = (M + CH_M - 1) / CH_M;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + CH_BAR);
   uint64_t* empty = full + CH_STAGES;
   uint64_t* act_full = empty + CH_STAGES;
   uint64_t* act_empty = act_full + 1;
-  const Halves hv{act_empty + 1, act_empty + 3};
-  // [2][8 warps][128 columns]: a layer's partials go to the other buffer than the previous layer's, so a warp that is
+  // [2][8 warps][256 columns]: a layer's partials go to the other buffer than the previous layer's, so a warp that is
   // ahead never overwrites partials that the rest of its warpgroup has still to read
   float* red = reinterpret_cast<float*>(smem + CH_ENC);
   if (threadIdx.x == 0) {
@@ -1512,86 +1551,76 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) dgrad_chain_kernel(const DgCh
     }
     mbar_init(act_full, 1);
     mbar_init(act_empty, CONSUMERS / 32);
-    for (int h = 0; h < 2; ++h) {
-      mbar_init(&hv.rd[h], CONSUMERS / 32);
-      mbar_init(&hv.wr[h], 4);
-    }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   __syncthreads();
   if (threadIdx.x >= CONSUMERS) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
-    if (threadIdx.x == CONSUMERS) dg_produce<DP>(c, M, tiles, full, empty, act_full, act_empty);
+    if (threadIdx.x == CONSUMERS) dg_produce<DP>(c, tiles, full, empty, act_full, act_empty);
     return;
   }
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
-  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // p: generations of the activation buffer the epilogues have written (G[l-1] at layers l > 1).  Layer top reads the
-  // producer's copy (act_full), a layer l < top generation p - 1; a layer l > 1 writes generation p once every warp has
-  // read what it overwrites, the same layer's input.  r: layers run, for the column sums' buffer.
-  int it = 0, n = 0, p = 0, r = 0;
+  const int wg = threadIdx.x >> 7, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // r: layers run, for the column sums' buffer
+  int it = 0, n = 0, r = 0;
   for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
-    if (t * CH_M >= M) {
-      dg_zero_tile<DP, TP>(c, t);
-      continue;
-    }
     mbar_wait(act_full, n & 1);
     ++n;
     for (int l = c.top; l >= 1; --l, ++r) {
-      uint4 wd[2];
-      dg_mask_words(wd, c.bits[l], M, t);
-      float acc[64];
-      chain_mma<false, DP>(acc, CH_KS, CH_KS, it, full, empty, hv, l == c.top ? -1 : (p - 1) & 1, l > 1);
-      if (l == 1 && lane == 0) mbar_arrive(act_empty);
-      float* rb = red + (r & 1) * (CONSUMERS / 32) * TN;
-      const uint32_t wds[2][4] = {{wd[0].x, wd[0].y, wd[0].z, wd[0].w}, {wd[1].x, wd[1].y, wd[1].z, wd[1].w}};
+      float* rb = red + (r & 1) * (CONSUMERS / 32) * CH_W;
+      uint16_t* row = c.row[l] ? c.row[l] + (size_t)t * CH_KS * 2 * TILE_ELEMS : nullptr;
+      ChainSplit<DP> held[CH_Q - 1];
 #pragma unroll
-      for (int i = 0; i < 64; i += 2) {     // columns 8 j + 2 (lane % 4) + {0, 1} of word j / 4, j = i / 4
-        const int j = i >> 2;
-        const uint32_t k = wds[(i >> 1) & 1][j >> 2] >> (8 * (j & 3) + 2 * (lane & 3));
-        if (!(k & 1)) acc[i] = 0.f;
-        if (!(k & 2)) acc[i + 1] = 0.f;
-      }
-      // column sums as tile_colsum's: over the 16 rows of each warp (shuffles), then its warpgroup's 4 warps
+      for (int q = 0; q < CH_Q; ++q) {
+        uint2 wd[2];
+        dg_mask_words(wd, c.bits[l], M, t, q);
+        float acc[32];
+        chain_mma<false, DP>(acc, CH_KS, CH_KS, it, full, empty);
+        if (q == CH_Q - 1 && l == 1 && lane == 0) mbar_arrive(act_empty);
+        const uint32_t wds[2][2] = {{wd[0].x, wd[0].y}, {wd[1].x, wd[1].y}};
 #pragma unroll
-      for (int j = 0; j < 16; ++j)
-#pragma unroll
-        for (int cc = 0; cc < 2; ++cc) {
-          float s = acc[4 * j + cc] + acc[4 * j + 2 + cc];
-#pragma unroll
-          for (int o = 4; o < 32; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-          if (lane < 4) rb[w * TN + 8 * j + 2 * lane + cc] = s;
+        for (int i = 0; i < 32; i += 2) {     // columns 8 j + 2 (lane % 4) + {0, 1} of word j / 4, j = i / 4
+          const int j = i >> 2;
+          const uint32_t k = wds[(i >> 1) & 1][j >> 2] >> (8 * (j & 3) + 2 * (lane & 3));
+          if (!(k & 1)) acc[i] = 0.f;
+          if (!(k & 2)) acc[i + 1] = 0.f;
         }
-      if (l > 1) {
-        mbar_wait(&hv.rd[wg], p & 1);     // every warp has read this half of G[l]
-        chain_split<false, DP>(acc, reinterpret_cast<uint16_t*>(smem), CH_HALF, CH_HALF / 2);
-        chain_written(hv);
-        ++p;
-      }
-      warpgroup_sync();         // the warpgroup's partials are in rb
-      {
-        float s = 0.f;
+        // column sums as tile_colsum's: over the 16 rows of each warp (shuffles), then its warpgroup's 4 warps
 #pragma unroll
-        for (int i = 0; i < 4; ++i) s += rb[(4 * wg + i) * TN + (threadIdx.x & (TN - 1))];
-        atomicAdd(c.db[l] + threadIdx.x, s);
-      }
-      // the transposed image as epilogue<..., TRP>'s: rows n (row tile wg), k = m (k-step 2 t + wq / 2)
-      const int kt = 2 * t + (wq >> 1);
-      if (kt < c.tr_ks) {
-        uint16_t* tp = c.tr[l] + ((size_t)wg * c.tr_ks + kt) * 2 * TILE_ELEMS;
+        for (int j = 0; j < 8; ++j)
 #pragma unroll
-        for (int j = 0; j < 16; ++j)
+          for (int cc = 0; cc < 2; ++cc) {
+            float s = acc[4 * j + cc] + acc[4 * j + 2 + cc];
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            uint32_t hi, lo;
-            split2<false>(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], hi, lo);
-            const int core = j * (TK / 8) + 2 * (wq & 1) + h;
-            reinterpret_cast<uint32_t*>(tp + core * 64)[lane] = movmatrix_trans(hi);
-            if (TP == 3) reinterpret_cast<uint32_t*>(tp + TILE_ELEMS + core * 64)[lane] = movmatrix_trans(lo);
+            for (int o = 4; o < 32; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            if (lane < 4) rb[w * CH_W + q * 64 + 8 * j + 2 * lane + cc] = s;
           }
+        ChainSplit<DP> s;
+        chain_split<false, DP>(acc, s);
+        if (q == CH_Q - 1) {    // every MMA on this warpgroup's rows of G[l] has retired
+          if (l > 1) {
+            uint16_t* buf = reinterpret_cast<uint16_t*>(smem);
+#pragma unroll
+            for (int p = 0; p < CH_Q - 1; ++p) chain_put<DP>(held[p], p, buf, 2 * TILE_ELEMS, TILE_ELEMS);
+            chain_put<DP>(s, q, buf, 2 * TILE_ELEMS, TILE_ELEMS);
+            fence_proxy_async();
+          }
+          warpgroup_sync();     // the warpgroup's partials are in rb, its split in the activation buffer
+#pragma unroll
+          for (int i = 0; i < CH_W / 128; ++i) {
+            const int col = (threadIdx.x & 127) + 128 * i;
+            float sum = 0.f;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) sum += rb[(4 * wg + k) * CH_W + col];
+            atomicAdd(c.db[l] + col, sum);
+          }
+        } else if (l > 1) {
+#pragma unroll
+          for (int i = 0; i < (DP == 3 ? 32 : 16); ++i) held[q][i] = s[i];
+        }
+        dg_put_tr<TP, DP>(s, q, c.tr[l], c.tr_ks, t);
+        if (row) chain_put<DP>(s, q, row, 2 * TILE_ELEMS, TILE_ELEMS);
       }
-      if (c.row[l])
-        chain_split<false, DP>(acc, c.row[l] + (size_t)(t >> 1) * CH_KS * 2 * TILE_ELEMS + (t & 1) * (CH_M * TK), 2 * TILE_ELEMS, TILE_ELEMS);
     }
   }
 }
@@ -1600,16 +1629,26 @@ template <int DP, int TP>
 static int launch_dgrad_chain(const DgChain& c, int ctas, RowCount rc, cudaStream_t st) {
   auto kernel = rc.rows ? dgrad_chain_kernel<DP, TP, true> : dgrad_chain_kernel<DP, TP>;
   SPARF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM));
-  kernel<<<std::min(2 * ceil_div(c.M, TM), ctas), GEMM_THREADS, CH_SMEM, st>>>(c, rc);
+  kernel<<<std::min(ceil_div(c.M, CH_M), ctas), GEMM_THREADS, CH_SMEM, st>>>(c, rc);
   SPARF_CHECK_LAUNCH("dgrad_chain_kernel");
   return SPARF_OK;
 }
 
-template <bool F16, int PASSES, bool KFAST, class F, bool DYN = false>
+template <bool F16, int PASSES, bool KFAST, class F, bool DYN = false, bool QUARTERS = false>
 static int launch_pack(F f, int rtiles, int ksteps, uint16_t* img, cudaStream_t st, RowCount rc = {nullptr, 0}) {
-  pack_kernel<F16, PASSES, KFAST, F, DYN><<<dim3(ksteps, rtiles), 256, 0, st>>>(f, ksteps, img, rc);
+  pack_kernel<F16, PASSES, KFAST, F, DYN, QUARTERS><<<dim3(ksteps, rtiles), 256, 0, st>>>(f, ksteps, img, rc);
   SPARF_CHECK_LAUNCH("pack_kernel");
   return SPARF_OK;
+}
+
+// a fused chain's weight image: CH_W rows of B in quarters (pack_kernel's QUARTERS layout)
+template <bool KFAST, class F>
+static int pack_chain_weights(const TcPrec& p, F f, int ksteps, uint16_t* img, cudaStream_t st) {
+  constexpr int RT = CH_W / TM;
+  return p.f16 ? (p.passes == 3 ? launch_pack<true, 3, KFAST, F, false, true>(f, RT, ksteps, img, st)
+                                : launch_pack<true, 1, KFAST, F, false, true>(f, RT, ksteps, img, st))
+               : (p.passes == 3 ? launch_pack<false, 3, KFAST, F, false, true>(f, RT, ksteps, img, st)
+                                : launch_pack<false, 1, KFAST, F, false, true>(f, RT, ksteps, img, st));
 }
 
 template <bool F16, int PASSES, bool F32, int ROWP, int TRP>
@@ -1768,15 +1807,15 @@ int tc_chain_ksteps(int l, int skip, int E3p) { return chain_ks(l, skip, ceil_di
 
 int tc_pack_nt(TcPrec p, int N, int ks1, int K1v, int ks2, int K2v, const float* W, int ldw, int wcol2, TcImage img,
                cudaStream_t st) {
-  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && img.p && img.ks == ks1 + ks2, "tc_pack_nt: passes=%d ks=%d, %d + %d k-steps",
-                p.passes, img.ks, ks1, ks2);
-  return SPARF_WG_PACK(true, NtB{W, ldw, wcol2, K1v, K2v, N, ks1}, ceil_div(N, TM), img.ks, img.p, st);
+  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && N == CH_W && img.p && img.ks == ks1 + ks2,
+                "tc_pack_nt: passes=%d N=%d ks=%d, %d + %d k-steps", p.passes, N, img.ks, ks1, ks2);
+  return pack_chain_weights<true>(p, NtB{W, ldw, wcol2, K1v, K2v, N, ks1}, img.ks, img.p, st);
 }
 
 int tc_pack_nn(TcPrec p, int Kout, int N, int Kv, const float* W, int ldw, int wcol, TcImage img, cudaStream_t st) {
-  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && img.p && img.ks == ceil_div(N, TK), "tc_pack_nn: passes=%d ks=%d N=%d",
-                p.passes, img.ks, N);
-  return SPARF_WG_PACK(false, NnB{W, ldw, wcol, Kv, N}, ceil_div(Kout, TM), img.ks, img.p, st);
+  SPARF_REQUIRE((p.passes == 1 || p.passes == 3) && Kout == CH_W && img.p && img.ks == ceil_div(N, TK),
+                "tc_pack_nn: passes=%d Kout=%d ks=%d N=%d", p.passes, Kout, img.ks, N);
+  return pack_chain_weights<false>(p, NnB{W, ldw, wcol, Kv, N}, img.ks, img.p, st);
 }
 
 int tc_dgrad_chain(TcPrec dg, TcPrec wg, int M, int W, int top, TcImage in, const TcImage* wimg, const uint32_t* const* bits,

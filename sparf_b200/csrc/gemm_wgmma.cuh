@@ -56,15 +56,15 @@ int tc_pack_cols(TcPrec p, int M, int N, const float* X, int ldx, TcImage img, c
 int tc_gemm_nt(TcPrec p, int act, int M, int N, TcImage a1, int K1v, TcImage a2, int K2v, const float* W, int ldw, int wcol2,
                const float* bias, float* Y, int ldy, const TcOut& out, cudaStream_t st);
 // The fused trunk forward (trunk_chain_kernel): layers l = 0 ... nt-1 of width W, H[l] = relu(in_l W_l^T + bias[l]) with
-// in_0 = enc, in_l = H[l-1], [H[l-1] | enc] at l == skip, in one launch that keeps a 64-row tile's activations in shared
+// in_0 = enc, in_l = H[l-1], [H[l-1] | enc] at l == skip, in one launch that keeps a 128-row tile's activations in shared
 // memory from layer to layer.  Every H[l], and the last layer's row image, is bit-identical to what the same layers give
 // through tc_gemm_nt chained by row images.
 // Whether the kernel is built for a trunk of this shape (width 256, an encoding of at most 64 padded columns, at least 3 layers):
 bool tc_chain_supported(int W, int E3p, int nt, int skip);
 // k-steps of layer l's weight image
 int tc_chain_ksteps(int l, int skip, int E3p);
-// img = the B operand image tc_gemm_nt packs of W (N rows): ks1 k-steps of W[n][k], k < K1v, then ks2 of W[n][wcol2 + k],
-// k < K2v
+// img = the fused forward's weight image of W (N = 256 rows): the values tc_gemm_nt packs, ks1 k-steps of W[n][k], k < K1v,
+// then ks2 of W[n][wcol2 + k], k < K2v, in the chains' layout: per quarter of 64 rows its k-steps one after another
 int tc_pack_nt(TcPrec p, int N, int ks1, int K1v, int ks2, int K2v, const float* W, int ldw, int wcol2, TcImage img,
                cudaStream_t st);
 // wimg[l]: layer l's weight image (tc_pack_nt, tc_chain_ksteps(l) k-steps), all alive at once.  H[l] == NULL: that
@@ -73,14 +73,15 @@ int tc_pack_nt(TcPrec p, int N, int ks1, int K1v, int ks2, int K2v, const float*
 // last layer's row image (row_passes = p.passes, or 0: none).  p.rows as for the GEMMs.
 int tc_trunk_chain(TcPrec p, int M, int W, int nt, int skip, TcImage enc, const TcImage* wimg, const float* const* bias,
                    float* const* H, uint32_t* const* bits, const TcOut& last, cudaStream_t st);
-// img = the B operand image tc_gemm_nn packs of W (Kout rows k, contraction over N): W[n][wcol + k], k < Kv
+// img = the fused input gradients' weight image of W (Kout = 256 rows k, contraction over N): the values tc_gemm_nn packs,
+// W[n][wcol + k], k < Kv, in the chains' layout (as tc_pack_nt's)
 int tc_pack_nn(TcPrec p, int Kout, int N, int Kv, const float* W, int ldw, int wcol, TcImage img, cudaStream_t st);
 // The trunk backward's input gradients in one launch (dgrad_chain_kernel), width W = 256, for layers l = top ... 1:
 //   G[l-1] = (bit k of bits[l][m]) * sum_n G[l][m][n] W_l[n][k],  db[l][k] += sum_m G[l-1][m][k]
 // from G[top] as its row image `in` (dg passes) and wimg[l] (tc_pack_nn of W_l's first 256 columns, dg passes), keeping a
-// 64-row tile's gradient in shared memory from layer to layer.  G[l-1] leaves as its transposed image tr[l] (wg passes)
+// 128-row tile's gradient in shared memory from layer to layer.  G[l-1] leaves as its transposed image tr[l] (wg passes)
 // and, where row[l].p is not NULL, its row image (dg passes).  Values and images are bit-identical to tc_gemm_nn's with
-// the same bit masks (bf16 halves); the column sums add 64-row tiles.  dg.rows as for the GEMMs.
+// the same bit masks (bf16 halves); the column sums add 64-row blocks.  dg.rows as for the GEMMs.
 int tc_dgrad_chain(TcPrec dg, TcPrec wg, int M, int W, int top, TcImage in, const TcImage* wimg, const uint32_t* const* bits,
                    float* const* db, const TcImage* tr, const TcImage* row, cudaStream_t st);
 // D[m][k] = mask(m,k) * ( sum_n G[m][n] W[n][wcol+k] + r1_vec[m]*r1_row[k] )   (= or +=), G [M x N] as its row image.

@@ -1079,7 +1079,7 @@ static int trunk_backward_simt(const SparfMLP* mlp, const Call& c, long long Mc,
 // Layer by layer they ping-pong.  With the chained input gradients every transposed image of G_{nt-2} ... G_0 is alive
 // until the weight gradients that follow the chain, G_0's in G_{nt-1}'s buffer (whose weight gradient ran before the
 // chain); the chain's input is G_{nt-2}'s row image, and the row images it writes for the encoding's gradient go to the
-// two row buffers: G_0's over G_{nt-1}'s, G_skip's over G_{nt-2}'s, each 64-row tile of which is read only by the CTA
+// two row buffers: G_0's over G_{nt-1}'s, G_skip's over G_{nt-2}'s, each 128-row tile of which is read only by the CTA
 // that writes it there afterwards.
 static int grad_tr_buf(const MlpDims& d, bool chained, int l) { return chained ? (l ? d.nt - 1 - l : 0) : (d.nt - 1 - l) & 1; }
 static int grad_row(const MlpDims& d, bool chained, int l) {
